@@ -1,5 +1,5 @@
 /*
- * ivid_b200 — C ABI of the B200-native (sm_100a) multiview RGBD diffusion sampling hot path.
+ * ivid_b200 — C ABI of the Hopper-native (H100, sm_90a) multiview RGBD diffusion sampling hot path.
  *
  * The reference (JeffreyXiang/ivid) has no FFI layer: its boundary for this path is the Python class surface that
  * inference/sample.py resolves by name (sample.py:183-184,191-192,47-50).  The Python package `ivid_b200` mirrors
@@ -232,7 +232,7 @@ int ivid_warp_forward_backward(ivid_warp_t* w, const float* lin_depth0_host, con
  * Operator-level entry points (unit parity tests, profiling): the kernels the UNet is assembled from.
  * ------------------------------------------------------------------------------------------------------------------ */
 
-/* nn.Conv2d 3x3 pad 1 / 1x1 as tcgen05 implicit GEMM.  act_dev fp16 NHWC [N,H,W,Cin] (Cin % 64 == 0); w_host fp32
+/* nn.Conv2d 3x3 pad 1 / 1x1 as wgmma implicit GEMM.  act_dev fp16 NHWC [N,H,W,Cin] (Cin % 64 == 0); w_host fp32
  * [Cout,Cin,k,k] reference layout; optional 1x1 skip over act2_dev [N,H,W,Cin2] with w2_host [Cout,Cin2,1,1];
  * optional fp32 NHWC residual; out fp32 NHWC [N,H,W,Cout] (out_fp16 = 1: fp16). */
 int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,

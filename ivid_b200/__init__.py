@@ -1,4 +1,4 @@
-"""ivid_b200 — B200-native (sm_100a) sampling hot path of JeffreyXiang/ivid.
+"""ivid_b200 — Hopper-native (H100, sm_90a) sampling hot path of JeffreyXiang/ivid.
 
 Drop-in surface (same names as the reference packages `diffusion.backbones`, `diffusion.frameworks`,
 `diffusion.samplers`, `rgbd_3d`):

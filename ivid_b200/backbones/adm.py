@@ -1,7 +1,7 @@
 """AdmUnet2d — host-side mirror of the reference backbone class (diffusion/backbones/adm.py:289-566).
 
 Same constructor kwargs, same state-dict keys/shapes (enumerated from the native topology builder, so there is a single
-source of truth), same `.forward(x, times, classes)` contract — but the forward runs the hand-written sm_100a kernels
+source of truth), same `.forward(x, times, classes)` contract — but the forward runs the hand-written sm_90a kernels
 behind the C ABI (include/ivid_b200.h) instead of ~625 ATen/cuDNN launches.  There is no CPU path: calling forward
 without a CUDA device raises.
 """
@@ -148,7 +148,7 @@ class AdmUnet2d(nn.Module):
         """Pack the current parameters into the native device arena (fp16 K-major conv/GEMM operands etc.)."""
         dev = self.device
         if dev.type != "cuda":
-            raise RuntimeError("ivid_b200.AdmUnet2d runs on CUDA (sm_100a) only: call .cuda() first — there is no CPU path")
+            raise RuntimeError("ivid_b200.AdmUnet2d runs on CUDA (sm_90a) only: call .cuda() first — there is no CPU path")
         L = _lib.lib()
         sd = self.state_dict()
         for key, shp, _ in self._schema:

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a CUDA library (libivid_b200.so) with nvcc.
+"""In-tree build of the sm_90a CUDA library (libivid_b200.so) with nvcc.
 
 `python -m ivid_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU; the resulting .so is
 git-ignored but travels to the GPU box with the repo snapshot.
@@ -17,7 +17,7 @@ LIB = os.path.join(HERE, "libivid_b200.so")
 OBJ_DIR = os.path.join(HERE, "_build")
 SOURCES = ["host_util.cu", "ops.cu", "unet.cu", "sampler.cu", "warp.cu", "api.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -70,7 +70,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(6, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

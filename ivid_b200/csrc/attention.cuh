@@ -1,18 +1,16 @@
-// Fused QKV self-attention core (FlashAttention-style, no T x T matrix in HBM) on tcgen05 / TMEM.
+// Fused QKV self-attention core (FlashAttention-style, no T x T matrix in HBM) on Hopper wgmma.
 //   reference: QKVAttention.forward adm.py:233-253 — per (sample, head): softmax_fp32((q*d^-1/4)^T (k*d^-1/4)) v,
 //   legacy channel order [head][q|k|v][64] of the qkv projection (adm.py:246), head dim 64.
 //
 // Input : qkv  fp16 [N][T][3C]  (NHWC output of the qkv 1x1 GEMM); head h owns channels [192h, 192h+192) = q|k|v.
 // Output: o    fp16 [N][T][C]   channel = 64*h + d   (== reshape(bs, -1, length) of the reference).
 //
-// One CTA per (sample, head, 128-query tile), 64 keys per step.  warp0 = TMA producer, warp1 = MMA issuer (+TMEM
-// alloc), warps2-5 = softmax / correction / output (one thread per query row).  Everything that is matrix-shaped lives
-// in TMEM (128 columns per CTA, so FOUR CTAs are resident per SM and hide each other's serial
-// S -> softmax -> PV chain; with head dim 64 the kernel is bound by the exp2 (MUFU) rate, not by the tensor pipe):
-//   S = Q K^T  fp32 in columns [0,64);  the un-normalised probabilities P overwrite the same columns as packed fp16 and
-//   are consumed directly as the A operand of P V (tcgen05.mma with A in TMEM, V in shared memory as an MN-major
-//   operand);  O accumulates in columns [64,128) across key blocks and is rescaled in place when the running maximum
-//   moves (online softmax).  (q*s)(k*s) with s = 64^-1/4 is evaluated as (q.k) * 0.125 — an exact power of two.
+// One CTA per (sample, head, 128-query tile), two warpgroups of 64 query rows each, 64 keys per step.  Thread 0 drives a
+// four-deep TMA ring of K / V tiles shared by both warpgroups.  Per key block a warpgroup computes S = Q K^T into
+// registers (wgmma, Q and K from shared memory), turns it into un-normalised fp16 probabilities P in place and
+// accumulates O += P V with P as the register A operand (its fragment layout is the accumulator's) and V as an MN-major
+// shared-memory operand; the online-softmax rescale of O happens in registers.  (q*s)(k*s) with s = 64^-1/4 is
+// evaluated as (q.k) * 0.125 — an exact power of two.
 #pragma once
 #include "common.cuh"
 
@@ -28,231 +26,24 @@ struct AttnCfg {
   static constexpr int KV = 64;
   static constexpr int Q_BYTES = 128 * 64 * 2;
   static constexpr int KV_BYTES = KV * 64 * 2;
-  static constexpr int STAGES = 2;
+  static constexpr int STAGES = 4;
   static constexpr int SMEM_BYTES = Q_BYTES + STAGES * 2 * KV_BYTES + 1024 /*barriers*/ + 1024 /*align*/;
-  static constexpr int TMEM_COLS = 128;     // S|P [0,64) , O [64,128)
-  static constexpr int COL_S = 0, COL_P = 0, COL_O = 64;
-  static constexpr int THREADS = 192;
+  static constexpr int THREADS = 256;
 };
 
-// 2^x on the SFU without exp2f()'s denormal pre/post-scaling (two predicated FMULs and an FSETP per call: 20 % of the kernel's
-// instructions): inputs here are <= 0 after the running-maximum subtraction, results below 2^-126 flush to 0 and contribute
-// nothing to a sum whose largest term is >= 2^-8.
+// 2^x on the SFU without exp2f()'s denormal pre/post-scaling: inputs here are <= 0 after the running-maximum subtraction,
+// results below 2^-126 flush to 0 and contribute nothing to a sum whose largest term is >= 2^-8.
 __device__ __forceinline__ float ex2_ftz(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-__global__ void __launch_bounds__(192, 4)
-attention_kernel_v1(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapKV,
-                 const AttnParams p) {
-  using Cfg = AttnCfg;
-  constexpr int KV = Cfg::KV;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip would turn every later access into
-  // a generic LD / ST with 64-bit address arithmetic instead of LDS / STS
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;
-  uint8_t* sKV = smem + Cfg::Q_BYTES;                       // stage s: K at sKV + s*2*KV_BYTES, V right after
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + Cfg::STAGES * 2 * Cfg::KV_BYTES);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;      // [2]
-  uint64_t* kv_empty = bars + 3;     // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* p_full = bars + 6;
-  uint64_t* o_full = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = blockIdx.x % p.q_tiles;
-  const int head = (blockIdx.x / p.q_tiles) % p.heads;
-  const int n = blockIdx.x / (p.q_tiles * p.heads);
-  const int nkv = p.T / KV;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapKV);
-    mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);      // one arrive per softmax warp
-    mbar_init(o_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0 && lane == 0) {
-    // ------------------------------ TMA producer ------------------------------
-    mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
-    tma_load_3d(&mapQ, q_full, sQ, head * 192, qt * 128, n);
-    for (int j = 0; j < nkv; ++j) {
-      const int st = j & 1;
-      const uint32_t ph = (j >> 1) & 1;
-      mbar_wait(&kv_empty[st], ph ^ 1);
-      uint8_t* sk = sKV + st * 2 * Cfg::KV_BYTES;
-      mbar_arrive_expect_tx(&kv_full[st], 2 * Cfg::KV_BYTES);
-      tma_load_3d(&mapKV, &kv_full[st], sk, head * 192 + 64, j * KV, n);
-      tma_load_3d(&mapKV, &kv_full[st], sk + Cfg::KV_BYTES, head * 192 + 128, j * KV, n);
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ------------------------------ MMA issuer ------------------------------
-    constexpr uint32_t idesc_s = make_idesc_f16(128, KV, false, false, false);   // S[128,KV] = Q[128,64] K[KV,64]^T
-    constexpr uint32_t idesc_o = make_idesc_f16(128, 64, false, false, true);    // O[128,64] += P[128,KV] V[KV,64]
-    mbar_wait(q_full, 0);
-    const uint64_t dq = make_smem_desc_sw128(smem_u32(sQ), 1024, 16);
-    for (int j = 0; j < nkv; ++j) {
-      const int st = j & 1;
-      const uint32_t ph = (j >> 1) & 1;
-      mbar_wait(&kv_full[st], ph);
-      tc_fence_after();
-      const uint32_t sk = smem_u32(sKV + st * 2 * Cfg::KV_BYTES);
-      const uint64_t dk = make_smem_desc_sw128(sk, 1024, 16);
-      // S_j overwrites the columns P_{j-1} lived in: ordered behind PV_{j-1} by the in-order MMA pipe
-#pragma unroll
-      for (int k = 0; k < 4; ++k) mma_f16_ss(tmem_base + Cfg::COL_S, dq + 2 * k, dk + 2 * k, idesc_s, k != 0);
-      tc_commit(s_full);
-      mbar_wait(p_full, j & 1);          // P_j written and O rescaled by the softmax warps
-      tc_fence_after();
-      // V tile [KV rows][64 d] is an MN-major B operand: 16 kv rows (one MMA K step) = 2048 B
-      const uint64_t dv = make_smem_desc_sw128(sk + Cfg::KV_BYTES, 1024, 1024);
-#pragma unroll
-      for (int k = 0; k < KV / 16; ++k)
-        mma_f16_ts(tmem_base + Cfg::COL_O, tmem_base + Cfg::COL_P + 8 * k, dv + 128 * k, idesc_o, (j | k) != 0);
-      tc_commit(&kv_empty[st]);
-      tc_commit(o_full);
-    }
-  } else if (warp >= 2) {
-    // ------------------------------ softmax / correction / output ------------------------------
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    constexpr float kScaleLog2 = 0.125f * 1.4426950408889634f;   // (64^-1/4)^2 * log2(e)
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      // pass 1: row maximum (two 32-column loads; S is re-read in pass 2 instead of being held in 64 registers so that
-      // four CTAs fit the register file)
-      float mx = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < KV; c += 32) {
-        uint32_t sv[32];
-        tmem_ld_32x32b_x32(lane_addr + Cfg::COL_S + c, sv);
-        tc_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(sv[i]));
-      }
-      // lazy online softmax: the reference maximum of a row only moves when the new maximum exceeds it by more than
-      // 2^kLazy (probabilities stay <= 2^kLazy, far inside fp16 range, and O / l is independent of the reference), and
-      // the in-place rescale of O is skipped whenever no row of the warp moved.
-      constexpr float kLazy = 8.0f;
-      const float m_cand = fmaxf(m_run, mx * kScaleLog2);
-      const float m_new = (m_cand - m_run > kLazy) ? m_cand : m_run;      // m_run = -inf on the first block: always taken
-      const float alpha = ex2_ftz(m_run - m_new);
-      const bool rescale = __any_sync(0xffffffffu, alpha != 1.0f);
-      // pass 2: probabilities -> fp16 -> TMEM (A operand of P V).  P columns [c/2, c/2+16) overwrite S columns that
-      // have already been consumed by this thread (its own TMEM lane), never the half still to be read.
-      float lsum = 0.f;
-#pragma unroll
-      for (int c = 0; c < KV; c += 32) {
-        uint32_t sv[32];
-        tmem_ld_32x32b_x32(lane_addr + Cfg::COL_S + c, sv);
-        tc_wait_ld();
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = ex2_ftz(__uint_as_float(sv[i]) * kScaleLog2 - m_new);
-          const float p1 = ex2_ftz(__uint_as_float(sv[i + 1]) * kScaleLog2 - m_new);
-          lsum += p0 + p1;
-          pk[i >> 1] = pack_h2(p0, p1);
-        }
-        tmem_st_32x32b_x16(lane_addr + Cfg::COL_P + (c >> 1), pk);
-      }
-      l_run = l_run * alpha + lsum;
-      m_run = m_new;
-      if (j > 0 && rescale) {
-        // correction: rescale the running output in place (PV_{j-1} must have landed)
-        mbar_wait(o_full, (j - 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int c = 0; c < 64; c += 16) {
-          uint32_t o[16];
-          tmem_ld_32x32b_x16(lane_addr + Cfg::COL_O + c, o);
-          tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st_32x32b_x16(lane_addr + Cfg::COL_O + c, o);
-        }
-      }
-      tc_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-    }
-    mbar_wait(o_full, (nkv - 1) & 1);
-    tc_fence_after();
-    const int t = qt * 128 + row;
-    const float inv = 1.0f / l_run;
-    __half* o = p.out + (static_cast<size_t>(n) * p.T + t) * p.C + head * 64;
-#pragma unroll
-    for (int c = 0; c < 64; c += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(lane_addr + Cfg::COL_O + c, r);
-      tc_wait_ld();
-      if (t < p.T) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 v;
-          v.x = pack_h2(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-          v.y = pack_h2(__uint_as_float(r[i + 2]) * inv, __uint_as_float(r[i + 3]) * inv);
-          v.z = pack_h2(__uint_as_float(r[i + 4]) * inv, __uint_as_float(r[i + 5]) * inv);
-          v.w = pack_h2(__uint_as_float(r[i + 6]) * inv, __uint_as_float(r[i + 7]) * inv);
-          *reinterpret_cast<uint4*>(o + c + i) = v;
-        }
-      }
-    }
-    tc_fence_before();
-  }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-}
-
-
-// ----------------------------------------------------------------------------------------------------------------------
-// v2 (default): same tile shape and numerics, but the scores are DOUBLE-BUFFERED in TMEM (S0 | S1 | O = 192 columns, two
-// CTAs per SM) and the K/V ring has four stages: the MMA thread issues Q K^T of block j+2 right behind P V of block j, so
-// the softmax warps find the next S tile already waiting and the tensor pipe works while they exponentiate.  With head dim
-// 64 the kernel is then bound by the SFU (64 ex2 per thread per 64-key block = 512 MUFU cycles per warp against 271 tensor
-// cycles per block), not by the S -> softmax -> P V round trip of v1 (ncu r02b: 22 % of v1's samples sit in the softmax
-// warps' wait for s_full).  The whole 64-column score row is held in registers (one TMEM read instead of two).
-// ----------------------------------------------------------------------------------------------------------------------
-struct AttnCfg2 {
-  static constexpr int KV = 64;
-  static constexpr int Q_BYTES = 128 * 64 * 2;
-  static constexpr int KV_BYTES = KV * 64 * 2;
-  static constexpr int STAGES = 4;
-  static constexpr int SMEM_BYTES = Q_BYTES + STAGES * 2 * KV_BYTES + 1024 /*barriers*/ + 1024 /*align*/;
-  static constexpr int TMEM_COLS = 256;     // S0|P0 [0,64), S1|P1 [64,128), O [128,192)
-  static constexpr int COL_S = 0, COL_O = 128;
-  static constexpr int THREADS = 192;
-};
-
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(256, 2)
 attention_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapKV, const AttnParams p) {
-  using Cfg = AttnCfg2;
+  using Cfg = AttnCfg;
   constexpr int KV = Cfg::KV, ST = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip would turn every later access into
-  // a generic LD / ST with 64-bit address arithmetic instead of LDS / STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
   uint8_t* sKV = smem + Cfg::Q_BYTES;                       // stage s: K at sKV + s*2*KV_BYTES, V right after
@@ -260,175 +51,126 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;          // [ST]
   uint64_t* kv_empty = kv_full + ST;     // [ST]
-  uint64_t* s_full = kv_empty + ST;      // [2]
-  uint64_t* p_full = s_full + 2;         // [2]
-  uint64_t* o_full = p_full + 2;         // [2]: P V_j signals o_full[j & 1]
-  uint64_t* o_done = o_full + 2;         // the last P V
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;
   const int qt = blockIdx.x % p.q_tiles;
   const int head = (blockIdx.x / p.q_tiles) % p.heads;
   const int n = blockIdx.x / (p.q_tiles * p.heads);
   const int nkv = p.T / KV;
 
-  if (warp == 0 && lane == 0) {
+  auto load_kv = [&](int j) {
+    const int st = j % ST;
+    if (j >= ST) mbar_wait(&kv_empty[st], ((j / ST) - 1) & 1);
+    uint8_t* sk = sKV + st * 2 * Cfg::KV_BYTES;
+    mbar_arrive_expect_tx(&kv_full[st], 2 * Cfg::KV_BYTES);
+    tma_load_3d(&mapKV, &kv_full[st], sk, head * 192 + 64, j * KV, n);
+    tma_load_3d(&mapKV, &kv_full[st], sk + Cfg::KV_BYTES, head * 192 + 128, j * KV, n);
+  };
+  if (tid == 0) {
     tma_prefetch_desc(&mapQ);
     tma_prefetch_desc(&mapKV);
     mbar_init(q_full, 1);
-    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&s_full[b], 1); mbar_init(&p_full[b], 4); }      // p_full: one arrive per softmax warp
-    mbar_init(&o_full[0], 1); mbar_init(&o_full[1], 1);
-    mbar_init(o_done, 1);
+    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 8); }      // kv_empty: one arrive per warp
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0 && lane == 0) {
-    // ------------------------------ TMA producer ------------------------------
+  if (tid == 0) {
     mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
     tma_load_3d(&mapQ, q_full, sQ, head * 192, qt * 128, n);
-    for (int j = 0; j < nkv; ++j) {
-      const int st = j % ST;
-      const uint32_t ph = (j / ST) & 1;
-      mbar_wait(&kv_empty[st], ph ^ 1);
-      uint8_t* sk = sKV + st * 2 * Cfg::KV_BYTES;
-      mbar_arrive_expect_tx(&kv_full[st], 2 * Cfg::KV_BYTES);
-      tma_load_3d(&mapKV, &kv_full[st], sk, head * 192 + 64, j * KV, n);
-      tma_load_3d(&mapKV, &kv_full[st], sk + Cfg::KV_BYTES, head * 192 + 128, j * KV, n);
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ------------------------------ MMA issuer ------------------------------
-    constexpr uint32_t idesc_s = make_idesc_f16(128, KV, false, false, false);   // S[128,KV] = Q[128,64] K[KV,64]^T
-    constexpr uint32_t idesc_o = make_idesc_f16(128, 64, false, false, true);    // O[128,64] += P[128,KV] V[KV,64]
-    mbar_wait(q_full, 0);
-    const uint64_t dq = make_smem_desc_sw128(smem_u32(sQ), 1024, 16);
-    auto issue_qk = [&](int j) {         // S_{j&1} = Q K_j^T ; signals s_full[j&1]
-      const int st = j % ST;
-      mbar_wait(&kv_full[st], (j / ST) & 1);
-      tc_fence_after();
-      const uint64_t dk = make_smem_desc_sw128(smem_u32(sKV + st * 2 * Cfg::KV_BYTES), 1024, 16);
-      const uint32_t ds = tmem_base + Cfg::COL_S + (j & 1) * 64;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) mma_f16_ss(ds, dq + 2 * k, dk + 2 * k, idesc_s, k != 0);
-      tc_commit(&s_full[j & 1]);
-    };
-    issue_qk(0);
-    if (nkv > 1) issue_qk(1);
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(&p_full[j & 1], (j >> 1) & 1);          // P_j written (and O rescaled) by the softmax warps
-      tc_fence_after();
-      const int st = j % ST;
-      // V tile [KV rows][64 d] is an MN-major B operand: 16 kv rows (one MMA K step) = 2048 B
-      const uint64_t dv = make_smem_desc_sw128(smem_u32(sKV + st * 2 * Cfg::KV_BYTES) + Cfg::KV_BYTES, 1024, 1024);
-      const uint32_t dp = tmem_base + Cfg::COL_S + (j & 1) * 64;
-#pragma unroll
-      for (int k = 0; k < KV / 16; ++k)
-        mma_f16_ts(tmem_base + Cfg::COL_O, dp + 8 * k, dv + 128 * k, idesc_o, (j | k) != 0);
-      tc_commit(&kv_empty[st]);
-      tc_commit(&o_full[j & 1]);
-      if (j == nkv - 1) tc_commit(o_done);
-      // S_{j+2} overwrites the columns P_j lives in: ordered behind P V_j by the in-order MMA pipe
-      if (j + 2 < nkv) issue_qk(j + 2);
-    }
-  } else if (warp >= 2) {
-    // ------------------------------ softmax / correction / output ------------------------------
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    constexpr float kScaleLog2 = 0.125f * 1.4426950408889634f;   // (64^-1/4)^2 * log2(e)
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      const uint32_t scol = lane_addr + Cfg::COL_S + (j & 1) * 64;
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tc_fence_after();
-      uint32_t s0[32], s1[32];
-      tmem_ld_32x32b_x32(scol, s0);
-      tmem_ld_32x32b_x32(scol + 32, s1);
-      tc_wait_ld();
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) mx = fmaxf(mx, fmaxf(__uint_as_float(s0[i]), __uint_as_float(s1[i])));
-      // lazy online softmax (see v1): the row reference only moves when the maximum grows by more than 2^kLazy
-      constexpr float kLazy = 8.0f;
-      const float m_cand = fmaxf(m_run, mx * kScaleLog2);
-      const float m_new = (m_cand - m_run > kLazy) ? m_cand : m_run;      // m_run = -inf on the first block: always taken
-      const float alpha = ex2_ftz(m_run - m_new);
-      const bool rescale = __any_sync(0xffffffffu, alpha != 1.0f);
-      float lsum = 0.f;
-      uint32_t pk[16];
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        const float p0 = ex2_ftz(__uint_as_float(s0[i]) * kScaleLog2 - m_new);
-        const float p1 = ex2_ftz(__uint_as_float(s0[i + 1]) * kScaleLog2 - m_new);
-        lsum += p0 + p1;
-        pk[i >> 1] = pack_h2(p0, p1);
-      }
-      tmem_st_32x32b_x16(scol, pk);
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        const float p0 = ex2_ftz(__uint_as_float(s1[i]) * kScaleLog2 - m_new);
-        const float p1 = ex2_ftz(__uint_as_float(s1[i + 1]) * kScaleLog2 - m_new);
-        lsum += p0 + p1;
-        pk[i >> 1] = pack_h2(p0, p1);
-      }
-      tmem_st_32x32b_x16(scol + 16, pk);
-      l_run = l_run * alpha + lsum;
-      m_run = m_new;
-      if (j > 0 && rescale) {
-        // correction: rescale the running output in place (P V_{j-1} must have landed; P V_j is not issued before p_full).
-        // One barrier per parity of j: with S double-buffered a warp may be two blocks ahead of the P V pipe (S_j was
-        // computed before P V_{j-2} finished), and a parity wait on a single barrier one phase further back returns at once.
-        mbar_wait(&o_full[(j - 1) & 1], ((j - 1) >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int c = 0; c < 64; c += 16) {
-          uint32_t o[16];
-          tmem_ld_32x32b_x16(lane_addr + Cfg::COL_O + c, o);
-          tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st_32x32b_x16(lane_addr + Cfg::COL_O + c, o);
-        }
-      }
-      tc_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[j & 1]);
-    }
-    mbar_wait(o_done, 0);
-    tc_fence_after();
-    const int t = qt * 128 + row;
-    const float inv = 1.0f / l_run;
-    __half* o = p.out + (static_cast<size_t>(n) * p.T + t) * p.C + head * 64;
-#pragma unroll
-    for (int c = 0; c < 64; c += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(lane_addr + Cfg::COL_O + c, r);
-      tc_wait_ld();
-      if (t < p.T) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 v;
-          v.x = pack_h2(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-          v.y = pack_h2(__uint_as_float(r[i + 2]) * inv, __uint_as_float(r[i + 3]) * inv);
-          v.z = pack_h2(__uint_as_float(r[i + 4]) * inv, __uint_as_float(r[i + 5]) * inv);
-          v.w = pack_h2(__uint_as_float(r[i + 6]) * inv, __uint_as_float(r[i + 7]) * inv);
-          *reinterpret_cast<uint4*>(o + c + i) = v;
-        }
-      }
-    }
-    tc_fence_before();
+    for (int j = 0; j < ST && j < nkv; ++j) load_kv(j);
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+  constexpr float kScaleLog2 = 0.125f * 1.4426950408889634f;   // (64^-1/4)^2 * log2(e)
+  // lazy online softmax: the reference maximum of a row only moves when the new maximum exceeds it by more than 2^kLazy
+  // (probabilities stay <= 2^kLazy, far inside fp16 range, and O / l does not depend on the reference)
+  constexpr float kLazy = 8.0f;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};     // rows lane/4 and lane/4 + 8 of the warp
+  mbar_wait(q_full, 0);
+  const uint64_t dq = make_smem_desc_sw128(smem_u32(sQ) + wg * 64 * 128, 1024, 16);
+#pragma unroll 1
+  for (int j = 0; j < nkv; ++j) {
+    const int st = j % ST;
+    mbar_wait(&kv_full[st], (j / ST) & 1);
+    const uint32_t sk = smem_u32(sKV + st * 2 * Cfg::KV_BYTES);
+    const uint64_t dk = make_smem_desc_sw128(sk, 1024, 16);
+    float s[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss<64>(s, dq + 2 * k, dk + 2 * k, k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    // row maxima: a thread holds 16 columns of each of its two rows; the four lanes of a row combine theirs
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[4 * c], s[4 * c + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[4 * c + 2], s[4 * c + 3]));
+    }
+    float alpha[2], m_new[2], lsum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_cand = fmaxf(m_run[r], mx[r] * kScaleLog2);
+      m_new[r] = (m_cand - m_run[r] > kLazy) ? m_cand : m_run[r];      // m_run = -inf on the first block: always taken
+      alpha[r] = ex2_ftz(m_run[r] - m_new[r]);
+      m_run[r] = m_new[r];
+    }
+    // P (fp16) as the A operand of P V: K step k covers key columns [16k, 16k + 16) = accumulator groups 2k and 2k + 1
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const float p0 = ex2_ftz(s[4 * c] * kScaleLog2 - m_new[0]), p1 = ex2_ftz(s[4 * c + 1] * kScaleLog2 - m_new[0]);
+      const float p2 = ex2_ftz(s[4 * c + 2] * kScaleLog2 - m_new[1]), p3 = ex2_ftz(s[4 * c + 3] * kScaleLog2 - m_new[1]);
+      lsum[0] += p0 + p1;
+      lsum[1] += p2 + p3;
+      pa[c >> 1][(c & 1) * 2 + 0] = pack_h2(p0, p1);
+      pa[c >> 1][(c & 1) * 2 + 1] = pack_h2(p2, p3);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + lsum[r];
+    if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        o[4 * c] *= alpha[0]; o[4 * c + 1] *= alpha[0];
+        o[4 * c + 2] *= alpha[1]; o[4 * c + 3] *= alpha[1];
+      }
+    }
+    // V tile [KV rows][64 d] is an MN-major B operand: 16 kv rows (one MMA K step) = 2048 B
+    const uint64_t dv = make_smem_desc_sw128(sk + Cfg::KV_BYTES, 1024, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_rs_tb<64>(o, pa[k], dv + 128 * k, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+    if (tid == 0 && j + ST < nkv) load_kv(j + ST);
+  }
+  // row sums: combine the four lanes of each row
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int t = qt * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    if (t >= p.T) continue;
+    const float inv = 1.0f / l_run[r];
+    __half* out = p.out + (static_cast<size_t>(n) * p.T + t) * p.C + head * 64 + 2 * (lane & 3);
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+      *reinterpret_cast<uint32_t*>(out + 8 * c) = pack_h2(o[4 * c + 2 * r] * inv, o[4 * c + 2 * r + 1] * inv);
   }
 }
 

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution (3x3 pad 1 / 1x1) for NHWC fp16 activations on tcgen05 tensor cores.
+// Implicit-GEMM convolution (3x3 pad 1 / 1x1) for NHWC fp16 activations on Hopper wgmma tensor cores.
 //
 // Replaces, on the ADM UNet hot path, every nn.Conv2d / nn.Conv1d the reference issues through cuDNN:
 //   ResBlock2d in_layers[2] / out_layers[3] / skip_connection   (reference diffusion/backbones/adm.py:160,182,190)
@@ -6,16 +6,29 @@
 //   input conv / final out conv                                  (adm.py:369,486)
 //
 // GEMM view:  D[M = N*H*W pixels, Cout] = A[M, K] * B[Cout, K]^T,   K = sum over segments of taps*C_seg.
-//   A is never materialised (no im2col buffer): for every filter tap the producer issues one 4-D TMA box load
-//   (64 channels x TW x TH x TN pixels) at the tap-shifted coordinate; TMA's out-of-bounds zero fill implements the
-//   conv zero padding.  A second "segment" lets a 1x1 skip convolution over a different tensor (raw x) accumulate
-//   into the same TMEM tile as extra K slabs (SURVEY K2), so  skip(x) + conv(h)  is one kernel.
+//   A is never materialised (no im2col buffer): for every filter tap one 4-D TMA box load (64 channels x TW x TH x TN
+//   pixels) at the tap-shifted coordinate; TMA's out-of-bounds zero fill implements the conv zero padding.  Further
+//   "segments" let a 1x1 skip convolution over a different tensor (raw x) accumulate into the same tile as extra K slabs
+//   (SURVEY K2), so  skip(x) + conv(h)  is one kernel.
 //   B (weights) is packed [Cout_pad][K] fp16, K-major, loaded by 2-D TMA.
-// Both operands land in shared memory in the 128-byte-swizzled K-major layout that tcgen05.mma consumes directly.
+// Both operands land in shared memory in the 128-byte-swizzled K-major layout that wgmma reads directly.
 //
-// Persistent, warp-specialised:  warp0 = TMA producer, warp1 = MMA issuer (single thread), warp2 = TMEM allocator,
-// warps4-7 = epilogue (TMEM -> registers -> bias / residual / cast -> global).  Accumulators are double-buffered in TMEM
-// (2 x BN columns) so the epilogue of tile i overlaps the main loop of tile i+1.
+// Two warpgroups per CTA (rows 0-63 / 64-127 of a 128-pixel x BN tile), accumulators in registers.  Thread 0 also drives
+// the TMA ring: STAGES k-blocks are in flight, a slot is refilled as soon as all eight warps have retired the wgmma group
+// that read it.  Two CTAs fit one SM (BN <= 128), so one CTA's epilogue overlaps the other's main loop.
+// The epilogue works on the accumulator fragments in place: bias, residual (optionally through a nearest-2x upsample),
+// fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.
+//
+// Opt-in variants, selected when a launch is created (see conv_launch_create):
+//   kMc    cluster multicast on the low-resolution levels: a cluster of mc_m pixel tiles x mc_n column blocks; every CTA loads
+//          a 1/mc_n slice of its activation tile and a 1/mc_m slice of its weight tile and multicasts them to the CTAs of its
+//          row / column, which cuts the L2 -> shared-memory operand traffic per CTA.  A slot may be refilled once every CTA
+//          that receives this CTA's slices has consumed it, so the empty barriers count the warps of the row and column.
+//   kSlab  3x3 tap reuse: 8 x 16 pixel tiles; per 64-channel chunk and horizontal shift one [18 rows][8 px] slab is loaded
+//          and its three vertical taps are the same shared-memory bytes read through descriptors one slab row (1024 B, one
+//          swizzle atom) apart, with the three weight tiles of the taps in the same stage.
+//   contig persistent CTAs, each owning a contiguous range of the work list with the column block slow and the pixel tile
+//          fast (any kernel but kMc).
 #pragma once
 #include "common.cuh"
 
@@ -26,11 +39,6 @@ struct ConvGemmParams {
   int TW, TH, TN;              // pixel tile (TW*TH*TN == 128)
   int tiles_w, tiles_h, tiles_n;
   int n_blocks;                // Cout_pad / BN
-  int num_tiles;               // tiles_w*tiles_h*tiles_n*n_blocks
-  // Work list of a CTA (pair): items [0, full_items) are full BN-wide tiles; items [full_items, num_items) are the remaining
-  // tiles cut into two BN/2-wide halves each, so that the last, partially filled round of a small layer costs half a tile
-  // (wave quantisation on the 16x16 / 32x32 levels).  No split: full_items = num_items = num_tiles / kCtas.
-  int full_items, num_items;
   int seg_chunks[3];           // channels/64 of each K segment (0 = segment unused)
   int seg_taps[3];             // 9 (3x3) or 1 (1x1)
   int Cout;                    // valid output channels
@@ -39,947 +47,310 @@ struct ConvGemmParams {
   int out_mode;                // 0 = fp32 NHWC, 1 = fp16 NHWC, 2 = fp32 NCHW (Cout planes)
   const float* bias;           // [Cout_pad] fp32
   const float* residual;       // fp32 NHWC or nullptr
+  int res_up;                  // the residual is the nearest-2x upsample of a [N][H/2][W/2][ldr] tensor
   void* out;
-  double* stats;               // optional [N][Cout][2] per-(sample, channel) sum / sum-of-squares of the output (GroupNorm)
-  int res_up;                  // epi_tma == 1 only: the residual is the nearest-2x upsample of a half-resolution tensor (TW == 16)
-  int out16;                   // epi_tma == 1 only: also emit an fp16 copy of the output tile through maps.out16
-  int epi_tma;                 // 1: fp32 NHWC output (+ residual) moved by TMA through swizzled smem tiles; 2: fp16 NHWC output
-  int slab_mode;               // kSlab kernel: 1 = three [18][8]-pixel slabs per chunk (one per horizontal shift, 1024-byte-aligned descriptor
-                               // starts); 2 = ONE [18][16]-pixel slab per chunk, horizontal taps as descriptor starts 128 B apart INSIDE
-                               // a swizzle atom; 3 = ONE [18][10]-pixel slab (pitch 10 rows of 128 B, 8-row groups 1280 B apart), three
-                               // slots.  Measured rule (profiles/slab_probe_r02w.json): the 128-byte swizzle of tcgen05.mma operands is a
-                               // function of the absolute shared-memory address, so unaligned starts need matrix base offset 0
-                               // (base offset = row offset gives wrong products)
-  int fold;                    // kSlab modes 2 / 3 only: the GroupNorm affine + SiLU of the 3x3 segments is applied to the raw fp16 slab in shared
-                               // memory by the two spare warps (y = silu(A x + B), (A, B) per (sample, channel) from fold_ab; pixels
-                               // outside the image stay zero), so the separate GroupNorm-apply pass of that operand disappears
-  const float2* fold_ab;       // [N][fold_C]
-  int fold_C;                  // channels of the coefficient table (virtual concat width)
-  int fold_off[3];             // channel offset of each segment in the table; < 0: segment is consumed as loaded
-  int contig;                  // 1: a CTA (pair) owns a CONTIGUOUS range of the work list, column block slow / pixel tile fast, so that
-                               // its consecutive tiles belong to the same (sample, column block) and the GroupNorm statistics are
-                               // summed in registers and flushed with ONE pair of fp64 atomics per channel and sample instead of
-                               // one per tile (the per-tile atomics cost 2.7 ms of a 22 ms step: profiles/bench_r02q_dbg*.json)
-  int res3;                    // epi_tma == 1 with a residual: THREE residual tiles in flight per epilogue warp (the output staging
-                               // tile is then single-buffered): 48 instead of 32 KB of residual reads in flight per SM
-  int mc_n, mc_m;              // cluster-multicast mode (kMc): cluster = mc_m pixel tiles x mc_n column blocks
-  int debug;                   // perf attribution only (IVID_CONV_DEBUG): 1 = skip stats atomics, 2 = skip global load/store, 4 = skip smem transpose
+  __half* out16;               // optional fp16 NHWC copy of an fp32 NHWC output (same ldc)
+  double* stats;               // optional [N][Cout][2] per-(sample, channel) sum / sum-of-squares of the output (GroupNorm);
+                               // of the ROUNDED values when the output is fp16 (exactly what the next GroupNorm reads)
+  int contig;                  // persistent CTAs over contiguous ranges of the work list (column block slow)
+  int mc_n, mc_m;              // kMc: cluster = mc_m pixel tiles x mc_n column blocks
 };
 
-// kCtas == 2: a CTA pair (cluster of 2, one TPC) computes a 256-pixel x BN tile with tcgen05.mma.cta_group::2 — each CTA
-// stages its own 128 pixels of A and HALF of the weight tile, which cuts the L2 -> shared-memory operand traffic per
-// FLOP by a third and the per-stage footprint to 32 KB (4 stages + the TMA epilogue buffers fit in 227 KB).
 // All TMA descriptors of one launch, passed as a single __grid_constant__ argument.
 struct ConvMaps {
   CUtensorMap a[3];            // activation segments (fp16 NHWC)
   CUtensorMap b;               // packed weights
-  CUtensorMap bh;              // packed weights, half-width box (split tail items)
-  CUtensorMap out, res;        // epilogue: output tile store, residual tile load
-  CUtensorMap out16;           // optional fp16 copy of an fp32 output ([32 px][64 ch] boxes)
-  CUtensorMap a_mc[3];         // kMc: activation slice (128 / mc_n pixels) of each segment
+  CUtensorMap a_mc[3];         // kMc: activation slice (128 / mc_n pixels) of each segment; kSlab: [18][8]-pixel slab boxes
   CUtensorMap b_mc;            // kMc: weight slice (BN / mc_m rows)
 };
 
-template <int BN, int kCtas = 1>
+enum { kConvDefault = 0, kConvMc = 1, kConvSlab = 2 };
+
+template <int BN, int kMode = kConvDefault>
 struct ConvGemmCfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;
-  static constexpr int A_BYTES = BM * BK * 2;                  // 16 KB
-  static constexpr int B_BYTES = (BN / kCtas) * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + ((B_BYTES + 1023) / 1024) * 1024;
-  static constexpr int STAGES = (kCtas == 2) ? 4 : (BN == 256) ? 3 : (BN == 128) ? 4 : (BN == 64) ? 5 : 6;
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
-  static constexpr int BAR_BYTES = 1024;
-  static constexpr int STAT_BYTES = 8 * BN * 4;                                // [4 warps][sum|sumsq][BN] fp32
-  // per epilogue warp: 2 output staging tiles + 2 residual tiles of [32 pixels][32 channels] fp32 (4 KB each, 128B-swizzled)
-  // (+ one [32 px][64 ch] fp16 tile for the optional fp16 copy; not available in the single-CTA N=256 configuration)
-  static constexpr bool kHas16 = !(BN == 256 && kCtas == 1);
-  static constexpr int EPI_PER_WARP = (kHas16 ? 5 : 4) * 4096;
-  static constexpr int EPI_BYTES = 4 * EPI_PER_WARP;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + STAT_BYTES + EPI_BYTES + 1024;   // +1024 alignment slack
-  static constexpr int THREADS = 256;
-  static constexpr int THREADS_SLAB = 320;      // + warps 8, 9: with warps 2, 3 one operand-transform warp per scheduler (fold mode)
-  // kSlab (3x3 tap reuse): activation ring of [18 rows][8 px][64 ch] slabs, weight ring of [BN / kCtas][64] tap tiles
   static constexpr int SLAB_ROWS = 18;
-  static constexpr int SLAB_A_BYTES = SLAB_ROWS * 8 * BK * 2;                  // 18 KB
-  static constexpr int SLAB_SA = 3, SLAB_SB = 5;
-  // mode 2: [18 rows][16 px] slabs (36 KB), two of them, and a four-deep weight ring; mode 3: [18][10 px] slabs (22.5 KB in
-  // 23 KB slots), three of them
-  static constexpr int SLAB2_A_BYTES = SLAB_ROWS * 16 * BK * 2, SLAB2_SA = 2, SLAB2_SB = 4;
-  static constexpr int SLAB3_A_BYTES = SLAB_ROWS * 10 * BK * 2, SLAB3_SLOT = ((SLAB3_A_BYTES + 1023) / 1024) * 1024, SLAB3_SA = 3;
-  static constexpr int SLAB1_OPER = SLAB_SA * SLAB_A_BYTES + SLAB_SB * B_BYTES, SLAB2_OPER = SLAB2_SA * SLAB2_A_BYTES + SLAB2_SB * B_BYTES;
-  static constexpr int SLAB_OPER_BYTES = SLAB1_OPER > SLAB2_OPER ? SLAB1_OPER : SLAB2_OPER;
-  static constexpr int SMEM_BYTES_SLAB = SLAB_OPER_BYTES + BAR_BYTES + STAT_BYTES + EPI_BYTES + 1024;
+  static constexpr int A_BYTES = BM * BK * 2;                  // 16 KB
+  static constexpr int SLAB_A_BYTES = SLAB_ROWS * 8 * BK * 2;  // 18 KB
+  static constexpr int A_AREA = kMode == kConvSlab ? SLAB_A_BYTES : A_BYTES;
+  static constexpr int B_BYTES = ((BN * BK * 2 + 1023) / 1024) * 1024;
+  static constexpr int NB = kMode == kConvSlab ? 3 : 1;       // weight tiles per stage (slab: one per vertical tap)
+  static constexpr int STAGE_BYTES = A_AREA + NB * B_BYTES;
+  static constexpr int STAGES = (kMode == kConvSlab || BN == 128) ? 3 : 4;
+  static constexpr int BAR_BYTES = 128;
+  static constexpr int STAT_BYTES = 8 * 2 * BN * 4;            // [8 warps][sum|sumsq][BN] fp32
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + STAT_BYTES + 1024;   // +1024 alignment slack
+  static constexpr int THREADS = 256;
 };
 
-// kMc (cluster multicast, low-resolution levels): a cluster of mc_m x mc_n CTAs computes mc_m pixel tiles x mc_n column blocks.
-// The mc_n CTAs of a row need the SAME activation tile and the mc_m CTAs of a column the SAME weight tile, so every CTA loads
-// only a 1/mc_n slice of its activation tile and a 1/mc_m slice of its weight tile and multicasts them to its row / column:
-// the L2 -> shared-memory traffic per CTA and k-block drops from 32 KB to 16/mc_n + 16/mc_m KB (12 KB for 2 x 4), which is what
-// bounds the 8x8 level (M = 2048 pixels: every CTA used to stream its own operands, 9 TB/s of L2 reads at 590 TFLOP/s).
-// A stage may be refilled once every CTA that RECEIVES this CTA's slices has consumed it: the MMA commits arrive (multicast) on
-// the empty barriers of the whole row and column, which therefore count mc_n + mc_m - 1 arrivals.
-//
-// kSlab (3x3 tap reuse, CTA pairs): the pixel tile is 8 wide x 16 high.  Instead of nine tap-shifted 128-pixel boxes per 64-channel
-// chunk, the producer loads THREE [18 rows][8 px] slabs (one per horizontal shift dx, rows y0-1 .. y0+16, zero-filled outside the
-// image) and the three vertical taps of a slab are the same shared-memory bytes read through descriptors that start one slab
-// row (1024 B = one 8-row swizzle atom) apart.  L2 -> shared-memory activation traffic per chunk: 3 x 18 KB instead of 9 x 16 KB;
-// with the nine 16 KB weight tiles (own ring) the operand traffic per FLOP drops by 1.45x.  maps.a_mc[] hold the slab boxes.
-// Modes 2 / 3 (ConvGemmParams::slab_mode) load ONE slab per chunk ([18][16] or [18][10] pixels) and read the horizontal taps
-// through descriptor starts 128 B apart inside a swizzle atom (swizzle by absolute address: matrix base offset 0).  On those,
-// fold mode (ConvGemmParams::fold) lets warps 2, 3, 8, 9 (the kernel then runs 320 threads) apply the GroupNorm affine + SiLU
-// to the raw slab in place between the TMA barrier and the MMA's "operand ready" barrier.  All of it is opt-in (IVID_SLAB,
-// IVID_FOLD): measured slower than the tap-by-tap kernel + separate GroupNorm pass (DESIGN.md section 4).
-template <int BN, int kCtas = 1, bool kMc = false, bool kSlab = false>
-__global__ void __launch_bounds__(kSlab ? 320 : 256, 1)
+// position in the K loop: segment, tap (default / kMc) or horizontal shift (kSlab 3x3 segments), 64-channel chunk, and the
+// first packed weight column of the segment
+struct ConvKCursor {
+  int seg = 0, t = 0, ch = 0, base = 0;
+};
+
+template <int BN, int kMode = kConvDefault>
+__global__ void __launch_bounds__(256, kMode == kConvSlab ? 1 : 2)
 conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const ConvGemmParams p) {
-  using Cfg = ConvGemmCfg<BN, kCtas>;
+  using Cfg = ConvGemmCfg<BN, kMode>;
+  constexpr bool kMc = kMode == kConvMc, kSlab = kMode == kConvSlab;
   constexpr int STAGES = Cfg::STAGES;
-  static_assert(!kMc || kCtas == 1, "multicast mode uses single-CTA MMAs");
-  static_assert(!kSlab || (kCtas == 2 && !kMc), "slab mode is built for CTA pairs");
-  constexpr int NA = kSlab ? Cfg::SLAB_SA : STAGES;        // activation (or unified) ring depth
-  constexpr int NB = kSlab ? Cfg::SLAB_SB : 0;             // weight ring depth (slab mode only)
-  const uint32_t cta_rank = (kCtas == 2) ? cluster_ctarank() : 0u;
-  const int mc_rank = kMc ? static_cast<int>(cluster_ctarank()) : 0;
-  const int mc_rn = kMc ? mc_rank % p.mc_n : 0, mc_rm = kMc ? mc_rank / p.mc_n : 0;
+  extern __shared__ uint8_t smem_raw[];
+  // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
+  float* stat_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES);
+
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;                      // warpgroup: tile rows [64 wg, 64 wg + 64)
+
+  int mc_rn = 0, mc_rm = 0, csize = 1;
   uint16_t row_mask = 0, col_mask = 0;
   if constexpr (kMc) {
+    const int rank = static_cast<int>(cluster_ctarank());
+    csize = p.mc_n * p.mc_m;
+    mc_rn = rank % p.mc_n;
+    mc_rm = rank / p.mc_n;
     row_mask = static_cast<uint16_t>(((1u << p.mc_n) - 1u) << (mc_rm * p.mc_n));
     for (int i = 0; i < p.mc_m; ++i) col_mask |= static_cast<uint16_t>(1u << (i * p.mc_n + mc_rn));
   }
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip would turn every later access into
-  // a generic LD / ST with 64-bit address arithmetic instead of LDS / STS
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* stage_smem = smem + (kSlab ? Cfg::SLAB_OPER_BYTES : STAGES * Cfg::STAGE_BYTES);     // 1024-aligned (TMA 128B swizzle)
-  uint8_t* bar_area = stage_smem + Cfg::EPI_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bar_area);
-  uint64_t* empty_bar = full_bar + NA;
-  uint64_t* bfull_bar = empty_bar + NA;
-  uint64_t* bempty_bar = bfull_bar + NB;
-  uint64_t* tmem_full = bempty_bar + NB;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* res_full = tmem_empty + 2;                               // [4 warps][2 or 3 buffers]
-  uint64_t* araw_bar = res_full + 12;                                // [NA] fold mode: this CTA's raw slab has landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(araw_bar + NA);
-  float* stat_smem = reinterpret_cast<float*>(bar_area + Cfg::BAR_BYTES);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  if (tid == 0) {
     tma_prefetch_desc(&maps.a[0]);
     tma_prefetch_desc(&maps.b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < NA; ++s) {
-      // fold mode: the MMA thread's "operand ready" barrier counts one arrive per CTA of the pair (its transform warps)
-      mbar_init(&full_bar[s], (kSlab && p.fold) ? 2u : 1u);
-      mbar_init(&empty_bar[s], kMc ? static_cast<uint32_t>(p.mc_n + p.mc_m - 1) : 1u);
-      mbar_init(&araw_bar[s], 1);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      // one arrive per warp of every CTA that reads what this CTA loads (kMc: its cluster row and column)
+      mbar_init(&empty_bar[s], kMc ? 8u * static_cast<uint32_t>(p.mc_n + p.mc_m - 1) : 8u);
     }
-    for (int s = 0; s < NB; ++s) {
-      mbar_init(&bfull_bar[s], 1);
-      mbar_init(&bempty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 4 * kCtas);   // one arrive per epilogue warp (of both CTAs of a pair)
-    }
-    for (int i = 0; i < 12; ++i) mbar_init(&res_full[i], 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (kCtas == 2) tmem_alloc_2sm<Cfg::TMEM_COLS>(tmem_slot);
-    else tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
-  if constexpr (kCtas == 2 || kMc) cluster_sync_all(); else __syncthreads();      // peer barriers initialised before any remote signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if constexpr (kMc) cluster_sync_all(); else __syncthreads();      // peer barriers initialised before any remote signal
 
-  // work items of this CTA: tiles (kCtas == 1), tile PAIRS of its cluster (kCtas == 2; CTA `rank` owns m-tile 2*pair+rank) or
-  // cluster tiles (kMc: mc_m pixel tiles x mc_n column blocks; every CTA of a cluster walks the same item sequence)
-  const int mc_size = kMc ? p.mc_n * p.mc_m : 1;
-  int w_first = kMc ? static_cast<int>(blockIdx.x) / mc_size : (kCtas == 2) ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  int w_stride = kMc ? static_cast<int>(gridDim.x) / mc_size : (kCtas == 2) ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  int w_limit = p.num_items;
+  // work list: tiles (kMc: cluster tiles, every CTA of a cluster takes the same one)
+  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  int w_first = static_cast<int>(blockIdx.x) / csize, w_limit = w_first + 1;
   if (!kMc && p.contig) {
-    // contiguous ranges balanced by cost: a full item counts two units, a half-width tail item one.  CTA c owns the items whose
-    // first unit lies in [ceil(c U / G), ceil((c + 1) U / G))
-    const long long G = w_stride, c = w_first, F = p.full_items;
-    const long long U = 2 * F + (p.num_items - F);
-    auto first_item = [&](long long cc) -> int {
-      const long long u = (cc * U + G - 1) / G;
-      return static_cast<int>(u >= 2 * F ? F + (u - 2 * F) : (u + 1) / 2);
-    };
-    w_first = first_item(c);
-    w_limit = first_item(c + 1);
-    w_stride = 1;
+    const long long T = static_cast<long long>(m_tiles) * p.n_blocks, G = gridDim.x, c = blockIdx.x;
+    w_first = static_cast<int>(c * T / G);
+    w_limit = static_cast<int>((c + 1) * T / G);
   }
-  // work item -> (pixel-tile index of the CTA (pair), first output column, width)
-  auto decode = [&](int w, int& mtp, int& colbase, int& ncols) {
-    if constexpr (kMc) {
-      const int ncb = p.n_blocks / p.mc_n;
-      const int mt_c = w / ncb, nb_c = w - mt_c * ncb;
-      mtp = mt_c * p.mc_m + mc_rm;
-      colbase = (nb_c * p.mc_n + mc_rn) * BN;
-      ncols = BN;
-      return;
+  int nunits = 0;                                // K blocks (kSlab: slab units) per tile
+  for (int sg = 0; sg < 3; ++sg) nunits += p.seg_chunks[sg] * ((kSlab && p.seg_taps[sg] == 9) ? 3 : p.seg_taps[sg]);
+  auto advance = [&](ConvKCursor& c) {
+    const int taps = p.seg_taps[c.seg], chunks = p.seg_chunks[c.seg];
+    if (kSlab && taps == 9) {                    // chunk slow, horizontal shift fast
+      if (++c.t == 3) { c.t = 0; if (++c.ch == chunks) { c.ch = 0; c.base += 9 * chunks * 64; ++c.seg; } }
+    } else {                                     // tap slow, chunk fast
+      if (++c.ch == chunks) { c.ch = 0; if (++c.t == taps) { c.t = 0; c.base += taps * chunks * 64; ++c.seg; } }
     }
-    int f = w, half = 0;
-    ncols = BN;
-    if (w >= p.full_items) {
-      const int hidx = w - p.full_items;
-      f = p.full_items + (hidx >> 1);
-      half = hidx & 1;
-      ncols = BN / 2;
-    }
-    if (p.contig) {          // column block slow, pixel tile fast
-      const int m_items = (p.num_tiles / kCtas) / p.n_blocks;
-      const int nb = f / m_items;
-      mtp = f - nb * m_items;
-      colbase = nb * BN + half * (BN / 2);
-    } else {
-      mtp = f / p.n_blocks;
-      colbase = (f - mtp * p.n_blocks) * BN + half * (BN / 2);
-    }
+    while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
   };
+  const uint32_t empty0 = kMc ? smem_u32(&empty_bar[0]) : 0u;
 
-  const int kblks = p.seg_chunks[0] * p.seg_taps[0] + p.seg_chunks[1] * p.seg_taps[1] + p.seg_chunks[2] * p.seg_taps[2];
-  const int tiles_per_img = p.tiles_w * p.tiles_h;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  uint32_t g0 = 0;                               // ring position of the current tile's first unit
 
-  if (kSlab && warp == 0 && lane == 0) {
-    // ===================================== TMA producer, slab mode =====================================
-    if constexpr (kSlab) {
-      int sa = 0, sb = 0;
-      uint32_t pa = 0, pb = 0;
-      const uint32_t afull0 = mapa_cluster(smem_u32(&full_bar[0]), 0), bfull0 = mapa_cluster(smem_u32(&bfull_bar[0]), 0);
-      const bool wide = p.slab_mode >= 2, narrow = p.slab_mode == 3;
-      const int na = narrow ? Cfg::SLAB3_SA : wide ? Cfg::SLAB2_SA : Cfg::SLAB_SA, nb = wide ? Cfg::SLAB2_SB : Cfg::SLAB_SB;
-      const int a_slot = narrow ? Cfg::SLAB3_SLOT : wide ? Cfg::SLAB2_A_BYTES : Cfg::SLAB_A_BYTES;
-      const uint32_t a_bytes = narrow ? Cfg::SLAB3_A_BYTES : Cfg::SLAB2_A_BYTES;       // wide modes: bytes of one slab load
-      uint8_t* b_ring = smem + na * a_slot;
-      for (int w = w_first; w < w_limit; w += w_stride) {
-        int mtp, colbase, ncols;
-        decode(w, mtp, colbase, ncols);
-        const int mt = mtp * 2 + static_cast<int>(cta_rank);
-        const int tn = mt / tiles_per_img;
-        const int rem = mt - tn * tiles_per_img;
-        const int th = rem / p.tiles_w;
-        const int tw = rem - th * p.tiles_w;
-        const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
-        const bool full = ncols == BN;
-        const CUtensorMap* mapB = full ? &maps.b : &maps.bh;
-        const uint32_t b_bytes = full ? Cfg::B_BYTES : Cfg::B_BYTES / 2;
-        const int bcol = colbase + static_cast<int>(cta_rank) * (ncols / 2);
-        int seg_base = 0;
-        auto load_b = [&](int kcol) {
-          mbar_wait(&bempty_bar[sb], pb ^ 1);
-          if (cta_rank == 0) mbar_arrive_expect_tx(&bfull_bar[sb], 2 * b_bytes);
-          tma_load_2d_2sm(mapB, bfull0 + sb * 8, b_ring + sb * Cfg::B_BYTES, kcol, bcol);
-          if (++sb == nb) { sb = 0; pb ^= 1; }
-        };
 #pragma unroll 1
-        for (int seg = 0; seg < 3; ++seg) {
-          const int taps = p.seg_taps[seg];
-          const int chunks = p.seg_chunks[seg];
-          if (chunks == 0) continue;
-#pragma unroll 1
-          for (int ch = 0; ch < chunks; ++ch) {
-            if (taps == 9 && wide) {
-              mbar_wait(&empty_bar[sa], pa ^ 1);
-              if (p.fold) {          // each CTA's slab lands on its own barrier; its transform warps release it to the MMA thread
-                mbar_arrive_expect_tx(&araw_bar[sa], a_bytes);
-                tma_load_4d(&maps.a_mc[seg], &araw_bar[sa], smem + sa * a_slot, ch * 64, w0 - 1, h0 - 1, n0);
-              } else {
-                if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[sa], 2 * a_bytes);
-                tma_load_4d_2sm(&maps.a_mc[seg], afull0 + sa * 8, smem + sa * a_slot, ch * 64, w0 - 1, h0 - 1, n0);
-              }
-              if (++sa == na) { sa = 0; pa ^= 1; }
-#pragma unroll 1
-              for (int t = 0; t < 9; ++t) load_b(seg_base + (t * chunks + ch) * 64);
-            } else if (taps == 9) {
-#pragma unroll 1
-              for (int dx = 0; dx < 3; ++dx) {
-                mbar_wait(&empty_bar[sa], pa ^ 1);
-                if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[sa], 2 * Cfg::SLAB_A_BYTES);
-                tma_load_4d_2sm(&maps.a_mc[seg], afull0 + sa * 8, smem + sa * a_slot, ch * 64, w0 + dx - 1, h0 - 1, n0);
-                if (++sa == na) { sa = 0; pa ^= 1; }
-#pragma unroll 1
-                for (int dy = 0; dy < 3; ++dy) load_b(seg_base + ((dy * 3 + dx) * chunks + ch) * 64);
-              }
-            } else {
-              mbar_wait(&empty_bar[sa], pa ^ 1);
-              if (p.fold) {
-                mbar_arrive_expect_tx(&araw_bar[sa], Cfg::A_BYTES);
-                tma_load_4d(&maps.a[seg], &araw_bar[sa], smem + sa * a_slot, ch * 64, w0, h0, n0);
-              } else {
-                if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[sa], 2 * Cfg::A_BYTES);
-                tma_load_4d_2sm(&maps.a[seg], afull0 + sa * 8, smem + sa * a_slot, ch * 64, w0, h0, n0);
-              }
-              if (++sa == na) { sa = 0; pa ^= 1; }
-              load_b(seg_base + ch * 64);
-            }
-          }
-          seg_base += taps * chunks * 64;
-        }
-      }
+  for (int w = w_first; w < w_limit; ++w) {
+    int mt, nb;
+    if (kMc) {
+      const int ncb = p.n_blocks / p.mc_n;
+      mt = (w / ncb) * p.mc_m + mc_rm;
+      nb = (w % ncb) * p.mc_n + mc_rn;
+    } else if (p.contig) {                       // column block slow, pixel tile fast
+      nb = w / m_tiles;
+      mt = w - nb * m_tiles;
+    } else {                                     // column block fast: the CTAs that share an activation tile run together
+      mt = w / p.n_blocks;
+      nb = w - mt * p.n_blocks;
     }
-  } else if (kSlab && warp == 1 && lane == 0 && cta_rank == 0) {
-    // ===================================== MMA issuer, slab mode =====================================
-    if constexpr (kSlab) {
-      constexpr uint32_t idesc_full = make_idesc_f16(256, BN, false, false, false);
-      constexpr uint32_t idesc_half = make_idesc_f16(256, BN / 2, false, false, false);
-      int sa = 0, sb = 0;
-      uint32_t pa = 0, pb = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const bool wide = p.slab_mode >= 2, narrow = p.slab_mode == 3;
-      const int na = narrow ? Cfg::SLAB3_SA : wide ? Cfg::SLAB2_SA : Cfg::SLAB_SA, nb = wide ? Cfg::SLAB2_SB : Cfg::SLAB_SB;
-      const int a_slot = narrow ? Cfg::SLAB3_SLOT : wide ? Cfg::SLAB2_A_BYTES : Cfg::SLAB_A_BYTES;
-      const uint32_t row_pitch = narrow ? 10u * 128u : 16u * 128u;      // bytes between slab rows = between the 8-row groups of a tile
-      const uint32_t b_ring = smem_u32(smem + na * a_slot);
-      for (int w = w_first; w < w_limit; w += w_stride) {
-        const uint32_t idesc = (w >= p.full_items) ? idesc_half : idesc_full;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        uint32_t accum = 0;
-        // one weight tile against the 128 activation rows starting at a_addr (8-row groups `sbo` bytes apart)
-        auto tap = [&](uint32_t a_addr, uint32_t sbo = 1024, uint32_t bo = 0) {
-          mbar_wait(&bfull_bar[sb], pb);
-          tc_fence_after();
-          const uint64_t da = make_smem_desc_sw128_bo(a_addr, sbo, 16, bo);
-          const uint64_t db = make_smem_desc_sw128(b_ring + sb * Cfg::B_BYTES, 1024, 16);
+    const int colbase = nb * BN;
+    const int tiles_per_img = p.tiles_w * p.tiles_h;
+    const int tn = mt / tiles_per_img;
+    const int rem = mt - tn * tiles_per_img;
+    const int th = rem / p.tiles_w;
+    const int tw = rem - th * p.tiles_w;
+    const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
+
+    // producer (thread 0): units are issued strictly in order
+    ConvKCursor pc;
+    while (p.seg_chunks[pc.seg] == 0) ++pc.seg;
+    auto issue_load = [&](int u) {
+      const uint32_t g = g0 + static_cast<uint32_t>(u);
+      const int s = static_cast<int>(g % STAGES);
+      if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
+      const int taps = p.seg_taps[pc.seg], chunks = p.seg_chunks[pc.seg];
+      uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
+      uint8_t* sb = sa + Cfg::A_AREA;
+      if (kSlab && taps == 9) {
+        mbar_arrive_expect_tx(&full_bar[s], Cfg::SLAB_A_BYTES + 3 * BN * Cfg::BK * 2);
+        // slab rows y0-1 .. y0+16 at horizontal shift t - 1 (zero fill outside the image)
+        tma_load_4d(&maps.a_mc[pc.seg], &full_bar[s], sa, pc.ch * 64, w0 + pc.t - 1, h0 - 1, n0);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            mma_f16_ss_2sm(tmem_d, da + 2 * k, db + 2 * k, idesc, accum);
-            accum = 1u;
-          }
-          tc_commit_2sm(&bempty_bar[sb]);
-          if (++sb == nb) { sb = 0; pb ^= 1; }
-        };
-#pragma unroll 1
-        for (int seg = 0; seg < 3; ++seg) {
-          const int taps = p.seg_taps[seg];
-          const int chunks = p.seg_chunks[seg];
-          if (chunks == 0) continue;
-#pragma unroll 1
-          for (int ch = 0; ch < chunks; ++ch) {
-            const int nslab = (taps == 9 && !wide) ? 3 : 1;
-#pragma unroll 1
-            for (int dx = 0; dx < nslab; ++dx) {
-              mbar_wait(&full_bar[sa], pa);
-              tc_fence_after();
-              const uint32_t a_addr = smem_u32(smem + sa * a_slot);
-              if (taps == 9 && wide) {
-                // slab row dy = image row y0 - 1 + dy; pixel column dx = image column x0 - 1 + dx: the tile rows of tap (dy, dx)
-                // start (dy * pitch + dx) 128-byte rows into the slab; swizzle by absolute address, base offset 0
-#pragma unroll 1
-                for (int t = 0; t < 9; ++t) {
-                  const uint32_t tdy = t / 3, tdx = t - 3 * tdy;
-                  tap(a_addr + tdy * row_pitch + tdx * 128, row_pitch, 0u);
-                }
-              } else if (taps == 9) {
-#pragma unroll 1
-                for (int dy = 0; dy < 3; ++dy) tap(a_addr + dy * 1024);      // slab row dy = image row y0 - 1 + dy
-              } else {
-                tap(a_addr);
-              }
-              tc_commit_2sm(&empty_bar[sa]);
-              if (++sa == na) { sa = 0; pa ^= 1; }
-            }
-          }
+        for (int dy = 0; dy < 3; ++dy)
+          tma_load_2d(&maps.b, &full_bar[s], sb + dy * Cfg::B_BYTES, pc.base + ((dy * 3 + pc.t) * chunks + pc.ch) * 64, colbase);
+      } else {
+        const int dy = (taps == 9) ? (pc.t / 3 - 1) : 0;
+        const int dx = (taps == 9) ? (pc.t % 3 - 1) : 0;
+        const int kcol = pc.base + (pc.t * chunks + pc.ch) * 64;
+        mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
+        if constexpr (kMc) {
+          const int srows = 128 / p.mc_n;        // pixels of one activation slice (multiple of 8)
+          const int r0 = mc_rn * srows;
+          const int dn = r0 / (p.TW * p.TH), dh = (r0 / p.TW) % p.TH;
+          tma_load_4d_mc(&maps.a_mc[pc.seg], &full_bar[s], sa + r0 * 128, pc.ch * 64, w0 + dx, h0 + dy + dh, n0 + dn, row_mask);
+          const int brows = BN / p.mc_m;
+          tma_load_2d_mc(&maps.b_mc, &full_bar[s], sb + mc_rm * brows * 128, kcol, colbase + mc_rm * brows, col_mask);
+        } else {
+          tma_load_4d(&maps.a[pc.seg], &full_bar[s], sa, pc.ch * 64, w0 + dx, h0 + dy, n0);
+          tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
         }
-        tc_commit_2sm(&tmem_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       }
+      advance(pc);
+    };
+    if (tid == 0) {
+      for (int u = 0; u < STAGES && u < nunits; ++u) issue_load(u);
     }
-  } else if (kSlab && (warp == 2 || warp == 3 || warp >= 8)) {
-    // ===================================== operand transform (fold mode): GroupNorm affine + SiLU in place =====================
-    if constexpr (kSlab) {
-      if (p.fold) {
-        const int tt = warp < 4 ? static_cast<int>(threadIdx.x) - 64 : static_cast<int>(threadIdx.x) - 192;       // 0..127
-        const int cq = tt & 7, pq = tt >> 3;                     // logical 16-byte channel chunk, pixel phase (0..15)
-        const bool narrow = p.slab_mode == 3;
-        const int na = narrow ? Cfg::SLAB3_SA : Cfg::SLAB2_SA, a_slot = narrow ? Cfg::SLAB3_SLOT : Cfg::SLAB2_A_BYTES;
-        const int ppr = narrow ? 10 : 16;                        // 128-byte rows (pixels) per slab row
-        int sa = 0;
-        uint32_t pa = 0;
-        const uint32_t ready0 = mapa_cluster(smem_u32(&full_bar[0]), 0);
-        for (int w = w_first; w < w_limit; w += w_stride) {
-          int mtp, colbase, ncols;
-          decode(w, mtp, colbase, ncols);
-          const int mt = mtp * 2 + static_cast<int>(cta_rank);
-          const int tn = mt / tiles_per_img;
-          const int rem = mt - tn * tiles_per_img;
-          const int th = rem / p.tiles_w;
-          const int tw = rem - th * p.tiles_w;
-          const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
+
+    // ===================================== main loop =====================================
+    ConvKCursor cc;
+    while (p.seg_chunks[cc.seg] == 0) ++cc.seg;
 #pragma unroll 1
-          for (int seg = 0; seg < 3; ++seg) {
-            const int taps = p.seg_taps[seg];
-            const int chunks = p.seg_chunks[seg];
-            if (chunks == 0) continue;
-            const bool xform = taps == 9 && p.fold_off[seg] >= 0;
-#pragma unroll 1
-            for (int ch = 0; ch < chunks; ++ch) {
-              float cA[8], cB[8];
-              if (xform) {      // this thread's 8 channels of the chunk: issued before the wait for the slab
-                const float4* ab = reinterpret_cast<const float4*>(p.fold_ab + static_cast<size_t>(n0) * p.fold_C + p.fold_off[seg] + ch * 64 + cq * 8);
+    for (int u = 0; u < nunits; ++u) {
+      const uint32_t g = g0 + static_cast<uint32_t>(u);
+      const int s = static_cast<int>(g % STAGES);
+      mbar_wait(&full_bar[s], (g / STAGES) & 1);
+      const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
+      const uint32_t sb = sa + Cfg::A_AREA;
+      wgmma_fence();
+      if (kSlab && p.seg_taps[cc.seg] == 9) {
+        // tap (dy, shift): tile rows start dy slab rows (1024 B each) into the slab; warpgroup wg owns image rows 8 wg ..
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const float4 v = __ldg(ab + i);
-                  cA[2 * i] = v.x; cB[2 * i] = v.y; cA[2 * i + 1] = v.z; cB[2 * i + 1] = v.w;
-                }
-              }
-              mbar_wait(&araw_bar[sa], pa);
-              if (xform) {
-                uint8_t* slab = smem + sa * a_slot;
-                // pixels (srow, px), px = 0..9 (image columns x0-1 .. x0+8), of the [18][16 or 10]-pixel slab; 128-byte rows, 16-byte
-                // chunks XOR-swizzled with the row index (TMA SWIZZLE_128B, a function of the address: slots are 1024-byte aligned)
-#pragma unroll 4
-                for (int pp = pq; pp < Cfg::SLAB_ROWS * 10; pp += 16) {
-                  const int srow = pp / 10, px = pp - srow * 10;
-                  const int y = h0 - 1 + srow, x = w0 - 1 + px;
-                  if (y < 0 || y >= p.H || x < 0 || x >= p.W) continue;        // conv zero padding stays zero
-                  const int r = srow * ppr + px;
-                  uint4* ptr = reinterpret_cast<uint4*>(slab + r * 128 + ((cq ^ (r & 7)) << 4));
-                  const uint4 raw = *ptr;
-                  const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
-                  uint32_t pk[4];
+        for (int dy = 0; dy < 3; ++dy) {
+          const uint64_t da = make_smem_desc_sw128(sa + (dy + 8 * wg) * 1024, 1024, 16);
+          const uint64_t db = make_smem_desc_sw128(sb + dy * Cfg::B_BYTES, 1024, 16);
 #pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    const float2 f = __half22float2(h2[j]);
-                    const float y0 = silu_f(fmaf(f.x, cA[2 * j], cB[2 * j]));
-                    const float y1 = silu_f(fmaf(f.y, cA[2 * j + 1], cB[2 * j + 1]));
-                    pk[j] = pack_h2(y0, y1);
-                  }
-                  *ptr = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                }
-                fence_proxy_async_smem();      // the tensor core reads the slab through the async proxy
-              }
-              asm volatile("bar.sync 2, 128;\n" ::: "memory");
-              if (tt == 0) mbar_arrive_cluster(ready0 + sa * 8);
-              if (++sa == na) { sa = 0; pa ^= 1; }
-            }
-          }
+          for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | dy | k) != 0 ? 1u : 0u);
         }
-      }
-    }
-  } else if (!kSlab && warp == 0 && lane == 0) {
-    // ===================================== TMA producer =====================================
-    int stage = 0;
-    uint32_t phase = 0;
-    // 2-CTA: every load of either CTA signals the LEADER's full barrier (its MMA thread consumes both halves)
-    const uint32_t full0 = (kCtas == 2) ? mapa_cluster(smem_u32(&full_bar[0]), 0) : 0u;
-    for (int w = w_first; w < w_limit; w += w_stride) {
-      int mtp, colbase, ncols;
-      decode(w, mtp, colbase, ncols);
-      const int mt = mtp * kCtas + static_cast<int>(cta_rank);
-      const int tn = mt / tiles_per_img;
-      const int rem = mt - tn * tiles_per_img;
-      const int th = rem / p.tiles_w;
-      const int tw = rem - th * p.tiles_w;
-      const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
-      const bool full = ncols == BN;
-      const CUtensorMap* mapB = full ? &maps.b : &maps.bh;
-      const uint32_t b_bytes = full ? Cfg::B_BYTES : Cfg::B_BYTES / 2;
-      int kcol = 0;
-#pragma unroll 1
-      for (int seg = 0; seg < 3; ++seg) {
-        const CUtensorMap* mapA = &maps.a[seg];
-        const int taps = p.seg_taps[seg];
-        const int chunks = p.seg_chunks[seg];
-        if (chunks == 0) continue;
-#pragma unroll 1
-        for (int tap = 0; tap < taps; ++tap) {
-          const int dy = (taps == 9) ? (tap / 3 - 1) : 0;
-          const int dx = (taps == 9) ? (tap % 3 - 1) : 0;
-#pragma unroll 1
-          for (int ch = 0; ch < chunks; ++ch) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-            uint8_t* sb = sa + Cfg::A_BYTES;
-            if constexpr (kMc) {
-              // own barrier expects the whole tile; the bytes arrive as slices multicast by the CTAs of this row / column
-              mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_BYTES + Cfg::B_BYTES);
-              const int srows = 128 / p.mc_n;                       // pixels of one activation slice (multiple of 8)
-              const int r0 = mc_rn * srows;
-              const int dn = r0 / (p.TW * p.TH), dh = (r0 / p.TW) % p.TH;
-              tma_load_4d_mc(&maps.a_mc[seg], &full_bar[stage], sa + r0 * 128, ch * 64, w0 + dx, h0 + dy + dh, n0 + dn, row_mask);
-              const int brows = BN / p.mc_m;
-              tma_load_2d_mc(&maps.b_mc, &full_bar[stage], sb + mc_rm * brows * 128, kcol, colbase + mc_rm * brows, col_mask);
-            } else if constexpr (kCtas == 2) {
-              if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * (Cfg::A_BYTES + b_bytes));
-              const uint32_t bar = full0 + stage * 8;
-              tma_load_4d_2sm(mapA, bar, sa, ch * 64, w0 + dx, h0 + dy, n0);
-              tma_load_2d_2sm(mapB, bar, sb, kcol, colbase + static_cast<int>(cta_rank) * (ncols / 2));
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_BYTES + b_bytes);
-              tma_load_4d(mapA, &full_bar[stage], sa, ch * 64, w0 + dx, h0 + dy, n0);
-              tma_load_2d(mapB, &full_bar[stage], sb, kcol, colbase);
-            }
-            kcol += 64;
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (!kSlab && warp == 1 && lane == 0 && cta_rank == 0) {
-    // ===================================== MMA issuer (leader CTA only in 2-CTA mode) =====================================
-    constexpr uint32_t idesc_full = make_idesc_f16(128 * kCtas, BN, false, false, false);
-    constexpr uint32_t idesc_half = make_idesc_f16(128 * kCtas, BN >= 32 ? BN / 2 : BN, false, false, false);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int w = w_first; w < w_limit; w += w_stride) {
-      const uint32_t idesc = (w >= p.full_items) ? idesc_half : idesc_full;
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
-#pragma unroll 1
-      for (int kb = 0; kb < kblks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint32_t sb = sa + Cfg::A_BYTES;
-        const uint64_t da = make_smem_desc_sw128(sa, 1024, 16);
+      } else {
+        const uint64_t da = make_smem_desc_sw128(sa + wg * 64 * 128, 1024, 16);
         const uint64_t db = make_smem_desc_sw128(sb, 1024, 16);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          // advance 16 elements (32 B) along K inside the 128 B swizzle atom: +2 in the (addr >> 4) field
-          if constexpr (kCtas == 2) mma_f16_ss_2sm(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          else mma_f16_ss(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        // frees the smem slot (in both CTAs / in every CTA that multicasts into it) once the MMAs above have consumed it
-        if constexpr (kMc) tc_commit_mc(&empty_bar[stage], static_cast<uint16_t>(row_mask | col_mask));
-        else if constexpr (kCtas == 2) tc_commit_2sm(&empty_bar[stage]);
-        else tc_commit(&empty_bar[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
       }
-      // accumulator complete -> epilogue (of both CTAs)
-      if constexpr (kCtas == 2) tc_commit_2sm(&tmem_full[acc]); else tc_commit(&tmem_full[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================================== epilogue =====================================
-    const int quarter = warp & 3;          // TMEM lane quarter this warp may access
-    const int row = quarter * 32 + lane;   // row of the 128-pixel tile
-    const int pw = row % p.TW;
-    const int ph = (row / p.TW) % p.TH;
-    const int pn = row / (p.TW * p.TH);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    constexpr int CH = (BN >= 32) ? 32 : 16;
-    // ---- TMA epilogue state (CH == 32, fp32 NHWC): the warp's 32 rows form one box (32 ch, TW, box_h, box_n)
-    constexpr int NCH = BN / 32;
-    uint8_t* epi_base = stage_smem + quarter * Cfg::EPI_PER_WARP;   // out0 | out1 | res0 | res1 | out16, 4 KB each
-                                                                    // (res3: out | res0 | res1 | res2 | out16)
-    const uint32_t RD = p.res3 ? 3u : 2u;                           // residual tiles in flight
-    uint64_t* res_bar = res_full + quarter * 3;
-    auto res_tile = [&](uint32_t seq) -> uint8_t* {
-      return p.res3 ? epi_base + 4096 + (seq % 3u) * 4096 : epi_base + 8192 + (seq & 1u) * 4096;
-    };
-    const int box_h0 = (p.TW * p.TH >= 32) ? ((quarter * 32) / p.TW) % p.TH : 0;
-    const int box_n0 = (quarter * 32) / (p.TW * p.TH);
-    const bool tma_res = p.epi_tma == 1 && p.residual != nullptr && !(p.debug & 2);
-    uint32_t res_cnt = 0, res_issued = 0, out_cnt = 0;
-    // GroupNorm statistics of this CTA's consecutive tiles of one (sample, column block): thread t of the 128 epilogue threads owns
-    // columns t and t + 128 of the block; the sums run in fp64 registers and are flushed when the (sample, column block) changes
-    // and after the last item (contig schedule: ~once per CTA and sample; strided schedule: every tile, as before)
-    double acc_s[2] = {0.0, 0.0}, acc_q[2] = {0.0, 0.0};
-    int acc_tn = -1, acc_col0 = 0, acc_ncols = 0;
-    auto stats_flush = [&]() {
-      if (acc_tn < 0) return;
-      const int t = static_cast<int>(threadIdx.x) - 128;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int c = t + 128 * j;
-        const int col = acc_col0 + c;
-        if (c < acc_ncols && col < p.Cout && acc_tn < p.N && !(p.debug & 1)) {
-          double* st = p.stats + (static_cast<size_t>(acc_tn) * p.Cout + col) * 2;
-          atomicAdd(st, acc_s[j]);
-          atomicAdd(st + 1, acc_q[j]);
-        }
-        acc_s[j] = 0.0; acc_q[j] = 0.0;
-      }
-      acc_tn = -1;
-    };
-    // end-of-tile: combine the four epilogue warps' column sums (stat_smem) into the running sums
-    auto stats_tile = [&](int tn, int colbase, int ncols) {
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");
-      if (tn != acc_tn || colbase != acc_col0 || ncols != acc_ncols) {
-        stats_flush();
-        acc_tn = tn; acc_col0 = colbase; acc_ncols = ncols;
-      }
-      const int t = static_cast<int>(threadIdx.x) - 128;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int c = t + 128 * j;
-        if (c < ncols) {
-          float ssum = 0.f, qsum = 0.f;
-#pragma unroll
-          for (int w4 = 0; w4 < 4; ++w4) { ssum += stat_smem[(w4 * 2 + 0) * BN + c]; qsum += stat_smem[(w4 * 2 + 1) * BN + c]; }
-          acc_s[j] += static_cast<double>(ssum);
-          acc_q[j] += static_cast<double>(qsum);
-        }
-      }
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");
-    };
-    const uint32_t my_tiles = (w_first < w_limit) ? static_cast<uint32_t>((w_limit - w_first + w_stride - 1) / w_stride) : 0u;
-    // this CTA's items: first `my_full` full-width ones (NCH chunks each), then half-width ones (NCH / 2 chunks each)
-    const uint32_t my_full = (p.full_items > w_first) ? static_cast<uint32_t>((p.full_items - w_first + w_stride - 1) / w_stride) : 0u;
-    const uint32_t my_full_c = my_full < my_tiles ? my_full : my_tiles;
-    constexpr uint32_t NCHH = NCH >= 2 ? NCH / 2 : 1;
-    const uint32_t total_seq = my_full_c * NCH + (my_tiles - my_full_c) * NCHH;
-    // Residual prefetch cursor: the residual tiles are requested in the order the chunks are consumed (items of this CTA, 32-column
-    // chunks of an item).  The cursor keeps the decoded tile of the item it is in, so the integer divisions of the work-item
-    // decode run once per item and not once per chunk (they sat on the single epilogue warp's critical path).
-    uint32_t pf_item = 0;
-    int pf_k = 0, pf_nch = 0, pf_col = 0, pf_x = 0, pf_y = 0, pf_n = 0;
-    auto pf_load_item = [&]() {
-      const int w2 = w_first + static_cast<int>(pf_item) * w_stride;
-      int mtp2, colbase2, ncols2;
-      decode(w2, mtp2, colbase2, ncols2);
-      const int mt2 = mtp2 * kCtas + static_cast<int>(cta_rank);
-      const int tn2 = mt2 / tiles_per_img, rem2 = mt2 - tn2 * tiles_per_img;
-      const int th2 = rem2 / p.tiles_w, tw2 = rem2 - th2 * p.tiles_w;
-      pf_nch = ncols2 / 32; pf_col = colbase2; pf_k = 0;
-      pf_x = p.res_up ? (tw2 * p.TW) >> 1 : tw2 * p.TW;
-      pf_y = p.res_up ? (th2 * p.TH + box_h0) >> 1 : th2 * p.TH + box_h0;
-      pf_n = tn2 * p.TN + box_n0;
-    };
-    auto issue_res = [&](uint32_t seq) {      // lane 0: residual tile of chunk `seq` (== the cursor position) of this CTA's chunk stream
-      uint64_t* bar = &res_bar[seq % RD];
-      // res_up: the warp's 16 x 2 output pixels are the 2x2 replicas of 8 x 1 source pixels: a [32 ch][8][1][1] box (1 KB)
-      mbar_arrive_expect_tx(bar, p.res_up ? 1024u : 4096u);
-      tma_load_4d(&maps.res, bar, res_tile(seq), pf_col + pf_k * 32, pf_x, pf_y, pf_n);
-      if (++pf_k == pf_nch) {
-        ++pf_item;
-        if (pf_item < my_tiles) pf_load_item();
-      }
-    };
-    if constexpr (CH == 32) {
-      if (tma_res) {
-        if (lane == 0 && my_tiles > 0) {
-          pf_load_item();
-          for (uint32_t i = 0; i < RD && i < total_seq; ++i) issue_res(i);
-        }
-        res_issued = total_seq < RD ? total_seq : RD;
-      }
-    }
-    const uint32_t tmem_empty0 = (kCtas == 2) ? mapa_cluster(smem_u32(&tmem_empty[0]), 0) : 0u;
-    for (int wi = w_first; wi < w_limit; wi += w_stride) {
-      int mtp, colbase, ncols;
-      decode(wi, mtp, colbase, ncols);
-      const int mt = mtp * kCtas + static_cast<int>(cta_rank);
-      const int tn = mt / tiles_per_img;
-      const int rem = mt - tn * tiles_per_img;
-      const int th = rem / p.tiles_w;
-      const int tw = rem - th * p.tiles_w;
-      const int n = tn * p.TN + pn, h = th * p.TH + ph, w = tw * p.TW + pw;
-      const bool valid = (n < p.N) && (h < p.H) && (w < p.W);
-      const bool all_valid = __all_sync(0xffffffffu, valid);
-      const size_t pix = (static_cast<size_t>(n) * p.H + h) * p.W + w;
-
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
-      const bool do_stats = (CH == 32) && (p.stats != nullptr);
-      const int n_warp = tn * p.TN + (quarter * 32) / (p.TW * p.TH);     // sample of this warp's 32 rows (TW*TH >= 32)
-      if constexpr (CH == 16) {
-        // narrow output head (Cout <= 16, fp32 NCHW eps planes or tiny NHWC): direct stores, one row per thread
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < ncols; c0 += CH) {
-          uint32_t r[CH];
-          tmem_ld_32x32b_x16(taddr + c0, r);
-          tc_wait_ld();
-          const int col0 = colbase + c0;
-          if (!valid || col0 >= p.Cout) continue;
-#pragma unroll
-          for (int j = 0; j < CH; ++j) {
-            const int c = col0 + j;
-            if (c >= p.Cout) continue;
-            float v = __uint_as_float(r[j]) + __ldg(p.bias + c);
-            if (p.out_mode == 2) {
-              reinterpret_cast<float*>(p.out)[((static_cast<size_t>(n) * p.Cout + c) * p.H + h) * p.W + w] = v;
-            } else {
-              if (p.residual != nullptr) v += __ldg(p.residual + pix * p.ldr + c);
-              if (p.out_mode == 0) reinterpret_cast<float*>(p.out)[pix * p.ldc + c] = v;
-              else reinterpret_cast<__half*>(p.out)[pix * p.ldc + c] = __float2half_rn(v);
-            }
-          }
-        }
-      } else if (p.epi_tma == 1) {
-        // TMA epilogue (fp32 NHWC): per 32-column chunk the warp adds bias (+ residual tile fetched by TMA two chunks
-        // ahead, across tile boundaries) in the row-per-lane layout, writes the 128B-swizzled [32 px][32 ch] tile to
-        // shared memory and one lane issues a bulk tensor store; posted LSU stores from a single warp per SM
-        // sub-partition cannot keep enough bytes in flight, the TMA engine can.
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll 1
-        for (int k = 0; k < ncols / 32; ++k) {
-          const int c0 = k * 32;
-          const int col0 = colbase + c0;
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(taddr + c0, r);
-          float4 b4[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) b4[j] = ldg_f4(p.bias + col0 + 4 * j);
-          if (tma_res) mbar_wait(&res_bar[res_cnt % RD], (res_cnt / RD) & 1);
-          tc_wait_ld();
-          if (lane == 0) {      // the store that last used this staging tile (two chunks ago; res3: the previous one) has read it
-            if (p.res3) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
-          }
-          __syncwarp();
-          float4* ob = reinterpret_cast<float4*>(p.res3 ? epi_base : epi_base + (out_cnt & 1) * 4096);
-          const float4* rb = reinterpret_cast<const float4*>(res_tile(res_cnt));
-          // optional fp16 copy of the same values (operand of the next GroupNorm / skip conv): two 32-column chunks fill one
-          // [32 px][64 ch] tile; its store is committed BEFORE the odd chunk's fp32 store so that wait_group.read<1> at the
-          // top of the next chunk also covers it.
-          uint4* o16 = reinterpret_cast<uint4*>(epi_base + 16384);
-          const bool want16 = Cfg::kHas16 && p.out16;
-          float4 vprev = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int pos = lane * 8 + (j ^ (lane & 7));
-            float4 v = make_float4(__uint_as_float(r[4 * j]) + b4[j].x, __uint_as_float(r[4 * j + 1]) + b4[j].y,
-                                   __uint_as_float(r[4 * j + 2]) + b4[j].z, __uint_as_float(r[4 * j + 3]) + b4[j].w);
-            if (tma_res) {
-              const int rrow = (lane & 15) >> 1;        // res_up: source pixel of this lane's output pixel
-              const float4 t = p.res_up ? rb[rrow * 8 + (j ^ rrow)] : rb[pos];
-              v.x += t.x; v.y += t.y; v.z += t.z; v.w += t.w;
-            }
-            if (!all_valid && !valid) v = make_float4(0.f, 0.f, 0.f, 0.f);      // rows of the batch tail: clipped by TMA, zero for the statistics
-            ob[pos] = v;
-            if (want16) {
-              if (j & 1) {
-                uint4 pk;
-                pk.x = pack_h2(vprev.x, vprev.y); pk.y = pack_h2(vprev.z, vprev.w); pk.z = pack_h2(v.x, v.y); pk.w = pack_h2(v.z, v.w);
-                o16[lane * 8 + ((((k & 1) << 2) + (j >> 1)) ^ (lane & 7))] = pk;
-              } else {
-                vprev = v;
-              }
-            }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (Cfg::kHas16) {
-              if (p.out16 && (k & 1)) {
-                if (!(p.debug & 2)) tma_store_4d(&maps.out16, epi_base + 16384, col0 - 32, tw * p.TW, th * p.TH + box_h0, tn * p.TN + box_n0);
-                tma_store_commit();
-              }
-            }
-            if (!(p.debug & 2)) tma_store_4d(&maps.out, ob, col0, tw * p.TW, th * p.TH + box_h0, tn * p.TN + box_n0);
-            tma_store_commit();
-            if (tma_res && res_issued < total_seq) issue_res(res_issued);
-          }
-          if (tma_res) { if (res_issued < total_seq) ++res_issued; ++res_cnt; }
-          ++out_cnt;
-          if (do_stats) {
-            // column sums over the warp's 32 rows straight from the staged tile: lane = column
-            const float* of = reinterpret_cast<const float*>(ob);
-            float ssum = 0.f, qsum = 0.f;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              const float x = of[rr * 32 + ((((lane >> 2) ^ (rr & 7)) << 2) | (lane & 3))];
-              ssum += x;
-              qsum = fmaf(x, x, qsum);
-            }
-            if (p.TN == 1) {
-              stat_smem[(quarter * 2 + 0) * BN + c0 + lane] = ssum;
-              stat_smem[(quarter * 2 + 1) * BN + c0 + lane] = qsum;
-            } else if (n_warp < p.N) {
-              double* st = p.stats + (static_cast<size_t>(n_warp) * p.Cout + col0 + lane) * 2;
-              atomicAdd(st, static_cast<double>(ssum));
-              atomicAdd(st + 1, static_cast<double>(qsum));
-            }
-          }
-        }
-        if (do_stats && p.TN == 1) stats_tile(tn, colbase, ncols);
-      } else if (p.epi_tma == 2) {
-        // TMA epilogue, fp16 NHWC output (qkv projections, ResBlock hidden tensor): 64 columns per bulk store
-        // ([32 px][64 ch] fp16 = 128-byte rows); no residual on these paths.
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll 1
-        for (int k = 0; k < ncols / 64; ++k) {
-          const int c0 = k * 64;
-          const int col0 = colbase + c0;
-          uint32_t r0[32], r1[32];
-          tmem_ld_32x32b_x32(taddr + c0, r0);
-          tmem_ld_32x32b_x32(taddr + c0 + 32, r1);
-          tc_wait_ld();
-          if (lane == 0) tma_store_wait_read<1>();
-          __syncwarp();
-          uint4* ob = reinterpret_cast<uint4*>(epi_base + (out_cnt & 1) * 4096);
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {          // 8 columns (16 bytes of fp16) per step
-            const uint32_t* src = jj < 4 ? r0 + 8 * jj : r1 + 8 * (jj - 4);
-            const float4 ba = ldg_f4(p.bias + col0 + 8 * jj), bb = ldg_f4(p.bias + col0 + 8 * jj + 4);
-            uint4 pk;
-            pk.x = pack_h2(__uint_as_float(src[0]) + ba.x, __uint_as_float(src[1]) + ba.y);
-            pk.y = pack_h2(__uint_as_float(src[2]) + ba.z, __uint_as_float(src[3]) + ba.w);
-            pk.z = pack_h2(__uint_as_float(src[4]) + bb.x, __uint_as_float(src[5]) + bb.y);
-            pk.w = pack_h2(__uint_as_float(src[6]) + bb.z, __uint_as_float(src[7]) + bb.w);
-            if (!valid) pk = make_uint4(0u, 0u, 0u, 0u);
-            ob[lane * 8 + (jj ^ (lane & 7))] = pk;
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (!(p.debug & 2)) tma_store_4d(&maps.out, ob, col0, tw * p.TW, th * p.TH + box_h0, tn * p.TN + box_n0);
-            tma_store_commit();
-          }
-          ++out_cnt;
-          if (do_stats) {
-            // statistics of the ROUNDED tensor (exactly what the next GroupNorm will read): lane owns columns 2l, 2l+1
-            const __half2* oh = reinterpret_cast<const __half2*>(ob);
-            float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              const float2 x = __half22float2(oh[rr * 32 + ((((lane >> 2) ^ (rr & 7)) << 2) | (lane & 3))]);
-              s0 += x.x; s1 += x.y;
-              q0 = fmaf(x.x, x.x, q0); q1 = fmaf(x.y, x.y, q1);
-            }
-            if (p.TN == 1) {
-              stat_smem[(quarter * 2 + 0) * BN + c0 + 2 * lane] = s0;
-              stat_smem[(quarter * 2 + 0) * BN + c0 + 2 * lane + 1] = s1;
-              stat_smem[(quarter * 2 + 1) * BN + c0 + 2 * lane] = q0;
-              stat_smem[(quarter * 2 + 1) * BN + c0 + 2 * lane + 1] = q1;
-            } else if (n_warp < p.N) {
-              double* st = p.stats + (static_cast<size_t>(n_warp) * p.Cout + col0 + 2 * lane) * 2;
-              atomicAdd(st, static_cast<double>(s0)); atomicAdd(st + 1, static_cast<double>(q0));
-              atomicAdd(st + 2, static_cast<double>(s1)); atomicAdd(st + 3, static_cast<double>(q1));
-            }
-          }
-        }
-        if (do_stats && p.TN == 1) stats_tile(tn, colbase, ncols);
-      } else {
-        // Coalesced epilogue: the warp's 32 rows x 32 columns chunk goes TMEM -> registers (row per lane) -> XOR-swizzled
-        // shared memory -> registers (8 lanes per row, 4 columns each), so every global access is a full 128-byte row
-        // segment.  Bias, residual, GroupNorm statistics and the output cast are applied in that second layout.
-        float4* stage = reinterpret_cast<float4*>(stage_smem) + quarter * 256;      // [32 rows][8 float4], 4 KB per warp
-        const int sub_row = lane >> 3, cq = lane & 7;
-        // pixel offsets / validity of the 8 rows this lane touches in the second layout
-        size_t pix_i[8];
-        bool ok_i[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int R = quarter * 32 + i * 4 + sub_row;
-          const int rw = R % p.TW, rh = (R / p.TW) % p.TH, rn = R / (p.TW * p.TH);
-          const int nn = tn * p.TN + rn, hh = th * p.TH + rh, ww = tw * p.TW + rw;
-          ok_i[i] = (nn < p.N) && (hh < p.H) && (ww < p.W);
-          pix_i[i] = (static_cast<size_t>(nn) * p.H + hh) * p.W + ww;
-        }
-        // residual / bias of the first chunk are requested before the accumulator is even ready; inside the loop the
-        // NEXT chunk's are requested before the current chunk is processed, so one warp keeps 2 x 4 KB of reads in flight
-        // (the single epilogue warp per SM sub-partition is otherwise bound by global-load latency, not bandwidth).
-        const bool has_res = p.residual != nullptr && !(p.debug & 2);
-        float4 res_nx[8], b4_nx;
-        auto prefetch = [&](int c0n) {
-          const int colq_n = colbase + c0n + cq * 4;
-          const bool okc = colq_n < p.Cout;
-          b4_nx = okc ? ldg_f4(p.bias + colq_n) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            res_nx[i] = (has_res && okc && ok_i[i]) ? ldg_f4(p.residual + pix_i[i] * p.ldr + colq_n) : make_float4(0.f, 0.f, 0.f, 0.f);
-        };
-        prefetch(0);
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < ncols; c0 += CH) {
-          uint32_t r[CH];
-          tmem_ld_32x32b_x32(taddr + c0, r);
-          tc_wait_ld();
-          const int col0 = colbase + c0;
-          if (col0 >= p.Cout) continue;                   // padded output columns (warp-uniform)
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            stage[lane * 8 + (j ^ (lane & 7))] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                                             __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-          __syncwarp();
-          const int colq = col0 + cq * 4;
-          const bool col_ok = colq < p.Cout;
-          float4 res[8];
-          const float4 b4 = b4_nx;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) res[i] = res_nx[i];
-          if (c0 + CH < ncols) prefetch(c0 + CH);
-          float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = i * 4 + sub_row;
-            float4 v = stage[rr * 8 + (cq ^ (rr & 7))];
-            if (ok_i[i] && col_ok && !(p.debug & 2)) {
-              v.x = (v.x + b4.x) + res[i].x; v.y = (v.y + b4.y) + res[i].y; v.z = (v.z + b4.z) + res[i].z; v.w = (v.w + b4.w) + res[i].w;
-              if (p.out_mode == 0) {
-                stg_f4(reinterpret_cast<float*>(p.out) + pix_i[i] * p.ldc + colq, v);
-              } else {
-                uint2 pk;
-                pk.x = pack_h2(v.x, v.y);
-                pk.y = pack_h2(v.z, v.w);
-                *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + pix_i[i] * p.ldc + colq) = pk;
-              }
-              s4[0] += v.x; s4[1] += v.y; s4[2] += v.z; s4[3] += v.w;
-              q4[0] += v.x * v.x; q4[1] += v.y * v.y; q4[2] += v.z * v.z; q4[3] += v.w * v.w;
-            }
-          }
-          __syncwarp();
-          if (do_stats) {
-            // GroupNorm statistics of the tensor being written (consumed by the NEXT norm): reduce the 4 lanes that
-            // share a column quad; lanes 0..7 then own columns [col0 + 4*lane, +4)
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              s4[k] += __shfl_xor_sync(0xffffffffu, s4[k], 8);
-              q4[k] += __shfl_xor_sync(0xffffffffu, q4[k], 8);
-              s4[k] += __shfl_xor_sync(0xffffffffu, s4[k], 16);
-              q4[k] += __shfl_xor_sync(0xffffffffu, q4[k], 16);
-            }
-            if (lane < 8) {
-              if (p.TN == 1) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  stat_smem[(quarter * 2 + 0) * BN + c0 + lane * 4 + k] = s4[k];
-                  stat_smem[(quarter * 2 + 1) * BN + c0 + lane * 4 + k] = q4[k];
-                }
-              } else if (n_warp < p.N && col_ok) {
-                double* st = p.stats + (static_cast<size_t>(n_warp) * p.Cout + colq) * 2;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  atomicAdd(st + 2 * k, static_cast<double>(s4[k]));
-                  atomicAdd(st + 2 * k + 1, static_cast<double>(q4[k]));
-                }
-              }
-            }
-          }
-        }
-        if (do_stats && p.TN == 1) stats_tile(tn, colbase, ncols);
-      }
-      tc_fence_before();
+      wgmma_commit();
+      // retired before the slot is released: a wgmma group still in flight across thread 0's refill branch would make ptxas
+      // serialise every wgmma; the other warpgroups on the SM keep the tensor cores busy meanwhile
+      wgmma_wait<0>();
+      reg_fence(acc);
       __syncwarp();
       if (lane == 0) {
-        if constexpr (kCtas == 2) mbar_arrive_cluster(tmem_empty0 + acc * 8);      // the leader's MMA thread waits for both CTAs
-        else mbar_arrive(&tmem_empty[acc]);
+        if constexpr (kMc) {
+          for (int r = 0; r < csize; ++r)
+            if (r / p.mc_n == mc_rm || r % p.mc_n == mc_rn) mbar_arrive_cluster(mapa_cluster(empty0 + s * 8, static_cast<uint32_t>(r)));
+        } else {
+          mbar_arrive(&empty_bar[s]);
+        }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      if (tid == 0 && u + STAGES < nunits) issue_load(u + STAGES);
+      advance(cc);
     }
-    stats_flush();
-    if (p.epi_tma && lane == 0) tma_store_wait_all();
-  }
+    g0 += static_cast<uint32_t>(nunits);
 
-  tc_fence_before();
-  if constexpr (kCtas == 2 || kMc) cluster_sync_all(); else __syncthreads();      // the peers' smem / TMEM stay alive until all are done
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (kCtas == 2) tmem_dealloc_2sm<Cfg::TMEM_COLS>(tmem_base);
-    else tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    // ===================================== epilogue =====================================
+    const int wr = warp & 3;
+    const int quad = lane & 3;
+    int pn[2], ph[2], pw[2];
+    bool ok[2];
+    size_t pix[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
+      const int n = n0 + row / (p.TW * p.TH), h = h0 + (row / p.TW) % p.TH, x = w0 + row % p.TW;
+      ok[i] = n < p.N;                           // rows of the batch tail (TMA zero fill) are not written
+      pix[i] = (static_cast<size_t>(n) * p.H + h) * p.W + x;
+      pn[i] = n; ph[i] = h; pw[i] = x;
+    }
+    const bool do_stats = p.stats != nullptr;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = colbase + 8 * j + 2 * quad;  // this thread's column pair
+      float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+      if (c < p.Cout) {
+        const float2 b = make_float2(__ldg(p.bias + c), __ldg(p.bias + c + 1));
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (!ok[i]) continue;
+          float v0 = acc[4 * j + 2 * i] + b.x, v1 = acc[4 * j + 2 * i + 1] + b.y;
+          if (p.out_mode == 2) {
+            float* o = reinterpret_cast<float*>(p.out);
+            o[((static_cast<size_t>(pn[i]) * p.Cout + c) * p.H + ph[i]) * p.W + pw[i]] = v0;
+            if (c + 1 < p.Cout) o[((static_cast<size_t>(pn[i]) * p.Cout + c + 1) * p.H + ph[i]) * p.W + pw[i]] = v1;
+            continue;
+          }
+          if (p.residual != nullptr) {
+            const size_t rpix = p.res_up ? (static_cast<size_t>(pn[i]) * (p.H >> 1) + (ph[i] >> 1)) * (p.W >> 1) + (pw[i] >> 1) : pix[i];
+            const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + rpix * p.ldr + c));
+            v0 += r.x; v1 += r.y;
+          }
+          if (p.out_mode == 0) {
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix[i] * p.ldc + c) = make_float2(v0, v1);
+            if (p.out16 != nullptr) *reinterpret_cast<uint32_t*>(p.out16 + pix[i] * p.ldc + c) = pack_h2(v0, v1);
+          } else {
+            const __half2 hv = __floats2half2_rn(v0, v1);
+            *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + pix[i] * p.ldc + c) = hv;
+            const float2 r = __half22float2(hv);
+            v0 = r.x; v1 = r.y;
+          }
+          s0 += v0; s1 += v1;
+          q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
+        }
+      }
+      if (do_stats) {
+        // column sums over the warp's 16 rows (the 8 lanes that share `quad`); lanes 0..3 keep them
+#pragma unroll
+        for (int off = 4; off < 32; off <<= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, off);
+          s1 += __shfl_xor_sync(0xffffffffu, s1, off);
+          q0 += __shfl_xor_sync(0xffffffffu, q0, off);
+          q1 += __shfl_xor_sync(0xffffffffu, q1, off);
+        }
+        if (lane < 4) {
+          float* st = stat_smem + warp * 2 * BN + 8 * j + 2 * quad;
+          st[0] = s0; st[1] = s1; st[BN] = q0; st[BN + 1] = q1;
+        }
+      }
+    }
+    if (do_stats) {
+      // a warp's 16 rows belong to one sample (TW*TH >= 32); the warps of each sample are combined in a fixed order, so the
+      // statistics are reproducible bit for bit, and one fp64 atomic pair per (sample, channel) and tile goes to global memory
+      __syncthreads();
+      const int rows_per_n = p.TW * p.TH;
+      const int n_tile = (128 + rows_per_n - 1) / rows_per_n;
+      for (int e = tid; e < n_tile * BN; e += Cfg::THREADS) {
+        const int sn = e / BN, c = e - sn * BN;
+        const int n = n0 + sn, col = colbase + c;
+        if (n >= p.N || col >= p.Cout) continue;
+        float ssum = 0.f, qsum = 0.f;
+        for (int w8 = 0; w8 < 8; ++w8) {
+          if ((w8 * 16) / rows_per_n != sn) continue;
+          ssum += stat_smem[w8 * 2 * BN + c];
+          qsum += stat_smem[w8 * 2 * BN + BN + c];
+        }
+        double* st = p.stats + (static_cast<size_t>(n) * p.Cout + col) * 2;
+        atomicAdd(st, static_cast<double>(ssum));
+        atomicAdd(st + 1, static_cast<double>(qsum));
+      }
+      __syncthreads();                           // stat_smem is rewritten by the next tile
+    }
   }
+  if constexpr (kMc) cluster_sync_all();         // peers keep multicasting into / arriving on this CTA until all are done
 }
 
 }  // namespace ivid

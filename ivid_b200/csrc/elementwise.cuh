@@ -240,18 +240,6 @@ __device__ __forceinline__ void gn_prologue(const GnApplyParams& p, float* s_ab,
 
 }
 
-// The same per-(sample, channel) affine written to global memory: coefficients of a GroupNorm whose apply is folded into the
-// consuming conv's operand path (conv_gemm_kernel, fold mode).  grid = (1, N), block = 256.
-__global__ void __launch_bounds__(256) gn_coeff_kernel(const GnApplyParams p, float2* __restrict__ out) {
-  extern __shared__ float s_ab[];
-  __shared__ float s_mean[64], s_rstd[64];
-  gn_prologue(p, s_ab, s_mean, s_rstd);
-  const int C = p.C0 + p.C1;
-  const int n = static_cast<int>(blockIdx.y);
-  for (int c = threadIdx.x; c < C; c += blockDim.x)
-    out[static_cast<size_t>(n) * C + c] = make_float2(s_ab[(c & 7) * (C >> 3) + (c >> 3)], s_ab[C + (c & 7) * (C >> 3) + (c >> 3)]);
-}
-
 __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p) {
   extern __shared__ float s_ab[];        // A then B, each stored [c % 8][c / 8] so a warp's reads are conflict-free
   __shared__ float s_mean[64], s_rstd[64];

@@ -67,9 +67,9 @@ int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return 148;
+    if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return 132;
     n = prop.multiProcessorCount;
   }
   return n;

@@ -20,9 +20,7 @@ struct ConvLaunch {
   ConvGemmParams p;
   int BN;
   int grid;
-  int ctas = 1;          // 2 = CTA-pair kernel (cluster of 2, cta_group::2 MMA)
-  int mc = 0;            // > 0: cluster-multicast kernel, cluster size mc = mc_n * mc_m
-  int slab = 0;          // 1: 3x3 tap-reuse kernel (8 x 16 pixel tiles, [18][8] activation slabs), CTA pairs only
+  int mode = kConvDefault;     // kConvMc: cluster of p.mc_n * p.mc_m CTAs; kConvSlab: 3x3 tap-reuse kernel
 };
 
 int conv_pad_cout(int cout) {
@@ -33,80 +31,16 @@ bool conv_can_fuse_stats(int H, int W) {
   const int TW = std::min(W, 16), TH = std::min(H, 128 / TW);
   return TW * TH >= 32;
 }
-int conv_pick_bn(int cout_pad, int m_tiles) {
-  if (cout_pad % 256 == 0) {
-    // Wave quantisation on the low-resolution levels (few 128-pixel tiles): a 128-wide N tile doubles the tile count at
-    // ~10% lower per-tile efficiency; take it when it shortens the predicted makespan on the 148 SMs.
-    if (m_tiles > 0) {
-      const int sms = sm_count();
-      const long t256 = static_cast<long>(m_tiles) * (cout_pad / 256), t128 = static_cast<long>(m_tiles) * (cout_pad / 128);
-      const double cost256 = static_cast<double>((t256 + sms - 1) / sms) * 1.0;
-      static const double f128 = getenv("IVID_BN128_COST") ? atof(getenv("IVID_BN128_COST")) : 0.72;
-      const double cost128 = static_cast<double>((t128 + sms - 1) / sms) * f128;   // half the work per tile at ~70% of the N=256 efficiency (smem-operand bound)
-      if (cost128 < cost256) return 128;
-    }
-    return 256;
-  }
+// 128-wide tiles keep the 64 x 128 fp32 accumulator of a warpgroup at 64 registers per thread, so two CTAs share an SM
+int conv_pick_bn(int cout_pad) {
   if (cout_pad % 128 == 0) return 128;
   if (cout_pad % 64 == 0) return 64;
   if (cout_pad % 16 == 0 && cout_pad <= 48) return 16;
   throw Error(kErrInvalidArgument, "conv: unsupported padded Cout " + std::to_string(cout_pad));
 }
 
-static bool conv_pairs(int m_tiles, int cout_pad) {
-  static const bool pair_ok = getenv("IVID_NO_2CTA") == nullptr;
-  return pair_ok && conv_pick_bn(cout_pad, m_tiles) == 256 && m_tiles % 2 == 0 && m_tiles >= 2;
-}
-bool conv_fold_ok(int N, int H, int W, int cout_pad, bool residual_up) {
-  const char* e = getenv("IVID_FOLD");
-  if (e == nullptr || e[0] != '1') return false;
-  if (H < 16 || W < 16 || residual_up) return false;
-  return conv_pairs(N * (H * W / 128), cout_pad);
-}
-
-template <int BN>
-static void set_conv_attr() {
-  static std::once_flag once;
-  std::call_once(once, [] {
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         ConvGemmCfg<BN, 1>::SMEM_BYTES));
-  });
-}
-
-bool conv_can_res_up(int W, int cout) {
-  static const int dbg = [] { const char* e = getenv("IVID_CONV_DEBUG"); return e ? atoi(e) : 0; }();
-  static const bool off = getenv("IVID_NO_RES_UP") != nullptr;
-  return W >= 16 && cout % 32 == 0 && !(dbg & 16) && !off;
-}
-
-bool conv_can_out16(int cout) {
-  static const int dbg = [] { const char* e = getenv("IVID_CONV_DEBUG"); return e ? atoi(e) : 0; }();
-  static const bool off = getenv("IVID_NO_OUT16") != nullptr;
-  return cout % 64 == 0 && !(dbg & 16) && !off;
-}
-
-// how many clusters of `csize` multicast-conv CTAs the device can hold at once (one CTA per SM, clusters stay inside a GPC)
-static int max_mc_clusters(int csize) {
-  static int cache[17] = {0};
-  if (cache[csize] == 0) {
-    using Cfg = ConvGemmCfg<128, 1>;
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<128, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(csize * (sm_count() / csize));
-    cfg.blockDim = dim3(Cfg::THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = csize; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, conv_gemm_kernel<128, 1, true>, &cfg);
-    if (e != cudaSuccess || n < 1) { cudaGetLastError(); n = std::max(1, (sm_count() / csize) * 3 / 4); }
-    cache[csize] = n;
-  }
-  return cache[csize];
-}
+bool conv_can_res_up(int W, int cout) { return W >= 16 && cout % 32 == 0; }
+bool conv_can_out16(int cout) { return cout % 64 == 0; }
 
 ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.C0 > 0 && d.C0 % 64 == 0, "conv: segment-0 channels must be a positive multiple of 64");
@@ -125,213 +59,107 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   p.tiles_w = d.W / p.TW;
   p.tiles_h = d.H / p.TH;
   p.tiles_n = (d.N + p.TN - 1) / p.TN;
-  l->BN = conv_pick_bn(d.cout_pad, p.tiles_w * p.tiles_h * p.tiles_n);
-  {
-    // N = 256 tiles run as CTA pairs; when the layer cannot be paired (odd number of pixel tiles) the 128-wide
-    // single-CTA configuration is used instead (it has the shared memory for every epilogue feature)
-    static const bool pair_ok = getenv("IVID_NO_2CTA") == nullptr;
-    const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-    l->ctas = (pair_ok && l->BN == 256 && m_tiles % 2 == 0 && m_tiles >= 2) ? 2 : 1;
-    if (l->BN == 256 && l->ctas == 1 && (pair_ok || d.out16 != nullptr)) l->BN = 128;
-    // 3x3 tap reuse (conv_gemm_kernel<.., kSlab>): 8 x 16 pixel tiles; not with the upsampled residual (16-wide boxes)
-    int slab_mode = getenv("IVID_SLAB") ? atoi(getenv("IVID_SLAB")) : 0;      // read per plan build (tests switch it)
-    if (d.fold_ab != nullptr && slab_mode < 2) slab_mode = 3;      // fold: single-slab modes only (default: the 10-pixel pitch)
-    if (slab_mode && l->ctas == 2 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && !d.residual_up) {
-      l->slab = 1;
-      p.slab_mode = slab_mode >= 2 ? slab_mode : 1;
-      p.TW = 8; p.TH = 16; p.TN = 1;
-      p.tiles_w = d.W / p.TW; p.tiles_h = d.H / p.TH; p.tiles_n = d.N;
-    }
-    p.fold = 0; p.fold_ab = nullptr; p.fold_C = 0; p.fold_off[0] = p.fold_off[1] = p.fold_off[2] = -1;
-    if (d.fold_ab != nullptr) {
-      IVID_REQUIRE(l->slab == 1 && p.slab_mode >= 2, "conv: fold mode needs the CTA-pair tap-reuse kernel (see conv_fold_ok)");
-      IVID_REQUIRE(d.fold_C % 8 == 0 && d.fold_off0 % 8 == 0, "conv: fold coefficient table alignment");
-      p.fold = 1; p.fold_ab = static_cast<const float2*>(d.fold_ab); p.fold_C = d.fold_C;
-      p.fold_off[0] = d.fold_off0; p.fold_off[1] = d.C1 > 0 ? d.fold_off1 : -1; p.fold_off[2] = d.C2 > 0 ? d.fold_off2 : -1;
-    }
+  l->BN = conv_pick_bn(d.cout_pad);
+  // 3x3 tap reuse (IVID_SLAB=1, read per launch creation): 8 x 16 pixel tiles; not with the upsampled residual (its index
+  // arithmetic assumes the 16-wide tiles of the default kernel)
+  const bool slab_on = getenv("IVID_SLAB") != nullptr && atoi(getenv("IVID_SLAB")) > 0;
+  if (slab_on && l->BN == 128 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && !d.residual_up) {
+    l->mode = kConvSlab;
+    p.TW = 8; p.TH = 16; p.TN = 1;
+    p.tiles_w = d.W / p.TW; p.tiles_h = d.H / p.TH; p.tiles_n = d.N;
   }
   p.n_blocks = d.cout_pad / l->BN;
-  p.num_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_blocks;
   p.seg_chunks[0] = d.C0 / 64; p.seg_taps[0] = d.taps0;
   p.seg_chunks[1] = d.C1 / 64; p.seg_taps[1] = d.C1 > 0 ? d.taps1 : 0;
   p.seg_chunks[2] = d.C2 / 64; p.seg_taps[2] = d.C2 > 0 ? d.taps2 : 0;
   p.Cout = d.cout; p.ldc = d.ldc; p.ldr = d.ldr; p.out_mode = d.out_mode;
   p.bias = d.bias; p.residual = d.residual; p.out = d.out;
-  {
-    const char* dbg = getenv("IVID_CONV_DEBUG");
-    p.debug = dbg ? atoi(dbg) : 0;
-    if (p.debug & 8) { /* 8 = no fused statistics at all */ }
-  }
   p.stats = (d.stats != nullptr && conv_can_fuse_stats(d.H, d.W) && d.out_mode != 2) ? d.stats : nullptr;
   IVID_REQUIRE(d.stats == nullptr || p.stats != nullptr, "conv: fused statistics need >= 32 pixels per sample per warp");
   IVID_REQUIRE(d.out_mode == 2 || (d.cout % 8 == 0 && d.ldc % 8 == 0), "conv: NHWC output needs Cout % 8 == 0");
+  IVID_REQUIRE(d.residual == nullptr || (d.out_mode != 2 && d.ldr % 2 == 0), "conv: residual needs an NHWC output and an even row pitch");
+  p.res_up = 0;
+  if (d.residual != nullptr && d.residual_up) {
+    IVID_REQUIRE(conv_can_res_up(d.W, d.cout) && d.H % 2 == 0, "conv: upsampled residual needs W >= 16 and Cout % 32 == 0");
+    p.res_up = 1;
+  }
+  p.out16 = nullptr;
+  if (d.out16 != nullptr) {
+    IVID_REQUIRE(d.out_mode == 0 && conv_can_out16(d.cout), "conv: fp16 output copy needs an fp32 NHWC output and Cout % 64 == 0");
+    p.out16 = static_cast<__half*>(d.out16);
+  }
   const int Ktot = d.taps0 * d.C0 + (d.C1 > 0 ? d.taps1 * d.C1 : 0) + (d.C2 > 0 ? d.taps2 * d.C2 : 0);
   ConvMaps& M = l->maps;
   M.a[0] = make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN);
   M.a[1] = d.C1 > 0 ? make_act_map(d.act1, d.N, d.H, d.W, d.C1, p.TW, p.TH, p.TN) : M.a[0];
   M.a[2] = d.C2 > 0 ? make_act_map(d.act2, d.N, d.H, d.W, d.C2, p.TW, p.TH, p.TN) : M.a[0];
-  M.b = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN / l->ctas);
-  M.bh = M.b;
-  // Work list: full tiles, and - when the last round of the persistent grid would be less than half full - its tiles as
-  // twice as many half-width items (see ConvGemmParams::full_items).  A half-width item costs ~0.6 of a full one.
-  {
-    const int T = p.num_tiles / l->ctas;
-    const int S = l->ctas == 2 ? sm_count() / 2 : sm_count();
-    p.full_items = T;
-    p.num_items = T;
-    static const bool split_ok = getenv("IVID_NO_TAILSPLIT") == nullptr;
-    if (split_ok && l->BN == 256 && T > S) {
-      const int F = (T / S) * S, R = T - F;
-      if (R > 0) {
-        const double old_cost = static_cast<double>((T + S - 1) / S);
-        const double new_cost = static_cast<double>(T / S) + 0.6 * static_cast<double>((2 * R + S - 1) / S);
-        if (new_cost < old_cost - 0.05) {
-          p.full_items = F;
-          p.num_items = F + 2 * R;
-          M.bh = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN / 2 / l->ctas);
-        }
-      }
-    }
+  M.b = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN);
+  M.a_mc[0] = M.a[0]; M.a_mc[1] = M.a[1]; M.a_mc[2] = M.a[2]; M.b_mc = M.b;
+  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  if (l->mode == kConvSlab) {
+    M.a_mc[0] = make_act_map(d.act0, d.N, d.H, d.W, d.C0, 8, ConvGemmCfg<128, kConvSlab>::SLAB_ROWS, 1);
+    if (d.C1 > 0 && d.taps1 == 9) M.a_mc[1] = make_act_map(d.act1, d.N, d.H, d.W, d.C1, 8, ConvGemmCfg<128, kConvSlab>::SLAB_ROWS, 1);
+    if (d.C2 > 0 && d.taps2 == 9) M.a_mc[2] = make_act_map(d.act2, d.N, d.H, d.W, d.C2, 8, ConvGemmCfg<128, kConvSlab>::SLAB_ROWS, 1);
   }
-  // Cluster multicast on the low-resolution levels (single-CTA N = 128 tiles, few pixel tiles): see conv_gemm_kernel<.., kMc>.
+  // Cluster multicast on the low-resolution levels (IVID_MC=1, read per launch creation): see conv_gemm_kernel<.., kConvMc>
   p.mc_n = 1; p.mc_m = 1;
-  {
-    // Measured on B200 (profiles/per_op_r02e_*.json): 1.3x (2 x 2 clusters) to 2.4x (2 x 4) SLOWER than independent CTAs - the
-    // lock-step of 4-8 CTAs per stage and the small multicast boxes cost more than the 2.7x lower L2 traffic saves.  Kept as an
-    // opt-in experiment (IVID_MC=1, read at plan-build time), exercised by tests/test_gpu_ops.py.
-    const bool mc_ok = getenv("IVID_MC") != nullptr && getenv("IVID_MC")[0] == '1';
-    const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-    if (mc_ok && l->ctas == 1 && l->BN == 128 && d.H <= 16 && m_tiles >= 2) {
-      const int cn = p.n_blocks % 4 == 0 ? 4 : (p.n_blocks % 2 == 0 ? 2 : 1);
-      const int cm = m_tiles % 2 == 0 ? 2 : 1;
-      if (cn * cm >= 2) {
-        p.mc_n = cn; p.mc_m = cm;
-        l->mc = cn * cm;
-        const int srows = 128 / cn;
-        const int bh = srows >= p.TW * p.TH ? p.TH : srows / p.TW, bn = srows >= p.TW * p.TH ? srows / (p.TW * p.TH) : 1;
-        IVID_REQUIRE(bh >= 1 && srows % 8 == 0, "conv: multicast slice geometry");
-        auto slice_map = [&](const void* base, int C) {
-          const uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(d.W), static_cast<uint64_t>(d.H), static_cast<uint64_t>(d.N)};
-          const uint64_t str[3] = {static_cast<uint64_t>(C) * 2, static_cast<uint64_t>(d.W) * C * 2, static_cast<uint64_t>(d.H) * d.W * C * 2};
-          const uint32_t box[4] = {64, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(bh), static_cast<uint32_t>(bn)};
-          return make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-        };
-        M.a_mc[0] = slice_map(d.act0, d.C0);
-        M.a_mc[1] = d.C1 > 0 ? slice_map(d.act1, d.C1) : M.a_mc[0];
-        M.a_mc[2] = d.C2 > 0 ? slice_map(d.act2, d.C2) : M.a_mc[0];
-        M.b_mc = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN / cm);
-        p.num_items = (m_tiles / cm) * (p.n_blocks / cn);
-        p.full_items = p.num_items;
-      }
+  const bool mc_on = getenv("IVID_MC") != nullptr && getenv("IVID_MC")[0] == '1';
+  if (mc_on && l->mode == kConvDefault && l->BN == 128 && d.H <= 16 && m_tiles >= 2) {
+    const int cn = p.n_blocks % 4 == 0 ? 4 : (p.n_blocks % 2 == 0 ? 2 : 1);
+    const int cm = m_tiles % 2 == 0 ? 2 : 1;
+    if (cn * cm >= 2) {
+      p.mc_n = cn; p.mc_m = cm;
+      l->mode = kConvMc;
+      const int srows = 128 / cn;
+      const int bh = srows >= p.TW * p.TH ? p.TH : srows / p.TW, bn = srows >= p.TW * p.TH ? srows / (p.TW * p.TH) : 1;
+      IVID_REQUIRE(bh >= 1 && srows % 8 == 0, "conv: multicast slice geometry");
+      auto slice_map = [&](const void* base, int C) {
+        const uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(d.W), static_cast<uint64_t>(d.H), static_cast<uint64_t>(d.N)};
+        const uint64_t str[3] = {static_cast<uint64_t>(C) * 2, static_cast<uint64_t>(d.W) * C * 2, static_cast<uint64_t>(d.H) * d.W * C * 2};
+        const uint32_t box[4] = {64, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(bh), static_cast<uint32_t>(bn)};
+        return make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+      };
+      M.a_mc[0] = slice_map(d.act0, d.C0);
+      M.a_mc[1] = d.C1 > 0 ? slice_map(d.act1, d.C1) : M.a_mc[0];
+      M.a_mc[2] = d.C2 > 0 ? slice_map(d.act2, d.C2) : M.a_mc[0];
+      M.b_mc = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN / cm);
     }
   }
-  if (l->mc == 0) { M.a_mc[0] = M.a[0]; M.a_mc[1] = M.a[0]; M.a_mc[2] = M.a[0]; M.b_mc = M.b; }
-  if (l->slab) {
-    const int sw = p.slab_mode == 3 ? 10 : p.slab_mode == 2 ? 16 : 8;        // slab width in pixels
-    M.a_mc[0] = make_act_map(d.act0, d.N, d.H, d.W, d.C0, sw, ConvGemmCfg<256, 2>::SLAB_ROWS, 1);
-    if (d.C1 > 0 && d.taps1 == 9) M.a_mc[1] = make_act_map(d.act1, d.N, d.H, d.W, d.C1, sw, ConvGemmCfg<256, 2>::SLAB_ROWS, 1);
-    if (d.C2 > 0 && d.taps2 == 9) M.a_mc[2] = make_act_map(d.act2, d.N, d.H, d.W, d.C2, sw, ConvGemmCfg<256, 2>::SLAB_ROWS, 1);
-  }
-  // TMA epilogue for fp32 NHWC outputs: one box = the 32 pixels of an epilogue warp x 32 channels
-  M.out = M.a[0]; M.res = M.a[0]; M.out16 = M.a[0];
-  p.out16 = 0;
-  p.epi_tma = 0;
-  if (d.out_mode == 0 && l->BN >= 32 && d.cout % 32 == 0 && !(p.debug & 16)) {
-    const int bh = std::min(p.TH, 32 / p.TW), bn = 32 / (p.TW * bh);
-    auto f32_map = [&](const void* base, int ld) {
-      const uint64_t dims[4] = {static_cast<uint64_t>(ld), static_cast<uint64_t>(d.W), static_cast<uint64_t>(d.H), static_cast<uint64_t>(d.N)};
-      const uint64_t str[3] = {static_cast<uint64_t>(ld) * 4, static_cast<uint64_t>(d.W) * ld * 4, static_cast<uint64_t>(d.H) * d.W * ld * 4};
-      const uint32_t box[4] = {32, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(bh), static_cast<uint32_t>(bn)};
-      return make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    };
-    M.out = f32_map(d.out, d.ldc);
-    p.res_up = 0;
-    if (d.residual != nullptr && d.residual_up) {
-      IVID_REQUIRE(p.TW == 16 && bh == 2 && d.H % 2 == 0, "conv: upsampled residual needs 16-pixel-wide tiles");
-      const uint64_t dims[4] = {static_cast<uint64_t>(d.ldr), static_cast<uint64_t>(d.W / 2), static_cast<uint64_t>(d.H / 2), static_cast<uint64_t>(d.N)};
-      const uint64_t str[3] = {static_cast<uint64_t>(d.ldr) * 4, static_cast<uint64_t>(d.W / 2) * d.ldr * 4,
-                               static_cast<uint64_t>(d.H / 2) * (d.W / 2) * d.ldr * 4};
-      const uint32_t box[4] = {32, 8, 1, 1};
-      M.res = make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(d.residual), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-      p.res_up = 1;
-    } else if (d.residual != nullptr) {
-      M.res = f32_map(d.residual, d.ldr);
-    }
-    p.epi_tma = 1;
-    if (d.out16 != nullptr) {
-      IVID_REQUIRE(d.cout % 64 == 0 && !(l->BN == 256 && l->ctas == 1), "conv: fp16 output copy needs Cout % 64 == 0");
-      const uint64_t dims[4] = {static_cast<uint64_t>(d.ldc), static_cast<uint64_t>(d.W), static_cast<uint64_t>(d.H), static_cast<uint64_t>(d.N)};
-      const uint64_t str[3] = {static_cast<uint64_t>(d.ldc) * 2, static_cast<uint64_t>(d.W) * d.ldc * 2, static_cast<uint64_t>(d.H) * d.W * d.ldc * 2};
-      const uint32_t box[4] = {64, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(bh), static_cast<uint32_t>(bn)};
-      M.out16 = make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, d.out16, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-      p.out16 = 1;
-    }
-  } else if (d.out_mode == 1 && l->BN >= 64 && d.cout % 64 == 0 && d.residual == nullptr && !(p.debug & 16)) {
-    const int bh = std::min(p.TH, 32 / p.TW), bn = 32 / (p.TW * bh);
-    const uint64_t dims[4] = {static_cast<uint64_t>(d.ldc), static_cast<uint64_t>(d.W), static_cast<uint64_t>(d.H), static_cast<uint64_t>(d.N)};
-    const uint64_t str[3] = {static_cast<uint64_t>(d.ldc) * 2, static_cast<uint64_t>(d.W) * d.ldc * 2, static_cast<uint64_t>(d.H) * d.W * d.ldc * 2};
-    const uint32_t box[4] = {64, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(bh), static_cast<uint32_t>(bn)};
-    M.out = make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, d.out, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    p.epi_tma = 2;
-  }
-  // contiguous work ranges + running GroupNorm statistics (conv_gemm.cuh, ConvGemmParams::contig)
-  // Measured (profiles/per_op_r02r_*.json, bench_r02s_*): with ONE column block (Cout <= BN: the 128^2 / 64^2 levels) the contiguous
-  // ranges are 2-8 % faster per isolated launch and +-0 inside the step; with several column blocks (32^2 and below) they are
-  // 25-50 % slower than the round-robin order, in which the CTAs that share an activation tile run at the same time.  Opt-in:
-  // IVID_CONV_CONTIG=1 (single-column-block layers) / IVID_CONV_CONTIG_ALL=1 (read per plan build).
-  p.contig = (l->mc == 0 && p.n_blocks == 1 && p.full_items == p.num_items && getenv("IVID_CONV_CONTIG") != nullptr) ? 1 : 0;
-  if (getenv("IVID_CONV_CONTIG_ALL") != nullptr && l->mc == 0) p.contig = 1;
-  // deeper residual prefetch (three tiles in flight per epilogue warp, single output staging tile): opt-in A/B
-  p.res3 = (p.epi_tma == 1 && d.residual != nullptr && getenv("IVID_RES3") != nullptr && getenv("IVID_RES3")[0] == '1') ? 1 : 0;
-  // fused statistics are produced by the TMA epilogues only
-  if (p.stats != nullptr && p.epi_tma == 0) throw Error(kErrInvalidArgument, "conv: fused statistics need a TMA epilogue (Cout % 64 == 0)");
-  l->grid = l->ctas == 2 ? 2 * std::min(p.num_items, sm_count() / 2) : std::min(p.num_items, sm_count());
-  if (l->mc > 0) l->grid = l->mc * std::min(p.num_items, max_mc_clusters(l->mc));
+  // contiguous work ranges of persistent CTAs (IVID_CONV_CONTIG_ALL=1; IVID_CONV_CONTIG=1: layers with one column block)
+  p.contig = 0;
+  if (l->mode != kConvMc && (getenv("IVID_CONV_CONTIG_ALL") != nullptr || (getenv("IVID_CONV_CONTIG") != nullptr && p.n_blocks == 1))) p.contig = 1;
+  const int tiles = m_tiles * p.n_blocks;
+  if (l->mode == kConvMc) l->grid = tiles;                       // (m_tiles / cm) * (n_blocks / cn) clusters of cm * cn CTAs
+  else if (p.contig) l->grid = std::min(tiles, sm_count() * (l->mode == kConvSlab ? 1 : 2));
+  else l->grid = tiles;
   return l;
 }
 void conv_launch_destroy(ConvLaunch* l) { delete l; }
 int conv_launch_bn(const ConvLaunch* l) { return l->BN; }
 
-template <int BN>
+template <int BN, int kMode = kConvDefault>
 static void run_conv(const ConvLaunch* l, cudaStream_t s) {
-  set_conv_attr<BN>();
-  conv_gemm_kernel<BN, 1><<<l->grid, ConvGemmCfg<BN, 1>::THREADS, ConvGemmCfg<BN, 1>::SMEM_BYTES, s>>>(l->maps, l->p);
-  IVID_CHECK_CUDA(cudaGetLastError());
-}
-static void run_conv_pair(const ConvLaunch* l, cudaStream_t s) {
-  using Cfg = ConvGemmCfg<256, 2>;
+  using Cfg = ConvGemmCfg<BN, kMode>;
   static std::once_flag once;
   std::call_once(once, [] {
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<256, 2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES_SLAB));
+    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   });
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(l->grid);
-  cfg.blockDim = dim3(l->slab ? Cfg::THREADS_SLAB : Cfg::THREADS);
-  cfg.dynamicSmemBytes = l->slab ? Cfg::SMEM_BYTES_SLAB : Cfg::SMEM_BYTES;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (l->slab) IVID_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<256, 2, false, true>, l->maps, l->p));
-  else IVID_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<256, 2>, l->maps, l->p));
-}
-static void run_conv_mc(const ConvLaunch* l, cudaStream_t s) {
-  using Cfg = ConvGemmCfg<128, 1>;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(l->grid);
-  cfg.blockDim = dim3(Cfg::THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = l->mc; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  IVID_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<128, 1, true>, l->maps, l->p));
+  if (kMode == kConvMc) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(l->grid);
+    cfg.blockDim = dim3(Cfg::THREADS);
+    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = l->p.mc_n * l->p.mc_m; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    IVID_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, kMode>, l->maps, l->p));
+    return;
+  }
+  conv_gemm_kernel<BN, kMode><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
+  IVID_CHECK_CUDA(cudaGetLastError());
 }
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
   ConvLaunch tmp = *l;
@@ -339,10 +167,9 @@ void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
   conv_launch_run(&tmp, s);
 }
 void conv_launch_run(const ConvLaunch* l, cudaStream_t s) {
-  if (l->mc > 0) { run_conv_mc(l, s); return; }
-  if (l->ctas == 2) { run_conv_pair(l, s); return; }
+  if (l->mode == kConvMc) { run_conv<128, kConvMc>(l, s); return; }
+  if (l->mode == kConvSlab) { run_conv<128, kConvSlab>(l, s); return; }
   switch (l->BN) {
-    case 256: run_conv<256>(l, s); break;
     case 128: run_conv<128>(l, s); break;
     case 64: run_conv<64>(l, s); break;
     default: run_conv<16>(l, s); break;
@@ -381,12 +208,9 @@ void attn_launch_destroy(AttnLaunch* l) { delete l; }
 void attn_launch_run(const AttnLaunch* l, cudaStream_t s) {
   static std::once_flag once;
   std::call_once(once, [] {
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel_v1, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnCfg::SMEM_BYTES));
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnCfg2::SMEM_BYTES));
+    IVID_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnCfg::SMEM_BYTES));
   });
-  static const bool v1 = getenv("IVID_ATTN_V1") != nullptr;      // previous kernel (single-buffered S, 4 CTAs / SM) for same-box A/B
-  if (v1) attention_kernel_v1<<<l->grid, AttnCfg::THREADS, AttnCfg::SMEM_BYTES, s>>>(l->mapQ, l->mapKV, l->p);
-  else attention_kernel<<<l->grid, AttnCfg2::THREADS, AttnCfg2::SMEM_BYTES, s>>>(l->mapQ, l->mapKV, l->p);
+  attention_kernel<<<l->grid, AttnCfg::THREADS, AttnCfg::SMEM_BYTES, s>>>(l->mapQ, l->mapKV, l->p);
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 
@@ -456,19 +280,6 @@ void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s) {
   }
   IVID_CHECK_CUDA(cudaGetLastError());
 }
-void launch_gn_coeff(const GnApplyDesc& d, void* out_ab, cudaStream_t s) {
-  const int C = d.C0 + d.C1;
-  IVID_REQUIRE(C % 8 == 0 && d.groups >= 1 && d.groups <= 64 && C % d.groups == 0, "gn_coeff: channel / group counts");
-  IVID_REQUIRE(d.stats0 != nullptr && d.gamma != nullptr && d.beta != nullptr && out_ab != nullptr, "gn_coeff: statistics / affine parameters missing");
-  GnApplyParams p = GnApplyParams();
-  p.C0 = d.C0; p.C1 = d.C1; p.N = d.N; p.H = d.H; p.W = d.W;
-  p.stats0 = d.stats0; p.stats1 = d.stats1; p.groups = d.groups; p.inv_count = 1.0 / (static_cast<double>(d.H) * d.W);
-  p.eps = d.eps; p.gamma = d.gamma; p.beta = d.beta; p.film = d.film; p.film_ld = d.film_ld; p.film_off = d.film_off;
-  p.film_add = d.film_add ? 1 : 0;
-  gn_coeff_kernel<<<dim3(1, d.N), 256, static_cast<size_t>(C) * 8, s>>>(p, static_cast<float2*>(out_ab));
-  IVID_CHECK_CUDA(cudaGetLastError());
-}
-
 void launch_im2col_s2(const void* x16, void* col, int N, int H, int W, int C, cudaStream_t s) {
   IVID_REQUIRE(C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "im2col_s2: C % 8, even spatial size");
   const size_t items = static_cast<size_t>(N) * (H / 2) * (W / 2) * 9 * (C / 8);

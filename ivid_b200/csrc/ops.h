@@ -1,4 +1,4 @@
-// Host-side launch descriptors for the sm_100a kernels (built once at plan time, replayed every step).
+// Host-side launch descriptors for the sm_90a kernels (built once at plan time, replayed every step).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -27,14 +27,7 @@ struct ConvDesc {
   void* out = nullptr; int ldc = 0; int out_mode = 0;      // 0 fp32 NHWC, 1 fp16 NHWC, 2 fp32 NCHW
   double* stats = nullptr;                                 // optional fused GroupNorm statistics of the output [N][cout][2]
   int N = 0, H = 0, W = 0;
-  // fold mode (conv_fold_ok): the 3x3 segments are RAW fp16 tensors and y = silu(A x + B) is applied in the kernel's operand path
-  const void* fold_ab = nullptr;                           // float2 [N][fold_C] from launch_gn_coeff
-  int fold_C = 0;
-  int fold_off0 = -1, fold_off1 = -1, fold_off2 = -1;      // channel offset of each segment in the table (< 0: not transformed)
 };
-// whether a 3x3 conv of this shape runs on the kernel variant that can fold a GroupNorm apply into its operand path
-// (CTA pairs, 8 x 16-pixel tiles; IVID_FOLD=1 opts in)
-bool conv_fold_ok(int N, int H, int W, int cout_pad, bool residual_up);
 
 // opaque, heap-allocated launch records (hold the CUtensorMaps)
 ConvLaunch* conv_launch_create(const ConvDesc& d);
@@ -42,7 +35,7 @@ void conv_launch_destroy(ConvLaunch* l);
 void conv_launch_run(const ConvLaunch* l, cudaStream_t s);
 int conv_launch_bn(const ConvLaunch* l);
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s);   // same launch, output pointer overridden
-int conv_pick_bn(int cout_pad, int m_tiles = 0);          // m_tiles > 0: wave-quantisation aware choice
+int conv_pick_bn(int cout_pad);
 // whether a conv with this many (unpadded) output channels can also emit the fp16 copy of its fp32 NHWC output
 bool conv_can_out16(int cout);
 // whether the conv epilogue can add a half-resolution residual through a nearest-2x upsample (output width W, Cout)
@@ -68,8 +61,6 @@ struct GnApplyDesc {
   void* out_lo = nullptr;      // optional low half of a two-term fp16 split of the output (fp16-source same-resolution path only)
 };
 void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s);
-// the affine of the same GroupNorm as a table float2 (A, B)[N][C0 + C1] (x0 / x1 / out_* of the descriptor are not used)
-void launch_gn_coeff(const GnApplyDesc& d, void* out_ab, cudaStream_t s);
 // eps[n][c][h][w] = bias[c] + sum_tap Y[n][h+dy][w+dx][tap*Co + c]  (output head, see eps_gather_kernel)
 void launch_eps_gather(const float* Y, const float* bias, float* eps, int N, int H, int W, int Co, int ldy, cudaStream_t s);
 // plain Downsample2d / Upsample2d layers (resblock_updown=False): see elementwise.cuh

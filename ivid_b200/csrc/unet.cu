@@ -511,7 +511,7 @@ Plan* Unet::build_plan(int N) {
   auto Wf = [&](size_t off) { return reinterpret_cast<const float*>(arena_ + off); };
 
   // ---- scratch maxima (walk the topology once for sizes) ----
-  size_t max_act16 = 0, max_raw16 = 0, max_f32 = 0, max_c = 0, max_qkv = 0, max_col = 0;
+  size_t max_act16 = 0, max_raw16 = 0, max_f32 = 0, max_qkv = 0, max_col = 0;
   {
     int res = S;
     auto upd_res = [&](const ResBlockDef& r) {
@@ -519,7 +519,6 @@ Plan* Unet::build_plan(int N) {
       max_act16 = std::max({max_act16, static_cast<size_t>(N) * ro * ro * r.cin, static_cast<size_t>(N) * ro * ro * r.cout});
       max_raw16 = std::max(max_raw16, static_cast<size_t>(N) * res * res * r.cin);
       max_f32 = std::max({max_f32, static_cast<size_t>(N) * ro * ro * r.cin, static_cast<size_t>(N) * ro * ro * r.cout});
-      max_c = std::max({max_c, static_cast<size_t>(r.cin), static_cast<size_t>(r.cout)});
       res = ro;
     };
     for (const auto& b : blocks_)
@@ -533,7 +532,6 @@ Plan* Unet::build_plan(int N) {
           const auto& a = attn_[l.idx];
           max_act16 = std::max(max_act16, static_cast<size_t>(N) * res * res * a.C);
           max_qkv = std::max(max_qkv, static_cast<size_t>(N) * res * res * 3 * a.C);
-          max_c = std::max(max_c, static_cast<size_t>(a.C));
         }
       }
     max_act16 = std::max(max_act16, static_cast<size_t>(N) * S * S * std::max(64, final_ch_));
@@ -589,7 +587,6 @@ Plan* Unet::build_plan(int N) {
     void* s_xh = bump.take(max_raw16 * 2);
     float* s_xr = static_cast<float*>(bump.take(max_f32 * 4));
     float* s_h = static_cast<float*>(bump.take(max_f32 * 4));
-    void* s_ab = bump.take(static_cast<size_t>(N) * max_c * 2 * 8);      // float2 per (n, c); 2x slack for concat
     void* s_qkv = bump.take(std::max<size_t>(max_qkv, 1) * 2);
     void* s_col = bump.take(std::max<size_t>(max_col, 1) * 2);           // im2col operand of the stride-2 Downsample2d conv
     float* s_pe = static_cast<float*>(bump.take(static_cast<size_t>(N) * cfg_.model_channels * 4));
@@ -624,9 +621,9 @@ Plan* Unet::build_plan(int N) {
                        (d.C2 > 0 ? static_cast<double>(d.taps2) * d.C2 : 0.0);
       const double M = static_cast<double>(d.N) * d.H * d.W;
       const double Nalg = n_alg > 0.0 ? n_alg : static_cast<double>(d.cout);
-      static const char* names[] = {"conv_gemm<16>", "conv_gemm<64>", "conv_gemm<128>", "conv_gemm<256>"};
+      static const char* names[] = {"conv_gemm<16>", "conv_gemm<64>", "conv_gemm<128>"};
       const int bn = conv_launch_bn(l);
-      pl->ops.tag(names[bn == 256 ? 3 : bn == 128 ? 2 : bn == 64 ? 1 : 0], 2.0 * M * K * Nalg,
+      pl->ops.tag(names[bn == 128 ? 2 : bn == 64 ? 1 : 0], 2.0 * M * K * Nalg,
                   M * (d.C0 + d.C1 + d.C2) * 2 + M * d.cout * ((d.out_mode == 1 ? 2 : 4) + (d.out16 ? 2 : 0) + (d.residual ? 4 : 0)) + K * d.cout_pad * 2,
                   std::to_string(d.H) + "x" + std::to_string(d.W) + " " + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") + (d.C2 ? "+" + std::to_string(d.C2) : "") +
                       "->" + std::to_string(d.cout) + " k" + std::to_string(d.taps0) + (d.residual ? " res" : "") + (d.stats ? " stats" : "") +
@@ -667,17 +664,6 @@ Plan* Unet::build_plan(int N) {
                         " m" + std::to_string(d.mode) + (d.x0_half ? " h16" : "") + (d.out_raw16 ? " raw16" : "") + (d.out_raw32 ? " raw32" : ""));
       }
       pl->ops.push_back([d](cudaStream_t s) { launch_gn_apply(d, s); });
-    };
-
-    // GroupNorm folded into the consuming conv (conv_fold_ok): only the per-(sample, channel) coefficients are computed here
-    // (gn_coeff_kernel -> s_ab); the conv reads the RAW fp16 tensor and applies silu(A x + B) in its operand path
-    auto add_fold_coeff = [&](const GnApplyDesc& g) {
-      if (!create) return;
-      GnApplyDesc d = g;
-      d.stats0 = pend.stats0; d.stats1 = pend.stats1; d.groups = pend.groups; d.eps = pend.eps; d.gamma = pend.gamma;
-      d.beta = pend.beta; d.film = pend.film; d.film_ld = pend.film_ld; d.film_off = pend.film_off; d.film_add = pend.film_add;
-      pl->ops.tag("gn_coeff", 0, static_cast<double>(d.N) * (d.C0 + d.C1) * 24, "C" + std::to_string(d.C0 + d.C1));
-      pl->ops.push_back([d, s_ab](cudaStream_t s) { launch_gn_coeff(d, s_ab, s); });
     };
 
     // ---- embeddings ----
@@ -756,8 +742,7 @@ Plan* Unet::build_plan(int N) {
       g1.N = N; g1.H = H; g1.W = Wd; g1.mode = r.mode; g1.silu = 1;
       g1.out_act = s_a1; g1.out_raw16 = (r.skip_conv && !use16) ? s_xh : nullptr; g1.out_raw32 = need_xr ? s_xr : nullptr;
       IVID_REQUIRE(!(r.skip_conv && r.mode != 0), "internal: up/down ResBlocks keep the channel count");
-      const bool fold1 = use16 && x1 == nullptr && conv_fold_ok(N, Ho, Wo, r.conv1.cout_pad, false);
-      if (fold1) add_fold_coeff(g1); else add_apply(g1);
+      add_apply(g1);
       // conv1 -> h (fp32) ; stats
       bool h_half = false;
       Act h; h.C = r.cout; h.H = Ho; h.W = Wo; h.data = s_h;
@@ -765,7 +750,6 @@ Plan* Unet::build_plan(int N) {
       {
         ConvDesc d;
         d.act0 = s_a1; d.C0 = r.cin; d.taps0 = 9;
-        if (fold1) { d.act0 = x0.d16; d.fold_ab = s_ab; d.fold_C = r.cin; d.fold_off0 = 0; }
         d.weight = W8(r.conv1.w_off); d.cout_pad = r.conv1.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv1.b_off);
         // the hidden tensor only feeds GroupNorm 2: stored as fp16 (half the epilogue and GN traffic); its statistics are
         // taken from the rounded values in the conv epilogue.  Tiny feature maps keep the fp32 + stats-kernel path.
@@ -779,14 +763,12 @@ Plan* Unet::build_plan(int N) {
       GnApplyDesc g2;
       g2.x0 = h.data; g2.x0_half = h_half; g2.C0 = r.cout; g2.N = N; g2.H = Ho; g2.W = Wo; g2.mode = 0; g2.silu = 1;
       g2.out_act = s_a2;
-      const bool fold2 = h_half && conv_fold_ok(N, Ho, Wo, r.conv2.cout_pad, res_up);
-      if (fold2) add_fold_coeff(g2); else add_apply(g2);
+      add_apply(g2);
       // conv2 (+ 1x1 skip as extra K) + residual -> out
       Act out = new_act(r.cout, Ho, Wo);
       {
         ConvDesc d;
         d.act0 = s_a2; d.C0 = r.cout; d.taps0 = 9;
-        if (fold2) { d.act0 = h.data; d.fold_ab = s_ab; d.fold_C = r.cout; d.fold_off0 = 0; }
         if (r.skip_conv && use16) {
           d.act1 = x0.d16; d.C1 = x0.C; d.taps1 = 1;
           if (x1 != nullptr) { d.act2 = x1->d16; d.C2 = x1->C; d.taps2 = 1; }
@@ -979,12 +961,9 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
   IVID_REQUIRE(hook == nullptr || can_fuse_head(), "forward: a head hook needs the tap-column output head");
   IVID_REQUIRE(hook != nullptr || eps != nullptr, "forward: eps output missing");
 
-  // Two half-batches on two streams: the HBM-bound GroupNorm passes of one half overlap the tensor-bound convolutions
-  // of the other (a persistent conv CTA leaves enough registers / shared memory on every SM for a gn_apply block).
-  // The halves are independent samples (typically the two classifier-free-guidance halves sharing x).
-  // Measured on B200 (api.cu: ivid_debug_overlap): the two kernels do NOT overlap today (conv alone 0.21 ms + gn alone
-  // 0.08 ms = 0.28 ms when issued concurrently), so the split is opt-in (IVID_SPLIT_BATCH=1) until the co-residency
-  // blocker is understood.
+  // Two half-batches on two streams: the HBM-bound GroupNorm passes of one half may overlap the tensor-bound convolutions
+  // of the other.  The halves are independent samples (typically the two classifier-free-guidance halves sharing x).
+  // Opt-in (IVID_SPLIT_BATCH=1): not measured to help.
   static const bool split_ok = getenv("IVID_SPLIT_BATCH") != nullptr;
   const bool can_split = split_ok && hook == nullptr && !profile_ && N % 2 == 0 && N >= 4 && (Nx == N || Nx == N / 2) &&
                          !(cnd.kind != 0 && Nx == N && cnd.noise_dev == nullptr);

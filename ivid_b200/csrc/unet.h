@@ -1,7 +1,7 @@
 // ADM UNet: topology / state-dict schema (host), packed device weights, per-batch execution plan.
 // Mirrors the constructor logic of the reference's AdmUnet2d (diffusion/backbones/adm.py:318-487) so that the
 // state-dict keys and shapes are identical (SURVEY.md §8b), but executes the forward (adm.py:526-566) as a static list
-// of sm_100a kernel launches over NHWC tensors.
+// of sm_90a kernel launches over NHWC tensors.
 #pragma once
 #include <functional>
 #include <map>

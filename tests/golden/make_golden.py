@@ -212,9 +212,12 @@ def main():
     assert torch.equal(ci_ref, sampler_ref.make_sr_inputs(xs, ys))
     out["sr_x"] = xs.numpy(); out["sr_y"] = ys.numpy(); out["sr_cond_inputs"] = ci_ref.numpy()
 
-    np.savez_compressed(os.path.join(HERE, "unet_sampler_golden.npz"), **out)
-    sz = os.path.getsize(os.path.join(HERE, "unet_sampler_golden.npz"))
-    print(f"wrote unet_sampler_golden.npz ({sz/1024:.0f} KiB)")
+    # written in two parts so that no fixture file exceeds 1 MB (arrays alternate by size)
+    keys = sorted(out, key=lambda k: -np.asarray(out[k]).nbytes)
+    for part in (0, 1):
+        np.savez_compressed(os.path.join(HERE, f"unet_sampler_golden_part{part}.npz"), **{k: out[k] for k in keys[part::2]})
+    sz = [os.path.getsize(os.path.join(HERE, f"unet_sampler_golden_part{i}.npz")) / 1024 for i in (0, 1)]
+    print(f"wrote unet_sampler_golden_part{{0,1}}.npz ({sz[0]:.0f}, {sz[1]:.0f} KiB)")
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 """Pin oracle/warp_ref.py against the reference's own rgbd_3d/utils.py (build container only) and write the warp
-golden fixture tests/golden/warp_golden.npz.
+golden fixture tests/golden/warp_golden_part{0,1}.npz.
 
 rgbd_3d/utils.py is imported by file path with stubbed `glm` (numpy-backed: inverse/mat3, mathematical orientation),
 `plyfile` and `easydict`; rgbd_3d/__init__.py (which pulls in moderngl) is bypassed.  The reference's
@@ -158,8 +158,11 @@ def main():
         out[f"mesh{i}_abssum"] = np.abs(vb.astype(np.float64)).sum(0)
         out[f"mesh{i}_flaghist"] = np.bincount(vb[:, 8].astype(np.int64), minlength=8)
         out[f"mesh{i}_faces_sum"] = np.array([m.faces.astype(np.int64).sum(), (m.faces.astype(np.int64) * np.arange(1, 4)).sum()])
-    np.savez_compressed(os.path.join(HERE, "warp_golden.npz"), **out)
-    print(f"wrote warp_golden.npz ({os.path.getsize(os.path.join(HERE, 'warp_golden.npz')) / 1024:.0f} KiB)")
+    # written in two parts so that no fixture file exceeds 1 MB (arrays alternate by size)
+    keys = sorted(out, key=lambda k: -np.asarray(out[k]).nbytes)
+    for part in (0, 1):
+        np.savez_compressed(os.path.join(HERE, f"warp_golden_part{part}.npz"), **{k: out[k] for k in keys[part::2]})
+    print("wrote warp_golden_part{0,1}.npz (" + ", ".join(f"{os.path.getsize(os.path.join(HERE, f'warp_golden_part{i}.npz')) / 1024:.0f}" for i in (0, 1)) + " KiB)")
 
 
 if __name__ == "__main__":

@@ -140,7 +140,7 @@ def rel(a, b):
 
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "tiny"
-    g = np.load(os.path.join(ROOT, "tests", "golden", "unet_sampler_golden.npz"))
+    g = {k: v for i in (0, 1) for k, v in np.load(os.path.join(ROOT, "tests", "golden", f"unet_sampler_golden_part{i}.npz")).items()}
     key = {"tiny": "tiny_cfg", "tiny_cond": "tiny_cond_cfg", "tiny_sr": "tiny_sr_cfg",
            "large": "schemacfg_rgbd_imagenet_adm_128_large_cfg", "small": "schemacfg_rgbd_singlecategory_adm_128_small"}[which]
     cfg = json.loads(bytes(g[key]).decode())

@@ -91,7 +91,7 @@ def test_multiview_chain_teacher_forced_large_models(golden):
     import gpu_util as G
     from conftest import ROOT
     from oracle import sampler_ref, warp_ref
-    wg = np.load(os.path.join(ROOT, "tests", "golden", "warp_golden.npz"))
+    wg = {k: v for i in (0, 1) for k, v in np.load(os.path.join(ROOT, "tests", "golden", f"warp_golden_part{i}.npz")).items()}
     near, far, fov, atol, rtol, erode = [float(v) for v in wg["params"]]
     p = dict(fov=fov, near=near, far=far, atol=atol, rtol=rtol, erode_rgb=int(erode))
     # stage 0: "view 0" of two samples = the smooth synthetic RGBD images of the warp fixture (a random-weight sampler would

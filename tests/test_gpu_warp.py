@@ -18,7 +18,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module")
 def wg():
-    return np.load(os.path.join(ROOT, "tests", "golden", "warp_golden.npz"))
+    return {k: v for i in (0, 1) for k, v in np.load(os.path.join(ROOT, "tests", "golden", f"warp_golden_part{i}.npz")).items()}
 
 
 def _params(wg):

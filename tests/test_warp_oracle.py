@@ -10,7 +10,7 @@ import os
 
 @pytest.fixture(scope="module")
 def wg():
-    return np.load(os.path.join(ROOT, "tests", "golden", "warp_golden.npz"))
+    return {k: v for i in (0, 1) for k, v in np.load(os.path.join(ROOT, "tests", "golden", f"warp_golden_part{i}.npz")).items()}
 
 
 def _meshes(wg, k):

@@ -1,9 +1,9 @@
 """Secondary baseline (SURVEY.md §8d): the PyTorch restatement of the reference path (oracle/unet_ref.py +
-oracle/sampler_ref.py, i.e. what the reference's own modules launch) run EAGERLY on the same B200 through stock
+oracle/sampler_ref.py, i.e. what the reference's own modules launch) run EAGERLY on the same GPU through stock
 PyTorch kernels (cuDNN / cuBLAS), for the bench workload: one DDPM + classifier-free-guidance denoising step of batch 16
 on the large 128x128 model (two sequential batch-16 forwards, as the reference does).  Measurement tooling only.
 
-    python tools/bench_torch_gpu.py [--steps 5] > profiles/torch_gpu_baseline.json
+    python tools/bench_torch_gpu.py [--steps 5]
 """
 import argparse
 import json
