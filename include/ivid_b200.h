@@ -244,6 +244,9 @@ int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1,
                        int silu, int mode, void* out_fp16_dev, void* stream);
 /* QKVAttention (adm.py:233-253): qkv fp16 [N,T,3C] (legacy head-major q|k|v order) -> fp16 [N,T,C]. */
 int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, void* stream);
+/* The same with head width head_channels = C / heads (a multiple of 64, dividing C): qkv fp16 [N,T,3C] in the order
+   [head][q|k|v][head_channels] -> fp16 [N,T,C].  head_channels = 64 computes exactly what ivid_op_attention computes. */
+int ivid_op_attention_heads(const void* qkv_dev, int N, int T, int C, int head_channels, void* out_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -88,6 +88,7 @@ SIGNATURES = {
     "ivid_op_group_norm": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                                    c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "ivid_op_attention_heads": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_warp_create": (c_int, [c_int, c_int, c_int, c_int, c_double, c_double, c_int, POINTER(c_void_p)]),
     "ivid_warp_destroy": (c_int, [c_void_p]),
     "ivid_warp_reset": (c_int, [c_void_p]),

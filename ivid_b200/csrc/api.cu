@@ -264,7 +264,17 @@ int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, v
   return guarded([&] {
     IVID_NOT_NULL(qkv_dev); IVID_NOT_NULL(out_dev);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    std::unique_ptr<AttnLaunch, void (*)(AttnLaunch*)> l(attn_launch_create(qkv_dev, N, T, C, out_dev), attn_launch_destroy);
+    std::unique_ptr<AttnLaunch, void (*)(AttnLaunch*)> l(attn_launch_create(qkv_dev, N, T, C, 64, out_dev), attn_launch_destroy);
+    attn_launch_run(l.get(), st);
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+  });
+}
+
+int ivid_op_attention_heads(const void* qkv_dev, int N, int T, int C, int head_channels, void* out_dev, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(qkv_dev); IVID_NOT_NULL(out_dev);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    std::unique_ptr<AttnLaunch, void (*)(AttnLaunch*)> l(attn_launch_create(qkv_dev, N, T, C, head_channels, out_dev), attn_launch_destroy);
     attn_launch_run(l.get(), st);
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
   });

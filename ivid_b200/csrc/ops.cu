@@ -2,10 +2,12 @@
 #include "ops.h"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <mutex>
 
 #include "attention.cuh"
+#include "attention_hd.cuh"
 #include "conv_gemm.cuh"
 #include "elementwise.cuh"
 #include "embed.cuh"
@@ -181,14 +183,22 @@ void conv_launch_run(const ConvLaunch* l, cudaStream_t s) {
 // --------------------------------------------------------------------------------------------------
 struct AttnLaunch {
   CUtensorMap mapQ, mapKV;
-  AttnParams p;
+  AttnParams p;          // head width 64: attention_kernel
+  AttnHdParams hp;       // other widths: attention_hd_kernel<nv, qres>
+  int head_ch = 64;
+  int nv = 0;
+  bool qres = false;
+  int smem = 0;
   int grid;
 };
 
-AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, void* out) {
-  IVID_REQUIRE(C % 64 == 0, "attention: channels must be a multiple of the head width 64");
+AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out) {
+  if (head_ch <= 0 || head_ch % 64 != 0)
+    throw Error(kErrNotImplemented, "attention: head width " + std::to_string(head_ch) + " is not a multiple of 64");
+  IVID_REQUIRE(C % head_ch == 0, "attention: channels must be a multiple of the head width " + std::to_string(head_ch));
   IVID_REQUIRE(T >= 64 && T % 64 == 0, "attention: sequence length must be a multiple of 64");
   auto* l = new AttnLaunch();
+  l->head_ch = head_ch;
   l->p.N = N; l->p.T = T; l->p.C = C; l->p.heads = C / 64;
   l->p.q_tiles = (T + 127) / 128;
   l->p.out = reinterpret_cast<__half*>(out);
@@ -201,11 +211,53 @@ AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, void* out) 
   l->mapKV = make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(qkv), dims, str, boxkv,
                              CU_TENSOR_MAP_SWIZZLE_128B);
   l->grid = N * l->p.heads * l->p.q_tiles;
+  if (head_ch == 64) return l;
+  // wider heads: k = d/64 chunks; ceil(k/4) output-column slices of nv <= 4 boxes (see attention_hd.cuh)
+  using Cfg = AttnHdCfg;
+  const int k = head_ch / 64;
+  const int slices = (k + 3) / 4;
+  l->nv = (k + slices - 1) / slices;
+  l->qres = k <= Cfg::RESIDENT_Q_MAX_CHUNKS;
+  AttnHdParams& hp = l->hp;
+  hp.N = N; hp.T = T; hp.C = C; hp.d = head_ch; hp.heads = C / head_ch; hp.chunks = k;
+  hp.q_tiles = l->p.q_tiles;
+  hp.slices = (k + l->nv - 1) / l->nv;          // every slice holds >= 1 box
+  hp.scale_log2 = static_cast<float>(1.4426950408889634 / std::sqrt(static_cast<double>(head_ch)));
+  hp.out = l->p.out;
+  const int q_bytes = l->qres ? k * Cfg::QCHUNK_BYTES : 0;
+  const int fixed = q_bytes + 1024 /*barriers*/ + 1024 /*align*/;
+  const int budget = l->nv == 2 ? Cfg::MAX_SMEM_2CTA : Cfg::MAX_SMEM;
+  hp.stages = std::min(Cfg::MAX_STAGES, (budget - fixed) / Cfg::stage_bytes(l->qres));
+  IVID_REQUIRE(hp.stages >= 4, "attention: shared-memory ring too shallow");
+  l->smem = fixed + hp.stages * Cfg::stage_bytes(l->qres);
+  l->grid = N * hp.heads * hp.q_tiles * hp.slices;
   return l;
 }
 void attn_launch_destroy(AttnLaunch* l) { delete l; }
 
+template <int NV, bool QRES>
+static void run_attn_hd(const AttnLaunch* l, cudaStream_t s) {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    IVID_CHECK_CUDA(cudaFuncSetAttribute(attention_hd_kernel<NV, QRES>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnHdCfg::MAX_SMEM));
+  });
+  attention_hd_kernel<NV, QRES><<<l->grid, AttnHdCfg::THREADS, l->smem, s>>>(l->mapQ, l->mapKV, l->hp);
+  IVID_CHECK_CUDA(cudaGetLastError());
+}
+
 void attn_launch_run(const AttnLaunch* l, cudaStream_t s) {
+  if (l->head_ch != 64) {
+    switch (l->nv * 2 + (l->qres ? 1 : 0)) {
+      case 5: run_attn_hd<2, true>(l, s); break;
+      case 7: run_attn_hd<3, true>(l, s); break;
+      case 9: run_attn_hd<4, true>(l, s); break;
+      case 4: run_attn_hd<2, false>(l, s); break;
+      case 6: run_attn_hd<3, false>(l, s); break;
+      case 8: run_attn_hd<4, false>(l, s); break;
+      default: throw Error(kErrState, "internal: attention slice width " + std::to_string(l->nv));
+    }
+    return;
+  }
   static std::once_flag once;
   std::call_once(once, [] {
     IVID_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnCfg::SMEM_BYTES));

@@ -43,7 +43,8 @@ bool conv_can_res_up(int W, int cout);
 bool conv_can_fuse_stats(int H, int W);                    // epilogue statistics need >= 32 pixels of one sample per warp
 int conv_pad_cout(int cout);
 
-AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, void* out);
+// head_ch = 64: attention_kernel; any other multiple of 64: attention_hd_kernel (kErrNotImplemented otherwise)
+AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out);
 void attn_launch_destroy(AttnLaunch* l);
 void attn_launch_run(const AttnLaunch* l, cudaStream_t s);
 

@@ -91,10 +91,21 @@ void Unet::build_topology() {
   add_param("time_embed.3.bias", {E});
   if (c.num_classes > 0) add_param("label_emb.weight", {c.num_classes, E});
 
-  auto heads_ok = [&](int ch) {
-    const int hc = c.num_head_channels == -1 ? ch / std::max(1, c.num_heads) : c.num_head_channels;
-    if (hc != 64 || ch % 64 != 0)
-      throw Error(kErrNotImplemented, "attention head width must be 64 channels (num_head_channels=64)");
+  // head width of an attention block over ch channels (AttentionBlock.__init__ adm.py:266-273, QKVAttention adm.py:244)
+  auto head_width = [&](int ch) {
+    int hc;
+    if (c.num_head_channels != -1) {
+      IVID_REQUIRE(c.num_head_channels > 0 && ch % c.num_head_channels == 0,
+                   "q,k,v channels " + std::to_string(ch) + " is not divisible by num_head_channels " + std::to_string(c.num_head_channels));
+      hc = c.num_head_channels;
+    } else {
+      IVID_REQUIRE(c.num_heads > 0 && ch % c.num_heads == 0,
+                   "attention channels " + std::to_string(ch) + " are not divisible by num_heads " + std::to_string(c.num_heads));
+      hc = ch / c.num_heads;
+    }
+    if (hc % 64 != 0)
+      throw Error(kErrNotImplemented, "attention head width " + std::to_string(hc) + " is not a multiple of 64 channels");
+    return hc;
   };
   auto add_res = [&](const std::string& pfx, int cin, int cout, int mode) {
     ResBlockDef r;
@@ -123,9 +134,8 @@ void Unet::build_topology() {
     return static_cast<int>(res_.size()) - 1;
   };
   auto add_attn = [&](const std::string& pfx, int ch) {
-    heads_ok(ch);
     AttnBlockDef a;
-    a.pfx = pfx; a.C = ch;
+    a.pfx = pfx; a.C = ch; a.head_ch = head_width(ch);
     add_param(pfx + ".norm.weight", {ch});
     add_param(pfx + ".norm.bias", {ch});
     add_param(pfx + ".qkv.weight", {3 * ch, ch, 1});
@@ -800,10 +810,10 @@ Plan* Unet::build_plan(int N) {
         add_conv(d);
       }
       if (create) {
-        AttnLaunch* l = attn_launch_create(s_qkv, N, T, a.C, s_a2);
+        AttnLaunch* l = attn_launch_create(s_qkv, N, T, a.C, a.head_ch, s_a2);
         pl->attns.push_back(l);
-        pl->ops.tag("attention", 4.0 * N * (a.C / 64) * static_cast<double>(T) * T * 64, static_cast<double>(N) * T * a.C * 8,
-                    "T=" + std::to_string(T) + " heads=" + std::to_string(a.C / 64));
+        pl->ops.tag("attention", 4.0 * N * static_cast<double>(T) * T * a.C, static_cast<double>(N) * T * a.C * 8,
+                    "T=" + std::to_string(T) + " heads=" + std::to_string(a.C / a.head_ch) + " d=" + std::to_string(a.head_ch));
         pl->ops.push_back([l](cudaStream_t s) { attn_launch_run(l, s); });
       }
       Act out = new_act(a.C, x.H, x.W);

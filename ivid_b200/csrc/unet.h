@@ -55,6 +55,7 @@ struct ResBlockDef {
 struct AttnBlockDef {
   std::string pfx;
   int C = 0;
+  int head_ch = 64;        // channels per head (a multiple of 64)
   GnW gn;
   ConvW qkv, proj;
 };
