@@ -62,6 +62,10 @@ int ivid_unet_weight_arena(const ivid_unet_t* h, void** dev_ptr, uint64_t* bytes
 int ivid_unet_forward(ivid_unet_t* h, const float* x_dev, int Nx, const int64_t* t_dev, const int64_t* classes_dev,
                       float* eps_dev, int N, void* stream);
 
+/* Pixel tile TW x TH x TN of the implicit-GEMM convolution at an H x W layer, and whether its epilogue can take the
+ * GroupNorm statistics (fused_stats).  Host-only query, no device needed. */
+int ivid_conv_tile(int H, int W, int* tw, int* th, int* tn, int* fused_stats);
+
 /* Parity aid (per-layer taps, tests/test_gpu_unet.py): output of the module `layer` (reference module path such as
  * "input_blocks.3.0", "middle_block.1", "output_blocks.14.0"; the stem is "input_blocks.0.0"; "emb" = time + class embedding
  * [N, 4*model_channels, 1, 1]; "film" = the stacked emb_layers outputs of all ResBlocks) of the LAST forward of batch
@@ -77,7 +81,8 @@ int ivid_unet_profile_end(ivid_unet_t* h, char* json_out, int capacity);
 /* Conditional inputs assembled on the fly (never materialised in fp32):
  *   kind 1: InpaintCFG.make_cond_inputs (frameworks/inpaint_cfg.py:24-49): cat[x, mask_rgb, y_rgb*m_rgb+z*(1-m_rgb),
  *           y_d*m+z*(1-m), m];  noise_dev = injected z [Nx,4,H,W] or NULL (in-kernel Philox(seed, stream)).
- *   kind 2: SuperResCFG.make_cond_inputs (frameworks/sr_cfg.py:23-36): cat[x, bilinear_up2(y)], y is [Nx,4,H/2,W/2]. */
+ *   kind 2: SuperResCFG.make_cond_inputs (frameworks/sr_cfg.py:23-36): cat[x, bilinear_up_s(y)], y is [Nx,4,H/s,W/s]
+ *           for the integer scale s = sr_scale (0 selects 2). */
 typedef struct {
   int kind;              /* 0 none, 1 inpaint, 2 super-resolution */
   const float* y_dev;
@@ -86,9 +91,18 @@ typedef struct {
   const float* noise_dev;
   uint64_t seed;
   uint32_t stream_id;
+  int sr_scale;          /* kind 2: integer upsampling factor s, y is [Nx,4,H/s,W/s]; 0 means 2 */
 } ivid_cond_t;
 int ivid_unet_forward_cond(ivid_unet_t* h, const float* x_dev, int Nx, const ivid_cond_t* cond, const int64_t* t_dev,
                            const int64_t* classes_dev, float* eps_dev, int N, void* stream);
+
+/* The forward at any input size H x W (x_dev [Nx, in_channels, H, W], eps_dev [N, out_channels, H, W]); cond may be
+ * NULL.  H and W must be positive multiples of 2^(len(channel_mult) - 1), as in the reference, whose skip
+ * concatenations fail otherwise: IVID_ERR_STATE.  Attention blocks stay at the levels image_size places them on and
+ * run over that level's h*w positions.  ivid_unet_forward and ivid_unet_forward_cond are this call with
+ * H = W = image_size.  Execution plans are cached per (N, H, W). */
+int ivid_unet_forward_hw(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
+                         const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Samplers — replace diffusion.samplers.DdpmSampler / DdimSampler (samplers/ddpm.py:12-187, samplers/ddim.py:12-165)
@@ -123,6 +137,7 @@ typedef struct {
   /* RNG: injected noise (parity tests) or in-kernel Philox4x32-10 keyed by (seed, step) */
   const float* step_noise_dev;         /* [N,C,H,W] noise of THIS step (ivid_sampler_step) or NULL */
   uint64_t seed;
+  int height, width;                   /* sample size H x W; 0 means the backbone's image_size */
 } ivid_step_args_t;
 
 /* sample_once: x_prev = f(x_t, t[, t_prev]).  `t` follows the reference's convention of each sampler:

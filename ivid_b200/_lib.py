@@ -29,6 +29,7 @@ class CondT(Structure):
         ("noise_dev", c_void_p),
         ("seed", c_uint64),
         ("stream_id", c_uint32),
+        ("sr_scale", c_int),          # kind 2: integer upsampling factor (0 = 2)
     ]
 
 
@@ -51,6 +52,8 @@ class StepArgsT(Structure):
         ("constrain_depth_weight", c_double),
         ("step_noise_dev", c_void_p),
         ("seed", c_uint64),
+        ("height", c_int),            # sample size; 0 = the backbone's image_size
+        ("width", c_int),
     ]
 
 
@@ -73,6 +76,9 @@ SIGNATURES = {
     "ivid_unet_weight_arena": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_uint64)]),
     "ivid_unet_forward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "ivid_unet_forward_cond": (c_int, [c_void_p, c_void_p, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "ivid_unet_forward_hw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p, c_int,
+                                     c_void_p]),
+    "ivid_conv_tile": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "ivid_unet_debug_tap": (c_int, [c_void_p, c_int, c_char_p, c_void_p, c_uint64, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "ivid_unet_profile_begin": (c_int, [c_void_p]),
     "ivid_unet_profile_end": (c_int, [c_void_p, c_char_p, c_int]),

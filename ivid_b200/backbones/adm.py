@@ -179,20 +179,22 @@ class AdmUnet2d(nn.Module):
         """Apply the model to an input batch (reference adm.py:526-566).
 
         x: [N, C, H, W] fp32 cuda; times: [N] long; classes: [N] long (-1 = null class) or None.  Returns eps [N, out, H, W].
+        H and W need not equal image_size (which only places the attention blocks): like the reference, any size divisible
+        by 2^(len(channel_mult) - 1) runs, and other sizes raise RuntimeError.
         """
         assert classes is None or self.num_classes is not None, "this model is not class-conditioned"
         if classes is not None:
             assert bool(torch.all(classes >= 0)) or self.has_null_class, "this model does not have a null class"
             assert classes.shape == (x.shape[0],), "classes must be a 1-D batch of labels"
-        assert x.dim() == 4 and x.shape[1] == self.in_channels and x.shape[2] == self.image_size and x.shape[3] == self.image_size, \
-            f"expected input [N,{self.in_channels},{self.image_size},{self.image_size}], got {tuple(x.shape)}"
+        assert x.dim() == 4 and x.shape[1] == self.in_channels, \
+            f"expected input [N,{self.in_channels},H,W], got {tuple(x.shape)}"
         self._ensure_packed()
-        N = x.shape[0]
+        N, _, H, W = x.shape
         xx = x.to(torch.float32).contiguous()
         tt = times.to(device=x.device, dtype=torch.int64).contiguous()
         cc = classes.to(device=x.device, dtype=torch.int64).contiguous() if classes is not None else None
-        out = torch.empty((N, self.out_channels, self.image_size, self.image_size), dtype=torch.float32, device=x.device)
+        out = torch.empty((N, self.out_channels, H, W), dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().ivid_unet_forward(self._handle, _lib.ptr(xx), N, _lib.ptr(tt), _lib.ptr(cc), _lib.ptr(out), N,
-                                                    _lib.cur_stream(x.device)))
+            _lib.check(_lib.lib().ivid_unet_forward_hw(self._handle, _lib.ptr(xx), N, H, W, None, _lib.ptr(tt), _lib.ptr(cc),
+                                                       _lib.ptr(out), N, _lib.cur_stream(x.device)))
         return out.type(x.dtype)

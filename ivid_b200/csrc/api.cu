@@ -101,18 +101,34 @@ int ivid_unet_weight_arena(const ivid_unet_t* h, void** dev_ptr, uint64_t* bytes
     if (bytes) *bytes = h->impl->arena_bytes();
   });
 }
-int ivid_unet_forward(ivid_unet_t* h, const float* x_dev, int Nx, const int64_t* t_dev, const int64_t* classes_dev,
-                      float* eps_dev, int N, void* stream) {
+int ivid_unet_forward_hw(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
+                         const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, void* stream) {
   return guarded([&] {
     IVID_NOT_NULL(h); IVID_NOT_NULL(x_dev); IVID_NOT_NULL(t_dev); IVID_NOT_NULL(eps_dev);
-    h->impl->forward(x_dev, Nx, nullptr, t_dev, classes_dev, eps_dev, N, static_cast<cudaStream_t>(stream));
+    h->impl->forward(x_dev, Nx, H, W, cond, t_dev, classes_dev, eps_dev, N, static_cast<cudaStream_t>(stream));
   });
+}
+// the square forwards at the backbone's image_size
+int ivid_unet_forward(ivid_unet_t* h, const float* x_dev, int Nx, const int64_t* t_dev, const int64_t* classes_dev,
+                      float* eps_dev, int N, void* stream) {
+  const int S = h != nullptr ? h->impl->cfg().image_size : 0;
+  return ivid_unet_forward_hw(h, x_dev, Nx, S, S, nullptr, t_dev, classes_dev, eps_dev, N, stream);
 }
 int ivid_unet_forward_cond(ivid_unet_t* h, const float* x_dev, int Nx, const ivid_cond_t* cond, const int64_t* t_dev,
                            const int64_t* classes_dev, float* eps_dev, int N, void* stream) {
+  if (cond == nullptr) return guarded([&] { IVID_NOT_NULL(cond); });
+  const int S = h != nullptr ? h->impl->cfg().image_size : 0;
+  return ivid_unet_forward_hw(h, x_dev, Nx, S, S, cond, t_dev, classes_dev, eps_dev, N, stream);
+}
+
+int ivid_conv_tile(int H, int W, int* tw, int* th, int* tn, int* fused_stats) {
   return guarded([&] {
-    IVID_NOT_NULL(h); IVID_NOT_NULL(x_dev); IVID_NOT_NULL(t_dev); IVID_NOT_NULL(eps_dev); IVID_NOT_NULL(cond);
-    h->impl->forward(x_dev, Nx, cond, t_dev, classes_dev, eps_dev, N, static_cast<cudaStream_t>(stream));
+    int a, b, c;
+    conv_tile(H, W, &a, &b, &c);
+    if (tw) *tw = a;
+    if (th) *th = b;
+    if (tn) *tn = c;
+    if (fused_stats) *fused_stats = conv_can_fuse_stats(H, W) ? 1 : 0;
   });
 }
 

@@ -11,6 +11,8 @@
 // accumulates O += P V with P as the register A operand (its fragment layout is the accumulator's) and V as an MN-major
 // shared-memory operand; the online-softmax rescale of O happens in registers.  (q*s)(k*s) with s = 64^-1/4 is
 // evaluated as (q.k) * 0.125 — an exact power of two.
+// Any T >= 1: ceil(T / 64) key blocks; TMA zero-fills K / V / Q rows past T (the tensor map's T dimension keeps them inside
+// the sample), the last block's keys >= T are masked to -inf (mask_key_tail) and query rows >= T are not stored.
 #pragma once
 #include "common.cuh"
 
@@ -39,6 +41,18 @@ __device__ __forceinline__ float ex2_ftz(float x) {
   return y;
 }
 
+// Sequence tail (T % 64 != 0): the last key block's rows >= T are TMA zero fill; their logits are set to -inf before the row
+// maximum, so their probabilities are exactly 0.  Accumulator group c of a thread holds key columns 8c + 2(lane & 3) + {0, 1}
+// for both of its rows.  Applied on that block only, so sequences of whole blocks keep their bits.
+__device__ __forceinline__ void mask_key_tail(float (&s)[32], int valid, int lane) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    const int col = 8 * c + 2 * (lane & 3);
+    if (col >= valid) { s[4 * c] = -INFINITY; s[4 * c + 2] = -INFINITY; }
+    if (col + 1 >= valid) { s[4 * c + 1] = -INFINITY; s[4 * c + 3] = -INFINITY; }
+  }
+}
+
 __global__ void __launch_bounds__(256, 2)
 attention_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapKV, const AttnParams p) {
   using Cfg = AttnCfg;
@@ -58,7 +72,8 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant
   const int qt = blockIdx.x % p.q_tiles;
   const int head = (blockIdx.x / p.q_tiles) % p.heads;
   const int n = blockIdx.x / (p.q_tiles * p.heads);
-  const int nkv = p.T / KV;
+  const int nkv = (p.T + KV - 1) / KV;
+  const int kv_tail = p.T - (nkv - 1) * KV;                 // valid keys of the last block (KV unless T % 64 != 0)
 
   auto load_kv = [&](int j) {
     const int st = j % ST;
@@ -107,6 +122,7 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
+    if (j == nkv - 1 && kv_tail != KV) mask_key_tail(s, kv_tail, lane);
     // row maxima: a thread holds 16 columns of each of its two rows; the four lanes of a row combine theirs
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll

@@ -75,7 +75,8 @@ attention_hd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
   const int slice = b % p.slices; b /= p.slices;
   const int head = b % p.heads;
   const int n = b / p.heads;
-  const int nkv = p.T / Cfg::KV;
+  const int nkv = (p.T + Cfg::KV - 1) / Cfg::KV;
+  const int kv_tail = p.T - (nkv - 1) * Cfg::KV;                    // valid keys of the last block (see mask_key_tail)
   const int nv = min(NV, p.chunks - slice * NV);                    // V boxes of this slice (>= 1)
   const int q_ch = head * 3 * p.d, k_ch = q_ch + p.d, v_ch = q_ch + 2 * p.d + slice * NV * 64;
 
@@ -157,6 +158,7 @@ attention_hd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
     wgmma_wait<0>();
     reg_fence(s);
     release();
+    if (j == nkv - 1 && kv_tail != Cfg::KV) mask_key_tail(s, kv_tail, lane);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int c = 0; c < 8; ++c) {

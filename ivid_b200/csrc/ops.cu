@@ -29,8 +29,23 @@ int conv_pad_cout(int cout) {
   if (cout >= 64) return ((cout + 63) / 64) * 64;
   return ((cout + 15) / 16) * 16;
 }
+// Pixel tile of the default kernel: TW = the largest power of two <= 16 that divides W, TH = the largest power of two
+// <= 128 / TW that divides H, TN = 128 / (TW * TH) samples.  For power-of-two sizes this is min(W, 16) x min(H, 128 / TW);
+// for any size the tiles never overhang the image, so only the batch tail is masked.
+static int pow2_divisor(int v, int cap) {
+  int t = 1;
+  while (t * 2 <= cap && v % (t * 2) == 0) t *= 2;
+  return t;
+}
+void conv_tile(int H, int W, int* TW, int* TH, int* TN) {
+  IVID_REQUIRE(H > 0 && W > 0, "conv: spatial size must be positive");
+  *TW = pow2_divisor(W, 16);
+  *TH = pow2_divisor(H, 128 / *TW);
+  *TN = 128 / (*TW * *TH);
+}
 bool conv_can_fuse_stats(int H, int W) {
-  const int TW = std::min(W, 16), TH = std::min(H, 128 / TW);
+  int TW, TH, TN;
+  conv_tile(H, W, &TW, &TH, &TN);
   return TW * TH >= 32;
 }
 // 128-wide tiles keep the 64 x 128 fp32 accumulator of a warpgroup at 64 registers per thread, so two CTAs share an SM
@@ -50,22 +65,18 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.taps0 == 9 || d.taps0 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.taps1 == 9 || d.taps1 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.C2 % 64 == 0 && (d.taps2 == 9 || d.taps2 == 1), "conv: segment 2 must be a multiple of 64 channels, 3x3 or 1x1");
-  auto is_pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
-  IVID_REQUIRE(is_pow2(d.H) && is_pow2(d.W), "conv: spatial size must be a power of two");
   auto* l = new ConvLaunch();
   ConvGemmParams& p = l->p;
   p.N = d.N; p.H = d.H; p.W = d.W;
-  p.TW = std::min(d.W, 16);
-  p.TH = std::min(d.H, 128 / p.TW);
-  p.TN = 128 / (p.TW * p.TH);
+  conv_tile(d.H, d.W, &p.TW, &p.TH, &p.TN);
   p.tiles_w = d.W / p.TW;
   p.tiles_h = d.H / p.TH;
   p.tiles_n = (d.N + p.TN - 1) / p.TN;
   l->BN = conv_pick_bn(d.cout_pad);
-  // 3x3 tap reuse (IVID_SLAB=1, read per launch creation): 8 x 16 pixel tiles; not with the upsampled residual (its index
-  // arithmetic assumes the 16-wide tiles of the default kernel)
+  // 3x3 tap reuse (IVID_SLAB=1, read per launch creation): 8 x 16 pixel tiles, where they divide the layer; not with the
+  // upsampled residual (its index arithmetic assumes the 16-wide tiles of the default kernel)
   const bool slab_on = getenv("IVID_SLAB") != nullptr && atoi(getenv("IVID_SLAB")) > 0;
-  if (slab_on && l->BN == 128 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && !d.residual_up) {
+  if (slab_on && l->BN == 128 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && d.H % 16 == 0 && d.W % 8 == 0 && !d.residual_up) {
     l->mode = kConvSlab;
     p.TW = 8; p.TH = 16; p.TN = 1;
     p.tiles_w = d.W / p.TW; p.tiles_h = d.H / p.TH; p.tiles_n = d.N;
@@ -196,7 +207,7 @@ AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch
   if (head_ch <= 0 || head_ch % 64 != 0)
     throw Error(kErrNotImplemented, "attention: head width " + std::to_string(head_ch) + " is not a multiple of 64");
   IVID_REQUIRE(C % head_ch == 0, "attention: channels must be a multiple of the head width " + std::to_string(head_ch));
-  IVID_REQUIRE(T >= 64 && T % 64 == 0, "attention: sequence length must be a multiple of 64");
+  IVID_REQUIRE(T >= 1, "attention: sequence length must be positive");
   auto* l = new AttnLaunch();
   l->head_ch = head_ch;
   l->p.N = N; l->p.T = T; l->p.C = C; l->p.heads = C / 64;

@@ -40,6 +40,8 @@ int conv_pick_bn(int cout_pad);
 bool conv_can_out16(int cout);
 // whether the conv epilogue can add a half-resolution residual through a nearest-2x upsample (output width W, Cout)
 bool conv_can_res_up(int W, int cout);
+// pixel tile TW x TH x TN (== 128) of the default conv kernel at an H x W layer (see ops.cu)
+void conv_tile(int H, int W, int* TW, int* TH, int* TN);
 bool conv_can_fuse_stats(int H, int W);                    // epilogue statistics need >= 32 pixels of one sample per warp
 int conv_pad_cout(int cout);
 
@@ -73,6 +75,7 @@ void launch_pack_input(const float* x, void* out, int N, int Nx, int Cin, int HW
 struct CondPackDesc {
   const float* x = nullptr; const float* y = nullptr; const float* mask = nullptr; const float* mask_rgb = nullptr;
   const float* noise = nullptr; void* out = nullptr; int N = 0, Nx = 0, H = 0, W = 0; int kind = 0;
+  int scale = 2;                                            // kind 2: y is [Nx][4][H/scale][W/scale]
   uint64_t seed = 0; uint32_t stream = 0; const int* stream_dev = nullptr;
 };
 void launch_cond_pack(const CondPackDesc& d, cudaStream_t s);   // sampler.cu

@@ -65,6 +65,9 @@ void launch_cond_pack(const CondPackDesc& d, cudaStream_t s) {
   cp.x = d.x; cp.y = d.y; cp.mask = d.mask; cp.mask_rgb = d.mask_rgb; cp.noise = d.noise;
   cp.out = reinterpret_cast<__half*>(d.out); cp.N = d.N; cp.Nx = d.Nx; cp.H = d.H; cp.W = d.W; cp.kind = d.kind;
   cp.seed = d.seed; cp.stream = d.stream; cp.stream_dev = d.stream_dev;
+  cp.scale = d.scale; cp.inv_scale = static_cast<float>(1.0 / d.scale);
+  IVID_REQUIRE(d.kind != 2 || (d.scale >= 1 && d.H % d.scale == 0 && d.W % d.scale == 0),
+               "cond inputs: the super-resolution scale must divide the output size");
   IVID_REQUIRE(d.kind == 1 || d.kind == 2, "cond inputs: kind must be 1 (inpaint) or 2 (super-resolution)");
   IVID_REQUIRE(d.y != nullptr, "cond inputs: y is required");
   IVID_REQUIRE(d.kind != 1 || d.mask != nullptr, "cond inputs: mask is required for inpainting");
@@ -160,7 +163,8 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
                    const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
                    const int64_t* t_prev_dev) {
   const UnetConfig& uc = unet.cfg();
-  const int C = uc.out_channels, S = uc.image_size, HW = S * S;
+  const int C = uc.out_channels, H = a.height > 0 ? a.height : uc.image_size, W = a.width > 0 ? a.width : uc.image_size;
+  const int HW = H * W;
   IVID_REQUIRE(N >= 1, "batch must be positive");
   IVID_REQUIRE(HW % 4 == 0, "image size");
   const bool ddim = a.kind == 1;
@@ -230,32 +234,32 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
   // node of the forward's CUDA graph.  Not taken when per-step pointers change every step (injected noise / trajectories inside
   // run(): every step would need its own graph) or when the model has no tap-column head.
   static const bool fuse_ok = getenv("IVID_NO_FUSED_STEP") == nullptr;
-  const bool fuse = fuse_ok && !no_fuse_ && unet.can_fuse_head() && C == 4 && S % 4 == 0;
+  const bool fuse = fuse_ok && !no_fuse_ && unet.can_fuse_head(W) && C == 4 && W % 4 == 0;
   if (fuse) {
     p.eps = nullptr;
     HeadStepParams hp;
     std::memset(&hp, 0, sizeof(hp));
-    hp.sp = p; hp.H = S; hp.W = S;
+    hp.sp = p; hp.H = H; hp.W = W;
     HeadHook hook;
     uint64_t h = 1469598103934665603ull ^ (ddim ? 0x9E37ull : 0ull);         // FNV-1a over everything the launcher bakes in
     const unsigned char* bytes = reinterpret_cast<const unsigned char*>(&p);
     for (size_t i = 0; i < sizeof(StepParams); ++i) { h ^= bytes[i]; h *= 1099511628211ull; }
     hook.key = h | 1ull;
-    hook.launch = [hp, ddim](const float* Y, const float* bias, int, int H, int W, int Co, int ldy, cudaStream_t st) mutable {
-      IVID_REQUIRE(Co == 4 && W % 4 == 0, "fused head step: 4 output channels, width % 4 == 0");
+    hook.launch = [hp, ddim](const float* Y, const float* bias, int, int Hy, int Wy, int Co, int ldy, cudaStream_t st) mutable {
+      IVID_REQUIRE(Co == 4 && Wy % 4 == 0, "fused head step: 4 output channels, width % 4 == 0");
       HeadStepParams q = hp;
-      q.Y = Y; q.bias = bias; q.H = H; q.W = W; q.ldy = ldy;
-      const size_t groups = static_cast<size_t>(q.sp.N) * H * (W / 4);
+      q.Y = Y; q.bias = bias; q.H = Hy; q.W = Wy; q.ldy = ldy;
+      const size_t groups = static_cast<size_t>(q.sp.N) * Hy * (Wy / 4);
       const int grid = static_cast<int>(std::min<size_t>((groups + 255) / 256, static_cast<size_t>(sm_count()) * 8));
       if (ddim) head_step_kernel<true><<<std::max(grid, 1), 256, 0, st>>>(q);
       else head_step_kernel<false><<<std::max(grid, 1), 256, 0, st>>>(q);
       IVID_CHECK_CUDA(cudaGetLastError());
     };
-    unet.forward(x_t, N, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, Nf, stream, &hook);
+    unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, Nf, stream, &hook);
     unet.set_cond_stream_dev(nullptr);
     return;
   }
-  unet.forward(x_t, N, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, Nf, stream);
+  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, Nf, stream);
   unet.set_cond_stream_dev(nullptr);
   const size_t total4 = static_cast<size_t>(N) * C * HW / 4;
   const int grid = static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8));
@@ -267,7 +271,8 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
 void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t& a, const float* noise_all,
                   const float* cond_noise_all, float* traj_x0, float* traj_xt, cudaStream_t stream) {
   const UnetConfig& uc = unet.cfg();
-  const size_t img = static_cast<size_t>(N) * uc.out_channels * uc.image_size * uc.image_size;
+  const size_t hw = static_cast<size_t>(a.height > 0 ? a.height : uc.image_size) * (a.width > 0 ? a.width : uc.image_size);
+  const size_t img = static_cast<size_t>(N) * uc.out_channels * hw;
   const bool ddim = a.kind == 1;
   if (!ddim) steps = T_;
   IVID_REQUIRE(steps >= 1 && steps <= T_, "steps out of range");
@@ -292,7 +297,7 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
     ivid_step_args_t ai = a;
     ai.step_noise_dev = noise_all ? noise_all + static_cast<size_t>(i) * img : nullptr;
     if (cond_noise_all && ai.cond.kind == 1)
-      ai.cond.noise_dev = cond_noise_all + static_cast<size_t>(i) * N * 4 * uc.image_size * uc.image_size;
+      ai.cond.noise_dev = cond_noise_all + static_cast<size_t>(i) * N * 4 * hw;
     float* dst = traj_xt ? traj_xt + static_cast<size_t>(i) * img : bufs[cur ^ 1];
     float* x0 = traj_x0 ? traj_x0 + static_cast<size_t>(i) * img : nullptr;
     const float* src = (traj_xt && i > 0) ? traj_xt + static_cast<size_t>(i - 1) * img : bufs[cur];

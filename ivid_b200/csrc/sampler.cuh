@@ -270,13 +270,15 @@ __global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) 
 // ----------------------------------------------------------------------------------------------
 struct CondPackParams {
   const float* x;         // [Nx,4,H,W]
-  const float* y;         // inpaint: [Nx,4,H,W] warped RGBD;  superres: [Nx,4,H/2,W/2] low-res RGBD
+  const float* y;         // inpaint: [Nx,4,H,W] warped RGBD;  superres: [Nx,4,H/s,W/s] low-res RGBD
   const float* mask;      // inpaint [Nx,1,H,W]
   const float* mask_rgb;  // inpaint [Nx,1,H,W] or nullptr (then mask is used and no mask_rgb channel is emitted)
   const float* noise;     // inpaint: injected [Nx,4,H,W] (rgb noise 3 + depth noise 1) or nullptr -> Philox
   __half* out;            // [N,H,W,64]
   int N, Nx, H, W;
   int kind;               // 1 = InpaintCFG, 2 = SuperResCFG
+  int scale;              // superres: integer upsampling factor s
+  float inv_scale;        // superres: (float)(1.0 / s), the source-index scale of ATen's upsample_bilinear2d(scale_factor=s)
   uint64_t seed;
   uint32_t stream;
   const int* stream_dev;
@@ -320,11 +322,12 @@ __global__ void __launch_bounds__(256) cond_pack_kernel(const CondPackParams p) 
         ch[o++] = p.y[(static_cast<size_t>(n) * 4 + 3) * HW + pix] * m + z[3] * (1.0f - m);
         ch[o++] = m;
       } else {
-        // bilinear 2x upsample, align_corners=False: src = (dst + 0.5)/2 - 0.5, clamped at 0 (ATen upsample_bilinear2d)
+        // bilinear s-x upsample, align_corners=False: src = (dst + 0.5) * (1/s) - 0.5, clamped at 0 (ATen upsample_bilinear2d
+        // with scale_factor=s); for s = 2 the factor is exactly 0.5
         const int h = pix / p.W, w = pix % p.W;
-        const int Hs = p.H / 2, Ws = p.W / 2;
-        float sy = (h + 0.5f) * 0.5f - 0.5f; if (sy < 0.f) sy = 0.f;
-        float sx = (w + 0.5f) * 0.5f - 0.5f; if (sx < 0.f) sx = 0.f;
+        const int Hs = p.H / p.scale, Ws = p.W / p.scale;
+        float sy = (h + 0.5f) * p.inv_scale - 0.5f; if (sy < 0.f) sy = 0.f;
+        float sx = (w + 0.5f) * p.inv_scale - 0.5f; if (sx < 0.f) sx = 0.f;
         const int y0 = static_cast<int>(sy), x0 = static_cast<int>(sx);
         const int y1 = y0 + (y0 < Hs - 1 ? 1 : 0), x1 = x0 + (x0 < Ws - 1 ? 1 : 0);
         const float ly = sy - y0, lx = sx - x0;

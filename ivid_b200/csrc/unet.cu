@@ -424,7 +424,9 @@ Unet::~Unet() {
 // ==================================================================================================
 struct Plan {
   int N = 0;
+  int H = 0, W = 0;        // input geometry
   int slot = 0;            // 0 = main stream, 1 = side stream (two half-batches run concurrently)
+  uint64_t last_use = 0;   // Unet::plan_uses_ at the latest forward
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
   double* stats_base = nullptr;
@@ -459,8 +461,9 @@ struct Plan {
     int kind; const void* y; const void* mask; const void* mask_rgb; const void* noise; uint64_t seed; uint32_t stream_id;
     const void* stream_dev;
     uint64_t hook_key;
+    int sr_scale;
     bool operator==(const GraphKey& o) const {
-      return hook_key == o.hook_key && x == o.x && Nx == o.Nx && t == o.t && classes == o.classes && eps == o.eps && kind == o.kind && y == o.y && mask == o.mask &&
+      return hook_key == o.hook_key && sr_scale == o.sr_scale && x == o.x && Nx == o.Nx && t == o.t && classes == o.classes && eps == o.eps && kind == o.kind && y == o.y && mask == o.mask &&
              mask_rgb == o.mask_rgb && noise == o.noise && seed == o.seed && stream_id == o.stream_id && stream_dev == o.stream_dev;
     }
   };
@@ -499,22 +502,36 @@ struct Bump {
 };
 }  // namespace
 
-Plan* Unet::get_plan(int N, int slot) {
-  for (auto& p : plans_) if (p->N == N && p->slot == slot) return p.get();
-  if (plans_.size() >= 4) {
-    IVID_CHECK_CUDA(cudaDeviceSynchronize());     // the evicted plan's workspace may still be in use by queued kernels
-    plans_.erase(plans_.begin());
-  }
-  plans_.emplace_back(build_plan(N));
-  plans_.back()->slot = slot;
-  return plans_.back().get();
+void Unet::check_geometry(int H, int W) const {
+  const int levels = static_cast<int>(cfg_.channel_mult.size());
+  const int m = 1 << (levels - 1);
+  if (H <= 0 || W <= 0 || H % m != 0 || W % m != 0)
+    throw Error(kErrState, "input size " + std::to_string(H) + "x" + std::to_string(W) + " is not a multiple of " + std::to_string(m) +
+                               " (2^(levels-1)): the skip connections' sizes would not match after " + std::to_string(levels - 1) + " downsamplings");
 }
 
-Plan* Unet::build_plan(int N) {
+Plan* Unet::get_plan(int N, int H, int W, int slot) {
+  Plan* found = nullptr;
+  for (auto& p : plans_) if (p->N == N && p->H == H && p->W == W && p->slot == slot) found = p.get();
+  if (found == nullptr) {
+    check_geometry(H, W);
+    if (plans_.size() >= 4) {
+      IVID_CHECK_CUDA(cudaDeviceSynchronize());     // the evicted plan's workspace may still be in use by queued kernels
+      plans_.erase(plans_.begin());
+    }
+    plans_.emplace_back(build_plan(N, H, W));
+    plans_.back()->slot = slot;
+    found = plans_.back().get();
+  }
+  found->last_use = ++plan_uses_;
+  return found;
+}
+
+Plan* Unet::build_plan(int N, int SH, int SW) {
   std::unique_ptr<Plan> plan(new Plan());
   plan->N = N;
+  plan->H = SH; plan->W = SW;
   Plan* pl = plan.get();
-  const int S = cfg_.image_size;
   const int G = cfg_.num_groups;
   const float eps = 1e-5f;
   auto W8 = [&](size_t off) { return arena_ + off; };
@@ -523,28 +540,30 @@ Plan* Unet::build_plan(int N) {
   // ---- scratch maxima (walk the topology once for sizes) ----
   size_t max_act16 = 0, max_raw16 = 0, max_f32 = 0, max_qkv = 0, max_col = 0;
   {
-    int res = S;
+    int rh = SH, rw = SW;
     auto upd_res = [&](const ResBlockDef& r) {
-      const int ro = r.mode == 1 ? res * 2 : (r.mode == 2 ? res / 2 : res);
-      max_act16 = std::max({max_act16, static_cast<size_t>(N) * ro * ro * r.cin, static_cast<size_t>(N) * ro * ro * r.cout});
-      max_raw16 = std::max(max_raw16, static_cast<size_t>(N) * res * res * r.cin);
-      max_f32 = std::max({max_f32, static_cast<size_t>(N) * ro * ro * r.cin, static_cast<size_t>(N) * ro * ro * r.cout});
-      res = ro;
+      const int oh = r.mode == 1 ? rh * 2 : (r.mode == 2 ? rh / 2 : rh);
+      const int ow = r.mode == 1 ? rw * 2 : (r.mode == 2 ? rw / 2 : rw);
+      const size_t po = static_cast<size_t>(N) * oh * ow;
+      max_act16 = std::max({max_act16, po * r.cin, po * r.cout});
+      max_raw16 = std::max(max_raw16, static_cast<size_t>(N) * rh * rw * r.cin);
+      max_f32 = std::max({max_f32, po * r.cin, po * r.cout});
+      rh = oh; rw = ow;
     };
     for (const auto& b : blocks_)
       for (const auto& l : b.layers) {
         if (l.kind == 1) upd_res(res_[l.idx]);
         else if (l.kind == 3) {
           const auto& r = resample_[l.idx];
-          if (r.mode == 2) { max_col = std::max(max_col, static_cast<size_t>(N) * (res / 2) * (res / 2) * 9 * r.C); res /= 2; }
-          else { max_act16 = std::max(max_act16, static_cast<size_t>(N) * (res * 2) * (res * 2) * r.C); res *= 2; }
+          if (r.mode == 2) { max_col = std::max(max_col, static_cast<size_t>(N) * (rh / 2) * (rw / 2) * 9 * r.C); rh /= 2; rw /= 2; }
+          else { max_act16 = std::max(max_act16, static_cast<size_t>(N) * (rh * 2) * (rw * 2) * r.C); rh *= 2; rw *= 2; }
         } else {
           const auto& a = attn_[l.idx];
-          max_act16 = std::max(max_act16, static_cast<size_t>(N) * res * res * a.C);
-          max_qkv = std::max(max_qkv, static_cast<size_t>(N) * res * res * 3 * a.C);
+          max_act16 = std::max(max_act16, static_cast<size_t>(N) * rh * rw * a.C);
+          max_qkv = std::max(max_qkv, static_cast<size_t>(N) * rh * rw * 3 * a.C);
         }
       }
-    max_act16 = std::max(max_act16, static_cast<size_t>(N) * S * S * std::max(64, final_ch_));
+    max_act16 = std::max(max_act16, static_cast<size_t>(N) * SH * SW * std::max(64, final_ch_));
   }
 
   // The same allocation sequence is run three times: once to find out which block outputs are ever read in fp32 (residual
@@ -558,14 +577,12 @@ Plan* Unet::build_plan(int N) {
     // (sized generously: every tensor needs N*C*16 bytes; bound by total params walk below)
     size_t stats_cap = 0;
     {
-      int res = S;
       stats_cap += static_cast<size_t>(N) * in_ch_stem_ * 16 + 1024;
       for (const auto& b : blocks_)
         for (const auto& l : b.layers) {
           if (l.kind == 1) {
             const auto& r = res_[l.idx];
             stats_cap += 2 * (static_cast<size_t>(N) * r.cout * 16 + 1024);
-            res = r.mode == 1 ? res * 2 : (r.mode == 2 ? res / 2 : res);
           } else if (l.kind == 3) {
             stats_cap += static_cast<size_t>(N) * resample_[l.idx].C * 16 + 1024;
           } else {
@@ -591,7 +608,7 @@ Plan* Unet::build_plan(int N) {
     };
 
     // scratch
-    void* s_in = bump.take(static_cast<size_t>(N) * S * S * 64 * 2);
+    void* s_in = bump.take(static_cast<size_t>(N) * SH * SW * 64 * 2);
     void* s_a1 = bump.take(max_act16 * 2);
     void* s_a2 = bump.take(max_act16 * 2);
     void* s_xh = bump.take(max_raw16 * 2);
@@ -667,8 +684,9 @@ Plan* Unet::build_plan(int N) {
       d.beta = pend.beta; d.film = pend.film; d.film_ld = pend.film_ld; d.film_off = pend.film_off; d.film_add = pend.film_add;
       {
         const int Ho = d.mode == 1 ? d.H * 2 : (d.mode == 2 ? d.H / 2 : d.H);
+        const int Wo = d.mode == 1 ? d.W * 2 : (d.mode == 2 ? d.W / 2 : d.W);
         const double in_el = static_cast<double>(d.N) * d.H * d.W * (d.C0 + d.C1);
-        const double out_el = static_cast<double>(d.N) * Ho * Ho * (d.C0 + d.C1);
+        const double out_el = static_cast<double>(d.N) * Ho * Wo * (d.C0 + d.C1);
         pl->ops.tag("gn_apply", 0, in_el * (d.x0_half ? 2 : 4) + out_el * 2 + (d.out_raw16 ? out_el * 2 : 0) + (d.out_raw32 ? out_el * 4 : 0),
                     std::to_string(d.H) + "x" + std::to_string(d.W) + " C" + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") +
                         " m" + std::to_string(d.mode) + (d.x0_half ? " h16" : "") + (d.out_raw16 ? " raw16" : "") + (d.out_raw32 ? " raw32" : ""));
@@ -701,7 +719,7 @@ Plan* Unet::build_plan(int N) {
 
     // ---- stem ----
     if (create) {
-      const int Cin = cfg_.in_channels, HW = S * S;
+      const int Cin = cfg_.in_channels, HW = SH * SW;
       pl->ops.tag("pack_input", 0, static_cast<double>(N) * HW * (Cin * 4 + 128));
       pl->ops.push_back([=](cudaStream_t s) {
         if (pl->cond.kind == 0) {
@@ -709,20 +727,21 @@ Plan* Unet::build_plan(int N) {
         } else {
           CondPackDesc cp;
           cp.x = pl->x; cp.y = pl->cond.y_dev; cp.mask = pl->cond.mask_dev; cp.mask_rgb = pl->cond.mask_rgb_dev;
-          cp.noise = pl->cond.noise_dev; cp.out = s_in; cp.N = N; cp.Nx = pl->Nx; cp.H = S; cp.W = S;
+          cp.noise = pl->cond.noise_dev; cp.out = s_in; cp.N = N; cp.Nx = pl->Nx; cp.H = SH; cp.W = SW;
           cp.kind = pl->cond.kind; cp.seed = pl->cond.seed; cp.stream = pl->cond.stream_id; cp.stream_dev = pl->cond_stream_dev;
+          cp.scale = pl->cond.sr_scale > 0 ? pl->cond.sr_scale : 2;
           launch_cond_pack(cp, s);
         }
       });
     }
-    Act cur = new_act(in_ch_stem_, S, S);
+    Act cur = new_act(in_ch_stem_, SH, SW);
     {
       ConvDesc d;
       d.act0 = s_in; d.C0 = 64; d.taps0 = 9;
       d.weight = W8(in_conv_.w_off); d.cout_pad = in_conv_.cout_pad; d.cout = in_conv_.cout; d.bias = Wf(in_conv_.b_off);
       if (only16(cur, false)) { d.out = cur.d16; d.out_mode = 1; }
       else { alloc32(cur); d.out = cur.data; d.out16 = cur.d16; d.out_mode = 0; }
-      d.ldc = cur.C; d.N = N; d.H = S; d.W = S;
+      d.ldc = cur.C; d.N = N; d.H = SH; d.W = SW;
       add_conv(d, &cur, 9.0 * cfg_.in_channels);
       add_stats(cur);
       if (create) pl->taps.push_back({"input_blocks.0.0", cur.data, cur.d16, cur.C, cur.H, cur.W});
@@ -903,7 +922,7 @@ Plan* Unet::build_plan(int N) {
     GnApplyDesc go;
     const bool split_head = out_split_ && cur.d16 != nullptr;
     if (cur.d16 != nullptr) { go.x0 = cur.d16; go.x0_half = true; } else go.x0 = use32(cur);
-    go.C0 = cur.C; go.N = N; go.H = S; go.W = S; go.mode = 0; go.silu = 1; go.out_act = s_a1;
+    go.C0 = cur.C; go.N = N; go.H = SH; go.W = SW; go.mode = 0; go.silu = 1; go.out_act = s_a1;
     if (split_head) go.out_lo = s_a2;
     add_apply(go);
     if (split_head) {
@@ -914,27 +933,27 @@ Plan* Unet::build_plan(int N) {
       d.act1 = s_a2; d.C1 = cur.C; d.taps1 = 1;
       d.act2 = s_a1; d.C2 = cur.C; d.taps2 = 1;
       d.weight = W8(out1x1_.w_off); d.cout_pad = 64; d.cout = 64; d.bias = Wf(out1x1_.b_off);
-      d.out = s_h; d.ldc = 64; d.out_mode = 0; d.N = N; d.H = S; d.W = S;
+      d.out = s_h; d.ldc = 64; d.out_mode = 0; d.N = N; d.H = SH; d.W = SW;
       add_conv(d, nullptr, 9.0 * cur.C, static_cast<double>(cfg_.out_channels));
       if (create) {
         const float* Y = s_h; const float* ob = Wf(out_conv_.b_off);
         const int Co = cfg_.out_channels;
-        pl->ops.tag("eps_gather", 0, static_cast<double>(N) * S * S * (9.0 * Co * 4 + Co * 4));
+        pl->ops.tag("eps_gather", 0, static_cast<double>(N) * SH * SW * (9.0 * Co * 4 + Co * 4));
         pl->ops.push_back([=](cudaStream_t s) {
-          if (pl->hook != nullptr) pl->hook->launch(Y, ob, N, S, S, Co, 64, s);
-          else launch_eps_gather(Y, ob, pl->eps, N, S, S, Co, 64, s);
+          if (pl->hook != nullptr) pl->hook->launch(Y, ob, N, SH, SW, Co, 64, s);
+          else launch_eps_gather(Y, ob, pl->eps, N, SH, SW, Co, 64, s);
         });
       }
     } else if (create) {
       ConvDesc d;
       d.act0 = s_a1; d.C0 = cur.C; d.taps0 = 9;
       d.weight = W8(out_conv_.w_off); d.cout_pad = out_conv_.cout_pad; d.cout = cfg_.out_channels; d.bias = Wf(out_conv_.b_off);
-      d.out = nullptr; d.ldc = 0; d.out_mode = 2; d.N = N; d.H = S; d.W = S;
+      d.out = nullptr; d.ldc = 0; d.out_mode = 2; d.N = N; d.H = SH; d.W = SW;
       ConvLaunch* l = conv_launch_create(d);
       pl->convs.push_back(l);
       // eps pointer is a per-call input: patched through the plan at run time
-      pl->ops.tag("conv_gemm<16>", 2.0 * N * S * S * 9.0 * cur.C * cfg_.out_channels,
-                  static_cast<double>(N) * S * S * (cur.C * 2 + cfg_.out_channels * 4));
+      pl->ops.tag("conv_gemm<16>", 2.0 * N * SH * SW * 9.0 * cur.C * cfg_.out_channels,
+                  static_cast<double>(N) * SH * SW * (cur.C * 2 + cfg_.out_channels * 4));
       pl->ops.push_back([l, pl](cudaStream_t s) { conv_launch_run_out(l, pl->eps, s); });
     }
     if (create) {
@@ -954,13 +973,14 @@ Plan* Unet::build_plan(int N) {
   return plan.release();
 }
 
-bool Unet::can_fuse_head() const {
-  return out_split_ && conv_can_out16(final_ch_) && cfg_.out_channels == 4 && cfg_.image_size % 4 == 0;
+bool Unet::can_fuse_head(int W) const {
+  return out_split_ && conv_can_out16(final_ch_) && cfg_.out_channels == 4 && W % 4 == 0;
 }
 
-void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes, float* eps,
-                   int N, cudaStream_t stream, const HeadHook* hook) {
+void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes,
+                   float* eps, int N, cudaStream_t stream, const HeadHook* hook) {
   if (!finalized()) throw Error(kErrState, "AdmUnet2d: forward before .cuda()/finalize");
+  check_geometry(H, W);
   IVID_REQUIRE(N >= 1 && Nx >= 1 && N % Nx == 0, "forward: N must be a positive multiple of Nx");
   // reference: "this model is not class-conditioned" (adm.py:540)
   IVID_REQUIRE(classes == nullptr || cfg_.num_classes > 0, "this model is not class-conditioned");
@@ -968,7 +988,9 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
   ivid_cond_t cnd = cond ? *cond : ivid_cond_t{};
   const int expect_in = cnd.kind == 1 ? (cnd.mask_rgb_dev ? 10 : 9) : (cnd.kind == 2 ? 8 : cfg_.in_channels);
   IVID_REQUIRE(expect_in == cfg_.in_channels, "forward: conditional inputs do not match the model's in_channels");
-  IVID_REQUIRE(hook == nullptr || can_fuse_head(), "forward: a head hook needs the tap-column output head");
+  IVID_REQUIRE(hook == nullptr || can_fuse_head(W), "forward: a head hook needs the tap-column output head");
+  IVID_REQUIRE(cnd.kind != 2 || (cnd.sr_scale >= 0 && H % std::max(cnd.sr_scale, 1) == 0 && W % std::max(cnd.sr_scale, 1) == 0),
+               "forward: the super-resolution scale must divide the input size");
   IVID_REQUIRE(hook != nullptr || eps != nullptr, "forward: eps output missing");
 
   // Two half-batches on two streams: the HBM-bound GroupNorm passes of one half may overlap the tensor-bound convolutions
@@ -979,7 +1001,7 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
                          !(cnd.kind != 0 && Nx == N && cnd.noise_dev == nullptr);
   if (can_split) {
     const int half = N / 2;
-    const size_t img = static_cast<size_t>(cfg_.image_size) * cfg_.image_size;
+    const size_t img = static_cast<size_t>(H) * W;
     if (side_stream_ == nullptr) {
       IVID_CHECK_CUDA(cudaStreamCreateWithFlags(&side_stream_, cudaStreamNonBlocking));
       IVID_CHECK_CUDA(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
@@ -988,7 +1010,7 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
     IVID_CHECK_CUDA(cudaEventRecord(ev_fork_, stream));
     IVID_CHECK_CUDA(cudaStreamWaitEvent(side_stream_, ev_fork_, 0));
     for (int hb = 0; hb < 2; ++hb) {
-      Plan* ph = get_plan(half, hb);
+      Plan* ph = get_plan(half, H, W, hb);
       cudaStream_t st = hb == 0 ? stream : side_stream_;
       const bool shift = (Nx == N) && hb == 1;            // rows [half, N) of per-sample inputs
       const size_t xs = static_cast<size_t>(cfg_.in_channels) * img;
@@ -1000,7 +1022,8 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
       ph->eps = eps + static_cast<size_t>(hb) * half * cfg_.out_channels * img;
       ph->cond = cnd;
       if (cnd.kind != 0 && shift) {
-        const size_t yimg = cnd.kind == 2 ? img / 4 : img;
+        const int s = cnd.sr_scale > 0 ? cnd.sr_scale : 2;
+        const size_t yimg = cnd.kind == 2 ? img / (static_cast<size_t>(s) * s) : img;
         ph->cond.y_dev = cnd.y_dev + static_cast<size_t>(half) * 4 * yimg;
         if (cnd.mask_dev) ph->cond.mask_dev = cnd.mask_dev + static_cast<size_t>(half) * img;
         if (cnd.mask_rgb_dev) ph->cond.mask_rgb_dev = cnd.mask_rgb_dev + static_cast<size_t>(half) * img;
@@ -1014,7 +1037,7 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
     return;
   }
 
-  Plan* pl = get_plan(N, 0);
+  Plan* pl = get_plan(N, H, W, 0);
   pl->x = x; pl->Nx = Nx; pl->t = t; pl->classes = classes; pl->eps = eps;
   pl->cond = cnd;
   pl->cond_stream_dev = cond_stream_dev_;
@@ -1028,7 +1051,7 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
     if (graphs_on && pl->runs > 1) {
       const Plan::GraphKey key{x, Nx, t, classes, eps, cnd.kind, cnd.y_dev, cnd.mask_dev, cnd.mask_rgb_dev, cnd.noise_dev,
                                cnd.kind != 0 ? cnd.seed : 0ull, cnd.kind != 0 ? cnd.stream_id : 0u, cond_stream_dev_,
-                               hook ? hook->key : 0ull};
+                               hook ? hook->key : 0ull, cnd.kind == 2 ? cnd.sr_scale : 0};
       for (auto& g : pl->graphs)
         if (g.key == key) {
           g.last_use = pl->runs;
@@ -1103,12 +1126,13 @@ void Unet::forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_
   for (auto& e : ev) cudaEventDestroy(e);
 }
 
-// Debug tap: output of the named layer (reference module path, e.g. "input_blocks.3.0") of the LAST forward of batch N,
-// converted to fp32 NCHW on the host.  Tensors that only exist as fp16 in the plan (outputs nobody reads in fp32) are
-// widened.  Synchronises the device; not on any hot path.
+// Debug tap: output of the named layer (reference module path, e.g. "input_blocks.3.0") of the LAST forward of batch N
+// (whatever its input size), converted to fp32 NCHW on the host.  Tensors that only exist as fp16 in the plan (outputs
+// nobody reads in fp32) are widened.  Synchronises the device; not on any hot path.
 void Unet::debug_tap(int N, const std::string& name, float* host_out, size_t capacity, int* C, int* H, int* W) {
   Plan* pl = nullptr;
-  for (auto& p : plans_) if (p->N == N && p->slot == 0) pl = p.get();
+  for (auto& p : plans_)
+    if (p->N == N && p->slot == 0 && (pl == nullptr || p->last_use > pl->last_use)) pl = p.get();
   if (pl == nullptr) throw Error(kErrState, "debug_tap: no forward of this batch size has run");
   for (const auto& t : pl->taps) {
     if (t.name != name) continue;

@@ -94,11 +94,14 @@ class Unet {
   size_t arena_bytes() const { return arena_bytes_; }
   int device() const { return device_; }
 
-  // forward over a batch of N samples; x rows are read modulo Nx (CFG halves share x)
-  void forward(const float* x, int Nx, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes, float* eps,
-               int N, cudaStream_t stream, const HeadHook* hook = nullptr);
-  // whether the output head runs as the tap-column GEMM whose last kernel a HeadHook can replace
-  bool can_fuse_head() const;
+  // forward over a batch of N samples of H x W pixels; x rows are read modulo Nx (CFG halves share x)
+  void forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes,
+               float* eps, int N, cudaStream_t stream, const HeadHook* hook = nullptr);
+  // whether the output head of an H x W forward runs as the tap-column GEMM whose last kernel a HeadHook can replace
+  bool can_fuse_head(int W) const;
+  // inputs the network accepts: H and W positive multiples of 2^(levels - 1), as in the reference (its skip concatenations
+  // fail otherwise); kErrState otherwise
+  void check_geometry(int H, int W) const;
   // Device-resident Philox stream id (step counter) of the conditional-input noise: the sampler points this at its step
   // state so that consecutive denoising steps replay the same CUDA graph (a by-value stream id would change the key).
   void set_cond_stream_dev(const int* p) { cond_stream_dev_ = p; }
@@ -111,8 +114,8 @@ class Unet {
   void build_topology();
   int add_param(const std::string& name, std::vector<int64_t> shape, bool is_buffer = false);
   const ParamSpec& P(const std::string& name) const;
-  Plan* get_plan(int N, int slot);
-  Plan* build_plan(int N);
+  Plan* get_plan(int N, int H, int W, int slot);
+  Plan* build_plan(int N, int H, int W);
 
   UnetConfig cfg_;
   int embed_dim_ = 0;
@@ -145,7 +148,8 @@ class Unet {
   bool profile_ = false;
   std::map<std::string, ProfAgg> profile_acc_;
   std::string profile_ops_;
-  std::vector<std::unique_ptr<Plan>> plans_;
+  std::vector<std::unique_ptr<Plan>> plans_;       // keyed by (N, H, W, slot)
+  uint64_t plan_uses_ = 0;                         // debug_tap reads the most recently run plan of a batch size
   friend struct Plan;
 };
 

@@ -80,7 +80,8 @@ class GaussianDiffusion:
         dev = x.device
         N = x.shape[0]
         xx = x.to(torch.float32).contiguous()
-        out_shape = (N, net.out_channels, net.image_size, net.image_size)
+        H, W = x.shape[-2:]
+        out_shape = (N, net.out_channels, H, W)
         # classes None: both halves of the reference's expression are the same null-class forward, (1+s)e - s*e = e
         two = strength > 0 and classes is not None
         if two:
@@ -99,11 +100,8 @@ class GaussianDiffusion:
         eps = torch.empty((nf,) + out_shape[1:], dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             st = _lib.cur_stream(dev)
-            if cond is None:
-                _lib.check(L.ivid_unet_forward(net._handle, _lib.ptr(xx), N, _lib.ptr(tt), _lib.ptr(cc), _lib.ptr(eps), nf, st))
-            else:
-                _lib.check(L.ivid_unet_forward_cond(net._handle, _lib.ptr(xx), N, ctypes.byref(cond), _lib.ptr(tt), _lib.ptr(cc),
-                                                    _lib.ptr(eps), nf, st))
+            _lib.check(L.ivid_unet_forward_hw(net._handle, _lib.ptr(xx), N, H, W, ctypes.byref(cond) if cond is not None else None,
+                                              _lib.ptr(tt), _lib.ptr(cc), _lib.ptr(eps), nf, st))
             if not two:
                 return eps if (strength >= 0 and (classes is None or strength == 0)) else (1 + strength) * eps
             out = torch.empty(out_shape, dtype=torch.float32, device=dev)
@@ -190,16 +188,25 @@ class SuperResCFG(GaussianDiffusion):
 
     def make_cond_inputs(self, x, y, **kwargs):
         """cat[x, bilinear-upsampled y] of sr_cfg.py:23-36 as an fp32 tensor (API parity; `model_inference` uses the fused
-        native assembly, which applies the same align_corners=False 2x stencil in-kernel)."""
-        up = F.interpolate(y, size=x.shape[-2:], mode="bilinear", align_corners=False)
+        native assembly, which applies the same align_corners=False stencil in-kernel)."""
+        scale = x.shape[-1] // y.shape[-1]
+        up = F.interpolate(y, scale_factor=scale, mode="bilinear", align_corners=False)
         return torch.cat([x, up], dim=1)
+
+    @staticmethod
+    def _scale(x, y):
+        """The integer upsampling factor s of y -> x; RuntimeError unless y * s == x in both dimensions."""
+        s = x.shape[-1] // y.shape[-1] if y.shape[-1] > 0 else 0
+        if s < 1 or y.shape[-1] * s != x.shape[-1] or y.shape[-2] * s != x.shape[-2]:
+            raise RuntimeError(f"SuperResCFG: x {tuple(x.shape[-2:])} is not an integer multiple of y {tuple(y.shape[-2:])}")
+        return s
 
     @torch.no_grad()
     def model_inference(self, x, t, y, classes=None, strength=3.0, **kwargs):
         # sr_cfg.py:39-60
-        assert x.shape[-1] == 2 * y.shape[-1], "SuperResCFG: the native path implements the 2x configuration of the reference"
         yy = y.to(device=x.device, dtype=torch.float32).contiguous()
         cond = _lib.CondT()
         cond.kind = 2
+        cond.sr_scale = self._scale(x, yy)
         cond.y_dev = yy.data_ptr()
         return self._native_forward(x, t, classes, strength if classes is not None else 0.0, cond, keep=(yy,))

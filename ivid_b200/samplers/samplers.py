@@ -64,7 +64,7 @@ class _NativeSampler:
         return out
 
     # ------------------------------------------------------------------------------------------------------------
-    def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0):
+    def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -97,6 +97,8 @@ class _NativeSampler:
             assert "y" in kwargs, "SuperResCFG.model_inference needs y"
             a.cond.kind = 2
             a.cond.y_dev = P(kwargs["y"])
+            if hw is not None:
+                a.cond.sr_scale = SuperResCFG._scale(torch.empty(0, 0, *hw), kwargs["y"])
         rr = kwargs.get("replace_rgb")
         if rr is not None:
             assert self.KIND == 1, "replace_rgb is a DdimSampler argument"
@@ -109,6 +111,8 @@ class _NativeSampler:
                 a.constrain_depth_weight = float(cd[0]); a.constrain_depth_dev = P(cd[1])
         a.step_noise_dev = P(step_noise)
         a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        if hw is not None:
+            a.height, a.width = int(hw[0]), int(hw[1])
         return a, keep
 
     def _net(self):
@@ -120,7 +124,8 @@ class _NativeSampler:
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
-        a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise)
+        a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
+                                  hw=x_t.shape[-2:])
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         with torch.cuda.device(dev):
@@ -135,7 +140,8 @@ class _NativeSampler:
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
-        a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise)
+        a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
+                                  hw=x_t.shape[-2:])
         td = t.to(device=dev, dtype=torch.int64).contiguous()
         tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
         x_prev = torch.empty_like(x_t)
@@ -162,12 +168,13 @@ class _NativeSampler:
         net.eval()
         if image_size is None:
             image_size = net.image_size
-        assert image_size == net.image_size, "image_size must match the backbone"
-        shape = (num, net.out_channels, image_size, image_size)
         device = net.device
-        img = noise if noise is not None else torch.randn(shape, device=device)
-        assert tuple(img.shape) == shape, f"noise must have shape {shape}"
+        # as in the reference (ddpm.py:168-176), given noise is used as-is and defines the sample size
+        img = noise if noise is not None else torch.randn((num, net.out_channels, image_size, image_size), device=device)
+        assert img.dim() == 4 and img.shape[1] == net.out_channels, f"noise must be [N,{net.out_channels},H,W], got {tuple(img.shape)}"
         img = _f32(img, device).clone()
+        num = img.shape[0]
+        shape = tuple(img.shape)
         T = self.framework.timesteps
         nsteps = T if self.KIND == 0 else (steps if steps is not None else T)
         ret = edict({"samples": None, "pred_x_t": [], "pred_x_0": []})
@@ -191,7 +198,7 @@ class _NativeSampler:
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed)
+            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:])
             traj0 = trajt = None
             if return_trajectory:
                 traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
