@@ -39,7 +39,10 @@ int ivid_device_info(int device, int* sm_count, int* cc_major, int* cc_minor);
  * ------------------------------------------------------------------------------------------------------------------ */
 
 /* AdmUnet2d.__init__ (adm.py:318-337).  `cfg_json` is the "backbone.args" object of a reference config file
- * (configs/(name).json), passed through unchanged.  No GPU work happens here (usable on a CPU-only host). */
+ * (configs/(name).json), passed through unchanged.  No GPU work happens here (usable on a CPU-only host).
+ * Channel widths: every level width (stem, ResBlock inputs and outputs including the up-path concatenations, final width)
+ * must be divisible by num_groups (IVID_ERR_INVALID_ARGUMENT otherwise, as the reference's GroupNorm rejects it) and a
+ * multiple of 8 (IVID_ERR_NOT_IMPLEMENTED otherwise). */
 int ivid_unet_create(const char* cfg_json, ivid_unet_t** out);
 int ivid_unet_destroy(ivid_unet_t* h);
 
@@ -247,9 +250,10 @@ int ivid_warp_forward_backward(ivid_warp_t* w, const float* lin_depth0_host, con
  * Operator-level entry points (unit parity tests, profiling): the kernels the UNet is assembled from.
  * ------------------------------------------------------------------------------------------------------------------ */
 
-/* nn.Conv2d 3x3 pad 1 / 1x1 as wgmma implicit GEMM.  act_dev fp16 NHWC [N,H,W,Cin] (Cin % 64 == 0); w_host fp32
- * [Cout,Cin,k,k] reference layout; optional 1x1 skip over act2_dev [N,H,W,Cin2] with w2_host [Cout,Cin2,1,1];
- * optional fp32 NHWC residual; out fp32 NHWC [N,H,W,Cout] (out_fp16 = 1: fp16). */
+/* nn.Conv2d 3x3 pad 1 / 1x1 as wgmma implicit GEMM.  act_dev fp16 NHWC [N,H,W,Cin] (Cin % 8 == 0: the 16-byte row pitch
+ * TMA needs); w_host fp32 [Cout,Cin,k,k] reference layout; optional 1x1 skip over act2_dev [N,H,W,Cin2] (Cin2 % 8 == 0)
+ * with w2_host [Cout,Cin2,1,1]; optional fp32 NHWC residual; out fp32 NHWC [N,H,W,Cout] (out_fp16 = 1: fp16), Cout % 8 == 0.
+ * Channel counts that are not multiples of 64 are padded to whole 64-channel chunks inside the GEMM only. */
 int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
                    int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
                    const float* residual_dev, void* out_dev, int out_fp16, void* stream);

@@ -219,19 +219,20 @@ int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const floa
   return guarded([&] {
     IVID_NOT_NULL(act_dev); IVID_NOT_NULL(w_host); IVID_NOT_NULL(out_dev);
     IVID_REQUIRE(ksize == 3 || ksize == 1, "conv: kernel size must be 3 or 1");
-    IVID_REQUIRE(Cin % 64 == 0 && Cin2 % 64 == 0, "conv: channels must be multiples of 64");
+    IVID_REQUIRE(Cin > 0 && Cin % 8 == 0 && Cin2 % 8 == 0, "conv: channels must be multiples of 8");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int taps = ksize * ksize;
     const int cout_pad = conv_pad_cout(Cout);
-    const int K = taps * Cin + (act2_dev ? Cin2 : 0);
+    const int cp = conv_pad_k(Cin);                // per-tap column pitch: whole 64-channel chunks, zero columns at the pad
+    const int K = taps * cp + (act2_dev ? conv_pad_k(Cin2) : 0);
     std::vector<__half> wp(static_cast<size_t>(cout_pad) * K, __float2half_rn(0.f));
     for (int co = 0; co < Cout; ++co) {
       for (int tap = 0; tap < taps; ++tap)
         for (int ci = 0; ci < Cin; ++ci)
-          wp[static_cast<size_t>(co) * K + tap * Cin + ci] = __float2half_rn(w_host[(static_cast<size_t>(co) * Cin + ci) * taps + tap]);
+          wp[static_cast<size_t>(co) * K + tap * cp + ci] = __float2half_rn(w_host[(static_cast<size_t>(co) * Cin + ci) * taps + tap]);
       if (act2_dev)
         for (int ci = 0; ci < Cin2; ++ci)
-          wp[static_cast<size_t>(co) * K + taps * Cin + ci] = __float2half_rn(w2_host[static_cast<size_t>(co) * Cin2 + ci]);
+          wp[static_cast<size_t>(co) * K + taps * cp + ci] = __float2half_rn(w2_host[static_cast<size_t>(co) * Cin2 + ci]);
     }
     std::vector<float> bias(cout_pad, 0.f);
     for (int i = 0; i < Cout; ++i) bias[i] = (bias_host ? bias_host[i] : 0.f) + ((act2_dev && bias2_host) ? bias2_host[i] : 0.f);

@@ -11,6 +11,9 @@
 //   "segments" let a 1x1 skip convolution over a different tensor (raw x) accumulate into the same tile as extra K slabs
 //   (SURVEY K2), so  skip(x) + conv(h)  is one kernel.
 //   B (weights) is packed [Cout_pad][K] fp16, K-major, loaded by 2-D TMA.
+//   Segments of C % 64 != 0 channels (C % 8 == 0) run ceil(C/64) chunks: the activation map keeps the real channel extent, so
+//   TMA zero-fills the channels past C of the last box, and the packed weights hold zero columns there.  Out-of-bounds
+//   elements still count toward the transaction bytes, so every stage expects the full box.
 // Both operands land in shared memory in the 128-byte-swizzled K-major layout that wgmma reads directly.
 //
 // Two warpgroups per CTA (rows 0-63 / 64-127 of a 128-pixel x BN tile), accumulators in registers.  Thread 0 also drives
@@ -39,7 +42,7 @@ struct ConvGemmParams {
   int TW, TH, TN;              // pixel tile (TW*TH*TN == 128)
   int tiles_w, tiles_h, tiles_n;
   int n_blocks;                // Cout_pad / BN
-  int seg_chunks[3];           // channels/64 of each K segment (0 = segment unused)
+  int seg_chunks[3];           // ceil(channels/64) of each K segment (0 = segment unused)
   int seg_taps[3];             // 9 (3x3) or 1 (1x1)
   int Cout;                    // valid output channels
   int ldc;                     // output channel stride (elements) for NHWC modes

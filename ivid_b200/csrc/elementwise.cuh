@@ -139,9 +139,10 @@ __device__ __forceinline__ void gn_prologue(const GnApplyParams& p, float* s_ab,
   int n, bx_unused;
   gn_block_pos(p, n, bx_unused);
   const int cpg = C / p.groups;
-  if ((cpg & (cpg - 1)) == 0 && cpg <= 32 && C <= 4 * 256 && blockDim.x == 256) {
+  if ((cpg & (cpg - 1)) == 0 && cpg <= 32 && C % 32 == 0 && C <= 4 * 256 && blockDim.x == 256) {
     // fast path (power-of-two group width): thread = channel; every global load of the prologue (statistics and affine /
-    // FiLM parameters) is issued up front, the group sums are formed by shuffles, and there is a single barrier
+    // FiLM parameters) is issued up front, the group sums are formed by shuffles, and there is a single barrier.
+    // C % 32 == 0 keeps the full-warp shuffles on whole warps; other widths (e.g. 40 = 8 groups of 5) take the loop below
     constexpr int PF = 4;
     double2 st[PF];
     float pg[PF], pb[PF], psc[PF], psh[PF];

@@ -56,15 +56,20 @@ int conv_pick_bn(int cout_pad) {
   throw Error(kErrInvalidArgument, "conv: unsupported padded Cout " + std::to_string(cout_pad));
 }
 
-bool conv_can_res_up(int W, int cout) { return W >= 16 && cout % 32 == 0; }
-bool conv_can_out16(int cout) { return cout % 64 == 0; }
+// The epilogue writes channel pairs (c, c + 1) under c < Cout: an NHWC output of Cout % 8 == 0 channels (the 16-byte row
+// pitch of the fp16 tensors that TMA reads next) keeps every pair inside the row and every 4- / 8-byte access aligned.
+bool conv_can_res_up(int W, int cout) { return W >= 16 && cout % 8 == 0; }
+bool conv_can_out16(int cout) { return cout % 8 == 0; }
+int conv_pad_k(int c) { return ((c + 63) / 64) * 64; }
 
 ConvLaunch* conv_launch_create(const ConvDesc& d) {
-  IVID_REQUIRE(d.C0 > 0 && d.C0 % 64 == 0, "conv: segment-0 channels must be a positive multiple of 64");
-  IVID_REQUIRE(d.C1 % 64 == 0, "conv: segment-1 channels must be a multiple of 64");
+  IVID_REQUIRE(d.C0 > 0 && d.C0 % 8 == 0, "conv: segment-0 channels must be a positive multiple of 8");
+  IVID_REQUIRE(d.C1 % 8 == 0, "conv: segment-1 channels must be a multiple of 8");
   IVID_REQUIRE(d.taps0 == 9 || d.taps0 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.taps1 == 9 || d.taps1 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
-  IVID_REQUIRE(d.C2 % 64 == 0 && (d.taps2 == 9 || d.taps2 == 1), "conv: segment 2 must be a multiple of 64 channels, 3x3 or 1x1");
+  IVID_REQUIRE(d.C2 % 8 == 0 && (d.taps2 == 9 || d.taps2 == 1), "conv: segment 2 must be a multiple of 8 channels, 3x3 or 1x1");
+  // the opt-in slab / multicast kernels are only used where no K segment has a partial 64-channel chunk
+  const bool k_full = d.C0 % 64 == 0 && d.C1 % 64 == 0 && d.C2 % 64 == 0;
   auto* l = new ConvLaunch();
   ConvGemmParams& p = l->p;
   p.N = d.N; p.H = d.H; p.W = d.W;
@@ -76,15 +81,15 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   // 3x3 tap reuse (IVID_SLAB=1, read per launch creation): 8 x 16 pixel tiles, where they divide the layer; not with the
   // upsampled residual (its index arithmetic assumes the 16-wide tiles of the default kernel)
   const bool slab_on = getenv("IVID_SLAB") != nullptr && atoi(getenv("IVID_SLAB")) > 0;
-  if (slab_on && l->BN == 128 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && d.H % 16 == 0 && d.W % 8 == 0 && !d.residual_up) {
+  if (slab_on && k_full && l->BN == 128 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && d.H % 16 == 0 && d.W % 8 == 0 && !d.residual_up) {
     l->mode = kConvSlab;
     p.TW = 8; p.TH = 16; p.TN = 1;
     p.tiles_w = d.W / p.TW; p.tiles_h = d.H / p.TH; p.tiles_n = d.N;
   }
   p.n_blocks = d.cout_pad / l->BN;
-  p.seg_chunks[0] = d.C0 / 64; p.seg_taps[0] = d.taps0;
-  p.seg_chunks[1] = d.C1 / 64; p.seg_taps[1] = d.C1 > 0 ? d.taps1 : 0;
-  p.seg_chunks[2] = d.C2 / 64; p.seg_taps[2] = d.C2 > 0 ? d.taps2 : 0;
+  p.seg_chunks[0] = conv_pad_k(d.C0) / 64; p.seg_taps[0] = d.taps0;
+  p.seg_chunks[1] = conv_pad_k(d.C1) / 64; p.seg_taps[1] = d.C1 > 0 ? d.taps1 : 0;
+  p.seg_chunks[2] = conv_pad_k(d.C2) / 64; p.seg_taps[2] = d.C2 > 0 ? d.taps2 : 0;
   p.Cout = d.cout; p.ldc = d.ldc; p.ldr = d.ldr; p.out_mode = d.out_mode;
   p.bias = d.bias; p.residual = d.residual; p.out = d.out;
   p.stats = (d.stats != nullptr && conv_can_fuse_stats(d.H, d.W) && d.out_mode != 2) ? d.stats : nullptr;
@@ -93,15 +98,17 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.residual == nullptr || (d.out_mode != 2 && d.ldr % 2 == 0), "conv: residual needs an NHWC output and an even row pitch");
   p.res_up = 0;
   if (d.residual != nullptr && d.residual_up) {
-    IVID_REQUIRE(conv_can_res_up(d.W, d.cout) && d.H % 2 == 0, "conv: upsampled residual needs W >= 16 and Cout % 32 == 0");
+    IVID_REQUIRE(conv_can_res_up(d.W, d.cout) && d.H % 2 == 0, "conv: upsampled residual needs W >= 16 and Cout % 8 == 0");
     p.res_up = 1;
   }
   p.out16 = nullptr;
   if (d.out16 != nullptr) {
-    IVID_REQUIRE(d.out_mode == 0 && conv_can_out16(d.cout), "conv: fp16 output copy needs an fp32 NHWC output and Cout % 64 == 0");
+    IVID_REQUIRE(d.out_mode == 0 && conv_can_out16(d.cout), "conv: fp16 output copy needs an fp32 NHWC output and Cout % 8 == 0");
     p.out16 = static_cast<__half*>(d.out16);
   }
-  const int Ktot = d.taps0 * d.C0 + (d.C1 > 0 ? d.taps1 * d.C1 : 0) + (d.C2 > 0 ? d.taps2 * d.C2 : 0);
+  // packed weight columns: every segment padded to whole 64-channel chunks per tap (zero columns); the activation maps keep
+  // the real channel extent, so TMA zero-fills the missing channels of a segment's last chunk
+  const int Ktot = d.taps0 * conv_pad_k(d.C0) + (d.C1 > 0 ? d.taps1 * conv_pad_k(d.C1) : 0) + (d.C2 > 0 ? d.taps2 * conv_pad_k(d.C2) : 0);
   ConvMaps& M = l->maps;
   M.a[0] = make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN);
   M.a[1] = d.C1 > 0 ? make_act_map(d.act1, d.N, d.H, d.W, d.C1, p.TW, p.TH, p.TN) : M.a[0];
@@ -117,7 +124,7 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   // Cluster multicast on the low-resolution levels (IVID_MC=1, read per launch creation): see conv_gemm_kernel<.., kConvMc>
   p.mc_n = 1; p.mc_m = 1;
   const bool mc_on = getenv("IVID_MC") != nullptr && getenv("IVID_MC")[0] == '1';
-  if (mc_on && l->mode == kConvDefault && l->BN == 128 && d.H <= 16 && m_tiles >= 2) {
+  if (mc_on && k_full && l->mode == kConvDefault && l->BN == 128 && d.H <= 16 && m_tiles >= 2) {
     const int cn = p.n_blocks % 4 == 0 ? 4 : (p.n_blocks % 2 == 0 ? 2 : 1);
     const int cm = m_tiles % 2 == 0 ? 2 : 1;
     if (cn * cm >= 2) {

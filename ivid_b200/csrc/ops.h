@@ -18,7 +18,7 @@ struct ConvDesc {
   const void* act1 = nullptr; int C1 = 0; int taps1 = 1;   // optional segment 1 (1x1 skip over another tensor)
   const void* act2 = nullptr; int C2 = 0; int taps2 = 1;   // optional segment 2 (second half of a virtual concat)
   void* out16 = nullptr;                                   // optional fp16 NHWC copy of an fp32 output (same ldc)
-  const void* weight = nullptr;                            // fp16 [cout_pad][Ktot], Ktot = taps0*C0 + taps1*C1
+  const void* weight = nullptr;                            // fp16 [cout_pad][Ktot], Ktot = sum of taps*conv_pad_k(C) over segments
   int cout_pad = 0;
   int cout = 0;                                            // valid output channels
   const float* bias = nullptr;                             // [cout_pad]
@@ -44,6 +44,8 @@ bool conv_can_res_up(int W, int cout);
 void conv_tile(int H, int W, int* TW, int* TH, int* TN);
 bool conv_can_fuse_stats(int H, int W);                    // epilogue statistics need >= 32 pixels of one sample per warp
 int conv_pad_cout(int cout);
+// packed weight columns per tap of a K segment of c channels (c % 8 == 0): whole 64-channel chunks, zero columns at the pad
+int conv_pad_k(int c);
 
 // head_ch = 64: attention_kernel; any other multiple of 64: attention_hd_kernel (kErrNotImplemented otherwise)
 AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out);

@@ -77,7 +77,6 @@ const ParamSpec& Unet::P(const std::string& name) const {
 // key names ("input_blocks.3.0.in_layers.0.weight", ...) and shapes match torch's registration order.
 void Unet::build_topology() {
   const UnetConfig& c = cfg_;
-  IVID_REQUIRE(c.model_channels % 64 == 0, "model_channels must be a multiple of 64 (tensor-core K slab)");
   IVID_REQUIRE(c.in_channels <= 16, "in_channels must be <= 16");
   IVID_REQUIRE(c.num_groups >= 1 && c.num_groups <= 64, "num_groups must be in [1,64]");
   const int mc = c.model_channels;
@@ -107,11 +106,15 @@ void Unet::build_topology() {
       throw Error(kErrNotImplemented, "attention head width " + std::to_string(hc) + " is not a multiple of 64 channels");
     return hc;
   };
-  auto add_res = [&](const std::string& pfx, int cin, int cout, int mode) {
+  // Level widths: num_groups must divide each (the reference's GroupNorm32 asserts it), checked as the blocks are made.  The
+  // kernels further need C % 8 == 0 (16-byte NHWC fp16 rows for TMA), checked once the whole topology stands, so that any
+  // network the reference rejects still raises its AssertionError.
+  std::vector<int> widths;
+  auto add_res = [&](const std::string& pfx, int cin, int cout, int mode, int cat0 = 0) {
     ResBlockDef r;
-    r.pfx = pfx; r.cin = cin; r.cout = cout; r.mode = mode;
-    IVID_REQUIRE(cin % 64 == 0 && cout % 64 == 0, "channel counts must be multiples of 64");
+    r.pfx = pfx; r.cin = cin; r.cout = cout; r.mode = mode; r.cat0 = cat0;
     IVID_REQUIRE(cin % c.num_groups == 0 && cout % c.num_groups == 0, "num_groups must divide channels");
+    widths.insert(widths.end(), {cin, cout, cat0});
     add_param(pfx + ".in_layers.0.weight", {cin});
     add_param(pfx + ".in_layers.0.bias", {cin});
     add_param(pfx + ".in_layers.2.weight", {cout, cin, 3, 3});
@@ -148,7 +151,7 @@ void Unet::build_topology() {
   auto add_resample = [&](const std::string& pfx, int ch, int mode) {
     ResampleDef r;
     r.pfx = pfx; r.C = ch; r.mode = mode; r.conv = c.conv_resample;
-    IVID_REQUIRE(ch % 64 == 0, "channel counts must be multiples of 64");
+    widths.push_back(ch);
     if (r.conv) {
       const std::string sub = mode == 2 ? ".op" : ".conv";      // Downsample2d.op (adm.py:111) / Upsample2d.conv (adm.py:81)
       add_param(pfx + sub + ".weight", {ch, ch, 3, 3});
@@ -216,7 +219,7 @@ void Unet::build_topology() {
       const int ich = input_block_chs.back();
       input_block_chs.pop_back();
       int li = 0;
-      b.layers.push_back({1, add_res(pfx + "." + std::to_string(li++), ch + ich, outc, 0)});
+      b.layers.push_back({1, add_res(pfx + "." + std::to_string(li++), ch + ich, outc, 0, ch)});
       ch = outc;
       if (in_attn(ds)) b.layers.push_back({2, add_attn(pfx + "." + std::to_string(li++), ch)});
       if (level != 0 && i == c.num_res_blocks) {
@@ -230,6 +233,9 @@ void Unet::build_topology() {
   }
   final_ch_ = ch;
   IVID_REQUIRE(ch == input_ch, "final channel count must equal the stem width (adm.py:486 uses input_ch)");
+  for (int w : widths)
+    if (w % 8 != 0)
+      throw Error(kErrNotImplemented, "channel width " + std::to_string(w) + " is not a multiple of 8 (16-byte NHWC fp16 rows)");
   add_param("out.0.weight", {ch});
   add_param("out.0.bias", {ch});
   add_param("out.2.weight", {c.out_channels, input_ch, 3, 3});
@@ -261,14 +267,15 @@ struct ArenaBuilder {
   template <class T> T* at(size_t off) { return reinterpret_cast<T*>(buf.data() + off); }
 };
 
-// [Cout][Cin][k][k] fp32 -> rows of [taps][cin_pad] fp16 written at column `kcol0` of a [cout_pad][Ktot] matrix
-void pack_conv_rows(__half* dst, int Ktot, int kcol0, const float* w, int cout, int cin, int cin_pad, int ksz) {
+// [Cout][Cin][k][k] fp32, input channels [ci0, ci0 + cn) -> rows of [taps][cn_pad] fp16 written at column `kcol0` of a
+// [cout_pad][Ktot] matrix (columns past cn in each tap stay zero)
+void pack_conv_rows(__half* dst, int Ktot, int kcol0, const float* w, int cout, int cin, int ci0, int cn, int cn_pad, int ksz) {
   const int taps = ksz * ksz;
   for (int co = 0; co < cout; ++co)
     for (int tap = 0; tap < taps; ++tap)
-      for (int ci = 0; ci < cin; ++ci)
-        dst[static_cast<size_t>(co) * Ktot + kcol0 + tap * cin_pad + ci] =
-            __float2half_rn(w[(static_cast<size_t>(co) * cin + ci) * taps + tap]);
+      for (int ci = 0; ci < cn; ++ci)
+        dst[static_cast<size_t>(co) * Ktot + kcol0 + tap * cn_pad + ci] =
+            __float2half_rn(w[(static_cast<size_t>(co) * cin + ci0 + ci) * taps + tap]);
 }
 // Stem: the 64 operand channels of the packed network input are  hi | lo | hi  of a two-term fp16 split of x
 // (pack_input_kernel); the matching weight columns are  Wh | Wh | Wl  with W = Wh + Wl, so that the fp16 tensor-core
@@ -286,9 +293,10 @@ void pack_stem_rows(__half* dst, int Ktot, const float* w, int cout, int cin, in
 }
 
 // Output head as a 1x1 GEMM over 9*Co columns (column tap*Co + c holds W[c][:, tap]), split precision:
-// K = [Wh | Wh | Wl] against the activation segments [a_hi | a_lo | a_hi] (GnApplyParams::out_lo).
-void pack_out_rows(__half* dst, int C, const float* w, int co_n) {
-  const int K = 3 * C;
+// K = [Wh | Wh | Wl] against the activation segments [a_hi | a_lo | a_hi] (GnApplyParams::out_lo), each third padded to
+// Cp = conv_pad_k(C) columns.
+void pack_out_rows(__half* dst, int C, int Cp, const float* w, int co_n) {
+  const int K = 3 * Cp;
   for (int tap = 0; tap < 9; ++tap)
     for (int c = 0; c < co_n; ++c)
       for (int ci = 0; ci < C; ++ci) {
@@ -296,7 +304,7 @@ void pack_out_rows(__half* dst, int C, const float* w, int co_n) {
         const __half hi = __float2half_rn(v);
         const __half lo = __float2half_rn(v - __half2float(hi));
         __half* row = dst + static_cast<size_t>(tap * co_n + c) * K;
-        row[ci] = hi; row[C + ci] = hi; row[2 * C + ci] = lo;
+        row[ci] = hi; row[Cp + ci] = hi; row[2 * Cp + ci] = lo;
       }
 }
 }  // namespace
@@ -321,20 +329,26 @@ void Unet::finalize(int device) {
     g.b_off = put_f32(P(pfx + ".bias").host);
     return g;
   };
-  // generic conv: main weight (ksz x ksz over cin, channel-padded to cin_pad) + optional 1x1 skip weight over cin2
+  // generic conv: main weight (ksz x ksz over cin, channel-padded to cin_pad per tap, the whole main part to 64-channel
+  // chunks) + optional 1x1 skip weight over cin2 channels, one K segment per part of a concatenated input (cin2a | rest;
+  // cin2a = 0: one segment), each padded to 64-channel chunks as conv_launch_create expects
   auto pack_conv = [&](const std::string& wname, const std::string& bname, int cout, int cin, int cin_pad, int ksz,
-                       const std::string& skip_w, const std::string& skip_b, int cin2) {
+                       const std::string& skip_w, const std::string& skip_b, int cin2, int cin2a = 0) {
     ConvW cw;
     cw.cout = cout;
     cw.cout_pad = conv_pad_cout(cout);
-    cw.K = ksz * ksz * cin_pad + cin2;
+    const int kmain = conv_pad_k(ksz * ksz * cin_pad);
+    const int s0 = cin2a > 0 ? cin2a : cin2, s1 = cin2 - s0;
+    cw.K = kmain + conv_pad_k(s0) + conv_pad_k(s1);
     cw.w_off = ab.alloc(static_cast<size_t>(cw.cout_pad) * cw.K * 2);
-    pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, 0, P(wname).host.data(), cout, cin, cin_pad, ksz);
+    pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, 0, P(wname).host.data(), cout, cin, 0, cin, cin_pad, ksz);
     std::vector<float> bias(cw.cout_pad, 0.f);
     const auto& b = P(bname).host;
     for (int i = 0; i < cout; ++i) bias[i] = b[i];
     if (cin2 > 0) {
-      pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, ksz * ksz * cin_pad, P(skip_w).host.data(), cout, cin2, cin2, 1);
+      const float* w2 = P(skip_w).host.data();
+      pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, kmain, w2, cout, cin2, 0, s0, s0, 1);
+      if (s1 > 0) pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, kmain + conv_pad_k(s0), w2, cout, cin2, s0, s1, s1, 1);
       const auto& b2 = P(skip_b).host;
       for (int i = 0; i < cout; ++i) bias[i] += b2[i];
     }
@@ -382,28 +396,30 @@ void Unet::finalize(int device) {
   for (auto& r : resample_)
     if (r.conv) {
       const std::string sub = r.mode == 2 ? ".op" : ".conv";
-      r.w = pack_conv(r.pfx + sub + ".weight", r.pfx + sub + ".bias", r.C, r.C, r.C, 3, "", "", 0);
+      // the stride-2 conv runs as a 1x1 GEMM over the 9C im2col channels (one segment, padded at its end); the upsample
+      // conv is an ordinary 3x3 conv over C channels
+      r.w = pack_conv(r.pfx + sub + ".weight", r.pfx + sub + ".bias", r.C, r.C, r.mode == 2 ? r.C : conv_pad_k(r.C), 3, "", "", 0);
     }
   for (auto& r : res_) {
     r.gn1 = pack_gn(r.pfx + ".in_layers.0", r.cin);
-    r.conv1 = pack_conv(r.pfx + ".in_layers.2.weight", r.pfx + ".in_layers.2.bias", r.cout, r.cin, r.cin, 3, "", "", 0);
+    r.conv1 = pack_conv(r.pfx + ".in_layers.2.weight", r.pfx + ".in_layers.2.bias", r.cout, r.cin, conv_pad_k(r.cin), 3, "", "", 0);
     r.gn2 = pack_gn(r.pfx + ".out_layers.0", r.cout);
-    r.conv2 = pack_conv(r.pfx + ".out_layers.3.weight", r.pfx + ".out_layers.3.bias", r.cout, r.cout, r.cout, 3,
-                        r.pfx + ".skip_connection.weight", r.pfx + ".skip_connection.bias", r.skip_conv ? r.cin : 0);
+    r.conv2 = pack_conv(r.pfx + ".out_layers.3.weight", r.pfx + ".out_layers.3.bias", r.cout, r.cout, conv_pad_k(r.cout), 3,
+                        r.pfx + ".skip_connection.weight", r.pfx + ".skip_connection.bias", r.skip_conv ? r.cin : 0, r.cat0);
   }
   for (auto& a : attn_) {
     a.gn = pack_gn(a.pfx + ".norm", a.C);
-    a.qkv = pack_conv(a.pfx + ".qkv.weight", a.pfx + ".qkv.bias", 3 * a.C, a.C, a.C, 1, "", "", 0);
-    a.proj = pack_conv(a.pfx + ".proj_out.weight", a.pfx + ".proj_out.bias", a.C, a.C, a.C, 1, "", "", 0);
+    a.qkv = pack_conv(a.pfx + ".qkv.weight", a.pfx + ".qkv.bias", 3 * a.C, a.C, conv_pad_k(a.C), 1, "", "", 0);
+    a.proj = pack_conv(a.pfx + ".proj_out.weight", a.pfx + ".proj_out.bias", a.C, a.C, conv_pad_k(a.C), 1, "", "", 0);
   }
   out_gn_ = pack_gn("out.0", final_ch_);
-  out_conv_ = pack_conv("out.2.weight", "out.2.bias", cfg_.out_channels, final_ch_, final_ch_, 3, "", "", 0);
+  out_conv_ = pack_conv("out.2.weight", "out.2.bias", cfg_.out_channels, final_ch_, conv_pad_k(final_ch_), 3, "", "", 0);
   // split-precision 1x1 form of the same conv (see pack_out_rows); bias is added by eps_gather_kernel
   out_split_ = 9 * cfg_.out_channels <= 64 && getenv("IVID_NO_OUTSPLIT") == nullptr;
   if (out_split_) {
-    out1x1_.cout = 64; out1x1_.cout_pad = 64; out1x1_.K = 3 * final_ch_;
+    out1x1_.cout = 64; out1x1_.cout_pad = 64; out1x1_.K = 3 * conv_pad_k(final_ch_);
     out1x1_.w_off = ab.alloc(static_cast<size_t>(64) * out1x1_.K * 2);
-    pack_out_rows(ab.at<__half>(out1x1_.w_off), final_ch_, P("out.2.weight").host.data(), cfg_.out_channels);
+    pack_out_rows(ab.at<__half>(out1x1_.w_off), final_ch_, conv_pad_k(final_ch_), P("out.2.weight").host.data(), cfg_.out_channels);
     out1x1_.b_off = put_f32(std::vector<float>(64, 0.f));
   }
 
@@ -801,7 +817,12 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
         if (r.skip_conv && use16) {
           d.act1 = x0.d16; d.C1 = x0.C; d.taps1 = 1;
           if (x1 != nullptr) { d.act2 = x1->d16; d.C2 = x1->C; d.taps2 = 1; }
-        } else if (r.skip_conv) { d.act1 = s_xh; d.C1 = r.cin; d.taps1 = 1; }
+        } else if (r.skip_conv) {
+          // one segment over the raw concat: the packed skip columns (one segment per concat part) only line up when the
+          // first part fills whole 64-channel chunks
+          IVID_REQUIRE(!create || r.cat0 % 64 == 0, "internal: raw-copy skip conv over a concat whose first part is not a multiple of 64");
+          d.act1 = s_xh; d.C1 = r.cin; d.taps1 = 1;
+        }
         d.weight = W8(r.conv2.w_off); d.cout_pad = r.conv2.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv2.b_off);
         if (identity) { d.residual = need_xr ? s_xr : use32(x0); d.ldr = r.cout; d.residual_up = res_up; }
         if (only16(out, identity)) { d.out = out.d16; d.out_mode = 1; }

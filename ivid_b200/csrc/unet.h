@@ -46,11 +46,12 @@ struct LinW { int O = 0, K = 0; size_t w_off = 0, b_off = 0; };
 struct ResBlockDef {
   std::string pfx;
   int cin = 0, cout = 0;
+  int cat0 = 0;            // up-path ResBlocks: width of the first part (h) of the concatenated input [h, skip]; 0 otherwise
   int mode = 0;            // 0 same, 1 up, 2 down
   bool skip_conv = false;
   int film_off = 0;        // column offset of this block's (scale|shift) in the FiLM table
   GnW gn1, gn2;
-  ConvW conv1, conv2;      // conv2 holds out_layers.3 (+ skip_connection as extra K columns)
+  ConvW conv1, conv2;      // conv2 holds out_layers.3 (+ skip_connection as extra K columns, one K segment per concat part)
 };
 struct AttnBlockDef {
   std::string pfx;
