@@ -298,57 +298,3 @@ int ivid_op_attention_heads(const void* qkv_dev, int N, int T, int C, int head_c
 }
 
 }  // extern "C"
-
-// ------------------------------------------------------------------------------------------------------------------
-// development probe (not part of the reference-facing surface): do a persistent conv and a GroupNorm-apply kernel issued
-// on two streams actually overlap on this device?  ms[0] = conv alone, ms[1] = gn alone, ms[2] = both concurrently.
-// ------------------------------------------------------------------------------------------------------------------
-extern "C" int ivid_debug_overlap(int N, int reps, float* ms) {
-  return guarded([&] {
-    const int H = 128, W = 128, C = 256;
-    const size_t px = static_cast<size_t>(N) * H * W;
-    DevBuf a16(px * C * 2), wgt(static_cast<size_t>(C) * 9 * C * 2), bias(C * 4), out32(px * C * 4), x32(px * C * 4), y16(px * C * 2),
-        st(static_cast<size_t>(N) * C * 16), gam(C * 4), bet(C * 4);
-    IVID_CHECK_CUDA(cudaMemset(a16.p, 0, px * C * 2));
-    IVID_CHECK_CUDA(cudaMemset(wgt.p, 0, static_cast<size_t>(C) * 9 * C * 2));
-    IVID_CHECK_CUDA(cudaMemset(bias.p, 0, C * 4));
-    IVID_CHECK_CUDA(cudaMemset(x32.p, 0, px * C * 4));
-    IVID_CHECK_CUDA(cudaMemset(st.p, 0, static_cast<size_t>(N) * C * 16));
-    IVID_CHECK_CUDA(cudaMemset(gam.p, 0, C * 4));
-    IVID_CHECK_CUDA(cudaMemset(bet.p, 0, C * 4));
-    ConvDesc d;
-    d.act0 = a16.p; d.C0 = C; d.taps0 = 9; d.weight = wgt.p; d.cout_pad = C; d.cout = C; d.bias = static_cast<float*>(bias.p);
-    d.out = out32.p; d.ldc = C; d.out_mode = 0; d.N = N; d.H = H; d.W = W;
-    std::unique_ptr<ConvLaunch, void (*)(ConvLaunch*)> cl(conv_launch_create(d), conv_launch_destroy);
-    GnApplyDesc g;
-    g.x0 = static_cast<float*>(x32.p); g.C0 = C; g.N = N; g.H = H; g.W = W; g.mode = 0; g.silu = 1; g.out_act = y16.p;
-    g.stats0 = static_cast<double*>(st.p); g.groups = 32; g.gamma = static_cast<float*>(gam.p); g.beta = static_cast<float*>(bet.p);
-    cudaStream_t s1, s2;
-    IVID_CHECK_CUDA(cudaStreamCreateWithFlags(&s1, cudaStreamNonBlocking));
-    IVID_CHECK_CUDA(cudaStreamCreateWithFlags(&s2, cudaStreamNonBlocking));
-    cudaEvent_t e0, e1, e2;
-    cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventCreate(&e2);
-    auto run = [&](bool conv, bool gn) {
-      IVID_CHECK_CUDA(cudaDeviceSynchronize());
-      IVID_CHECK_CUDA(cudaEventRecord(e0, s1));
-      IVID_CHECK_CUDA(cudaStreamWaitEvent(s2, e0, 0));
-      for (int i = 0; i < reps; ++i) {
-        if (conv) conv_launch_run(cl.get(), s1);
-        if (gn) launch_gn_apply(g, s2);
-      }
-      IVID_CHECK_CUDA(cudaEventRecord(e2, s2));
-      IVID_CHECK_CUDA(cudaStreamWaitEvent(s1, e2, 0));
-      IVID_CHECK_CUDA(cudaEventRecord(e1, s1));
-      IVID_CHECK_CUDA(cudaEventSynchronize(e1));
-      float t = 0.f;
-      IVID_CHECK_CUDA(cudaEventElapsedTime(&t, e0, e1));
-      return t;
-    };
-    run(true, true);
-    ms[0] = run(true, false);
-    ms[1] = run(false, true);
-    ms[2] = run(true, true);
-    cudaStreamDestroy(s1); cudaStreamDestroy(s2);
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
-  });
-}

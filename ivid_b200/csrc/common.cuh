@@ -1,4 +1,4 @@
-// Common sm_90a device helpers: mbarrier, TMA (cp.async.bulk.tensor), clusters and wgmma PTX wrappers.
+// Common sm_90a device helpers: mbarrier, TMA (cp.async.bulk.tensor) and wgmma PTX wrappers.
 // Everything here is hand-written inline PTX for Hopper (H100, sm_90a); no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -15,7 +15,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ float silu_wrapped(float x) { return __fdividef(x, 1.0f + __expf(-x)); }   // previous form (A/B: IVID_SILU_WRAPPED)
 // x * sigmoid(x) with the two SFU approximations issued directly: __expf / __fdividef wrap the same ex2.approx / rcp.approx in
 // range fix-ups (an FSETP, two predicated FMULs and a branch per call) that matter in the GroupNorm-apply kernels, where SiLU
 // is most of the arithmetic.  x -> -inf: e = +inf, rcp = 0, result -0; x -> +inf: e = 0, result x.
@@ -107,44 +106,6 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
       "[%2];\n" ::"r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// clusters: rank, cluster-wide barrier, remote mbarrier arrive, TMA multicast to the CTAs of a mask
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// shared::cluster address of `smem_addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_cluster(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
-}
-// one CTA's TMA load lands at the same shared-memory offset of every CTA in `mask` and completes bytes on the mbarrier at the
-// same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mc(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;\n"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_mc(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2], %7;\n" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask)
       : "memory");
 }
 

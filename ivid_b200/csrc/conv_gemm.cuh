@@ -16,22 +16,13 @@
 //   elements still count toward the transaction bytes, so every stage expects the full box.
 // Both operands land in shared memory in the 128-byte-swizzled K-major layout that wgmma reads directly.
 //
-// Two warpgroups per CTA (rows 0-63 / 64-127 of a 128-pixel x BN tile), accumulators in registers.  Thread 0 also drives
-// the TMA ring: STAGES k-blocks are in flight, a slot is refilled as soon as all eight warps have retired the wgmma group
-// that read it.  Two CTAs fit one SM (BN <= 128), so one CTA's epilogue overlaps the other's main loop.
+// Every CTA computes one 128-pixel x BN output tile.  Block b takes pixel tile b / n_blocks and column block b % n_blocks, so
+// the CTAs that share an activation tile run together.  Two warpgroups per CTA (rows 0-63 / 64-127 of the tile),
+// accumulators in registers.  Thread 0 also drives the TMA ring: STAGES k-blocks are in flight, a slot is refilled as soon
+// as all eight warps have retired the wgmma group that read it.  Two CTAs fit one SM (BN <= 128), so one CTA's epilogue
+// overlaps the other's main loop.
 // The epilogue works on the accumulator fragments in place: bias, residual (optionally through a nearest-2x upsample),
 // fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.
-//
-// Opt-in variants, selected when a launch is created (see conv_launch_create):
-//   kMc    cluster multicast on the low-resolution levels: a cluster of mc_m pixel tiles x mc_n column blocks; every CTA loads
-//          a 1/mc_n slice of its activation tile and a 1/mc_m slice of its weight tile and multicasts them to the CTAs of its
-//          row / column, which cuts the L2 -> shared-memory operand traffic per CTA.  A slot may be refilled once every CTA
-//          that receives this CTA's slices has consumed it, so the empty barriers count the warps of the row and column.
-//   kSlab  3x3 tap reuse: 8 x 16 pixel tiles; per 64-channel chunk and horizontal shift one [18 rows][8 px] slab is loaded
-//          and its three vertical taps are the same shared-memory bytes read through descriptors one slab row (1024 B, one
-//          swizzle atom) apart, with the three weight tiles of the taps in the same stage.
-//   contig persistent CTAs, each owning a contiguous range of the work list with the column block slow and the pixel tile
-//          fast (any kernel but kMc).
 #pragma once
 #include "common.cuh"
 
@@ -55,49 +46,39 @@ struct ConvGemmParams {
   __half* out16;               // optional fp16 NHWC copy of an fp32 NHWC output (same ldc)
   double* stats;               // optional [N][Cout][2] per-(sample, channel) sum / sum-of-squares of the output (GroupNorm);
                                // of the ROUNDED values when the output is fp16 (exactly what the next GroupNorm reads)
-  int contig;                  // persistent CTAs over contiguous ranges of the work list (column block slow)
-  int mc_n, mc_m;              // kMc: cluster = mc_m pixel tiles x mc_n column blocks
 };
 
 // All TMA descriptors of one launch, passed as a single __grid_constant__ argument.
 struct ConvMaps {
   CUtensorMap a[3];            // activation segments (fp16 NHWC)
   CUtensorMap b;               // packed weights
-  CUtensorMap a_mc[3];         // kMc: activation slice (128 / mc_n pixels) of each segment; kSlab: [18][8]-pixel slab boxes
-  CUtensorMap b_mc;            // kMc: weight slice (BN / mc_m rows)
 };
 
-enum { kConvDefault = 0, kConvMc = 1, kConvSlab = 2 };
-
-template <int BN, int kMode = kConvDefault>
+template <int BN>
 struct ConvGemmCfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;
-  static constexpr int SLAB_ROWS = 18;
   static constexpr int A_BYTES = BM * BK * 2;                  // 16 KB
-  static constexpr int SLAB_A_BYTES = SLAB_ROWS * 8 * BK * 2;  // 18 KB
-  static constexpr int A_AREA = kMode == kConvSlab ? SLAB_A_BYTES : A_BYTES;
   static constexpr int B_BYTES = ((BN * BK * 2 + 1023) / 1024) * 1024;
-  static constexpr int NB = kMode == kConvSlab ? 3 : 1;       // weight tiles per stage (slab: one per vertical tap)
-  static constexpr int STAGE_BYTES = A_AREA + NB * B_BYTES;
-  static constexpr int STAGES = (kMode == kConvSlab || BN == 128) ? 3 : 4;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGES = BN == 128 ? 3 : 4;
   static constexpr int BAR_BYTES = 128;
   static constexpr int STAT_BYTES = 8 * 2 * BN * 4;            // [8 warps][sum|sumsq][BN] fp32
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + STAT_BYTES + 1024;   // +1024 alignment slack
   static constexpr int THREADS = 256;
 };
 
-// position in the K loop: segment, tap (default / kMc) or horizontal shift (kSlab 3x3 segments), 64-channel chunk, and the
-// first packed weight column of the segment
+// position in the K loop: segment, tap, 64-channel chunk, and the first packed weight column of the segment
 struct ConvKCursor {
   int seg = 0, t = 0, ch = 0, base = 0;
 };
 
-template <int BN, int kMode = kConvDefault>
-__global__ void __launch_bounds__(256, kMode == kConvSlab ? 1 : 2)
-conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const ConvGemmParams p) {
-  using Cfg = ConvGemmCfg<BN, kMode>;
-  constexpr bool kMc = kMode == kConvMc, kSlab = kMode == kConvSlab;
+// p is read in place (__grid_constant__): the K cursor indexes seg_chunks / seg_taps at run time, and without it the compiler
+// may copy the whole struct to a local-memory stack frame to do so.
+template <int BN>
+__global__ void __launch_bounds__(256, 2)
+conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ ConvGemmParams p) {
+  using Cfg = ConvGemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array
@@ -110,250 +91,169 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const ConvGemmParams p) 
   const int warp = tid >> 5, lane = tid & 31;
   const int wg = warp >> 2;                      // warpgroup: tile rows [64 wg, 64 wg + 64)
 
-  int mc_rn = 0, mc_rm = 0, csize = 1;
-  uint16_t row_mask = 0, col_mask = 0;
-  if constexpr (kMc) {
-    const int rank = static_cast<int>(cluster_ctarank());
-    csize = p.mc_n * p.mc_m;
-    mc_rn = rank % p.mc_n;
-    mc_rm = rank / p.mc_n;
-    row_mask = static_cast<uint16_t>(((1u << p.mc_n) - 1u) << (mc_rm * p.mc_n));
-    for (int i = 0; i < p.mc_m; ++i) col_mask |= static_cast<uint16_t>(1u << (i * p.mc_n + mc_rn));
-  }
-
   if (tid == 0) {
     tma_prefetch_desc(&maps.a[0]);
     tma_prefetch_desc(&maps.b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      // one arrive per warp of every CTA that reads what this CTA loads (kMc: its cluster row and column)
-      mbar_init(&empty_bar[s], kMc ? 8u * static_cast<uint32_t>(p.mc_n + p.mc_m - 1) : 8u);
+      mbar_init(&empty_bar[s], 8u);              // one arrive per warp
     }
     fence_barrier_init();
   }
-  if constexpr (kMc) cluster_sync_all(); else __syncthreads();      // peer barriers initialised before any remote signal
+  __syncthreads();
 
-  // work list: tiles (kMc: cluster tiles, every CTA of a cluster takes the same one)
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  int w_first = static_cast<int>(blockIdx.x) / csize, w_limit = w_first + 1;
-  if (!kMc && p.contig) {
-    const long long T = static_cast<long long>(m_tiles) * p.n_blocks, G = gridDim.x, c = blockIdx.x;
-    w_first = static_cast<int>(c * T / G);
-    w_limit = static_cast<int>((c + 1) * T / G);
-  }
-  int nunits = 0;                                // K blocks (kSlab: slab units) per tile
-  for (int sg = 0; sg < 3; ++sg) nunits += p.seg_chunks[sg] * ((kSlab && p.seg_taps[sg] == 9) ? 3 : p.seg_taps[sg]);
-  auto advance = [&](ConvKCursor& c) {
+  int nunits = 0;                                // K blocks of the tile
+  for (int sg = 0; sg < 3; ++sg) nunits += p.seg_chunks[sg] * p.seg_taps[sg];
+  auto advance = [&](ConvKCursor& c) {           // tap slow, chunk fast
     const int taps = p.seg_taps[c.seg], chunks = p.seg_chunks[c.seg];
-    if (kSlab && taps == 9) {                    // chunk slow, horizontal shift fast
-      if (++c.t == 3) { c.t = 0; if (++c.ch == chunks) { c.ch = 0; c.base += 9 * chunks * 64; ++c.seg; } }
-    } else {                                     // tap slow, chunk fast
-      if (++c.ch == chunks) { c.ch = 0; if (++c.t == taps) { c.t = 0; c.base += taps * chunks * 64; ++c.seg; } }
-    }
+    if (++c.ch == chunks) { c.ch = 0; if (++c.t == taps) { c.t = 0; c.base += taps * chunks * 64; ++c.seg; } }
     while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
   };
-  const uint32_t empty0 = kMc ? smem_u32(&empty_bar[0]) : 0u;
 
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  uint32_t g0 = 0;                               // ring position of the current tile's first unit
 
+  // column block fast: the CTAs that share an activation tile run together
+  const int mt = static_cast<int>(blockIdx.x) / p.n_blocks, nb = static_cast<int>(blockIdx.x) % p.n_blocks;
+  const int colbase = nb * BN;
+  const int tiles_per_img = p.tiles_w * p.tiles_h;
+  const int tn = mt / tiles_per_img;
+  const int rem = mt - tn * tiles_per_img;
+  const int th = rem / p.tiles_w;
+  const int tw = rem - th * p.tiles_w;
+  const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
+
+  // producer (thread 0): units are issued strictly in order
+  ConvKCursor pc;
+  while (p.seg_chunks[pc.seg] == 0) ++pc.seg;
+  auto issue_load = [&](int u) {
+    const uint32_t g = static_cast<uint32_t>(u);
+    const int s = static_cast<int>(g % STAGES);
+    if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
+    const int taps = p.seg_taps[pc.seg], chunks = p.seg_chunks[pc.seg];
+    uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
+    uint8_t* sb = sa + Cfg::A_BYTES;
+    const int dy = (taps == 9) ? (pc.t / 3 - 1) : 0;
+    const int dx = (taps == 9) ? (pc.t % 3 - 1) : 0;
+    const int kcol = pc.base + (pc.t * chunks + pc.ch) * 64;
+    mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
+    tma_load_4d(&maps.a[pc.seg], &full_bar[s], sa, pc.ch * 64, w0 + dx, h0 + dy, n0);
+    tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
+    advance(pc);
+  };
+  if (tid == 0) {
+    for (int u = 0; u < STAGES && u < nunits; ++u) issue_load(u);
+  }
+
+  // ===================================== main loop =====================================
 #pragma unroll 1
-  for (int w = w_first; w < w_limit; ++w) {
-    int mt, nb;
-    if (kMc) {
-      const int ncb = p.n_blocks / p.mc_n;
-      mt = (w / ncb) * p.mc_m + mc_rm;
-      nb = (w % ncb) * p.mc_n + mc_rn;
-    } else if (p.contig) {                       // column block slow, pixel tile fast
-      nb = w / m_tiles;
-      mt = w - nb * m_tiles;
-    } else {                                     // column block fast: the CTAs that share an activation tile run together
-      mt = w / p.n_blocks;
-      nb = w - mt * p.n_blocks;
-    }
-    const int colbase = nb * BN;
-    const int tiles_per_img = p.tiles_w * p.tiles_h;
-    const int tn = mt / tiles_per_img;
-    const int rem = mt - tn * tiles_per_img;
-    const int th = rem / p.tiles_w;
-    const int tw = rem - th * p.tiles_w;
-    const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
-
-    // producer (thread 0): units are issued strictly in order
-    ConvKCursor pc;
-    while (p.seg_chunks[pc.seg] == 0) ++pc.seg;
-    auto issue_load = [&](int u) {
-      const uint32_t g = g0 + static_cast<uint32_t>(u);
-      const int s = static_cast<int>(g % STAGES);
-      if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
-      const int taps = p.seg_taps[pc.seg], chunks = p.seg_chunks[pc.seg];
-      uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
-      uint8_t* sb = sa + Cfg::A_AREA;
-      if (kSlab && taps == 9) {
-        mbar_arrive_expect_tx(&full_bar[s], Cfg::SLAB_A_BYTES + 3 * BN * Cfg::BK * 2);
-        // slab rows y0-1 .. y0+16 at horizontal shift t - 1 (zero fill outside the image)
-        tma_load_4d(&maps.a_mc[pc.seg], &full_bar[s], sa, pc.ch * 64, w0 + pc.t - 1, h0 - 1, n0);
+  for (int u = 0; u < nunits; ++u) {
+    const uint32_t g = static_cast<uint32_t>(u);
+    const int s = static_cast<int>(g % STAGES);
+    mbar_wait(&full_bar[s], (g / STAGES) & 1);
+    const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
+    const uint32_t sb = sa + Cfg::A_BYTES;
+    wgmma_fence();
+    const uint64_t da = make_smem_desc_sw128(sa + wg * 64 * 128, 1024, 16);
+    const uint64_t db = make_smem_desc_sw128(sb, 1024, 16);
 #pragma unroll
-        for (int dy = 0; dy < 3; ++dy)
-          tma_load_2d(&maps.b, &full_bar[s], sb + dy * Cfg::B_BYTES, pc.base + ((dy * 3 + pc.t) * chunks + pc.ch) * 64, colbase);
-      } else {
-        const int dy = (taps == 9) ? (pc.t / 3 - 1) : 0;
-        const int dx = (taps == 9) ? (pc.t % 3 - 1) : 0;
-        const int kcol = pc.base + (pc.t * chunks + pc.ch) * 64;
-        mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
-        if constexpr (kMc) {
-          const int srows = 128 / p.mc_n;        // pixels of one activation slice (multiple of 8)
-          const int r0 = mc_rn * srows;
-          const int dn = r0 / (p.TW * p.TH), dh = (r0 / p.TW) % p.TH;
-          tma_load_4d_mc(&maps.a_mc[pc.seg], &full_bar[s], sa + r0 * 128, pc.ch * 64, w0 + dx, h0 + dy + dh, n0 + dn, row_mask);
-          const int brows = BN / p.mc_m;
-          tma_load_2d_mc(&maps.b_mc, &full_bar[s], sb + mc_rm * brows * 128, kcol, colbase + mc_rm * brows, col_mask);
+    for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    // retired before the slot is released: a wgmma group still in flight across thread 0's refill branch would make ptxas
+    // serialise every wgmma; the other warpgroups on the SM keep the tensor cores busy meanwhile
+    wgmma_wait<0>();
+    reg_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+    if (tid == 0 && u + STAGES < nunits) issue_load(u + STAGES);
+  }
+
+  // ===================================== epilogue =====================================
+  const int wr = warp & 3;
+  const int quad = lane & 3;
+  int pn[2], ph[2], pw[2];
+  bool ok[2];
+  size_t pix[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
+    const int n = n0 + row / (p.TW * p.TH), h = h0 + (row / p.TW) % p.TH, x = w0 + row % p.TW;
+    ok[i] = n < p.N;                             // rows of the batch tail (TMA zero fill) are not written
+    pix[i] = (static_cast<size_t>(n) * p.H + h) * p.W + x;
+    pn[i] = n; ph[i] = h; pw[i] = x;
+  }
+  const bool do_stats = p.stats != nullptr;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = colbase + 8 * j + 2 * quad;    // this thread's column pair
+    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+    if (c < p.Cout) {
+      const float2 b = make_float2(__ldg(p.bias + c), __ldg(p.bias + c + 1));
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (!ok[i]) continue;
+        float v0 = acc[4 * j + 2 * i] + b.x, v1 = acc[4 * j + 2 * i + 1] + b.y;
+        if (p.out_mode == 2) {
+          float* o = reinterpret_cast<float*>(p.out);
+          o[((static_cast<size_t>(pn[i]) * p.Cout + c) * p.H + ph[i]) * p.W + pw[i]] = v0;
+          if (c + 1 < p.Cout) o[((static_cast<size_t>(pn[i]) * p.Cout + c + 1) * p.H + ph[i]) * p.W + pw[i]] = v1;
+          continue;
+        }
+        if (p.residual != nullptr) {
+          const size_t rpix = p.res_up ? (static_cast<size_t>(pn[i]) * (p.H >> 1) + (ph[i] >> 1)) * (p.W >> 1) + (pw[i] >> 1) : pix[i];
+          const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + rpix * p.ldr + c));
+          v0 += r.x; v1 += r.y;
+        }
+        if (p.out_mode == 0) {
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix[i] * p.ldc + c) = make_float2(v0, v1);
+          if (p.out16 != nullptr) *reinterpret_cast<uint32_t*>(p.out16 + pix[i] * p.ldc + c) = pack_h2(v0, v1);
         } else {
-          tma_load_4d(&maps.a[pc.seg], &full_bar[s], sa, pc.ch * 64, w0 + dx, h0 + dy, n0);
-          tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
+          const __half2 hv = __floats2half2_rn(v0, v1);
+          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + pix[i] * p.ldc + c) = hv;
+          const float2 r = __half22float2(hv);
+          v0 = r.x; v1 = r.y;
         }
-      }
-      advance(pc);
-    };
-    if (tid == 0) {
-      for (int u = 0; u < STAGES && u < nunits; ++u) issue_load(u);
-    }
-
-    // ===================================== main loop =====================================
-    ConvKCursor cc;
-    while (p.seg_chunks[cc.seg] == 0) ++cc.seg;
-#pragma unroll 1
-    for (int u = 0; u < nunits; ++u) {
-      const uint32_t g = g0 + static_cast<uint32_t>(u);
-      const int s = static_cast<int>(g % STAGES);
-      mbar_wait(&full_bar[s], (g / STAGES) & 1);
-      const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
-      const uint32_t sb = sa + Cfg::A_AREA;
-      wgmma_fence();
-      if (kSlab && p.seg_taps[cc.seg] == 9) {
-        // tap (dy, shift): tile rows start dy slab rows (1024 B each) into the slab; warpgroup wg owns image rows 8 wg ..
-#pragma unroll
-        for (int dy = 0; dy < 3; ++dy) {
-          const uint64_t da = make_smem_desc_sw128(sa + (dy + 8 * wg) * 1024, 1024, 16);
-          const uint64_t db = make_smem_desc_sw128(sb + dy * Cfg::B_BYTES, 1024, 16);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | dy | k) != 0 ? 1u : 0u);
-        }
-      } else {
-        const uint64_t da = make_smem_desc_sw128(sa + wg * 64 * 128, 1024, 16);
-        const uint64_t db = make_smem_desc_sw128(sb, 1024, 16);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
-      }
-      wgmma_commit();
-      // retired before the slot is released: a wgmma group still in flight across thread 0's refill branch would make ptxas
-      // serialise every wgmma; the other warpgroups on the SM keep the tensor cores busy meanwhile
-      wgmma_wait<0>();
-      reg_fence(acc);
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (kMc) {
-          for (int r = 0; r < csize; ++r)
-            if (r / p.mc_n == mc_rm || r % p.mc_n == mc_rn) mbar_arrive_cluster(mapa_cluster(empty0 + s * 8, static_cast<uint32_t>(r)));
-        } else {
-          mbar_arrive(&empty_bar[s]);
-        }
-      }
-      if (tid == 0 && u + STAGES < nunits) issue_load(u + STAGES);
-      advance(cc);
-    }
-    g0 += static_cast<uint32_t>(nunits);
-
-    // ===================================== epilogue =====================================
-    const int wr = warp & 3;
-    const int quad = lane & 3;
-    int pn[2], ph[2], pw[2];
-    bool ok[2];
-    size_t pix[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
-      const int n = n0 + row / (p.TW * p.TH), h = h0 + (row / p.TW) % p.TH, x = w0 + row % p.TW;
-      ok[i] = n < p.N;                           // rows of the batch tail (TMA zero fill) are not written
-      pix[i] = (static_cast<size_t>(n) * p.H + h) * p.W + x;
-      pn[i] = n; ph[i] = h; pw[i] = x;
-    }
-    const bool do_stats = p.stats != nullptr;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int c = colbase + 8 * j + 2 * quad;  // this thread's column pair
-      float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-      if (c < p.Cout) {
-        const float2 b = make_float2(__ldg(p.bias + c), __ldg(p.bias + c + 1));
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          if (!ok[i]) continue;
-          float v0 = acc[4 * j + 2 * i] + b.x, v1 = acc[4 * j + 2 * i + 1] + b.y;
-          if (p.out_mode == 2) {
-            float* o = reinterpret_cast<float*>(p.out);
-            o[((static_cast<size_t>(pn[i]) * p.Cout + c) * p.H + ph[i]) * p.W + pw[i]] = v0;
-            if (c + 1 < p.Cout) o[((static_cast<size_t>(pn[i]) * p.Cout + c + 1) * p.H + ph[i]) * p.W + pw[i]] = v1;
-            continue;
-          }
-          if (p.residual != nullptr) {
-            const size_t rpix = p.res_up ? (static_cast<size_t>(pn[i]) * (p.H >> 1) + (ph[i] >> 1)) * (p.W >> 1) + (pw[i] >> 1) : pix[i];
-            const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + rpix * p.ldr + c));
-            v0 += r.x; v1 += r.y;
-          }
-          if (p.out_mode == 0) {
-            *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix[i] * p.ldc + c) = make_float2(v0, v1);
-            if (p.out16 != nullptr) *reinterpret_cast<uint32_t*>(p.out16 + pix[i] * p.ldc + c) = pack_h2(v0, v1);
-          } else {
-            const __half2 hv = __floats2half2_rn(v0, v1);
-            *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + pix[i] * p.ldc + c) = hv;
-            const float2 r = __half22float2(hv);
-            v0 = r.x; v1 = r.y;
-          }
-          s0 += v0; s1 += v1;
-          q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
-        }
-      }
-      if (do_stats) {
-        // column sums over the warp's 16 rows (the 8 lanes that share `quad`); lanes 0..3 keep them
-#pragma unroll
-        for (int off = 4; off < 32; off <<= 1) {
-          s0 += __shfl_xor_sync(0xffffffffu, s0, off);
-          s1 += __shfl_xor_sync(0xffffffffu, s1, off);
-          q0 += __shfl_xor_sync(0xffffffffu, q0, off);
-          q1 += __shfl_xor_sync(0xffffffffu, q1, off);
-        }
-        if (lane < 4) {
-          float* st = stat_smem + warp * 2 * BN + 8 * j + 2 * quad;
-          st[0] = s0; st[1] = s1; st[BN] = q0; st[BN + 1] = q1;
-        }
+        s0 += v0; s1 += v1;
+        q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
       }
     }
     if (do_stats) {
-      // a warp's 16 rows belong to one sample (TW*TH >= 32); the warps of each sample are combined in a fixed order, so the
-      // statistics are reproducible bit for bit, and one fp64 atomic pair per (sample, channel) and tile goes to global memory
-      __syncthreads();
-      const int rows_per_n = p.TW * p.TH;
-      const int n_tile = (128 + rows_per_n - 1) / rows_per_n;
-      for (int e = tid; e < n_tile * BN; e += Cfg::THREADS) {
-        const int sn = e / BN, c = e - sn * BN;
-        const int n = n0 + sn, col = colbase + c;
-        if (n >= p.N || col >= p.Cout) continue;
-        float ssum = 0.f, qsum = 0.f;
-        for (int w8 = 0; w8 < 8; ++w8) {
-          if ((w8 * 16) / rows_per_n != sn) continue;
-          ssum += stat_smem[w8 * 2 * BN + c];
-          qsum += stat_smem[w8 * 2 * BN + BN + c];
-        }
-        double* st = p.stats + (static_cast<size_t>(n) * p.Cout + col) * 2;
-        atomicAdd(st, static_cast<double>(ssum));
-        atomicAdd(st + 1, static_cast<double>(qsum));
+      // column sums over the warp's 16 rows (the 8 lanes that share `quad`); lanes 0..3 keep them
+#pragma unroll
+      for (int off = 4; off < 32; off <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, off);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, off);
+        q0 += __shfl_xor_sync(0xffffffffu, q0, off);
+        q1 += __shfl_xor_sync(0xffffffffu, q1, off);
       }
-      __syncthreads();                           // stat_smem is rewritten by the next tile
+      if (lane < 4) {
+        float* st = stat_smem + warp * 2 * BN + 8 * j + 2 * quad;
+        st[0] = s0; st[1] = s1; st[BN] = q0; st[BN + 1] = q1;
+      }
     }
   }
-  if constexpr (kMc) cluster_sync_all();         // peers keep multicasting into / arriving on this CTA until all are done
+  if (do_stats) {
+    // a warp's 16 rows belong to one sample (TW*TH >= 32); the warps of each sample are combined in a fixed order, so the
+    // statistics are reproducible bit for bit, and one fp64 atomic pair per (sample, channel) and tile goes to global memory
+    __syncthreads();
+    const int rows_per_n = p.TW * p.TH;
+    const int n_tile = (128 + rows_per_n - 1) / rows_per_n;
+    for (int e = tid; e < n_tile * BN; e += Cfg::THREADS) {
+      const int sn = e / BN, c = e - sn * BN;
+      const int n = n0 + sn, col = colbase + c;
+      if (n >= p.N || col >= p.Cout) continue;
+      float ssum = 0.f, qsum = 0.f;
+      for (int w8 = 0; w8 < 8; ++w8) {
+        if ((w8 * 16) / rows_per_n != sn) continue;
+        ssum += stat_smem[w8 * 2 * BN + c];
+        qsum += stat_smem[w8 * 2 * BN + BN + c];
+      }
+      double* st = p.stats + (static_cast<size_t>(n) * p.Cout + col) * 2;
+      atomicAdd(st, static_cast<double>(ssum));
+      atomicAdd(st + 1, static_cast<double>(qsum));
+    }
+  }
 }
 
 }  // namespace ivid

@@ -94,7 +94,7 @@ struct GnApplyParams {
   int C0, C1;
   int N, H, W;                          // INPUT spatial size
   int mode;                             // 0 same, 1 up, 2 down
-  int silu;                             // 0 none, 1 SiLU (silu_f), 2 SiLU through __expf / __fdividef (same-box A/B)
+  int silu;                             // 0 none, 1 SiLU (silu_f)
   const double* stats0; const double* stats1;   // [N][C0][2], [N][C1][2] (sum, sum of squares over H*W)
   int groups; double inv_count; float eps;
   const float* gamma; const float* beta;
@@ -266,7 +266,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float y = fmaf(raw[j], s_ab[j * c8 + cg], s_ab[C + j * c8 + cg]);
-        if (p.silu) y = (p.silu == 1) ? silu_f(y) : silu_wrapped(y);
+        if (p.silu) y = silu_f(y);
         act[j] = y;
       }
       uint4 pk;
@@ -327,7 +327,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           float y = fmaf(raw[u][j], s_ab[j * c8 + cg], s_ab[C + j * c8 + cg]);
-          if (p.silu) y = (p.silu == 1) ? silu_f(y) : silu_wrapped(y);
+          if (p.silu) y = silu_f(y);
           act[j] = y;
         }
         uint4 pk;
@@ -368,7 +368,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             float y = fmaf(v[j], A[j], B[j]);
-            if (p.silu) y = (p.silu == 1) ? silu_f(y) : silu_wrapped(y);
+            if (p.silu) y = silu_f(y);
             act[j] += y;
             raw[j] += v[j];
           }
@@ -382,7 +382,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float y = fmaf(raw[j], A[j], B[j]);
-        if (p.silu) y = (p.silu == 1) ? silu_f(y) : silu_wrapped(y);
+        if (p.silu) y = silu_f(y);
         act[j] = y;
       }
     }
@@ -507,7 +507,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_h16_kernel(const GnApplyParam
         y0 = fmaf(f.x, s_ab[(2 * j) * c8 + cg], s_ab[C + (2 * j) * c8 + cg]);
         y1 = fmaf(f.y, s_ab[(2 * j + 1) * c8 + cg], s_ab[C + (2 * j + 1) * c8 + cg]);
       }
-      if (p.silu) { y0 = (p.silu == 1) ? silu_f(y0) : silu_wrapped(y0); y1 = (p.silu == 1) ? silu_f(y1) : silu_wrapped(y1); }
+      if (p.silu) { y0 = silu_f(y0); y1 = silu_f(y1); }
       pk[j] = pack_h2(y0, y1);
       if (kLo) {
         const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&pk[j]));

@@ -3,7 +3,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <mutex>
 
 #include "attention.cuh"
@@ -22,7 +21,6 @@ struct ConvLaunch {
   ConvGemmParams p;
   int BN;
   int grid;
-  int mode = kConvDefault;     // kConvMc: cluster of p.mc_n * p.mc_m CTAs; kConvSlab: 3x3 tap-reuse kernel
 };
 
 int conv_pad_cout(int cout) {
@@ -68,8 +66,6 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.taps0 == 9 || d.taps0 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.taps1 == 9 || d.taps1 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.C2 % 8 == 0 && (d.taps2 == 9 || d.taps2 == 1), "conv: segment 2 must be a multiple of 8 channels, 3x3 or 1x1");
-  // the opt-in slab / multicast kernels are only used where no K segment has a partial 64-channel chunk
-  const bool k_full = d.C0 % 64 == 0 && d.C1 % 64 == 0 && d.C2 % 64 == 0;
   auto* l = new ConvLaunch();
   ConvGemmParams& p = l->p;
   p.N = d.N; p.H = d.H; p.W = d.W;
@@ -78,14 +74,6 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   p.tiles_h = d.H / p.TH;
   p.tiles_n = (d.N + p.TN - 1) / p.TN;
   l->BN = conv_pick_bn(d.cout_pad);
-  // 3x3 tap reuse (IVID_SLAB=1, read per launch creation): 8 x 16 pixel tiles, where they divide the layer; not with the
-  // upsampled residual (its index arithmetic assumes the 16-wide tiles of the default kernel)
-  const bool slab_on = getenv("IVID_SLAB") != nullptr && atoi(getenv("IVID_SLAB")) > 0;
-  if (slab_on && k_full && l->BN == 128 && d.taps0 == 9 && d.H >= 16 && d.W >= 16 && d.H % 16 == 0 && d.W % 8 == 0 && !d.residual_up) {
-    l->mode = kConvSlab;
-    p.TW = 8; p.TH = 16; p.TN = 1;
-    p.tiles_w = d.W / p.TW; p.tiles_h = d.H / p.TH; p.tiles_n = d.N;
-  }
   p.n_blocks = d.cout_pad / l->BN;
   p.seg_chunks[0] = conv_pad_k(d.C0) / 64; p.seg_taps[0] = d.taps0;
   p.seg_chunks[1] = conv_pad_k(d.C1) / 64; p.seg_taps[1] = d.C1 > 0 ? d.taps1 : 0;
@@ -114,71 +102,20 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   M.a[1] = d.C1 > 0 ? make_act_map(d.act1, d.N, d.H, d.W, d.C1, p.TW, p.TH, p.TN) : M.a[0];
   M.a[2] = d.C2 > 0 ? make_act_map(d.act2, d.N, d.H, d.W, d.C2, p.TW, p.TH, p.TN) : M.a[0];
   M.b = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN);
-  M.a_mc[0] = M.a[0]; M.a_mc[1] = M.a[1]; M.a_mc[2] = M.a[2]; M.b_mc = M.b;
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  if (l->mode == kConvSlab) {
-    M.a_mc[0] = make_act_map(d.act0, d.N, d.H, d.W, d.C0, 8, ConvGemmCfg<128, kConvSlab>::SLAB_ROWS, 1);
-    if (d.C1 > 0 && d.taps1 == 9) M.a_mc[1] = make_act_map(d.act1, d.N, d.H, d.W, d.C1, 8, ConvGemmCfg<128, kConvSlab>::SLAB_ROWS, 1);
-    if (d.C2 > 0 && d.taps2 == 9) M.a_mc[2] = make_act_map(d.act2, d.N, d.H, d.W, d.C2, 8, ConvGemmCfg<128, kConvSlab>::SLAB_ROWS, 1);
-  }
-  // Cluster multicast on the low-resolution levels (IVID_MC=1, read per launch creation): see conv_gemm_kernel<.., kConvMc>
-  p.mc_n = 1; p.mc_m = 1;
-  const bool mc_on = getenv("IVID_MC") != nullptr && getenv("IVID_MC")[0] == '1';
-  if (mc_on && k_full && l->mode == kConvDefault && l->BN == 128 && d.H <= 16 && m_tiles >= 2) {
-    const int cn = p.n_blocks % 4 == 0 ? 4 : (p.n_blocks % 2 == 0 ? 2 : 1);
-    const int cm = m_tiles % 2 == 0 ? 2 : 1;
-    if (cn * cm >= 2) {
-      p.mc_n = cn; p.mc_m = cm;
-      l->mode = kConvMc;
-      const int srows = 128 / cn;
-      const int bh = srows >= p.TW * p.TH ? p.TH : srows / p.TW, bn = srows >= p.TW * p.TH ? srows / (p.TW * p.TH) : 1;
-      IVID_REQUIRE(bh >= 1 && srows % 8 == 0, "conv: multicast slice geometry");
-      auto slice_map = [&](const void* base, int C) {
-        const uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(d.W), static_cast<uint64_t>(d.H), static_cast<uint64_t>(d.N)};
-        const uint64_t str[3] = {static_cast<uint64_t>(C) * 2, static_cast<uint64_t>(d.W) * C * 2, static_cast<uint64_t>(d.H) * d.W * C * 2};
-        const uint32_t box[4] = {64, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(bh), static_cast<uint32_t>(bn)};
-        return make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
-      };
-      M.a_mc[0] = slice_map(d.act0, d.C0);
-      M.a_mc[1] = d.C1 > 0 ? slice_map(d.act1, d.C1) : M.a_mc[0];
-      M.a_mc[2] = d.C2 > 0 ? slice_map(d.act2, d.C2) : M.a_mc[0];
-      M.b_mc = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN / cm);
-    }
-  }
-  // contiguous work ranges of persistent CTAs (IVID_CONV_CONTIG_ALL=1; IVID_CONV_CONTIG=1: layers with one column block)
-  p.contig = 0;
-  if (l->mode != kConvMc && (getenv("IVID_CONV_CONTIG_ALL") != nullptr || (getenv("IVID_CONV_CONTIG") != nullptr && p.n_blocks == 1))) p.contig = 1;
-  const int tiles = m_tiles * p.n_blocks;
-  if (l->mode == kConvMc) l->grid = tiles;                       // (m_tiles / cm) * (n_blocks / cn) clusters of cm * cn CTAs
-  else if (p.contig) l->grid = std::min(tiles, sm_count() * (l->mode == kConvSlab ? 1 : 2));
-  else l->grid = tiles;
+  l->grid = p.tiles_w * p.tiles_h * p.tiles_n * p.n_blocks;     // one CTA per (pixel tile, column block)
   return l;
 }
 void conv_launch_destroy(ConvLaunch* l) { delete l; }
 int conv_launch_bn(const ConvLaunch* l) { return l->BN; }
 
-template <int BN, int kMode = kConvDefault>
+template <int BN>
 static void run_conv(const ConvLaunch* l, cudaStream_t s) {
-  using Cfg = ConvGemmCfg<BN, kMode>;
+  using Cfg = ConvGemmCfg<BN>;
   static std::once_flag once;
   std::call_once(once, [] {
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   });
-  if (kMode == kConvMc) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(l->grid);
-    cfg.blockDim = dim3(Cfg::THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = l->p.mc_n * l->p.mc_m; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    IVID_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, kMode>, l->maps, l->p));
-    return;
-  }
-  conv_gemm_kernel<BN, kMode><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
+  conv_gemm_kernel<BN><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
@@ -187,8 +124,6 @@ void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
   conv_launch_run(&tmp, s);
 }
 void conv_launch_run(const ConvLaunch* l, cudaStream_t s) {
-  if (l->mode == kConvMc) { run_conv<128, kConvMc>(l, s); return; }
-  if (l->mode == kConvSlab) { run_conv<128, kConvSlab>(l, s); return; }
   switch (l->BN) {
     case 128: run_conv<128>(l, s); break;
     case 64: run_conv<64>(l, s); break;
@@ -309,8 +244,7 @@ void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s) {
   p.x0 = static_cast<const float*>(d.x0); p.x1 = static_cast<const float*>(d.x1); p.C0 = d.C0; p.C1 = d.C1; p.N = d.N; p.H = d.H; p.W = d.W; p.mode = d.mode;
   p.x0h = d.x0_half ? reinterpret_cast<const __half*>(d.x0) : nullptr;
   p.x1h = d.x0_half ? reinterpret_cast<const __half*>(d.x1) : nullptr;
-  static const bool silu_wrapped = getenv("IVID_SILU_WRAPPED") != nullptr;
-  p.silu = d.silu ? (silu_wrapped ? 2 : 1) : 0;
+  p.silu = d.silu ? 1 : 0;
   p.stats0 = d.stats0; p.stats1 = d.stats1; p.groups = d.groups; p.inv_count = 1.0 / (static_cast<double>(d.H) * d.W);
   p.eps = d.eps; p.gamma = d.gamma; p.beta = d.beta; p.film = d.film; p.film_ld = d.film_ld; p.film_off = d.film_off;
   p.film_add = d.film_add ? 1 : 0;
@@ -326,9 +260,8 @@ void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s) {
   {
     const int blocks_per_n = std::max(1, (sm_count() * 3) / std::max(d.N, 1));
     const int by_wave = (Ho * Wo + blocks_per_n - 1) / blocks_per_n;
-    static const int mode = getenv("IVID_GN_BLOCK") ? atoi(getenv("IVID_GN_BLOCK")) : 1;
     const int small = std::max(1, 1024 / (C / 8));      // at least ~4 work items per thread
-    p.pix_per_block = std::max(1, std::min(Ho * Wo, mode == 0 ? small : (mode == 2 ? std::max(by_wave / 4, small) : std::max(by_wave, small))));
+    p.pix_per_block = std::max(1, std::min(Ho * Wo, std::max(by_wave, small)));
   }
   // the upsampling path walks SOURCE pixels (each written to its 2x2 outputs)
   int pix_space = Ho * Wo;

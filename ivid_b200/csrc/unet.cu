@@ -429,7 +429,6 @@ void Unet::finalize(int device) {
 }
 
 Unet::~Unet() {
-  if (side_stream_) { cudaStreamDestroy(side_stream_); cudaEventDestroy(ev_fork_); cudaEventDestroy(ev_join_); }
   plans_.clear();
   if (cap_stream_) cudaStreamDestroy(cap_stream_);
   if (arena_) cudaFree(arena_);
@@ -441,7 +440,6 @@ Unet::~Unet() {
 struct Plan {
   int N = 0;
   int H = 0, W = 0;        // input geometry
-  int slot = 0;            // 0 = main stream, 1 = side stream (two half-batches run concurrently)
   uint64_t last_use = 0;   // Unet::plan_uses_ at the latest forward
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
@@ -526,9 +524,9 @@ void Unet::check_geometry(int H, int W) const {
                                " (2^(levels-1)): the skip connections' sizes would not match after " + std::to_string(levels - 1) + " downsamplings");
 }
 
-Plan* Unet::get_plan(int N, int H, int W, int slot) {
+Plan* Unet::get_plan(int N, int H, int W) {
   Plan* found = nullptr;
-  for (auto& p : plans_) if (p->N == N && p->H == H && p->W == W && p->slot == slot) found = p.get();
+  for (auto& p : plans_) if (p->N == N && p->H == H && p->W == W) found = p.get();
   if (found == nullptr) {
     check_geometry(H, W);
     if (plans_.size() >= 4) {
@@ -536,7 +534,6 @@ Plan* Unet::get_plan(int N, int H, int W, int slot) {
       plans_.erase(plans_.begin());
     }
     plans_.emplace_back(build_plan(N, H, W));
-    plans_.back()->slot = slot;
     found = plans_.back().get();
   }
   found->last_use = ++plan_uses_;
@@ -1014,51 +1011,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
                "forward: the super-resolution scale must divide the input size");
   IVID_REQUIRE(hook != nullptr || eps != nullptr, "forward: eps output missing");
 
-  // Two half-batches on two streams: the HBM-bound GroupNorm passes of one half may overlap the tensor-bound convolutions
-  // of the other.  The halves are independent samples (typically the two classifier-free-guidance halves sharing x).
-  // Opt-in (IVID_SPLIT_BATCH=1): not measured to help.
-  static const bool split_ok = getenv("IVID_SPLIT_BATCH") != nullptr;
-  const bool can_split = split_ok && hook == nullptr && !profile_ && N % 2 == 0 && N >= 4 && (Nx == N || Nx == N / 2) &&
-                         !(cnd.kind != 0 && Nx == N && cnd.noise_dev == nullptr);
-  if (can_split) {
-    const int half = N / 2;
-    const size_t img = static_cast<size_t>(H) * W;
-    if (side_stream_ == nullptr) {
-      IVID_CHECK_CUDA(cudaStreamCreateWithFlags(&side_stream_, cudaStreamNonBlocking));
-      IVID_CHECK_CUDA(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
-      IVID_CHECK_CUDA(cudaEventCreateWithFlags(&ev_join_, cudaEventDisableTiming));
-    }
-    IVID_CHECK_CUDA(cudaEventRecord(ev_fork_, stream));
-    IVID_CHECK_CUDA(cudaStreamWaitEvent(side_stream_, ev_fork_, 0));
-    for (int hb = 0; hb < 2; ++hb) {
-      Plan* ph = get_plan(half, H, W, hb);
-      cudaStream_t st = hb == 0 ? stream : side_stream_;
-      const bool shift = (Nx == N) && hb == 1;            // rows [half, N) of per-sample inputs
-      const size_t xs = static_cast<size_t>(cfg_.in_channels) * img;
-      ph->x = x + (shift && cnd.kind == 0 ? static_cast<size_t>(half) * xs : 0);
-      if (cnd.kind != 0) ph->x = x + (shift ? static_cast<size_t>(half) * cfg_.out_channels * img : 0);
-      ph->Nx = half;
-      ph->t = t + hb * half;
-      ph->classes = classes ? classes + hb * half : nullptr;
-      ph->eps = eps + static_cast<size_t>(hb) * half * cfg_.out_channels * img;
-      ph->cond = cnd;
-      if (cnd.kind != 0 && shift) {
-        const int s = cnd.sr_scale > 0 ? cnd.sr_scale : 2;
-        const size_t yimg = cnd.kind == 2 ? img / (static_cast<size_t>(s) * s) : img;
-        ph->cond.y_dev = cnd.y_dev + static_cast<size_t>(half) * 4 * yimg;
-        if (cnd.mask_dev) ph->cond.mask_dev = cnd.mask_dev + static_cast<size_t>(half) * img;
-        if (cnd.mask_rgb_dev) ph->cond.mask_rgb_dev = cnd.mask_rgb_dev + static_cast<size_t>(half) * img;
-        if (cnd.noise_dev) ph->cond.noise_dev = cnd.noise_dev + static_cast<size_t>(half) * 4 * img;
-      }
-      IVID_CHECK_CUDA(cudaMemsetAsync(ph->stats_base, 0, ph->stats_bytes, st));
-      for (auto& op : ph->ops.v) op.fn(st);
-    }
-    IVID_CHECK_CUDA(cudaEventRecord(ev_join_, side_stream_));
-    IVID_CHECK_CUDA(cudaStreamWaitEvent(stream, ev_join_, 0));
-    return;
-  }
-
-  Plan* pl = get_plan(N, H, W, 0);
+  Plan* pl = get_plan(N, H, W);
   pl->x = x; pl->Nx = Nx; pl->t = t; pl->classes = classes; pl->eps = eps;
   pl->cond = cnd;
   pl->cond_stream_dev = cond_stream_dev_;
@@ -1153,7 +1106,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
 void Unet::debug_tap(int N, const std::string& name, float* host_out, size_t capacity, int* C, int* H, int* W) {
   Plan* pl = nullptr;
   for (auto& p : plans_)
-    if (p->N == N && p->slot == 0 && (pl == nullptr || p->last_use > pl->last_use)) pl = p.get();
+    if (p->N == N && (pl == nullptr || p->last_use > pl->last_use)) pl = p.get();
   if (pl == nullptr) throw Error(kErrState, "debug_tap: no forward of this batch size has run");
   for (const auto& t : pl->taps) {
     if (t.name != name) continue;

@@ -115,7 +115,7 @@ class Unet {
   void build_topology();
   int add_param(const std::string& name, std::vector<int64_t> shape, bool is_buffer = false);
   const ParamSpec& P(const std::string& name) const;
-  Plan* get_plan(int N, int H, int W, int slot);
+  Plan* get_plan(int N, int H, int W);
   Plan* build_plan(int N, int H, int W);
 
   UnetConfig cfg_;
@@ -143,13 +143,11 @@ class Unet {
 
   const int* cond_stream_dev_ = nullptr;
   cudaStream_t cap_stream_ = nullptr;
-  cudaStream_t side_stream_ = nullptr;
-  cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
   struct ProfAgg { int launches = 0; double ms = 0, flops = 0, bytes = 0; };
   bool profile_ = false;
   std::map<std::string, ProfAgg> profile_acc_;
   std::string profile_ops_;
-  std::vector<std::unique_ptr<Plan>> plans_;       // keyed by (N, H, W, slot)
+  std::vector<std::unique_ptr<Plan>> plans_;       // keyed by (N, H, W)
   uint64_t plan_uses_ = 0;                         // debug_tap reads the most recently run plan of a batch size
   friend struct Plan;
 };

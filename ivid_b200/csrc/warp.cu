@@ -235,7 +235,6 @@ __device__ __forceinline__ void rtri_scan_small32(const RTri& r, int S, unsigned
 // frustum ring and faces stretched across depth discontinuities) are broadcast to the warp and scanned by all 32 lanes.
 // `stash` = this warp's 32 rows of a shared-memory table: a lane parks its big triangle there and the warp reads the leader's row
 // (a broadcast load) instead of keeping two set-up triangles in registers and shuffling 36 words per triangle.
-template <bool kSmemTri>
 __device__ __forceinline__ void rtri_raster(RTri& r, int S, unsigned long long* vis, int lane, int simple, uint32_t (*stash)[kRTriWords]) {
   constexpr int kSmall = 48;
   const int w = r.valid ? (r.px1 - r.px0 + 1) : 0, h = r.valid ? (r.py1 - r.py0 + 1) : 0;
@@ -272,13 +271,7 @@ __device__ __forceinline__ void rtri_raster(RTri& r, int S, unsigned long long* 
     mask &= mask - 1;
     // the leader's record is read in place (warp-uniform addresses: broadcast loads), which keeps the kernel at 96 registers
     // (5 blocks per SM) instead of 122 with a register copy
-    RTri breg;
-    if (!kSmemTri) {
-      uint32_t* dst = reinterpret_cast<uint32_t*>(&breg);
-#pragma unroll
-      for (int i = 0; i < kRTriWords; ++i) dst[i] = stash[leader][i];
-    }
-    const RTri& b = kSmemTri ? *reinterpret_cast<const RTri*>(stash[leader]) : breg;
+    const RTri& b = *reinterpret_cast<const RTri*>(stash[leader]);
     // 8x8-pixel tiles of the bounding box; a tile is skipped when one edge function is negative at its most-inside corner
     // (exact integer test, so the surviving pixels are decided by the same arithmetic as the small path).  The tiles are
     // TESTED 32 at a time (one tile per lane: the frustum-ring slivers have bounding boxes of thousands of tiles of which a
@@ -333,8 +326,7 @@ __device__ __forceinline__ void rtri_raster(RTri& r, int S, unsigned long long* 
   __syncwarp();      // the stash rows are reused by the next sub-triangle of this warp
 }
 
-template <bool kSmemTri, int kMinBlocks>
-__global__ void __launch_bounds__(128, kMinBlocks) raster_kernel(const RasterParams p) {
+__global__ void __launch_bounds__(128, 5) raster_kernel(const RasterParams p) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   const int view = blockIdx.y, b = blockIdx.z;
   const int lane = threadIdx.x & 31;
@@ -368,7 +360,7 @@ __global__ void __launch_bounds__(128, kMinBlocks) raster_kernel(const RasterPar
     }
     if (n >= 3) rtri_make(poly, p.S, static_cast<uint32_t>(fi) * 2u, t);
   }
-  rtri_raster<kSmemTri>(t, p.S, vis, lane, p.simple, stash);
+  rtri_raster(t, p.S, vis, lane, p.simple, stash);
   if (__any_sync(0xffffffffu, second)) {      // atomicMin commutes: the order of the two sub-triangles is irrelevant
     t.valid = 0;
     if (second) {
@@ -376,15 +368,8 @@ __global__ void __launch_bounds__(128, kMinBlocks) raster_kernel(const RasterPar
 #pragma unroll
       for (int i = 0; i < kRTriWords; ++i) dst[i] = s_second[threadIdx.x][i];
     }
-    rtri_raster<kSmemTri>(t, p.S, vis, lane, p.simple, stash);
+    rtri_raster(t, p.S, vis, lane, p.simple, stash);
   }
-}
-
-// IVID_RASTER_REGTRI=1 selects the variant that copies a big triangle into registers (122 registers, 4 blocks per SM): A/B only.
-static void launch_raster(dim3 grid, const RasterParams& rp, cudaStream_t st) {
-  static const bool regtri = [] { const char* e = std::getenv("IVID_RASTER_REGTRI"); return e != nullptr && e[0] == '1'; }();
-  if (regtri) raster_kernel<false, 4><<<grid, 128, 0, st>>>(rp);
-  else raster_kernel<true, 5><<<grid, 128, 0, st>>>(rp);
 }
 
 // ----------------------------------------------------------------------------------------------------------------------
@@ -1121,7 +1106,7 @@ class Warp {
     RasterParams rp;
     rp.views = views_dev_; rp.mvp = mvp_dev_; rp.vis = vis_; rp.nviews = nviews_; rp.F = F_; rp.S = S_; rp.simple = 0;
     dim3 gr((F_ + 127) / 128, nviews_, B_);
-    launch_raster(gr, rp, st);
+    raster_kernel<<<gr, 128, 0, st>>>(rp);
     ResolveParams sp;
     sp.views = views_dev_; sp.mvp = mvp_dev_; sp.vis = vis_; sp.nviews = nviews_; sp.S = S_; sp.T = n_;
     sp.nf_f = static_cast<float>(near_ * far_); sp.far_f = static_cast<float>(far_); sp.fn_f = static_cast<float>(far_ - near_);
@@ -1173,7 +1158,7 @@ class Warp {
     RasterParams rp;
     rp.views = views_dev_; rp.mvp = mvp_dev_; rp.vis = vis_; rp.nviews = 1; rp.F = 2 * (m - 1) * (m - 1); rp.S = S_; rp.simple = 1;
     dim3 gr((rp.F + 127) / 128, 1, B_);
-    launch_raster(gr, rp, st);
+    raster_kernel<<<gr, 128, 0, st>>>(rp);
     ResolveParams sp;
     sp.views = views_dev_; sp.mvp = mvp_dev_; sp.vis = vis_; sp.nviews = 1; sp.S = S_; sp.T = n_;
     sp.nf_f = static_cast<float>(near_ * far_); sp.far_f = static_cast<float>(far_); sp.fn_f = static_cast<float>(far_ - near_);

@@ -33,42 +33,23 @@ CONV_CASES = [
     (2, 64, 64, 64, 16, 3),      # narrow Cout (BN=16 path, output head shape)
     (1, 128, 128, 256, 256, 3),  # the dominant shape of the large model
     (2, 64, 64, 64, 768, 3),     # 6 column blocks, more than one wave of resident CTAs
-    # cluster-multicast kernel (low-resolution levels, N = 128 tiles): clusters of mc_m pixel tiles x mc_n column blocks
-    (4, 8, 8, 256, 512, 3),      # 2 x 4 cluster (8 CTAs): activation slices of 32 pixels, weight slices of 64 rows
-    (8, 8, 8, 128, 256, 3),      # 2 x 2 cluster, 2 cluster items per cluster row
-    (32, 8, 8, 1024, 1024, 3),   # the 8x8 level of the large model at the benchmark batch: 16 clusters of 8
-    (6, 16, 16, 128, 384, 1),    # 16x16 tiles (slices along rows), 3 column blocks: 2 x 1 cluster
-    (4, 16, 16, 64, 640, 3),     # 5 column blocks (odd): 2 x 1 cluster, weight multicast only
-    # 3x3 tap-reuse kernel (8 x 16 pixel tiles)
-    (5, 32, 32, 192, 512, 3),    # odd batch, 3 channel chunks, 40 pixel tiles x 4 column blocks
-    (13, 16, 16, 128, 768, 3),   # 16x16 images: one tile row per image (slab rows -1 and 16 are zero fill), 6 column blocks
+    # low-resolution levels: several samples per pixel tile, several column blocks per tile
+    (4, 8, 8, 256, 512, 3),      # TN=2, 4 column blocks
+    (8, 8, 8, 128, 256, 3),      # TN=2, 2 column blocks
+    (32, 8, 8, 1024, 1024, 3),   # the 8x8 level of the large model at the benchmark batch: 16 K chunks per tap, 8 column blocks
+    (6, 16, 16, 128, 384, 1),    # 1x1 on 16x16 images, 3 column blocks (odd)
+    (4, 16, 16, 64, 640, 3),     # 5 column blocks (odd)
+    (5, 32, 32, 192, 512, 3),    # odd batch, 3 channel chunks, 4 column blocks
+    (13, 16, 16, 128, 768, 3),   # 16x16 images, odd batch of 13, 6 column blocks
 ]
 
 
-@pytest.fixture(params=["default", "multicast", "slab", "contig"])
-def conv_mode(request, monkeypatch):
-    """Every conv case runs through the default kernels, through the opt-in cluster-multicast kernel (IVID_MC=1 is read when
-    a launch is created; it only takes effect on low-resolution N = 128 layers) and through the 3x3 tap-reuse ("slab") kernel
-    (IVID_SLAB=1, 3x3 layers with H >= 16 and 128-column blocks); "contig" = contiguous work ranges per CTA (IVID_CONV_CONTIG_ALL=1) instead of the
-    default round-robin schedule."""
-    monkeypatch.delenv("IVID_MC", raising=False)
-    monkeypatch.delenv("IVID_SLAB", raising=False)
-    monkeypatch.delenv("IVID_CONV_CONTIG_ALL", raising=False)
-    if request.param == "multicast":
-        monkeypatch.setenv("IVID_MC", "1")
-    elif request.param == "slab":
-        monkeypatch.setenv("IVID_SLAB", "1")
-    elif request.param == "contig":
-        monkeypatch.setenv("IVID_CONV_CONTIG_ALL", "1")
-    return request.param
-
-
 @pytest.mark.parametrize("N,H,W,Cin,Cout,k", CONV_CASES)
-def test_conv_matches_torch(N, H, W, Cin, Cout, k, conv_mode):
-    if conv_mode == "multicast" and H > 16:
-        pytest.skip("multicast mode only changes low-resolution layers")
-    if conv_mode == "slab" and (k != 3 or H < 16 or Cout % 128 != 0):
-        pytest.skip("slab mode only changes 3x3 layers with H >= 16 and 128-column blocks")
+@pytest.mark.parametrize("epilogue", ["default", "fp16_out", "residual", "skip"])
+def test_conv_matches_torch(N, H, W, Cin, Cout, k, epilogue):
+    """Every conv case through each epilogue / K path of the kernel: "default" = fp32 NHWC output, "fp16_out" = fp16 output,
+    "residual" = fp32 identity residual added in the epilogue, "skip" = a 1x1 skip segment over a second tensor of Cin
+    channels as extra K chunks (ResBlock tail)."""
     rng = _rng(hash((N, H, W, Cin, Cout, k)) % 2**31)
     x = _t(rng, N, Cin, H, W)
     w = _t(rng, Cout, Cin, k, k, scale=1 / math.sqrt(Cin * k * k))
@@ -76,11 +57,26 @@ def test_conv_matches_torch(N, H, W, Cin, Cout, k, conv_mode):
     xh = x.half()
     ref16 = F.conv2d(xh.float(), w.half().float(), b, padding=k // 2)       # same rounded operands, fp32 math
     ref32 = F.conv2d(x, w, b, padding=k // 2)
-    out = G.conv2d(xh.permute(0, 2, 3, 1).contiguous().cuda(), w, b, k)
-    got = out.permute(0, 3, 1, 2).cpu()
-    r16 = G.report(f"conv N{N} {H}x{W} {Cin}->{Cout} k{k} (vs fp16-rounded operands)", got, ref16)
-    r32 = G.report(f"conv N{N} {H}x{W} {Cin}->{Cout} k{k} (vs fp32)", got, ref32)
-    assert r16 < 2e-5
+    nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous().cuda()
+    kw = {}
+    if epilogue == "fp16_out":
+        kw["out_fp16"] = True
+    elif epilogue == "residual":
+        res = _t(rng, N, Cout, H, W)
+        ref16 = ref16 + res; ref32 = ref32 + res
+        kw["residual"] = nhwc(res)
+    elif epilogue == "skip":
+        x2 = _t(rng, N, Cin, H, W)
+        ws = _t(rng, Cout, Cin, 1, 1, scale=1 / math.sqrt(Cin)); bs = _t(rng, Cout, scale=0.1)
+        ref16 = ref16 + F.conv2d(x2.half().float(), ws.half().float(), bs)
+        ref32 = ref32 + F.conv2d(x2, ws, bs)
+        kw.update(act2=nhwc(x2.half()), w2=ws, b2=bs)
+    out = G.conv2d(nhwc(xh), w, b, k, **kw)
+    got = out.float().permute(0, 3, 1, 2).cpu()
+    tag = f"conv N{N} {H}x{W} {Cin}->{Cout} k{k} {epilogue}"
+    r16 = G.report(f"{tag} (vs fp16-rounded operands)", got, ref16)
+    r32 = G.report(f"{tag} (vs fp32)", got, ref32)
+    assert r16 < (5e-4 if epilogue == "fp16_out" else 2e-5)      # fp16 output: one rounding of the result
     assert r32 < 2e-3
 
 
@@ -103,9 +99,9 @@ def test_conv_skip_segment_residual_and_fp16_out():
     assert G.report("conv3x3 fp16 out", out3.float().permute(0, 3, 1, 2), F.conv2d(a.half().float(), w.half().float(), b, padding=1)) < 5e-4
 
 
-def test_conv_slab_segments_residual_and_fp16_out(monkeypatch):
-    """3x3 tap-reuse kernel with a 1x1 skip segment over a second tensor (mixed 9-tap / 1-tap segments share the ring), a
-    two-segment 3x3 input (virtual concat), the identity residual and the fp16 output; same shapes through the default kernel."""
+def test_conv_skip_segment_residual_and_fp16_out_4_column_blocks():
+    """The paths of test_conv_skip_segment_residual_and_fp16_out on a layer of 4 column blocks and 128 pixel tiles: a 1x1
+    skip segment over a second tensor (9-tap and 1-tap segments share the ring), the identity residual and the fp16 output."""
     rng = _rng(31)
     N, H, W, C, Cx = 4, 64, 64, 128, 192
     Co = 512
@@ -117,23 +113,17 @@ def test_conv_slab_segments_residual_and_fp16_out(monkeypatch):
     an = a.half().permute(0, 2, 3, 1).contiguous().cuda()
     xn = x.half().permute(0, 2, 3, 1).contiguous().cuda()
     rn = res.permute(0, 2, 3, 1).contiguous().cuda()
-    for mode in ("1", None):
-        if mode:
-            monkeypatch.setenv("IVID_SLAB", mode)
-        else:
-            monkeypatch.delenv("IVID_SLAB", raising=False)
-        tag = "slab" if mode else "default"
-        out = G.conv2d(an, w, b, 3, act2=xn, w2=ws, b2=bs)
-        assert G.report(f"{tag}: conv3x3 + 1x1 skip segment", out.permute(0, 3, 1, 2), base + skip) < 2e-5
-        out2 = G.conv2d(an, w, b, 3, residual=rn)
-        assert G.report(f"{tag}: conv3x3 + identity residual", out2.permute(0, 3, 1, 2), base + res) < 2e-5
-        out3 = G.conv2d(an, w, b, 3, out_fp16=True)
-        assert G.report(f"{tag}: conv3x3 fp16 out", out3.float().permute(0, 3, 1, 2), base) < 5e-4
+    out = G.conv2d(an, w, b, 3, act2=xn, w2=ws, b2=bs)
+    assert G.report("conv3x3 + 1x1 skip segment", out.permute(0, 3, 1, 2), base + skip) < 2e-5
+    out2 = G.conv2d(an, w, b, 3, residual=rn)
+    assert G.report("conv3x3 + identity residual", out2.permute(0, 3, 1, 2), base + res) < 2e-5
+    out3 = G.conv2d(an, w, b, 3, out_fp16=True)
+    assert G.report("conv3x3 fp16 out", out3.float().permute(0, 3, 1, 2), base) < 5e-4
 
 
-def test_conv_multicast_residual_stats_paths(monkeypatch):
-    """Cluster-multicast kernel through the residual epilogue, the fp16-output epilogue and the 1x1 skip segment."""
-    monkeypatch.setenv("IVID_MC", "1")
+def test_conv_low_resolution_residual_fp16_out_and_skip_segment():
+    """An 8x8 layer (two samples per pixel tile, 4 column blocks) through the residual epilogue, the fp16-output epilogue and
+    the 1x1 skip segment."""
     rng = _rng(21)
     N, H, W, C, Cx = 8, 8, 8, 512, 256
     a = _t(rng, N, C, H, W); x = _t(rng, N, Cx, H, W); res = _t(rng, N, C, H, W)
@@ -142,11 +132,11 @@ def test_conv_multicast_residual_stats_paths(monkeypatch):
     base = F.conv2d(a.half().float(), w.half().float(), b, padding=1)
     an = a.half().permute(0, 2, 3, 1).contiguous().cuda()
     out = G.conv2d(an, w, b, 3, residual=res.permute(0, 2, 3, 1).contiguous().cuda())
-    assert G.report("multicast: conv3x3 + residual", out.permute(0, 3, 1, 2), base + res) < 2e-5
+    assert G.report("8x8: conv3x3 + residual", out.permute(0, 3, 1, 2), base + res) < 2e-5
     out16 = G.conv2d(an, w, b, 3, out_fp16=True)
-    assert G.report("multicast: conv3x3 fp16 out", out16.float().permute(0, 3, 1, 2), base) < 5e-4
+    assert G.report("8x8: conv3x3 fp16 out", out16.float().permute(0, 3, 1, 2), base) < 5e-4
     outs = G.conv2d(an, w, b, 3, act2=x.half().permute(0, 2, 3, 1).contiguous().cuda(), w2=ws, b2=bs)
-    assert G.report("multicast: conv3x3 + 1x1 skip segment", outs.permute(0, 3, 1, 2),
+    assert G.report("8x8: conv3x3 + 1x1 skip segment", outs.permute(0, 3, 1, 2),
                     base + F.conv2d(x.half().float(), ws.half().float(), bs)) < 2e-5
 
 
