@@ -184,9 +184,9 @@ void Unet::build_topology() {
       BlockDef b;
       b.is_input = true;
       const std::string pfx = "input_blocks." + std::to_string(ib);
-      b.layers.push_back({1, add_res(pfx + ".0", ch, outc, 0)});
+      b.layers.push_back({LayerKind::kResBlock, add_res(pfx + ".0", ch, outc, 0)});
       ch = outc;
-      if (in_attn(ds)) b.layers.push_back({2, add_attn(pfx + ".1", ch)});
+      if (in_attn(ds)) b.layers.push_back({LayerKind::kAttention, add_attn(pfx + ".1", ch)});
       blocks_.push_back(b);
       input_block_chs.push_back(ch);
       ++ib;
@@ -194,8 +194,8 @@ void Unet::build_topology() {
     if (level != levels - 1) {
       BlockDef b;
       b.is_input = true;
-      if (c.resblock_updown) b.layers.push_back({1, add_res("input_blocks." + std::to_string(ib) + ".0", ch, ch, 2)});
-      else b.layers.push_back({3, add_resample("input_blocks." + std::to_string(ib) + ".0", ch, 2)});      // adm.py:409-412
+      if (c.resblock_updown) b.layers.push_back({LayerKind::kResBlock, add_res("input_blocks." + std::to_string(ib) + ".0", ch, ch, 2)});
+      else b.layers.push_back({LayerKind::kResample, add_resample("input_blocks." + std::to_string(ib) + ".0", ch, 2)});      // adm.py:409-412
       blocks_.push_back(b);
       input_block_chs.push_back(ch);
       ++ib;
@@ -204,9 +204,9 @@ void Unet::build_topology() {
   }
   {
     BlockDef b;
-    b.layers.push_back({1, add_res("middle_block.0", ch, ch, 0)});
-    b.layers.push_back({2, add_attn("middle_block.1", ch)});
-    b.layers.push_back({1, add_res("middle_block.2", ch, ch, 0)});
+    b.layers.push_back({LayerKind::kResBlock, add_res("middle_block.0", ch, ch, 0)});
+    b.layers.push_back({LayerKind::kAttention, add_attn("middle_block.1", ch)});
+    b.layers.push_back({LayerKind::kResBlock, add_res("middle_block.2", ch, ch, 0)});
     blocks_.push_back(b);
   }
   int ob = 0;
@@ -219,12 +219,12 @@ void Unet::build_topology() {
       const int ich = input_block_chs.back();
       input_block_chs.pop_back();
       int li = 0;
-      b.layers.push_back({1, add_res(pfx + "." + std::to_string(li++), ch + ich, outc, 0, ch)});
+      b.layers.push_back({LayerKind::kResBlock, add_res(pfx + "." + std::to_string(li++), ch + ich, outc, 0, ch)});
       ch = outc;
-      if (in_attn(ds)) b.layers.push_back({2, add_attn(pfx + "." + std::to_string(li++), ch)});
+      if (in_attn(ds)) b.layers.push_back({LayerKind::kAttention, add_attn(pfx + "." + std::to_string(li++), ch)});
       if (level != 0 && i == c.num_res_blocks) {
-        if (c.resblock_updown) b.layers.push_back({1, add_res(pfx + "." + std::to_string(li++), ch, ch, 1)});
-        else b.layers.push_back({3, add_resample(pfx + "." + std::to_string(li++), ch, 1)});               // adm.py:475-478
+        if (c.resblock_updown) b.layers.push_back({LayerKind::kResBlock, add_res(pfx + "." + std::to_string(li++), ch, ch, 1)});
+        else b.layers.push_back({LayerKind::kResample, add_resample(pfx + "." + std::to_string(li++), ch, 1)});               // adm.py:475-478
         ds *= 2;
       }
       blocks_.push_back(b);
@@ -446,21 +446,26 @@ struct Plan {
   double* stats_base = nullptr;
   size_t stats_bytes = 0;
   struct OpRec {
-    std::function<void(cudaStream_t)> fn;
     const char* label;      // kernel family (profile aggregation key)
     double flops;           // algorithmic FLOPs of this launch (tensor-core ops)
     double bytes;           // algorithmic HBM bytes of this launch (memory-bound ops)
     std::string note;       // shape description (per-op profile dump)
+    std::function<void(cudaStream_t)> fn;
   };
-  struct OpList {
-    std::vector<OpRec> v;
-    const char* label = "other"; double flops = 0, bytes = 0; std::string note;    // metadata of the next push
-    void tag(const char* l, double f, double b, std::string n = "") { label = l; flops = f; bytes = b; note = std::move(n); }
-    void push_back(std::function<void(cudaStream_t)> fn) {
-      v.push_back(OpRec{std::move(fn), label, flops, bytes, note});
-      label = "other"; flops = 0; bytes = 0; note.clear();
+  std::vector<OpRec> ops;
+  void add_op(const char* label, double flops, double bytes, std::string note, std::function<void(cudaStream_t)> fn) {
+    ops.push_back(OpRec{label, flops, bytes, std::move(note), std::move(fn)});
+  }
+  // One forward: zero the statistics arena, then enqueue every op on s.  With `ev` (ops.size() + 1 events), ev[i] and
+  // ev[i + 1] bracket op i.
+  void run(cudaStream_t s, cudaEvent_t* ev = nullptr) const {
+    IVID_CHECK_CUDA(cudaMemsetAsync(stats_base, 0, stats_bytes, s));
+    if (ev) IVID_CHECK_CUDA(cudaEventRecord(ev[0], s));
+    for (size_t i = 0; i < ops.size(); ++i) {
+      ops[i].fn(s);
+      if (ev) IVID_CHECK_CUDA(cudaEventRecord(ev[i + 1], s));
     }
-  } ops;
+  }
   std::vector<ConvLaunch*> convs;
   std::vector<AttnLaunch*> attns;
   // per-call inputs
@@ -497,22 +502,23 @@ struct Plan {
 };
 
 namespace {
+// scratch buffers of a plan, each reused by every layer that needs it
+enum Slot { kIn, kA1, kA2, kXh, kXr, kH, kQkv, kCol, kPe, kE1, kEmb, kFilm, kXt, kSlots };
 struct Act {          // fp32 NHWC residual-stream tensor with per-(n,channel) statistics
-  float* data = nullptr;
+  float* data = nullptr;    // null when the layout keeps the tensor as fp16 only, and in the sizing pass
   __half* d16 = nullptr;    // fp16 copy written by the producing conv (operand of the next GroupNorm / 1x1 skip conv)
   double* stats = nullptr;
-  int id = -1;              // position in creation order (fp32 liveness table of build_plan)
+  bool has16 = false;       // the producing conv writes the fp16 copy
+  int id = -1;              // position in creation order (index of its BlockOut)
   int C = 0, H = 0, W = 0;
 };
-struct Bump {
-  uint8_t* base; size_t off = 0;
-  explicit Bump(uint8_t* b) : base(b) {}
-  void* take(size_t bytes) {
-    off = (off + 1023) & ~size_t(1023);
-    void* p = base ? base + off : nullptr;
-    off += bytes;
-    return p;
-  }
+// a block output as the sizing pass records it and the layout places it
+struct BlockOut {
+  int C, H, W;
+  bool may16;               // the producing conv can write it as fp16 only
+  bool need32 = false;      // some consumer keeps its fp32 storage
+  bool only16 = false;      // layout: may16 && !need32
+  size_t off16 = 0, off32 = 0;
 };
 }  // namespace
 
@@ -550,110 +556,70 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
   auto W8 = [&](size_t off) { return arena_ + off; };
   auto Wf = [&](size_t off) { return reinterpret_cast<const float*>(arena_ + off); };
 
-  // ---- scratch maxima (walk the topology once for sizes) ----
-  size_t max_act16 = 0, max_raw16 = 0, max_f32 = 0, max_qkv = 0, max_col = 0;
-  {
-    int rh = SH, rw = SW;
-    auto upd_res = [&](const ResBlockDef& r) {
-      const int oh = r.mode == 1 ? rh * 2 : (r.mode == 2 ? rh / 2 : rh);
-      const int ow = r.mode == 1 ? rw * 2 : (r.mode == 2 ? rw / 2 : rw);
-      const size_t po = static_cast<size_t>(N) * oh * ow;
-      max_act16 = std::max({max_act16, po * r.cin, po * r.cout});
-      max_raw16 = std::max(max_raw16, static_cast<size_t>(N) * rh * rw * r.cin);
-      max_f32 = std::max({max_f32, po * r.cin, po * r.cout});
-      rh = oh; rw = ow;
+  // One walk over the topology, run twice.  The sizing pass (base == nullptr) creates no ops: it records the largest
+  // request made of each scratch slot, the shape and storage needs of each block output, and the statistics bytes.  The
+  // layout then places them, and the create pass (base = the workspace) walks again with real pointers, builds the
+  // launches and checks every scratch and statistics request against what the layout gave it.
+  size_t slot_bytes[kSlots] = {}, slot_off[kSlots] = {};
+  std::vector<BlockOut> outs;
+  size_t stats_bytes = 0, stats_off = 0;
+  auto walk = [&](uint8_t* base) {
+    const bool create = base != nullptr;
+    auto scratch = [&](Slot s, size_t bytes) -> void* {
+      if (!create) { slot_bytes[s] = std::max(slot_bytes[s], bytes); return nullptr; }
+      IVID_REQUIRE(bytes <= slot_bytes[s], "internal: scratch request exceeds its slot");
+      return base + slot_off[s];
     };
-    for (const auto& b : blocks_)
-      for (const auto& l : b.layers) {
-        if (l.kind == 1) upd_res(res_[l.idx]);
-        else if (l.kind == 3) {
-          const auto& r = resample_[l.idx];
-          if (r.mode == 2) { max_col = std::max(max_col, static_cast<size_t>(N) * (rh / 2) * (rw / 2) * 9 * r.C); rh /= 2; rw /= 2; }
-          else { max_act16 = std::max(max_act16, static_cast<size_t>(N) * (rh * 2) * (rw * 2) * r.C); rh *= 2; rw *= 2; }
-        } else {
-          const auto& a = attn_[l.idx];
-          max_act16 = std::max(max_act16, static_cast<size_t>(N) * rh * rw * a.C);
-          max_qkv = std::max(max_qkv, static_cast<size_t>(N) * rh * rw * 3 * a.C);
-        }
-      }
-    max_act16 = std::max(max_act16, static_cast<size_t>(N) * SH * SW * std::max(64, final_ch_));
-  }
-
-  // The same allocation sequence is run three times: once to find out which block outputs are ever read in fp32 (residual
-  // adds, resampling blocks; everything else consumes the fp16 copy), once to size the workspace, once to build the launches.
-  std::vector<char> need32;
-  bool collect = true;
-  auto layout = [&](uint8_t* base, bool create) -> size_t {
-    Bump bump(base);
-    int next_id = 0;
-    // statistics arena is placed first so that its base is known while creating ops
-    // (sized generously: every tensor needs N*C*16 bytes; bound by total params walk below)
-    size_t stats_cap = 0;
-    {
-      stats_cap += static_cast<size_t>(N) * in_ch_stem_ * 16 + 1024;
-      for (const auto& b : blocks_)
-        for (const auto& l : b.layers) {
-          if (l.kind == 1) {
-            const auto& r = res_[l.idx];
-            stats_cap += 2 * (static_cast<size_t>(N) * r.cout * 16 + 1024);
-          } else if (l.kind == 3) {
-            stats_cap += static_cast<size_t>(N) * resample_[l.idx].C * 16 + 1024;
-          } else {
-            stats_cap += static_cast<size_t>(N) * attn_[l.idx].C * 16 + 1024;
-          }
-        }
-    }
-    uint8_t* stats_base = static_cast<uint8_t*>(bump.take(stats_cap));
+    // N x H x W x C elements of a slot
+    auto s16 = [&](Slot s, int H, int Wd, int C) { return scratch(s, static_cast<size_t>(N) * H * Wd * C * 2); };
+    auto s32 = [&](Slot s, int H, int Wd, int C) { return static_cast<float*>(scratch(s, static_cast<size_t>(N) * H * Wd * C * 4)); };
     size_t soff = 0;
     auto take_stats = [&](int C) -> double* {
       const size_t o = soff;
       soff += (static_cast<size_t>(N) * C * 16 + 255) & ~size_t(255);
-      return stats_base ? reinterpret_cast<double*>(stats_base + o) : nullptr;
+      if (!create) return nullptr;
+      IVID_REQUIRE(soff <= stats_bytes, "internal: statistics request exceeds the arena");
+      return reinterpret_cast<double*>(base + stats_off + o);
     };
-    auto stats_ptr = [&](const Act& a) { return a.stats; };
-    auto new_act = [&](int C, int H, int Wd) {
+    int next_id = 0;
+    // may16: the producer's epilogue has no residual add, so it could write the output as fp16 only
+    auto new_act = [&](int C, int H, int Wd, bool may16) {
       Act a; a.C = C; a.H = H; a.W = Wd;
       a.id = next_id++;
-      if (collect) need32.resize(a.id + 1, 0);
-      if (conv_can_out16(C)) a.d16 = static_cast<__half*>(bump.take(static_cast<size_t>(N) * H * Wd * C * 2));
+      a.has16 = conv_can_out16(C);
+      if (!create) {
+        outs.push_back(BlockOut{C, H, Wd, may16 && a.has16 && conv_can_fuse_stats(H, Wd)});
+      } else {
+        IVID_REQUIRE(a.id < static_cast<int>(outs.size()) && outs[a.id].C == C && outs[a.id].H == H && outs[a.id].W == Wd,
+                     "internal: block output differs from the sizing pass");
+        const BlockOut& o = outs[a.id];
+        if (a.has16) a.d16 = reinterpret_cast<__half*>(base + o.off16);
+        if (!o.only16) a.data = reinterpret_cast<float*>(base + o.off32);
+      }
       a.stats = take_stats(C);
       return a;
     };
-
-    // scratch
-    void* s_in = bump.take(static_cast<size_t>(N) * SH * SW * 64 * 2);
-    void* s_a1 = bump.take(max_act16 * 2);
-    void* s_a2 = bump.take(max_act16 * 2);
-    void* s_xh = bump.take(max_raw16 * 2);
-    float* s_xr = static_cast<float*>(bump.take(max_f32 * 4));
-    float* s_h = static_cast<float*>(bump.take(max_f32 * 4));
-    void* s_qkv = bump.take(std::max<size_t>(max_qkv, 1) * 2);
-    void* s_col = bump.take(std::max<size_t>(max_col, 1) * 2);           // im2col operand of the stride-2 Downsample2d conv
-    float* s_pe = static_cast<float*>(bump.take(static_cast<size_t>(N) * cfg_.model_channels * 4));
-    float* s_e1 = static_cast<float*>(bump.take(static_cast<size_t>(N) * embed_dim_ * 4));
-    float* s_emb = static_cast<float*>(bump.take(static_cast<size_t>(N) * embed_dim_ * 4));
-    float* s_film = static_cast<float*>(bump.take(static_cast<size_t>(N) * film_total_ * 4));
-    float* s_xt = static_cast<float*>(bump.take(static_cast<size_t>((N + 31) / 32) * embed_dim_ * 32 * 4));
-
-    // fp32 storage of a block output is allocated by its producer, and only when some consumer reads it (or the fp16-only
-    // epilogue is not available: no fp16 copy, residual add, statistics not fusable)
-    auto alloc32 = [&](Act& a) { a.data = static_cast<float*>(bump.take(static_cast<size_t>(N) * a.H * a.W * a.C * 4)); };
-    auto only16 = [&](const Act& a, bool has_residual) {
-      return !collect && !need32[a.id] && a.d16 != nullptr && !has_residual && conv_can_fuse_stats(a.H, a.W);
-    };
     auto use32 = [&](const Act& a) -> const float* {
-      if (collect) need32[a.id] = 1;
-      else if (create) IVID_REQUIRE(a.data != nullptr, "internal: fp32 tensor was not materialised");
+      if (!create) outs[a.id].need32 = true;
+      else IVID_REQUIRE(a.data != nullptr, "internal: fp32 tensor was not materialised");
       return a.data;
     };
-    Act pending_stats; bool has_pending_stats = false;
+    // ResBlocks and the output head keep the fp32 storage of their inputs even where they read the fp16 copies, so only an
+    // output that a resampling conv alone reads is written as fp16 only.  Storing more outputs as fp16 only would change
+    // their convs' epilogues and take their statistics from the rounded values: a change of results, not of layout.
+    auto keep32 = [&](const Act& a) { use32(a); };
+    // a block output as the conv's output: fp32 NHWC plus the fp16 copy, or fp16 only where the layout gave it no fp32
+    auto write_to = [&](ConvDesc& d, const Act& a) {
+      if (a.data != nullptr) { d.out = a.data; d.out16 = a.d16; d.out_mode = 0; }
+      else { d.out = a.d16; d.out_mode = 1; }
+      d.ldc = a.C; d.N = N; d.H = a.H; d.W = a.W;
+    };
+    // GroupNorm statistics of the output are accumulated in the conv epilogue whenever the tile geometry allows; otherwise
+    // a separate pass reads the fp32 NHWC output right after the conv
     auto add_conv = [&](ConvDesc d, const Act* stats_of = nullptr, double k_alg = 0.0, double n_alg = 0.0) {
-      // GroupNorm statistics of the output are accumulated in the conv epilogue whenever the tile geometry allows
+      if (!create) return;
       const bool fused = stats_of != nullptr && conv_can_fuse_stats(d.H, d.W);
       if (fused) d.stats = stats_of->stats;
-      if (stats_of != nullptr && !fused) pending_stats = *stats_of;
-      has_pending_stats = stats_of != nullptr && !fused;
-      if (!create) return;
       ConvLaunch* l = conv_launch_create(d);
       pl->convs.push_back(l);
       // ALGORITHMIC work: operand padding (stem: 9*Cin of 9*64 columns) and split-precision segments do not count
@@ -663,51 +629,26 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       const double Nalg = n_alg > 0.0 ? n_alg : static_cast<double>(d.cout);
       static const char* names[] = {"conv_gemm<16>", "conv_gemm<64>", "conv_gemm<128>"};
       const int bn = conv_launch_bn(l);
-      pl->ops.tag(names[bn == 128 ? 2 : bn == 64 ? 1 : 0], 2.0 * M * K * Nalg,
-                  M * (d.C0 + d.C1 + d.C2) * 2 + M * d.cout * ((d.out_mode == 1 ? 2 : 4) + (d.out16 ? 2 : 0) + (d.residual ? 4 : 0)) + K * d.cout_pad * 2,
-                  std::to_string(d.H) + "x" + std::to_string(d.W) + " " + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") + (d.C2 ? "+" + std::to_string(d.C2) : "") +
-                      "->" + std::to_string(d.cout) + " k" + std::to_string(d.taps0) + (d.residual ? " res" : "") + (d.stats ? " stats" : "") +
-                      (d.out_mode == 1 ? " f16" : "") + (d.out16 ? " +f16" : ""));
-      pl->ops.push_back([l](cudaStream_t s) { conv_launch_run(l, s); });
-    };
-    auto add_stats = [&](const Act& a) {
-      if (!create || !has_pending_stats) return;      // already fused into the producing conv
-      has_pending_stats = false;
-      const float* x = a.data; double* st = stats_ptr(a);
-      IVID_REQUIRE(!create || x != nullptr, "internal: statistics pass over a tensor without fp32 storage");
-      const int HW = a.H * a.W, C = a.C;
-      pl->ops.tag("gn_stats", 0, static_cast<double>(N) * HW * C * 4);
-      pl->ops.push_back([=](cudaStream_t s) { launch_gn_stats(x, st, N, HW, C, s); });
-    };
-    // GroupNorm coefficients are computed in the prologue of the apply kernel: add_coeff only records its inputs
-    GnApplyDesc pend;
-    auto add_coeff = [&](const Act& a0, const Act* a1, const GnW& g, int film_off) {
-      pend = GnApplyDesc();
-      pend.stats0 = stats_ptr(a0);
-      pend.stats1 = a1 ? stats_ptr(*a1) : nullptr;
-      pend.groups = G; pend.eps = eps;
-      pend.gamma = Wf(g.g_off); pend.beta = Wf(g.b_off);
-      pend.film = film_off >= 0 ? s_film : nullptr;
-      pend.film_ld = film_total_; pend.film_off = std::max(film_off, 0);
-      pend.film_add = film_off >= 0 && !cfg_.use_scale_shift_norm;
-    };
-    auto add_apply = [&](GnApplyDesc d) {
-      if (!create) return;
-      d.stats0 = pend.stats0; d.stats1 = pend.stats1; d.groups = pend.groups; d.eps = pend.eps; d.gamma = pend.gamma;
-      d.beta = pend.beta; d.film = pend.film; d.film_ld = pend.film_ld; d.film_off = pend.film_off; d.film_add = pend.film_add;
-      {
-        const int Ho = d.mode == 1 ? d.H * 2 : (d.mode == 2 ? d.H / 2 : d.H);
-        const int Wo = d.mode == 1 ? d.W * 2 : (d.mode == 2 ? d.W / 2 : d.W);
-        const double in_el = static_cast<double>(d.N) * d.H * d.W * (d.C0 + d.C1);
-        const double out_el = static_cast<double>(d.N) * Ho * Wo * (d.C0 + d.C1);
-        pl->ops.tag("gn_apply", 0, in_el * (d.x0_half ? 2 : 4) + out_el * 2 + (d.out_raw16 ? out_el * 2 : 0) + (d.out_raw32 ? out_el * 4 : 0),
-                    std::to_string(d.H) + "x" + std::to_string(d.W) + " C" + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") +
-                        " m" + std::to_string(d.mode) + (d.x0_half ? " h16" : "") + (d.out_raw16 ? " raw16" : "") + (d.out_raw32 ? " raw32" : ""));
+      pl->add_op(names[bn == 128 ? 2 : bn == 64 ? 1 : 0], 2.0 * M * K * Nalg,
+                 M * (d.C0 + d.C1 + d.C2) * 2 + M * d.cout * ((d.out_mode == 1 ? 2 : 4) + (d.out16 ? 2 : 0) + (d.residual ? 4 : 0)) + K * d.cout_pad * 2,
+                 std::to_string(d.H) + "x" + std::to_string(d.W) + " " + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") + (d.C2 ? "+" + std::to_string(d.C2) : "") +
+                     "->" + std::to_string(d.cout) + " k" + std::to_string(d.taps0) + (d.residual ? " res" : "") + (d.stats ? " stats" : "") +
+                     (d.out_mode == 1 ? " f16" : "") + (d.out16 ? " +f16" : ""),
+                 [l](cudaStream_t s) { conv_launch_run(l, s); });
+      if (stats_of != nullptr && !fused) {
+        const float* x = stats_of->data; double* st = stats_of->stats;
+        IVID_REQUIRE(x != nullptr, "internal: statistics pass over a tensor without fp32 storage");
+        const int HW = stats_of->H * stats_of->W, C = stats_of->C;
+        pl->add_op("gn_stats", 0, static_cast<double>(N) * HW * C * 4, "", [=](cudaStream_t s) { launch_gn_stats(x, st, N, HW, C, s); });
       }
-      pl->ops.push_back([d](cudaStream_t s) { launch_gn_apply(d, s); });
     };
 
     // ---- embeddings ----
+    float* s_pe = s32(kPe, 1, 1, cfg_.model_channels);
+    float* s_e1 = s32(kE1, 1, 1, embed_dim_);
+    float* s_emb = s32(kEmb, 1, 1, embed_dim_);
+    float* s_film = s32(kFilm, 1, 1, film_total_);
+    float* s_xt = static_cast<float*>(scratch(kXt, static_cast<size_t>((N + 31) / 32) * embed_dim_ * 32 * 4));
     if (create) {
       const float* freqs = Wf(freqs_off_);
       const int half = cfg_.model_channels / 2, mc = cfg_.model_channels, E = embed_dim_;
@@ -715,26 +656,43 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       const float* lab = cfg_.num_classes > 0 ? Wf(label_off_) : nullptr;
       const float *wf = Wf(film_.w_off), *bf = Wf(film_.b_off);
       const int FT = film_total_;
-      pl->ops.tag("embed", 2.0 * N * E * (mc + E), 4.0 * E * (mc + E), "posenc+time_embed");
-      pl->ops.push_back([=](cudaStream_t s) {
+      pl->add_op("embed", 2.0 * N * E * (mc + E), 4.0 * E * (mc + E), "posenc+time_embed", [=](cudaStream_t s) {
         launch_posenc(pl->t, N, freqs, half, s_pe, N, s);
         launch_linear(s_pe, w1, b1, s_e1, N, mc, E, 0, nullptr, nullptr, 1, s);
         launch_linear(s_e1, w2, b2, s_emb, N, E, E, 1, pl->classes ? lab : nullptr, pl->classes, N, s);
       });
       pl->taps.push_back({"emb", s_emb, nullptr, E, 1, 1});                 // time (+ class) embedding [N, E] (adm.py:545-555)
       pl->taps.push_back({"film", s_film, nullptr, FT, 1, 1});              // all emb_layers outputs [N, sum 2*Cout] (adm.py:174-177, 214)
-      pl->ops.tag("embed", 2.0 * N * E * FT, 4.0 * E * FT, "film table O=" + std::to_string(FT));
-      pl->ops.push_back([=](cudaStream_t s) {
+      pl->add_op("embed", 2.0 * N * E * FT, 4.0 * E * FT, "film table O=" + std::to_string(FT), [=](cudaStream_t s) {
         if (E % 32 == 0) launch_film_table(s_emb, wf, bf, s_xt, s_film, N, E, FT, s);
         else launch_linear(s_emb, wf, bf, s_film, N, E, FT, 1, nullptr, nullptr, 1, s);
       });
     }
+    // GroupNorm (+ FiLM from column film_off of the table; -1: none) of a0 [| a1]; the coefficients are computed in the
+    // prologue of the apply kernel.  d carries the source pointers (fp32 or the fp16 copies), the geometry and the outputs.
+    auto add_gn = [&](GnApplyDesc d, const Act& a0, const Act* a1, const GnW& g, int film_off) {
+      if (!create) return;
+      d.stats0 = a0.stats; d.stats1 = a1 ? a1->stats : nullptr;
+      d.groups = G; d.eps = eps;
+      d.gamma = Wf(g.g_off); d.beta = Wf(g.b_off);
+      d.film = film_off >= 0 ? s_film : nullptr;
+      d.film_ld = film_total_; d.film_off = std::max(film_off, 0);
+      d.film_add = film_off >= 0 && !cfg_.use_scale_shift_norm;
+      const int Ho = d.mode == 1 ? d.H * 2 : (d.mode == 2 ? d.H / 2 : d.H);
+      const int Wo = d.mode == 1 ? d.W * 2 : (d.mode == 2 ? d.W / 2 : d.W);
+      const double in_el = static_cast<double>(d.N) * d.H * d.W * (d.C0 + d.C1);
+      const double out_el = static_cast<double>(d.N) * Ho * Wo * (d.C0 + d.C1);
+      pl->add_op("gn_apply", 0, in_el * (d.x0_half ? 2 : 4) + out_el * 2 + (d.out_raw16 ? out_el * 2 : 0) + (d.out_raw32 ? out_el * 4 : 0),
+                 std::to_string(d.H) + "x" + std::to_string(d.W) + " C" + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") +
+                     " m" + std::to_string(d.mode) + (d.x0_half ? " h16" : "") + (d.out_raw16 ? " raw16" : "") + (d.out_raw32 ? " raw32" : ""),
+                 [d](cudaStream_t s) { launch_gn_apply(d, s); });
+    };
 
     // ---- stem ----
+    void* s_in = s16(kIn, SH, SW, 64);
     if (create) {
       const int Cin = cfg_.in_channels, HW = SH * SW;
-      pl->ops.tag("pack_input", 0, static_cast<double>(N) * HW * (Cin * 4 + 128));
-      pl->ops.push_back([=](cudaStream_t s) {
+      pl->add_op("pack_input", 0, static_cast<double>(N) * HW * (Cin * 4 + 128), "", [=](cudaStream_t s) {
         if (pl->cond.kind == 0) {
           launch_pack_input(pl->x, s_in, N, pl->Nx, Cin, HW, s);
         } else {
@@ -747,16 +705,13 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
         }
       });
     }
-    Act cur = new_act(in_ch_stem_, SH, SW);
+    Act cur = new_act(in_ch_stem_, SH, SW, true);
     {
       ConvDesc d;
       d.act0 = s_in; d.C0 = 64; d.taps0 = 9;
       d.weight = W8(in_conv_.w_off); d.cout_pad = in_conv_.cout_pad; d.cout = in_conv_.cout; d.bias = Wf(in_conv_.b_off);
-      if (only16(cur, false)) { d.out = cur.d16; d.out_mode = 1; }
-      else { alloc32(cur); d.out = cur.data; d.out16 = cur.d16; d.out_mode = 0; }
-      d.ldc = cur.C; d.N = N; d.H = SH; d.W = SW;
+      write_to(d, cur);
       add_conv(d, &cur, 9.0 * cfg_.in_channels);
-      add_stats(cur);
       if (create) pl->taps.push_back({"input_blocks.0.0", cur.data, cur.d16, cur.C, cur.H, cur.W});
     }
     std::vector<Act> skips;
@@ -765,6 +720,8 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     auto run_res = [&](const ResBlockDef& r, const Act& x0, const Act* x1) -> Act {
       const int Cin = x0.C + (x1 ? x1->C : 0);
       IVID_REQUIRE(Cin == r.cin, "internal: ResBlock input width mismatch at " + r.pfx);
+      keep32(x0);
+      if (x1) keep32(*x1);
       const int H = x0.H, Wd = x0.W;
       const int Ho = r.mode == 1 ? H * 2 : (r.mode == 2 ? H / 2 : H);
       const int Wo = r.mode == 1 ? Wd * 2 : (r.mode == 2 ? Wd / 2 : Wd);
@@ -773,60 +730,58 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       const bool res_up = identity && r.mode == 1 && x1 == nullptr && conv_can_res_up(Wo, r.cout);
       const bool need_xr = identity && (r.mode != 0 || x1 != nullptr) && !res_up;   // resampled / concatenated identity skip
       // GN1 + SiLU (+ resample) -> a1 ; raw fp16 copy for the 1x1 skip conv ; raw fp32 for resampled identity skip
-      add_coeff(x0, x1, r.gn1, -1);
       GnApplyDesc g1;
       // same-resolution blocks read the fp16 copies their producers wrote (half the GroupNorm read traffic, and the 1x1 skip
       // conv takes them directly as K segments: no raw copy pass)
-      const bool use16 = r.mode == 0 && !need_xr && x0.d16 != nullptr && (x1 == nullptr || x1->d16 != nullptr);
+      const bool use16 = r.mode == 0 && !need_xr && x0.has16 && (x1 == nullptr || x1->has16);
       if (use16) { g1.x0 = x0.d16; g1.x1 = x1 ? x1->d16 : nullptr; g1.x0_half = true; }
       else { g1.x0 = use32(x0); g1.x1 = x1 ? use32(*x1) : nullptr; }
       g1.C0 = x0.C; g1.C1 = x1 ? x1->C : 0;
       g1.N = N; g1.H = H; g1.W = Wd; g1.mode = r.mode; g1.silu = 1;
-      g1.out_act = s_a1; g1.out_raw16 = (r.skip_conv && !use16) ? s_xh : nullptr; g1.out_raw32 = need_xr ? s_xr : nullptr;
       IVID_REQUIRE(!(r.skip_conv && r.mode != 0), "internal: up/down ResBlocks keep the channel count");
-      add_apply(g1);
-      // conv1 -> h (fp32) ; stats
-      bool h_half = false;
-      Act h; h.C = r.cout; h.H = Ho; h.W = Wo; h.data = s_h;
+      void* a1 = s16(kA1, Ho, Wo, r.cin);
+      void* xh = r.skip_conv && !use16 ? s16(kXh, H, Wd, r.cin) : nullptr;
+      float* xr = need_xr ? s32(kXr, Ho, Wo, r.cin) : nullptr;
+      g1.out_act = a1; g1.out_raw16 = xh; g1.out_raw32 = xr;
+      add_gn(g1, x0, x1, r.gn1, -1);
+      // conv1 -> h ; stats.  The hidden tensor only feeds GroupNorm 2: stored as fp16 (half the epilogue and GN traffic);
+      // its statistics are taken from the rounded values in the conv epilogue.  Tiny feature maps keep the fp32 +
+      // stats-kernel path.
+      const bool h_half = conv_can_fuse_stats(Ho, Wo);
+      Act h; h.C = r.cout; h.H = Ho; h.W = Wo;
+      h.data = static_cast<float*>(scratch(kH, static_cast<size_t>(N) * Ho * Wo * r.cout * (h_half ? 2 : 4)));
       h.stats = take_stats(r.cout);
       {
         ConvDesc d;
-        d.act0 = s_a1; d.C0 = r.cin; d.taps0 = 9;
+        d.act0 = a1; d.C0 = r.cin; d.taps0 = 9;
         d.weight = W8(r.conv1.w_off); d.cout_pad = r.conv1.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv1.b_off);
-        // the hidden tensor only feeds GroupNorm 2: stored as fp16 (half the epilogue and GN traffic); its statistics are
-        // taken from the rounded values in the conv epilogue.  Tiny feature maps keep the fp32 + stats-kernel path.
-        h_half = conv_can_fuse_stats(Ho, Wo);
         d.out = h.data; d.ldc = r.cout; d.out_mode = h_half ? 1 : 0; d.N = N; d.H = Ho; d.W = Wo;
         add_conv(d, &h);
-        add_stats(h);
       }
       // GN2 * (1+scale) + shift, SiLU -> a2
-      add_coeff(h, nullptr, r.gn2, r.film_off);
+      void* a2 = s16(kA2, Ho, Wo, r.cout);
       GnApplyDesc g2;
       g2.x0 = h.data; g2.x0_half = h_half; g2.C0 = r.cout; g2.N = N; g2.H = Ho; g2.W = Wo; g2.mode = 0; g2.silu = 1;
-      g2.out_act = s_a2;
-      add_apply(g2);
+      g2.out_act = a2;
+      add_gn(g2, h, nullptr, r.gn2, r.film_off);
       // conv2 (+ 1x1 skip as extra K) + residual -> out
-      Act out = new_act(r.cout, Ho, Wo);
+      Act out = new_act(r.cout, Ho, Wo, !identity);
       {
         ConvDesc d;
-        d.act0 = s_a2; d.C0 = r.cout; d.taps0 = 9;
+        d.act0 = a2; d.C0 = r.cout; d.taps0 = 9;
         if (r.skip_conv && use16) {
           d.act1 = x0.d16; d.C1 = x0.C; d.taps1 = 1;
           if (x1 != nullptr) { d.act2 = x1->d16; d.C2 = x1->C; d.taps2 = 1; }
         } else if (r.skip_conv) {
           // one segment over the raw concat: the packed skip columns (one segment per concat part) only line up when the
           // first part fills whole 64-channel chunks
-          IVID_REQUIRE(!create || r.cat0 % 64 == 0, "internal: raw-copy skip conv over a concat whose first part is not a multiple of 64");
-          d.act1 = s_xh; d.C1 = r.cin; d.taps1 = 1;
+          IVID_REQUIRE(r.cat0 % 64 == 0, "internal: raw-copy skip conv over a concat whose first part is not a multiple of 64");
+          d.act1 = xh; d.C1 = r.cin; d.taps1 = 1;
         }
         d.weight = W8(r.conv2.w_off); d.cout_pad = r.conv2.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv2.b_off);
-        if (identity) { d.residual = need_xr ? s_xr : use32(x0); d.ldr = r.cout; d.residual_up = res_up; }
-        if (only16(out, identity)) { d.out = out.d16; d.out_mode = 1; }
-        else { alloc32(out); d.out = out.data; d.out16 = out.d16; d.out_mode = 0; }
-        d.ldc = r.cout; d.N = N; d.H = Ho; d.W = Wo;
+        if (identity) { d.residual = need_xr ? xr : use32(x0); d.ldr = r.cout; d.residual_up = res_up; }
+        write_to(d, out);
         add_conv(d, &out);
-        add_stats(out);
       }
       if (create) pl->taps.push_back({r.pfx, out.data, out.d16, out.C, out.H, out.W});
       return out;
@@ -834,35 +789,35 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     auto run_attn = [&](const AttnBlockDef& a, const Act& x) -> Act {
       IVID_REQUIRE(x.C == a.C, "internal: attention width mismatch at " + a.pfx);
       const int T = x.H * x.W;
-      add_coeff(x, nullptr, a.gn, -1);
+      void* a1 = s16(kA1, x.H, x.W, a.C);
+      void* qkv = s16(kQkv, x.H, x.W, 3 * a.C);
+      void* a2 = s16(kA2, x.H, x.W, a.C);
       GnApplyDesc g;
-      if (x.d16 != nullptr) { g.x0 = x.d16; g.x0_half = true; } else g.x0 = use32(x);
-      g.C0 = a.C; g.N = N; g.H = x.H; g.W = x.W; g.mode = 0; g.silu = 0; g.out_act = s_a1;
-      add_apply(g);
+      if (x.has16) { g.x0 = x.d16; g.x0_half = true; } else g.x0 = use32(x);
+      g.C0 = a.C; g.N = N; g.H = x.H; g.W = x.W; g.mode = 0; g.silu = 0; g.out_act = a1;
+      add_gn(g, x, nullptr, a.gn, -1);
       {
         ConvDesc d;
-        d.act0 = s_a1; d.C0 = a.C; d.taps0 = 1;
+        d.act0 = a1; d.C0 = a.C; d.taps0 = 1;
         d.weight = W8(a.qkv.w_off); d.cout_pad = a.qkv.cout_pad; d.cout = 3 * a.C; d.bias = Wf(a.qkv.b_off);
-        d.out = s_qkv; d.ldc = 3 * a.C; d.out_mode = 1; d.N = N; d.H = x.H; d.W = x.W;
+        d.out = qkv; d.ldc = 3 * a.C; d.out_mode = 1; d.N = N; d.H = x.H; d.W = x.W;
         add_conv(d);
       }
       if (create) {
-        AttnLaunch* l = attn_launch_create(s_qkv, N, T, a.C, a.head_ch, s_a2);
+        AttnLaunch* l = attn_launch_create(qkv, N, T, a.C, a.head_ch, a2);
         pl->attns.push_back(l);
-        pl->ops.tag("attention", 4.0 * N * static_cast<double>(T) * T * a.C, static_cast<double>(N) * T * a.C * 8,
-                    "T=" + std::to_string(T) + " heads=" + std::to_string(a.C / a.head_ch) + " d=" + std::to_string(a.head_ch));
-        pl->ops.push_back([l](cudaStream_t s) { attn_launch_run(l, s); });
+        pl->add_op("attention", 4.0 * N * static_cast<double>(T) * T * a.C, static_cast<double>(N) * T * a.C * 8,
+                   "T=" + std::to_string(T) + " heads=" + std::to_string(a.C / a.head_ch) + " d=" + std::to_string(a.head_ch),
+                   [l](cudaStream_t s) { attn_launch_run(l, s); });
       }
-      Act out = new_act(a.C, x.H, x.W);
+      Act out = new_act(a.C, x.H, x.W, false);
       {
         ConvDesc d;
-        d.act0 = s_a2; d.C0 = a.C; d.taps0 = 1;
+        d.act0 = a2; d.C0 = a.C; d.taps0 = 1;
         d.weight = W8(a.proj.w_off); d.cout_pad = a.proj.cout_pad; d.cout = a.C; d.bias = Wf(a.proj.b_off);
         d.residual = use32(x); d.ldr = a.C;
-        alloc32(out);
-        d.out = out.data; d.out16 = out.d16; d.ldc = a.C; d.out_mode = 0; d.N = N; d.H = x.H; d.W = x.W;
+        write_to(d, out);
         add_conv(d, &out);
-        add_stats(out);
       }
       if (create) pl->taps.push_back({a.pfx, out.data, out.d16, out.C, out.H, out.W});
       return out;
@@ -872,40 +827,36 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     auto run_resample = [&](const ResampleDef& r, const Act& x) -> Act {
       IVID_REQUIRE(x.C == r.C, "internal: resampling layer width mismatch at " + r.pfx);
       const int Ho = r.mode == 1 ? x.H * 2 : x.H / 2, Wo = r.mode == 1 ? x.W * 2 : x.W / 2;
-      Act out = new_act(r.C, Ho, Wo);
-      alloc32(out);
+      Act out = new_act(r.C, Ho, Wo, false);
+      const int H = x.H, Wd = x.W, C = r.C;
       if (r.conv) {
-        IVID_REQUIRE(!create || x.d16 != nullptr, "internal: resampling conv needs the fp16 copy of its input");
+        IVID_REQUIRE(x.has16, "internal: resampling conv needs the fp16 copy of its input");
         const void* x16 = x.d16;
-        const int H = x.H, Wd = x.W, C = r.C;
         ConvDesc d;
         if (r.mode == 2) {
-          if (create) {
-            pl->ops.tag("resample", 0, static_cast<double>(N) * Ho * Wo * 9 * C * 4, "im2col s2 " + std::to_string(H) + "x" + std::to_string(Wd) + " C" + std::to_string(C));
-            pl->ops.push_back([=](cudaStream_t s) { launch_im2col_s2(x16, s_col, N, H, Wd, C, s); });
-          }
-          d.act0 = s_col; d.C0 = 9 * C; d.taps0 = 1;
+          void* col = s16(kCol, Ho, Wo, 9 * C);           // im2col operand of the stride-2 Downsample2d conv
+          if (create)
+            pl->add_op("resample", 0, static_cast<double>(N) * Ho * Wo * 9 * C * 4, "im2col s2 " + std::to_string(H) + "x" + std::to_string(Wd) + " C" + std::to_string(C),
+                       [=](cudaStream_t s) { launch_im2col_s2(x16, col, N, H, Wd, C, s); });
+          d.act0 = col; d.C0 = 9 * C; d.taps0 = 1;
         } else {
-          if (create) {
-            pl->ops.tag("resample", 0, static_cast<double>(N) * Ho * Wo * C * 2.5, "nearest 2x " + std::to_string(H) + "x" + std::to_string(Wd) + " C" + std::to_string(C));
-            pl->ops.push_back([=](cudaStream_t s) { launch_upsample2x_h16(x16, s_a1, N, H, Wd, C, s); });
-          }
-          d.act0 = s_a1; d.C0 = C; d.taps0 = 9;
+          void* up = s16(kA1, Ho, Wo, C);
+          if (create)
+            pl->add_op("resample", 0, static_cast<double>(N) * Ho * Wo * C * 2.5, "nearest 2x " + std::to_string(H) + "x" + std::to_string(Wd) + " C" + std::to_string(C),
+                       [=](cudaStream_t s) { launch_upsample2x_h16(x16, up, N, H, Wd, C, s); });
+          d.act0 = up; d.C0 = C; d.taps0 = 9;
         }
         d.weight = W8(r.w.w_off); d.cout_pad = r.w.cout_pad; d.cout = C; d.bias = Wf(r.w.b_off);
-        d.out = out.data; d.out16 = out.d16; d.out_mode = 0; d.ldc = C; d.N = N; d.H = Ho; d.W = Wo;
+        write_to(d, out);
         add_conv(d, &out, 9.0 * C);
-        add_stats(out);
       } else {
         const float* src = use32(x);
         if (create) {
-          float* dst = out.data; void* dst16 = out.d16;
-          const int H = x.H, Wd = x.W, C = r.C, mode = r.mode;
-          pl->ops.tag("resample", 0, static_cast<double>(N) * (H * Wd + Ho * Wo * 1.5) * C * 4, (mode == 1 ? "nearest 2x f32 " : "avgpool f32 ") + std::to_string(H) + "x" + std::to_string(Wd));
-          pl->ops.push_back([=](cudaStream_t s) { launch_resample_f32(src, dst, dst16, N, H, Wd, C, mode, s); });
-          double* st = stats_ptr(out);
-          pl->ops.tag("gn_stats", 0, static_cast<double>(N) * Ho * Wo * C * 4);
-          pl->ops.push_back([=](cudaStream_t s) { launch_gn_stats(dst, st, N, Ho * Wo, C, s); });
+          float* dst = out.data; void* dst16 = out.d16; double* st = out.stats;
+          const int mode = r.mode;
+          pl->add_op("resample", 0, static_cast<double>(N) * (H * Wd + Ho * Wo * 1.5) * C * 4, (mode == 1 ? "nearest 2x f32 " : "avgpool f32 ") + std::to_string(H) + "x" + std::to_string(Wd),
+                     [=](cudaStream_t s) { launch_resample_f32(src, dst, dst16, N, H, Wd, C, mode, s); });
+          pl->add_op("gn_stats", 0, static_cast<double>(N) * Ho * Wo * C * 4, "", [=](cudaStream_t s) { launch_gn_stats(dst, st, N, Ho * Wo, C, s); });
         }
       }
       if (create) pl->taps.push_back({r.pfx, out.data, out.d16, out.C, out.H, out.W});
@@ -916,18 +867,18 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       const BlockDef& b = blocks_[bi];
       bool first = true;
       for (const auto& l : b.layers) {
-        if (l.kind == 1) {
-          if (b.is_output && first) {
-            Act sk = skips.back();
-            skips.pop_back();
-            cur = run_res(res_[l.idx], cur, &sk);
-          } else {
-            cur = run_res(res_[l.idx], cur, nullptr);
-          }
-        } else if (l.kind == 3) {
-          cur = run_resample(resample_[l.idx], cur);
-        } else {
-          cur = run_attn(attn_[l.idx], cur);
+        switch (l.kind) {
+          case LayerKind::kResBlock:
+            if (b.is_output && first) {
+              Act sk = skips.back();
+              skips.pop_back();
+              cur = run_res(res_[l.idx], cur, &sk);
+            } else {
+              cur = run_res(res_[l.idx], cur, nullptr);
+            }
+            break;
+          case LayerKind::kAttention: cur = run_attn(attn_[l.idx], cur); break;
+          case LayerKind::kResample: cur = run_resample(resample_[l.idx], cur); break;
         }
         first = false;
       }
@@ -936,58 +887,69 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     IVID_REQUIRE(skips.empty(), "internal: skip stack not consumed");
 
     // ---- output head: GN + SiLU + conv3x3 -> eps (fp32 NCHW) ----
-    add_coeff(cur, nullptr, out_gn_, -1);
+    keep32(cur);
+    const bool split_head = out_split_ && cur.has16;
+    void* a1 = s16(kA1, SH, SW, cur.C);
+    void* a2 = split_head ? s16(kA2, SH, SW, cur.C) : nullptr;
     GnApplyDesc go;
-    const bool split_head = out_split_ && cur.d16 != nullptr;
-    if (cur.d16 != nullptr) { go.x0 = cur.d16; go.x0_half = true; } else go.x0 = use32(cur);
-    go.C0 = cur.C; go.N = N; go.H = SH; go.W = SW; go.mode = 0; go.silu = 1; go.out_act = s_a1;
-    if (split_head) go.out_lo = s_a2;
-    add_apply(go);
+    if (cur.has16) { go.x0 = cur.d16; go.x0_half = true; } else go.x0 = use32(cur);
+    go.C0 = cur.C; go.N = N; go.H = SH; go.W = SW; go.mode = 0; go.silu = 1; go.out_act = a1; go.out_lo = a2;
+    add_gn(go, cur, nullptr, out_gn_, -1);
     if (split_head) {
       // 1x1 GEMM over 9*Co tap columns on [a_hi | a_lo | a_hi] x [Wh | Wh | Wl], then shift-and-add + bias (eps_gather_kernel):
       // each activation element is read once instead of nine times, and the product carries ~21 mantissa bits
+      float* Y = s32(kH, SH, SW, 64);
       ConvDesc d;
-      d.act0 = s_a1; d.C0 = cur.C; d.taps0 = 1;
-      d.act1 = s_a2; d.C1 = cur.C; d.taps1 = 1;
-      d.act2 = s_a1; d.C2 = cur.C; d.taps2 = 1;
+      d.act0 = a1; d.C0 = cur.C; d.taps0 = 1;
+      d.act1 = a2; d.C1 = cur.C; d.taps1 = 1;
+      d.act2 = a1; d.C2 = cur.C; d.taps2 = 1;
       d.weight = W8(out1x1_.w_off); d.cout_pad = 64; d.cout = 64; d.bias = Wf(out1x1_.b_off);
-      d.out = s_h; d.ldc = 64; d.out_mode = 0; d.N = N; d.H = SH; d.W = SW;
+      d.out = Y; d.ldc = 64; d.out_mode = 0; d.N = N; d.H = SH; d.W = SW;
       add_conv(d, nullptr, 9.0 * cur.C, static_cast<double>(cfg_.out_channels));
       if (create) {
-        const float* Y = s_h; const float* ob = Wf(out_conv_.b_off);
+        const float* ob = Wf(out_conv_.b_off);
         const int Co = cfg_.out_channels;
-        pl->ops.tag("eps_gather", 0, static_cast<double>(N) * SH * SW * (9.0 * Co * 4 + Co * 4));
-        pl->ops.push_back([=](cudaStream_t s) {
+        pl->add_op("eps_gather", 0, static_cast<double>(N) * SH * SW * (9.0 * Co * 4 + Co * 4), "", [=](cudaStream_t s) {
           if (pl->hook != nullptr) pl->hook->launch(Y, ob, N, SH, SW, Co, 64, s);
           else launch_eps_gather(Y, ob, pl->eps, N, SH, SW, Co, 64, s);
         });
       }
     } else if (create) {
       ConvDesc d;
-      d.act0 = s_a1; d.C0 = cur.C; d.taps0 = 9;
+      d.act0 = a1; d.C0 = cur.C; d.taps0 = 9;
       d.weight = W8(out_conv_.w_off); d.cout_pad = out_conv_.cout_pad; d.cout = cfg_.out_channels; d.bias = Wf(out_conv_.b_off);
       d.out = nullptr; d.ldc = 0; d.out_mode = 2; d.N = N; d.H = SH; d.W = SW;
       ConvLaunch* l = conv_launch_create(d);
       pl->convs.push_back(l);
       // eps pointer is a per-call input: patched through the plan at run time
-      pl->ops.tag("conv_gemm<16>", 2.0 * N * SH * SW * 9.0 * cur.C * cfg_.out_channels,
-                  static_cast<double>(N) * SH * SW * (cur.C * 2 + cfg_.out_channels * 4));
-      pl->ops.push_back([l, pl](cudaStream_t s) { conv_launch_run_out(l, pl->eps, s); });
+      pl->add_op("conv_gemm<16>", 2.0 * N * SH * SW * 9.0 * cur.C * cfg_.out_channels,
+                 static_cast<double>(N) * SH * SW * (cur.C * 2 + cfg_.out_channels * 4), "",
+                 [l, pl](cudaStream_t s) { conv_launch_run_out(l, pl->eps, s); });
     }
-    if (create) {
-      pl->stats_base = reinterpret_cast<double*>(stats_base);
-      pl->stats_bytes = soff;
-      IVID_REQUIRE(soff <= stats_cap, "internal: statistics arena overflow");
-    }
-    return bump.off;
+    if (!create) stats_bytes = soff;
   };
 
-  layout(nullptr, false);
-  collect = false;
-  const size_t total = layout(nullptr, false);
+  walk(nullptr);
+  // layout: statistics, scratch slots, then block outputs in creation order, each 1024-byte aligned
+  size_t total = 0;
+  auto place = [&](size_t bytes) {
+    const size_t off = (total + 1023) & ~size_t(1023);
+    total = off + bytes;
+    return off;
+  };
+  stats_off = place(stats_bytes);
+  for (int s = 0; s < kSlots; ++s) slot_off[s] = place(slot_bytes[s]);
+  for (auto& o : outs) {
+    const size_t n = static_cast<size_t>(N) * o.H * o.W * o.C;
+    if (conv_can_out16(o.C)) o.off16 = place(n * 2);
+    o.only16 = o.may16 && !o.need32;
+    if (!o.only16) o.off32 = place(n * 4);
+  }
   IVID_CHECK_CUDA(cudaMalloc(&pl->ws, total + 4096));
   pl->ws_bytes = total;
-  layout(pl->ws, true);
+  pl->stats_base = reinterpret_cast<double*>(pl->ws + stats_off);
+  pl->stats_bytes = stats_bytes;
+  walk(pl->ws);
   return plan.release();
 }
 
@@ -1037,8 +999,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
       // hands fresh buffers to every call (e.g. a Python loop that keeps every x_{t-1}): replay the launches on the stream
       const bool thrash = pl->graph_captures >= 32 && pl->graph_hits < pl->graph_captures;
       if (thrash) {
-        IVID_CHECK_CUDA(cudaMemsetAsync(pl->stats_base, 0, pl->stats_bytes, stream));
-        for (auto& op : pl->ops.v) op.fn(stream);
+        pl->run(stream);
         return;
       }
       ++pl->graph_captures;
@@ -1046,8 +1007,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
       cudaGraph_t graph = nullptr;
       IVID_CHECK_CUDA(cudaStreamBeginCapture(cap_stream_, cudaStreamCaptureModeRelaxed));
       try {
-        IVID_CHECK_CUDA(cudaMemsetAsync(pl->stats_base, 0, pl->stats_bytes, cap_stream_));
-        for (auto& op : pl->ops.v) op.fn(cap_stream_);
+        pl->run(cap_stream_);
       } catch (...) {
         cudaStreamEndCapture(cap_stream_, &graph);
         if (graph) cudaGraphDestroy(graph);
@@ -1070,29 +1030,23 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
       IVID_CHECK_CUDA(cudaGraphLaunch(exec, stream));
       return;
     }
-    IVID_CHECK_CUDA(cudaMemsetAsync(pl->stats_base, 0, pl->stats_bytes, stream));
-    for (auto& op : pl->ops.v) op.fn(stream);
+    pl->run(stream);
     return;
   }
-  IVID_CHECK_CUDA(cudaMemsetAsync(pl->stats_base, 0, pl->stats_bytes, stream));
   // profiling pass: every launch bracketed by CUDA events on the launching stream (serialised; shares, not absolutes)
-  std::vector<cudaEvent_t> ev(pl->ops.v.size() + 1);
+  std::vector<cudaEvent_t> ev(pl->ops.size() + 1);
   for (auto& e : ev) IVID_CHECK_CUDA(cudaEventCreate(&e));
-  IVID_CHECK_CUDA(cudaEventRecord(ev[0], stream));
-  for (size_t i = 0; i < pl->ops.v.size(); ++i) {
-    pl->ops.v[i].fn(stream);
-    IVID_CHECK_CUDA(cudaEventRecord(ev[i + 1], stream));
-  }
+  pl->run(stream, ev.data());
   IVID_CHECK_CUDA(cudaStreamSynchronize(stream));
-  for (size_t i = 0; i < pl->ops.v.size(); ++i) {
+  for (size_t i = 0; i < pl->ops.size(); ++i) {
+    const Plan::OpRec& op = pl->ops[i];
     float ms = 0.f;
     IVID_CHECK_CUDA(cudaEventElapsedTime(&ms, ev[i], ev[i + 1]));
-    auto& agg = profile_acc_[pl->ops.v[i].label];
-    agg.launches += 1; agg.ms += ms; agg.flops += pl->ops.v[i].flops; agg.bytes += pl->ops.v[i].bytes;
-    if (!pl->ops.v[i].note.empty()) {
+    auto& agg = profile_acc_[op.label];
+    agg.launches += 1; agg.ms += ms; agg.flops += op.flops; agg.bytes += op.bytes;
+    if (!op.note.empty()) {
       char buf[256];
-      snprintf(buf, sizeof(buf), "[\"%s\", \"%s\", %.5f, %.4e, %.4e]", pl->ops.v[i].label, pl->ops.v[i].note.c_str(), ms, pl->ops.v[i].flops,
-               pl->ops.v[i].bytes);
+      snprintf(buf, sizeof(buf), "[\"%s\", \"%s\", %.5f, %.4e, %.4e]", op.label, op.note.c_str(), ms, op.flops, op.bytes);
       if (!profile_ops_.empty()) profile_ops_ += ", ";
       profile_ops_ += buf;
     }

@@ -67,7 +67,8 @@ struct ResampleDef {       // plain Downsample2d / Upsample2d layer (resblock_up
   bool conv = false;       // conv_resample
   ConvW w;                 // op / conv weights, packed as an ordinary 3x3 conv
 };
-struct LayerRef { int kind; int idx; };   // kind 1 = ResBlock, 2 = AttentionBlock, 3 = plain resampling layer
+enum class LayerKind { kResBlock, kAttention, kResample };   // kResample: plain Downsample2d / Upsample2d layer
+struct LayerRef { LayerKind kind; int idx; };                 // idx into res_, attn_ or resample_
 struct BlockDef { std::vector<LayerRef> layers; bool is_input = false; bool is_output = false; };
 
 struct Plan;

@@ -7,6 +7,8 @@ int(channel_mult[i] * model_channels) channels (adm.py:367,385,454) and only nee
     mc32      model_channels=32, channel_mult=[1,2,4], attention at 8            GroupNorm groups of one channel
     frac      model_channels=64, channel_mult=[1,1.5,2], attention at 8          widths 64, 96, 128
     g8        num_groups=8, model_channels=40, channel_mult=[1,2,3.2], none       widths 40, 80, 128 (groups of 5 and 10)
+    narrow8   num_groups=8, model_channels=8, channel_mult=[1,2,8], none          widths 8, 16, 64: the output head runs at
+              final width 8, and no full-resolution ResBlock reaches 64 channels
     legacy96  mc96 with use_scale_shift_norm=False, resblock_updown=False         stride-2 conv (im2col) and upsample conv
     inpaint96 InpaintCFG.model_inference at mc96 with in_channels=10, classes, strength 0.5, injected hole noise
     g4_20     num_groups=4, model_channels=20, channel_mult=[1,3.2]              widths 20, 64, 84, 40: the reference runs it,
@@ -32,6 +34,7 @@ UNET_CASES = (("mc96", MC96),
               ("mc32", dict(model_channels=32, channel_mult=[1, 2, 4], attention_resolutions=[8])),
               ("frac", dict(model_channels=64, channel_mult=[1, 1.5, 2], attention_resolutions=[8])),
               ("g8", dict(num_groups=8, model_channels=40, channel_mult=[1, 2, 3.2], attention_resolutions=[])),
+              ("narrow8", dict(num_groups=8, model_channels=8, channel_mult=[1, 2, 8], attention_resolutions=[])),
               ("legacy96", dict(MC96, use_scale_shift_norm=False, resblock_updown=False)))
 INPAINT = dict(MC96, in_channels=10)
 G4_20 = dict(num_groups=4, model_channels=20, channel_mult=[1, 3.2], attention_resolutions=[])

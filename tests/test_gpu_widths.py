@@ -24,7 +24,7 @@ pytestmark = pytest.mark.gpu
 NORTH_STAR = 1e-3
 HARD_CAP = 1.6e-3
 STEP_TOL = 1e-3
-UNET_TAGS = ["mc96", "mc32", "frac", "g8", "legacy96"]
+UNET_TAGS = ["mc96", "mc32", "frac", "g8", "narrow8", "legacy96"]
 STRENGTH = 0.5
 WIDTHS = [8, 24, 32, 40, 96, 160, 288]
 

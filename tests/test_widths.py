@@ -14,7 +14,7 @@ import ivid_b200.backbones as backbones
 from ivid_b200 import _lib
 from oracle import sampler_ref, unet_ref
 
-UNET_TAGS = ["mc96", "mc32", "frac", "g8", "legacy96"]
+UNET_TAGS = ["mc96", "mc32", "frac", "g8", "narrow8", "legacy96"]
 STRENGTH = 0.5
 
 
