@@ -17,10 +17,12 @@
 // Both operands land in shared memory in the 128-byte-swizzled K-major layout that wgmma reads directly.
 //
 // Every CTA computes one 128-pixel x BN output tile.  Block b takes pixel tile b / n_blocks and column block b % n_blocks, so
-// the CTAs that share an activation tile run together.  Two warpgroups per CTA (rows 0-63 / 64-127 of the tile),
-// accumulators in registers.  Thread 0 also drives the TMA ring: STAGES k-blocks are in flight, a slot is refilled as soon
-// as all eight warps have retired the wgmma group that read it.  Two CTAs fit one SM (BN <= 128), so one CTA's epilogue
-// overlaps the other's main loop.
+// the CTAs that share an activation tile run together.  Two consumer warpgroups per CTA (rows 0-63 / 64-127 of the tile),
+// accumulators in registers, and one producer warp (warp 8) whose elected lane drives the TMA ring: it runs STAGES k-blocks
+// ahead and refills a slot as soon as all eight consumer warps have released it.  A consumer keeps one wgmma group in
+// flight: it issues the group of k-block u, waits for group u - 1 to retire and only then releases u - 1's slot, so its
+// tensor work never stops for a refill.  Two CTAs fit one SM (BN <= 128), so one CTA's epilogue overlaps the other's main
+// loop.
 // The epilogue works on the accumulator fragments in place: bias, residual (optionally through a nearest-2x upsample),
 // fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.
 #pragma once
@@ -65,7 +67,8 @@ struct ConvGemmCfg {
   static constexpr int BAR_BYTES = 128;
   static constexpr int STAT_BYTES = 8 * 2 * BN * 4;            // [8 warps][sum|sumsq][BN] fp32
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + STAT_BYTES + 1024;   // +1024 alignment slack
-  static constexpr int THREADS = 256;
+  static constexpr int CONSUMER_THREADS = 256;                 // two warpgroups: MMA and epilogue
+  static constexpr int THREADS = CONSUMER_THREADS + 32;        // + one producer warp: TMA loads
 };
 
 // position in the K loop: segment, tap, 64-channel chunk, and the first packed weight column of the segment
@@ -76,7 +79,7 @@ struct ConvKCursor {
 // p is read in place (__grid_constant__): the K cursor indexes seg_chunks / seg_taps at run time, and without it the compiler
 // may copy the whole struct to a local-memory stack frame to do so.
 template <int BN>
-__global__ void __launch_bounds__(256, 2)
+__global__ void __launch_bounds__(ConvGemmCfg<BN>::THREADS, 2)
 conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ ConvGemmParams p) {
   using Cfg = ConvGemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
@@ -89,14 +92,12 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
-  const int wg = warp >> 2;                      // warpgroup: tile rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2;                      // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
 
   if (tid == 0) {
-    tma_prefetch_desc(&maps.a[0]);
-    tma_prefetch_desc(&maps.b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8u);              // one arrive per warp
+      mbar_init(&empty_bar[s], 8u);              // one arrive per consumer warp
     }
     fence_barrier_init();
   }
@@ -104,15 +105,6 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
 
   int nunits = 0;                                // K blocks of the tile
   for (int sg = 0; sg < 3; ++sg) nunits += p.seg_chunks[sg] * p.seg_taps[sg];
-  auto advance = [&](ConvKCursor& c) {           // tap slow, chunk fast
-    const int taps = p.seg_taps[c.seg], chunks = p.seg_chunks[c.seg];
-    if (++c.ch == chunks) { c.ch = 0; if (++c.t == taps) { c.t = 0; c.base += taps * chunks * 64; ++c.seg; } }
-    while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
-  };
-
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
   // column block fast: the CTAs that share an activation tile run together
   const int mt = static_cast<int>(blockIdx.x) / p.n_blocks, nb = static_cast<int>(blockIdx.x) % p.n_blocks;
@@ -124,29 +116,39 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
   const int tw = rem - th * p.tiles_w;
   const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
 
-  // producer (thread 0): units are issued strictly in order
-  ConvKCursor pc;
-  while (p.seg_chunks[pc.seg] == 0) ++pc.seg;
-  auto issue_load = [&](int u) {
-    const uint32_t g = static_cast<uint32_t>(u);
-    const int s = static_cast<int>(g % STAGES);
-    if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
-    const int taps = p.seg_taps[pc.seg], chunks = p.seg_chunks[pc.seg];
-    uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
-    uint8_t* sb = sa + Cfg::A_BYTES;
-    const int dy = (taps == 9) ? (pc.t / 3 - 1) : 0;
-    const int dx = (taps == 9) ? (pc.t % 3 - 1) : 0;
-    const int kcol = pc.base + (pc.t * chunks + pc.ch) * 64;
-    mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
-    tma_load_4d(&maps.a[pc.seg], &full_bar[s], sa, pc.ch * 64, w0 + dx, h0 + dy, n0);
-    tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
-    advance(pc);
-  };
-  if (tid == 0) {
-    for (int u = 0; u < STAGES && u < nunits; ++u) issue_load(u);
+  // ===================================== producer warp =====================================
+  if (warp == Cfg::CONSUMER_THREADS / 32) {
+    if (lane == 0) {
+      tma_prefetch_desc(&maps.a[0]);
+      tma_prefetch_desc(&maps.b);
+      ConvKCursor c;                             // units are issued strictly in order: segment, tap slow, chunk fast
+      while (p.seg_chunks[c.seg] == 0) ++c.seg;
+#pragma unroll 1
+      for (int u = 0; u < nunits; ++u) {
+        const uint32_t g = static_cast<uint32_t>(u);
+        const int s = static_cast<int>(g % STAGES);
+        if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
+        const int taps = p.seg_taps[c.seg], chunks = p.seg_chunks[c.seg];
+        uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
+        uint8_t* sb = sa + Cfg::A_BYTES;
+        const int dy = (taps == 9) ? (c.t / 3 - 1) : 0;
+        const int dx = (taps == 9) ? (c.t % 3 - 1) : 0;
+        const int kcol = c.base + (c.t * chunks + c.ch) * 64;
+        mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
+        tma_load_4d(&maps.a[c.seg], &full_bar[s], sa, c.ch * 64, w0 + dx, h0 + dy, n0);
+        tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
+        if (++c.ch == chunks) { c.ch = 0; if (++c.t == taps) { c.t = 0; c.base += taps * chunks * 64; ++c.seg; } }
+        while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
+      }
+    }
+    return;                                      // the consumers' barriers below count 256 threads
   }
 
   // ===================================== main loop =====================================
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+
 #pragma unroll 1
   for (int u = 0; u < nunits; ++u) {
     const uint32_t g = static_cast<uint32_t>(u);
@@ -160,28 +162,28 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
 #pragma unroll
     for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
     wgmma_commit();
-    // retired before the slot is released: a wgmma group still in flight across thread 0's refill branch would make ptxas
-    // serialise every wgmma; the other warpgroups on the SM keep the tensor cores busy meanwhile
-    wgmma_wait<0>();
-    reg_fence(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[s]);
-    if (tid == 0 && u + STAGES < nunits) issue_load(u + STAGES);
+    // group u stays in flight; group u - 1 has retired, so its slot goes back to the producer
+    wgmma_wait<1>();
+    if (u > 0 && lane == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
   }
+  wgmma_wait<0>();
+  reg_fence(acc);
+  if (lane == 0) mbar_arrive(&empty_bar[static_cast<uint32_t>(nunits - 1) % STAGES]);
 
   // ===================================== epilogue =====================================
   const int wr = warp & 3;
   const int quad = lane & 3;
-  int pn[2], ph[2], pw[2];
+  // 32-bit pixel indices (conv_launch_create requires N*H*W < 2^31): with the producer warp in the CTA, two CTAs per SM
+  // leave 96 registers per thread, and the 64 accumulators plus 64-bit row coordinates would spill
+  uint32_t pix[2], rpix[2];                      // output pixel, residual pixel (the 2x-upsample source under res_up)
   bool ok[2];
-  size_t pix[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
     const int n = n0 + row / (p.TW * p.TH), h = h0 + (row / p.TW) % p.TH, x = w0 + row % p.TW;
     ok[i] = n < p.N;                             // rows of the batch tail (TMA zero fill) are not written
-    pix[i] = (static_cast<size_t>(n) * p.H + h) * p.W + x;
-    pn[i] = n; ph[i] = h; pw[i] = x;
+    pix[i] = (static_cast<uint32_t>(n) * p.H + h) * p.W + x;
+    rpix[i] = p.res_up ? (static_cast<uint32_t>(n) * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (x >> 1) : pix[i];
   }
   const bool do_stats = p.stats != nullptr;
 #pragma unroll
@@ -195,22 +197,22 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
         if (!ok[i]) continue;
         float v0 = acc[4 * j + 2 * i] + b.x, v1 = acc[4 * j + 2 * i + 1] + b.y;
         if (p.out_mode == 2) {
-          float* o = reinterpret_cast<float*>(p.out);
-          o[((static_cast<size_t>(pn[i]) * p.Cout + c) * p.H + ph[i]) * p.W + pw[i]] = v0;
-          if (c + 1 < p.Cout) o[((static_cast<size_t>(pn[i]) * p.Cout + c + 1) * p.H + ph[i]) * p.W + pw[i]] = v1;
+          const uint32_t hw = static_cast<uint32_t>(p.H) * p.W, n = pix[i] / hw;
+          float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(n) * p.Cout + c) * hw + (pix[i] - n * hw);
+          o[0] = v0;
+          if (c + 1 < p.Cout) o[hw] = v1;
           continue;
         }
         if (p.residual != nullptr) {
-          const size_t rpix = p.res_up ? (static_cast<size_t>(pn[i]) * (p.H >> 1) + (ph[i] >> 1)) * (p.W >> 1) + (pw[i] >> 1) : pix[i];
-          const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + rpix * p.ldr + c));
+          const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + static_cast<size_t>(rpix[i]) * p.ldr + c));
           v0 += r.x; v1 += r.y;
         }
         if (p.out_mode == 0) {
-          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix[i] * p.ldc + c) = make_float2(v0, v1);
-          if (p.out16 != nullptr) *reinterpret_cast<uint32_t*>(p.out16 + pix[i] * p.ldc + c) = pack_h2(v0, v1);
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + static_cast<size_t>(pix[i]) * p.ldc + c) = make_float2(v0, v1);
+          if (p.out16 != nullptr) *reinterpret_cast<uint32_t*>(p.out16 + static_cast<size_t>(pix[i]) * p.ldc + c) = pack_h2(v0, v1);
         } else {
           const __half2 hv = __floats2half2_rn(v0, v1);
-          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + pix[i] * p.ldc + c) = hv;
+          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + static_cast<size_t>(pix[i]) * p.ldc + c) = hv;
           const float2 r = __half22float2(hv);
           v0 = r.x; v1 = r.y;
         }
@@ -235,11 +237,12 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
   }
   if (do_stats) {
     // a warp's 16 rows belong to one sample (TW*TH >= 32); the warps of each sample are combined in a fixed order, so the
-    // statistics are reproducible bit for bit, and one fp64 atomic pair per (sample, channel) and tile goes to global memory
-    __syncthreads();
+    // statistics are reproducible bit for bit, and one fp64 atomic pair per (sample, channel) and tile goes to global memory.
+    // Named barrier 1 over the consumer warps only: the producer warp has exited.
+    asm volatile("bar.sync 1, %0;\n" ::"n"(Cfg::CONSUMER_THREADS) : "memory");
     const int rows_per_n = p.TW * p.TH;
     const int n_tile = (128 + rows_per_n - 1) / rows_per_n;
-    for (int e = tid; e < n_tile * BN; e += Cfg::THREADS) {
+    for (int e = tid; e < n_tile * BN; e += Cfg::CONSUMER_THREADS) {
       const int sn = e / BN, c = e - sn * BN;
       const int n = n0 + sn, col = colbase + c;
       if (n >= p.N || col >= p.Cout) continue;

@@ -66,6 +66,8 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.taps0 == 9 || d.taps0 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.taps1 == 9 || d.taps1 == 1, "conv: only 3x3 (pad 1) and 1x1 kernels are on this path");
   IVID_REQUIRE(d.C2 % 8 == 0 && (d.taps2 == 9 || d.taps2 == 1), "conv: segment 2 must be a multiple of 8 channels, 3x3 or 1x1");
+  IVID_REQUIRE(d.N > 0 && static_cast<int64_t>(d.N) * d.H * d.W < (int64_t{1} << 31),
+               "conv: N*H*W must be below 2^31 (32-bit pixel indices in the epilogue)");
   auto* l = new ConvLaunch();
   ConvGemmParams& p = l->p;
   p.N = d.N; p.H = d.H; p.W = d.W;
