@@ -54,6 +54,9 @@ class StepArgsT(Structure):
         ("seed", c_uint64),
         ("height", c_int),            # sample size; 0 = the backbone's image_size
         ("width", c_int),
+        ("order", c_int),             # kind 2 (DPM-Solver++): 1 or 2 (0 = 2)
+        ("prev_x0_dev", c_void_p),    # kind 2, single step: the previous step's pred_x0 (NULL = first order)
+        ("t_last", c_int),            # kind 2, single step: the previous step's t
     ]
 
 

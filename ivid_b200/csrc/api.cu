@@ -181,7 +181,7 @@ int ivid_sampler_step_dev(ivid_sampler_t* s, ivid_unet_t* unet, const float* x_t
                           int N, const int64_t* t_dev, const int64_t* t_prev_dev, const ivid_step_args_t* args, void* stream) {
   return guarded([&] {
     IVID_NOT_NULL(s); IVID_NOT_NULL(unet); IVID_NOT_NULL(x_t_dev); IVID_NOT_NULL(x_prev_dev); IVID_NOT_NULL(args); IVID_NOT_NULL(t_dev);
-    IVID_REQUIRE(args->kind != 1 || t_prev_dev != nullptr, "DDIM step needs t_prev");
+    IVID_REQUIRE(args->kind == 0 || t_prev_dev != nullptr, "DDIM / DPM-Solver++ step needs t_prev");
     s->impl->step(*unet->impl, x_t_dev, x_prev_dev, pred_x0_dev, N, 0, 0, *args, 0, static_cast<cudaStream_t>(stream), t_dev, t_prev_dev);
   });
 }

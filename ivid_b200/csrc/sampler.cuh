@@ -1,8 +1,10 @@
-// Fused denoising-step kernels: classifier-free-guidance mix + DDPM / DDIM update (+ multiview replace/constrain
-// guidance) in ONE HBM pass over [N,4,H,W], coefficients read from a device-resident table (no per-step H2D).
+// Fused denoising-step kernels: classifier-free-guidance mix + DDPM / DDIM / DPM-Solver++(2M) update (+ multiview
+// replace/constrain guidance) in ONE HBM pass over [N,4,H,W], coefficients read from a device-resident table and step
+// state (no per-step H2D).
 //   reference: ClassifierFreeGuidance.model_inference classifier_free_guidance.py:39-42
 //              DdpmSampler.p_mean_variance / sample_once   samplers/ddpm.py:85-100,127-131
 //              DdimSampler.sample_once                      samplers/ddim.py:81-103
+//              DPM-Solver++(2M), data-prediction multistep  Lu et al. 2022, arXiv:2211.01095 (no reference counterpart)
 //              InpaintCFG.make_cond_inputs                  frameworks/inpaint_cfg.py:33-49
 //              SuperResCFG.make_cond_inputs                 frameworks/sr_cfg.py:31-36
 #pragma once
@@ -60,6 +62,18 @@ struct GuideParams {           // DDIM multiview guidance (all maps fp32 NCHW, n
   float w_convex, w_convex_c;
 };
 
+// Step kinds (template argument of the step kernels; ivid_step_args_t.kind)
+constexpr int kStepDdpm = 0, kStepDdim = 1, kStepDpm = 2;
+
+// DPM-Solver++ per-step scalars, computed in double by the step-state kernel and rounded to fp32 (sampler.cu):
+//   x_p = c_xt * x_t - c_d * D,  D = D0 (order 1) or w0 * D0 + w1 * D_{-1} (order 2)
+struct DpmStep {
+  float c_xt;                  // sigma_p / sigma_s
+  float c_d;                   // alpha_p * (exp(-h) - 1)
+  float w0, w1;                // 1 + 1/(2r), -1/(2r)
+  int order;                   // 1 or 2
+};
+
 struct StepParams {
   const float* x_t;            // [N,C,H,W]
   const float* eps;            // [2N or N,C,H,W]: rows [0,N) conditional, [N,2N) unconditional when cfg
@@ -78,6 +92,9 @@ struct StepParams {
   uint32_t stream;             // Philox stream id (step counter supplied by caller) when noise == nullptr
   const int* stream_dev;       // optional device step counter added to `stream`
   GuideParams g;
+  // DPM-Solver++ only (appended, so the DDPM / DDIM layout is unchanged)
+  const DpmStep* dpm;          // device step state
+  float* hist;                 // [N,C,H,W] D_{-1} on entry (order 2), overwritten in place with this step's D0
 };
 
 // (1 + strength) * eps_c - strength * eps_u (only evaluated with strength > 0).  Every product / sum of the step arithmetic is
@@ -108,17 +125,27 @@ __global__ void __launch_bounds__(256) cfg_mix_kernel(const float* __restrict__ 
 // Per-step scalars derived once per thread from the device-resident step state.
 struct StepScalars {
   StepCoef k;
-  float nz;          // DDPM: t != 0 ; DDIM: t_prev != 0
+  float nz;          // DDPM: t != 0 ; DDIM / DPM: t_prev != 0
   float sd;          // DDPM: exp(0.5 * posterior_log_variance_clipped)
   float sigma, c_x0, c_eps;    // DDIM
+  DpmStep d;                   // DPM-Solver++
   uint32_t stream;
 };
-template <bool kDdim>
+// whether the step draws N(0,1) noise (DPM-Solver++ is deterministic)
+template <int kKind>
+__device__ __forceinline__ bool step_draws_noise(const StepScalars& s) {
+  return kKind == kStepDdpm || (kKind == kStepDdim && s.sigma != 0.0f);
+}
+template <int kKind>
 __device__ __forceinline__ StepScalars step_scalars(const StepParams& p) {
   StepScalars s;
   s.k = p.table[*p.t_index];
   s.stream = p.stream + (p.stream_dev ? static_cast<uint32_t>(*p.stream_dev) : 0u);
-  if (!kDdim) {
+  if (kKind == kStepDpm) {
+    s.nz = (*p.t_prev != 0) ? 1.0f : 0.0f;
+    s.d = *p.dpm;
+    s.sigma = 0.f; s.c_x0 = 0.f; s.c_eps = 0.f; s.sd = 0.f;
+  } else if (kKind == kStepDdpm) {
     s.nz = (*p.t_index != 0) ? 1.0f : 0.0f;
     s.sd = expf(__fmul_rn(0.5f, s.k.post_logvar));
     s.sigma = 0.f; s.c_x0 = 0.f; s.c_eps = 0.f;
@@ -134,17 +161,18 @@ __device__ __forceinline__ StepScalars step_scalars(const StepParams& p) {
   }
   return s;
 }
-// x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, the (already guidance-mixed) eps and the N(0,1) draw z
-template <bool kDdim>
+// x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, the (already guidance-mixed) eps and the N(0,1) draw z.
+// DPM-Solver++: z is unused, dprev is D_{-1} of the element (read only at order 2) and x0o the guided D0.
+template <int kKind>
 __device__ __forceinline__ void step_element(const StepParams& p, const StepScalars& s, int n, int c, size_t pix, float xt, float e, float z,
-                                             float& xo, float& x0o) {
+                                             float dprev, float& xo, float& x0o) {
   const StepCoef& k = s.k;
   auto mul = [](float a, float b) { return __fmul_rn(a, b); };
   auto add = [](float a, float b) { return __fadd_rn(a, b); };
   auto sub = [](float a, float b) { return __fsub_rn(a, b); };
   float x0 = sub(mul(k.sqrt_recip_acp, xt), mul(k.sqrt_recipm1_acp, e));
   if (p.clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
-  if (!kDdim) {
+  if (kKind == kStepDdpm) {
     const float mean = add(mul(k.post_mean_coef1, x0), mul(k.post_mean_coef2, xt));
     xo = add(mean, mul(mul(s.nz, s.sd), z));
     x0o = x0;
@@ -165,6 +193,13 @@ __device__ __forceinline__ void step_element(const StepParams& p, const StepScal
       x0 = add(mul(x0, m), mul(add(mul(p.g.w_convex, fmaxf(x0, cv)), mul(p.g.w_convex_c, x0)), sub(1.0f, m)));
     }
   }
+  if (kKind == kStepDpm) {
+    // D_{-1} is not read at order 1: the history may hold anything (first step of a run)
+    const float d = s.d.order == 2 ? add(mul(s.d.w0, x0), mul(s.d.w1, dprev)) : x0;
+    xo = sub(mul(s.d.c_xt, xt), mul(s.d.c_d, d));
+    x0o = x0;
+    return;
+  }
   const float e2 = __fdiv_rn(sub(mul(k.sqrt_recip_acp, xt), x0), k.sqrt_recipm1_acp);
   const float mean = add(mul(s.c_x0, x0), mul(s.c_eps, e2));
   xo = add(mean, mul(mul(s.nz, s.sigma), z));
@@ -178,30 +213,46 @@ __device__ __forceinline__ void step_noise4(const StepParams& p, const StepScala
   z[0] = t.x; z[1] = t.y; z[2] = t.z; z[3] = t.w;
 }
 
+// DPM-Solver++ history of elements [i, i+4): D_{-1} before the step (only at order 2; every thread reads and then overwrites
+// its own elements, so the buffer is updated in place)
+template <int kKind>
+__device__ __forceinline__ void hist_load4(const StepParams& p, const StepScalars& s, size_t i, float (&h)[4]) {
+  h[0] = h[1] = h[2] = h[3] = 0.f;
+  if (kKind != kStepDpm || s.d.order != 2) return;
+  const float4 t = *reinterpret_cast<const float4*>(p.hist + i);
+  h[0] = t.x; h[1] = t.y; h[2] = t.z; h[3] = t.w;
+}
+template <int kKind>
+__device__ __forceinline__ void hist_store4(const StepParams& p, size_t i, const float (&x0o)[4]) {
+  if (kKind == kStepDpm) stg_f4(p.hist + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
+}
+
 // one thread = 4 consecutive pixels of one (n, c) plane
-template <bool kDdim>
+template <int kKind>
 __global__ void __launch_bounds__(256) step_kernel(const StepParams p) {
   const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
-  const StepScalars s = step_scalars<kDdim>(p);
+  const StepScalars s = step_scalars<kKind>(p);
   for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
        i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const size_t i = i4 * 4;
     const int plane = static_cast<int>(i / p.HW);      // n*C + c
     const int n = plane / p.C, c = plane % p.C;
     const size_t pix = i - static_cast<size_t>(plane) * p.HW;
-    float z[4];
-    step_noise4(p, s, i, !kDdim || s.sigma != 0.0f, z);
+    float z[4], hp[4];
+    step_noise4(p, s, i, step_draws_noise<kKind>(s), z);
+    hist_load4<kKind>(p, s, i, hp);
     float xo[4], x0o[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) step_element<kDdim>(p, s, n, c, pix + j, p.x_t[i + j], mix_eps(p, i + j, total), z[j], xo[j], x0o[j]);
+    for (int j = 0; j < 4; ++j) step_element<kKind>(p, s, n, c, pix + j, p.x_t[i + j], mix_eps(p, i + j, total), z[j], hp[j], xo[j], x0o[j]);
     stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
     if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
+    hist_store4<kKind>(p, i, x0o);
   }
 }
 
 // Output head + denoising step in ONE kernel (the last node of the forward's CUDA graph): eps of both guidance halves is formed
 // from the tap columns Y of the output head's 1x1 GEMM (the shift-and-add of eps_gather_kernel, same summation order), mixed, and
-// pushed through the DDPM / DDIM update without ever being written to HBM.  One thread = 4 consecutive pixels (one row segment)
+// pushed through the DDPM / DDIM / DPM-Solver++ update without ever being written to HBM.  One thread = 4 consecutive pixels (one row segment)
 // of one sample, all Co = 4 channels; noise indices and arithmetic are those of step_kernel, so both routes agree bit for bit.
 struct HeadStepParams {
   StepParams sp;
@@ -221,10 +272,10 @@ __device__ __forceinline__ void head_eps4(const HeadStepParams& h, int n, int y,
 #pragma unroll
   for (int c = 0; c < 4; ++c) e[c] += __ldg(h.bias + c);
 }
-template <bool kDdim>
+template <int kKind>
 __global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) {
   const StepParams& p = h.sp;
-  const StepScalars s = step_scalars<kDdim>(p);
+  const StepScalars s = step_scalars<kKind>(p);
   const int w4 = h.W / 4;
   const size_t groups = static_cast<size_t>(p.N) * h.H * w4;
   for (size_t g = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; g < groups; g += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -252,15 +303,17 @@ __global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) 
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       const size_t i = (static_cast<size_t>(n) * 4 + c) * p.HW + pix;
-      float z[4];
-      step_noise4(p, s, i, !kDdim || s.sigma != 0.0f, z);
+      float z[4], hp[4];
+      step_noise4(p, s, i, step_draws_noise<kKind>(s), z);
+      hist_load4<kKind>(p, s, i, hp);
       const float4 xt = ldg_f4(p.x_t + i);
       const float xtv[4] = {xt.x, xt.y, xt.z, xt.w};
       float xo[4], x0o[4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) step_element<kDdim>(p, s, n, c, pix + j, xtv[j], e[j][c], z[j], xo[j], x0o[j]);
+      for (int j = 0; j < 4; ++j) step_element<kKind>(p, s, n, c, pix + j, xtv[j], e[j][c], z[j], hp[j], xo[j], x0o[j]);
       stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
       if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
+      hist_store4<kKind>(p, i, x0o);
     }
   }
 }

@@ -1,4 +1,4 @@
-// DDPM / DDIM samplers (host class).  See sampler.cu / sampler.cuh.
+// DDPM / DDIM / DPM-Solver++ samplers (host class).  See sampler.cu / sampler.cuh.
 #pragma once
 #include <vector>
 
@@ -24,10 +24,14 @@ class Sampler {
 
  private:
   void ensure_device(int N2, size_t eps_elems);
+  void ensure_hist(size_t elems);
   int T_;
   std::vector<double> betas_, acp_, acp_prev_, srac_, srm1_, pvar_, plogvar_, pc1_, pc2_;
   void* d_table_ = nullptr;
   void* d_state_ = nullptr;
+  double* d_acp_ = nullptr;                // float64 alphas_cumprod (DPM-Solver++ step scalars)
+  float* d_hist_ = nullptr;                // DPM-Solver++ history D_{-1} [N,C,H,W], updated in place by the step kernels
+  size_t cap_hist_ = 0;
   int64_t* d_t_ = nullptr;
   int64_t* d_classes2_ = nullptr;
   float* d_eps_ = nullptr;

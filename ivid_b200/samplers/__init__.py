@@ -1,1 +1,1 @@
-from .samplers import DdpmSampler, DdimSampler
+from .samplers import DdpmSampler, DdimSampler, DpmSolverSampler

@@ -1,5 +1,6 @@
 """DdpmSampler / DdimSampler — host-side mirrors of the reference samplers
-(diffusion/samplers/ddpm.py:12-187, diffusion/samplers/ddim.py:12-165).
+(diffusion/samplers/ddpm.py:12-187, diffusion/samplers/ddim.py:12-165) — and DpmSolverSampler, a DPM-Solver++(2M)
+sampler with the same surface that the reference does not have.
 
 Same constructor (`Sampler(framework)`), same float64 numpy table attributes, same `.sample(...)` / `.sample_once(...)`
 signatures and return dict (`samples`, `pred_x_t`, `pred_x_0`).  The step itself — UNet forward with both
@@ -22,7 +23,7 @@ from .. import _lib
 from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG
 from ..utils import edict
 
-__all__ = ["DdpmSampler", "DdimSampler"]
+__all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler"]
 
 
 def _unwrap(backbone):
@@ -64,7 +65,8 @@ class _NativeSampler:
         return out
 
     # ------------------------------------------------------------------------------------------------------------
-    def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None):
+    def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
+                   order=0, prev=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -101,7 +103,7 @@ class _NativeSampler:
                 a.cond.sr_scale = SuperResCFG._scale(torch.empty(0, 0, *hw), kwargs["y"])
         rr = kwargs.get("replace_rgb")
         if rr is not None:
-            assert self.KIND == 1, "replace_rgb is a DdimSampler argument"
+            assert self.KIND in (1, 2), "replace_rgb is a DdimSampler / DpmSolverSampler argument"
             a.replace_rgb_weight = float(rr[0]); a.replace_rgb_dev = P(rr[1]); a.replace_rgb_mask_dev = P(rr[2])
         rd = kwargs.get("replace_depth")
         if rd:
@@ -113,6 +115,11 @@ class _NativeSampler:
         a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
         if hw is not None:
             a.height, a.width = int(hw[0]), int(hw[1])
+        a.order = int(order)
+        if prev is not None:
+            t_last, x0_last = prev
+            a.t_last = int(t_last[0]) if torch.is_tensor(t_last) and t_last.dim() > 0 else int(t_last)
+            a.prev_x0_dev = P(x0_last)
         return a, keep
 
     def _net(self):
@@ -120,12 +127,12 @@ class _NativeSampler:
         net._ensure_packed()
         return net
 
-    def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise):
+    def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None):
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:])
+                                  hw=x_t.shape[-2:], order=order, prev=prev)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         with torch.cuda.device(dev):
@@ -135,13 +142,13 @@ class _NativeSampler:
         del keep
         return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
 
-    def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise):
+    def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None):
         """Same step with the timestep taken on the device from the [N] tensors the caller passed (no host sync)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:])
+                                  hw=x_t.shape[-2:], order=order, prev=prev)
         td = t.to(device=dev, dtype=torch.int64).contiguous()
         tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
         x_prev = torch.empty_like(x_t)
@@ -163,7 +170,7 @@ class _NativeSampler:
             cond_noise = torch.cat([n_rgb, n_d], dim=1)
         return torch.randn_like(x_t), cond_noise
 
-    def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs):
+    def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0):
         net = self._net()
         net.eval()
         if image_size is None:
@@ -184,6 +191,7 @@ class _NativeSampler:
             else:
                 jump = T // nsteps
                 sched = [(jump * (i + 1), jump * i) for i in reversed(range(nsteps))]
+            prev = None
             for (t, t_prev) in sched:
                 # the reference draws the model-input noise first (inside model_inference), then randn_like(x_t)
                 cond_noise = None
@@ -191,14 +199,20 @@ class _NativeSampler:
                     y = kwargs["y"]
                     cond_noise = torch.cat([torch.randn_like(y[:, :3]), torch.randn_like(y[:, 3:])], dim=1)
                 z = torch.randn_like(img)
-                out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise)
+                if self.KIND == 2:
+                    # deterministic: z is drawn only to consume the torch RNG as DdimSampler does
+                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, None, cond_noise, order=order,
+                                            prev=prev if order != 1 else None)
+                    prev = (t, out.pred_x_0)
+                else:
+                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise)
                 img = out.pred_x_prev
                 if return_trajectory:
                     ret.pred_x_t.append(out.pred_x_prev)
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:])
+            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order)
             traj0 = trajt = None
             if return_trajectory:
                 traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
@@ -276,3 +290,37 @@ class DdimSampler(_NativeSampler):
                verbose=True, rng="philox", return_trajectory=False, **kwargs):
         """Run `steps` DDIM steps (ddim.py:106-165)."""
         return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs)
+
+
+class DpmSolverSampler(_NativeSampler):
+    """DPM-Solver++(2M) (Lu et al. 2022), the second-order multistep ODE solver in data-prediction form, on DdimSampler's
+    time grid (jump = T // steps, model called at t - 1) with the same guidance (classifier-free mix, multiview replace /
+    constrain applied to x_0 exactly as DdimSampler.sample_once applies it).  Order 1 is DDIM with eta = 0.  Deterministic:
+    no step noise.  The update is fused into the output head like the DDPM / DDIM steps (include/ivid_b200.h, kind 2)."""
+    KIND = 2
+
+    @torch.no_grad()
+    def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
+                    constrain_depth=None, noise=None, **kwargs):
+        """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
+        `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
+        `noise` is not used by the update: when it is None the torch RNG is consumed exactly as DdimSampler.sample_once
+        consumes it (InpaintCFG hole noise, then one randn_like(x_t)); `cond_noise` injects the hole noise."""
+        B = x_t.shape[0]
+        assert t.shape == (B,) and t_prev.shape == (B,)
+        kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
+        if noise is None:
+            _, cond_noise = self._draw_step_noise(x_t, kw)
+        else:
+            cond_noise = kw.pop("cond_noise", None)
+        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, None, cond_noise,
+                                     order=2 if prev is not None else 1, prev=prev)
+
+    @torch.no_grad()
+    def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
+               rng="philox", return_trajectory=False, **kwargs):
+        """Run `steps` DPM-Solver++ steps of order `order` (1 or 2).  The first step and the final step (to t_prev = 0,
+        which returns x_0 as DDIM does) are first order.  Same return dict as DdimSampler.sample."""
+        assert order in (1, 2), f"order must be 1 or 2, got {order}"
+        return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
+                         order=order)
