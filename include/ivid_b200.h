@@ -54,6 +54,16 @@ int ivid_unet_param_info(const ivid_unet_t* h, int index, const char** name, int
 int ivid_unet_set_param(ivid_unet_t* h, const char* name, const float* host_data, const int64_t* shape, int ndim);
 /* .cuda() : pack all parameters (fp16 K-major GEMM operands, fp32 norms/embeddings) into one device arena. */
 int ivid_unet_finalize(ivid_unet_t* h, int device);
+/* Operand precision of the ResBlock 3x3 convs (in_layers.2, out_layers.3): 0 = fp16 (default), 1 = fp8, e4m3 activations
+ * and power-of-two-scaled e4m3 weights with fp32 accumulation (DESIGN.md §2 gives the rules, and which convs stay fp16).
+ * Any other value returns IVID_ERR_INVALID_ARGUMENT.  Takes effect at the next ivid_unet_finalize.  The packed arena's size
+ * and layout depend on it, so ranks that share a broadcast arena must all use the same precision. */
+int ivid_unet_set_precision(ivid_unet_t* h, int precision);
+/* The fp8 mode's host conversion, no device needed: fp32 -> e4m3 (E4M3FN) bytes, round to nearest even, saturated to
+ * +-448, NaN -> 0x7F with the input's sign. */
+int ivid_fp8_e4m3_quantize(const float* in, uint8_t* out, uint64_t count);
+/* The fp8 mode's weight scale, no device needed: the e with max|w| * 2^e in (224, 448] (0 when every w is zero). */
+int ivid_fp8_weight_exponent(const float* w, uint64_t count, int* e_out);
 /* Device arena (for the NCCL weight broadcast at init, sample.py:186-195 loads per rank instead). */
 int ivid_unet_weight_arena(const ivid_unet_t* h, void** dev_ptr, uint64_t* bytes);
 
@@ -276,10 +286,20 @@ int ivid_warp_forward_backward(ivid_warp_t* w, const float* lin_depth0_host, con
 int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
                    int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
                    const float* residual_dev, void* out_dev, int out_fp16, void* stream);
+/* The fp8 twin of ivid_op_conv2d: act_dev e4m3 NHWC [N,H,W,Cin] (Cin % 16 == 0); w_host fp32, quantized as the packer
+ * does (e4m3(w * 2^e), the e of ivid_fp8_weight_exponent, written to *e_out when e_out is not NULL); the optional fp16
+ * 1x1 skip segment is packed as fp16(w2 * 2^e); out = acc * 2^-e + bias (+ residual). */
+int ivid_op_conv2d_e4m3(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
+                        int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
+                        const float* residual_dev, void* out_dev, int out_fp16, int* e_out, void* stream);
 /* GroupNorm32 (+FiLM) (+SiLU) (+2x up / 2x2 avg-pool) over a virtual concat of two fp32 NHWC tensors -> fp16 NHWC. */
 int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
                        float eps, const float* gamma_host, const float* beta_host, const float* film_dev /*[N,2C]*/,
                        int silu, int mode, void* out_fp16_dev, void* stream);
+/* The same with an e4m3 NHWC output (satfinite, round to nearest even; C0 + C1 a multiple of 16). */
+int ivid_op_group_norm_e4m3(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
+                            float eps, const float* gamma_host, const float* beta_host, const float* film_dev,
+                            int silu, int mode, void* out_e4m3_dev, void* stream);
 /* QKVAttention (adm.py:233-253): qkv fp16 [N,T,3C] (legacy head-major q|k|v order) -> fp16 [N,T,C]. */
 int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, void* stream);
 /* The same with head width head_channels = C / heads (a multiple of 64, dividing C): qkv fp16 [N,T,3C] in the order

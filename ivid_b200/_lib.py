@@ -77,6 +77,9 @@ SIGNATURES = {
     "ivid_unet_set_param": (c_int, [c_void_p, c_char_p, c_void_p, POINTER(c_int64), c_int]),
     "ivid_unet_finalize": (c_int, [c_void_p, c_int]),
     "ivid_unet_weight_arena": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_uint64)]),
+    "ivid_unet_set_precision": (c_int, [c_void_p, c_int]),
+    "ivid_fp8_e4m3_quantize": (c_int, [c_void_p, c_void_p, c_uint64]),
+    "ivid_fp8_weight_exponent": (c_int, [c_void_p, c_uint64, POINTER(c_int)]),
     "ivid_unet_forward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "ivid_unet_forward_cond": (c_int, [c_void_p, c_void_p, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "ivid_unet_forward_hw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p, c_int,
@@ -96,6 +99,10 @@ SIGNATURES = {
                                c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "ivid_op_group_norm": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                                    c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "ivid_op_conv2d_e4m3": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), c_void_p]),
+    "ivid_op_group_norm_e4m3": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
+                                        c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention_heads": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_warp_create": (c_int, [c_int, c_int, c_int, c_int, c_double, c_double, c_int, POINTER(c_void_p)]),

@@ -78,6 +78,7 @@ class AdmUnet2d(nn.Module):
         _lib.check(L.ivid_unet_create(self._cfg_json.encode(), ctypes.byref(self._handle)))
         self._packed_device = None     # device index the native arena currently lives on
         self._packed_version = None
+        self.precision = "fp16"
 
         # Parameters / buffers with the reference's names, shapes and default initialisation
         # (nn.Conv/Linear defaults, zero_module for out_layers.3 / proj_out / out.2: adm.py:182,278,486).
@@ -160,6 +161,15 @@ class AdmUnet2d(nn.Module):
         _lib.check(L.ivid_unet_finalize(self._handle, idx))
         self._packed_device = idx
         self._packed_version = self._version()
+
+    def set_precision(self, precision: str) -> None:
+        """Operands of the ResBlock 3x3 convs: "fp16" (default) or "fp8" (e4m3 activations, power-of-two-scaled e4m3
+        weights, fp32 accumulation; DESIGN.md §2).  fp8 changes the numbers.  The weights are repacked at the next use."""
+        if precision not in ("fp16", "fp8"):
+            raise ValueError(f"precision must be 'fp16' or 'fp8', got {precision!r}")
+        _lib.check(_lib.lib().ivid_unet_set_precision(self._handle, 0 if precision == "fp16" else 1))
+        self.precision = precision
+        self._packed_device = None
 
     def _ensure_packed(self):
         if self._packed_device is None or self._packed_version != self._version():

@@ -1,4 +1,6 @@
 // C ABI (include/ivid_b200.h): exception -> status-code translation, op-level entry points.
+#include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -91,6 +93,27 @@ int ivid_unet_finalize(ivid_unet_t* h, int device) {
   return guarded([&] {
     IVID_NOT_NULL(h);
     h->impl->finalize(device);
+  });
+}
+int ivid_unet_set_precision(ivid_unet_t* h, int precision) {
+  return guarded([&] {
+    IVID_NOT_NULL(h);
+    h->impl->set_precision(precision);
+  });
+}
+int ivid_fp8_e4m3_quantize(const float* in, uint8_t* out, uint64_t count) {
+  return guarded([&] {
+    IVID_REQUIRE(count == 0 || (in != nullptr && out != nullptr), "in and out must not be NULL");
+    for (uint64_t i = 0; i < count; ++i) out[i] = fp8_e4m3_from_float(in[i]);
+  });
+}
+int ivid_fp8_weight_exponent(const float* w, uint64_t count, int* e_out) {
+  return guarded([&] {
+    IVID_REQUIRE(count == 0 || w != nullptr, "w must not be NULL");
+    IVID_NOT_NULL(e_out);
+    float mx = 0.f;
+    for (uint64_t i = 0; i < count; ++i) mx = std::max(mx, std::fabs(w[i]));
+    *e_out = fp8_weight_exponent(mx);
   });
 }
 int ivid_unet_weight_arena(const ivid_unet_t* h, void** dev_ptr, uint64_t* bytes) {
@@ -251,9 +274,59 @@ int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const floa
   });
 }
 
-int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
-                       float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
-                       int mode, void* out_fp16_dev, void* stream) {
+int ivid_op_conv2d_e4m3(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
+                        int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
+                        const float* residual_dev, void* out_dev, int out_fp16, int* e_out, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(act_dev); IVID_NOT_NULL(w_host); IVID_NOT_NULL(out_dev);
+    IVID_REQUIRE(ksize == 3 || ksize == 1, "conv: kernel size must be 3 or 1");
+    IVID_REQUIRE(Cin > 0 && Cin % 16 == 0, "conv: an e4m3 operand needs a multiple of 16 channels");
+    IVID_REQUIRE(Cin2 % 8 == 0 && (act2_dev == nullptr || w2_host != nullptr), "conv: skip channels must be a multiple of 8");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int taps = ksize * ksize;
+    const int cout_pad = conv_pad_cout(Cout);
+    const size_t nw = static_cast<size_t>(Cout) * Cin * taps;
+    float mx = 0.f;
+    for (size_t i = 0; i < nw; ++i) mx = std::max(mx, std::fabs(w_host[i]));
+    const int e = fp8_weight_exponent(mx);
+    const float scale = std::ldexp(1.0f, e);
+    const int cp8 = conv_pad_k8(Cin), K8 = taps * cp8;
+    std::vector<uint8_t> w8(static_cast<size_t>(cout_pad) * K8, 0);
+    for (int co = 0; co < Cout; ++co)
+      for (int tap = 0; tap < taps; ++tap)
+        for (int ci = 0; ci < Cin; ++ci)
+          w8[static_cast<size_t>(co) * K8 + tap * cp8 + ci] = fp8_e4m3_from_float(w_host[(static_cast<size_t>(co) * Cin + ci) * taps + tap] * scale);
+    const int K = act2_dev ? conv_pad_k(Cin2) : 0;
+    std::vector<__half> wp(static_cast<size_t>(cout_pad) * std::max(K, 1), __float2half_rn(0.f));
+    for (int co = 0; co < Cout && act2_dev; ++co)
+      for (int ci = 0; ci < Cin2; ++ci) {
+        const float v = w2_host[static_cast<size_t>(co) * Cin2 + ci] * scale;
+        IVID_REQUIRE(std::fabs(v) <= 65504.f, "conv: skip weights times 2^e leave the fp16 range");
+        wp[static_cast<size_t>(co) * K + ci] = __float2half_rn(v);
+      }
+    std::vector<float> bias(cout_pad, 0.f);
+    for (int i = 0; i < Cout; ++i) bias[i] = (bias_host ? bias_host[i] : 0.f) + ((act2_dev && bias2_host) ? bias2_host[i] : 0.f);
+    DevBuf dw8(w8.size()), dw(wp.size() * 2), db(bias.size() * 4);
+    IVID_CHECK_CUDA(cudaMemcpyAsync(dw8.p, w8.data(), w8.size(), cudaMemcpyHostToDevice, st));
+    IVID_CHECK_CUDA(cudaMemcpyAsync(dw.p, wp.data(), wp.size() * 2, cudaMemcpyHostToDevice, st));
+    IVID_CHECK_CUDA(cudaMemcpyAsync(db.p, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice, st));
+    ConvDesc d;
+    d.act0 = act_dev; d.C0 = Cin; d.taps0 = taps;
+    if (act2_dev) { d.act1 = act2_dev; d.C1 = Cin2; d.taps1 = 1; }
+    d.weight8 = dw8.p; d.weight = act2_dev ? dw.p : nullptr; d.acc_scale = std::ldexp(1.0f, -e);
+    d.cout_pad = cout_pad; d.cout = Cout; d.bias = static_cast<const float*>(db.p);
+    d.residual = residual_dev; d.ldr = Cout; d.out = out_dev; d.ldc = Cout; d.out_mode = out_fp16 ? 1 : 0;
+    d.N = N; d.H = H; d.W = W;
+    std::unique_ptr<ConvLaunch, void (*)(ConvLaunch*)> l(conv_launch_create(d), conv_launch_destroy);
+    conv_launch_run(l.get(), st);
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+    if (e_out) *e_out = e;
+  });
+}
+
+static int op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
+                         float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
+                         int mode, void* out_fp16_dev, bool e4m3, void* stream) {
   return guarded([&] {
     IVID_NOT_NULL(x0_dev); IVID_NOT_NULL(gamma_host); IVID_NOT_NULL(beta_host); IVID_NOT_NULL(out_fp16_dev);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -268,13 +341,26 @@ int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1,
     if (C1 > 0) launch_gn_stats(x1_dev, static_cast<double*>(st1.p), N, H * W, C1, st);
     GnApplyDesc g;
     g.x0 = x0_dev; g.x1 = C1 > 0 ? x1_dev : nullptr; g.C0 = C0; g.C1 = C1; g.N = N; g.H = H; g.W = W; g.mode = mode;
-    g.silu = silu; g.out_act = out_fp16_dev;
+    g.silu = silu; g.out_act = out_fp16_dev; g.out_e4m3 = e4m3;
     g.stats0 = static_cast<double*>(st0.p); g.stats1 = C1 > 0 ? static_cast<double*>(st1.p) : nullptr;
     g.groups = groups; g.eps = eps; g.gamma = static_cast<float*>(dg.p); g.beta = static_cast<float*>(dbt.p);
     g.film = film_dev; g.film_ld = 2 * C; g.film_off = 0;
     launch_gn_apply(g, st);
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
   });
+}
+
+int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
+                       float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
+                       int mode, void* out_fp16_dev, void* stream) {
+  return op_group_norm(x0_dev, C0, x1_dev, C1, N, H, W, groups, eps, gamma_host, beta_host, film_dev, silu, mode, out_fp16_dev,
+                       false, stream);
+}
+int ivid_op_group_norm_e4m3(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
+                            float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
+                            int mode, void* out_e4m3_dev, void* stream) {
+  return op_group_norm(x0_dev, C0, x1_dev, C1, N, H, W, groups, eps, gamma_host, beta_host, film_dev, silu, mode, out_e4m3_dev,
+                       true, stream);
 }
 
 int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, void* stream) {

@@ -25,7 +25,15 @@
 // loop.
 // The epilogue works on the accumulator fragments in place: bias, residual (optionally through a nearest-2x upsample),
 // fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.
+//
+// fp8 operand mode (A8): segment 0 is e4m3.  Its 128-byte box row is 128 channels, so an e4m3 k-block has exactly the
+// shared-memory layout, TMA bytes and wgmma descriptors of an fp16 one; only the instruction differs (k32 e4m3 for k16
+// f16) and a chunk covers 128 channels.  Its weights come from a second map (b8) over e4m3 columns pre-scaled by 2^e; the
+// fp16 skip segments keep the b map with columns pre-scaled by the same 2^e, so all of K sums into one accumulator, and
+// the epilogue takes v = acc * 2^-e + bias.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ivid {
@@ -48,12 +56,17 @@ struct ConvGemmParams {
   __half* out16;               // optional fp16 NHWC copy of an fp32 NHWC output (same ldc)
   double* stats;               // optional [N][Cout][2] per-(sample, channel) sum / sum-of-squares of the output (GroupNorm);
                                // of the ROUNDED values when the output is fp16 (exactly what the next GroupNorm reads)
+  float acc_scale;             // A8 only: 2^-e, the inverse of the weights' power-of-two scale
 };
 
 // All TMA descriptors of one launch, passed as a single __grid_constant__ argument.
 struct ConvMaps {
   CUtensorMap a[3];            // activation segments (fp16 NHWC)
   CUtensorMap b;               // packed weights
+};
+// the A8 kernels' maps: also the e4m3 weight columns of segment 0
+struct ConvMaps8 : ConvMaps {
+  CUtensorMap b8;
 };
 
 template <int BN>
@@ -78,9 +91,9 @@ struct ConvKCursor {
 
 // p is read in place (__grid_constant__): the K cursor indexes seg_chunks / seg_taps at run time, and without it the compiler
 // may copy the whole struct to a local-memory stack frame to do so.
-template <int BN>
+template <int BN, bool A8 = false>
 __global__ void __launch_bounds__(ConvGemmCfg<BN>::THREADS, 2)
-conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ ConvGemmParams p) {
+conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvMaps> maps, const __grid_constant__ ConvGemmParams p) {
   using Cfg = ConvGemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -105,6 +118,7 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
 
   int nunits = 0;                                // K blocks of the tile
   for (int sg = 0; sg < 3; ++sg) nunits += p.seg_chunks[sg] * p.seg_taps[sg];
+  const int nunits8 = A8 ? p.seg_chunks[0] * p.seg_taps[0] : 0;   // the first nunits8 k-blocks are e4m3
 
   // column block fast: the CTAs that share an activation tile run together
   const int mt = static_cast<int>(blockIdx.x) / p.n_blocks, nb = static_cast<int>(blockIdx.x) % p.n_blocks;
@@ -121,6 +135,7 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
     if (lane == 0) {
       tma_prefetch_desc(&maps.a[0]);
       tma_prefetch_desc(&maps.b);
+      if constexpr (A8) tma_prefetch_desc(&maps.b8);
       ConvKCursor c;                             // units are issued strictly in order: segment, tap slow, chunk fast
       while (p.seg_chunks[c.seg] == 0) ++c.seg;
 #pragma unroll 1
@@ -133,11 +148,24 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
         uint8_t* sb = sa + Cfg::A_BYTES;
         const int dy = (taps == 9) ? (c.t / 3 - 1) : 0;
         const int dx = (taps == 9) ? (c.t % 3 - 1) : 0;
-        const int kcol = c.base + (c.t * chunks + c.ch) * 64;
         mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
-        tma_load_4d(&maps.a[c.seg], &full_bar[s], sa, c.ch * 64, w0 + dx, h0 + dy, n0);
-        tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
-        if (++c.ch == chunks) { c.ch = 0; if (++c.t == taps) { c.t = 0; c.base += taps * chunks * 64; ++c.seg; } }
+        bool e4m3 = false;
+        if constexpr (A8) {
+          if (c.seg == 0) {                      // e4m3: 128 channels per box row; columns of b8 (c.base stays 0)
+            tma_load_4d(&maps.a[0], &full_bar[s], sa, c.ch * 128, w0 + dx, h0 + dy, n0);
+            tma_load_2d(&maps.b8, &full_bar[s], sb, (c.t * chunks + c.ch) * 128, colbase);
+            e4m3 = true;
+          }
+        }
+        if (!e4m3) {
+          const int kcol = c.base + (c.t * chunks + c.ch) * 64;
+          tma_load_4d(&maps.a[c.seg], &full_bar[s], sa, c.ch * 64, w0 + dx, h0 + dy, n0);
+          tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
+        }
+        if (++c.ch == chunks) {
+          c.ch = 0;
+          if (++c.t == taps) { c.t = 0; if (!A8 || c.seg != 0) c.base += taps * chunks * 64; ++c.seg; }
+        }
         while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
       }
     }
@@ -159,8 +187,13 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
     wgmma_fence();
     const uint64_t da = make_smem_desc_sw128(sa + wg * 64 * 128, 1024, 16);
     const uint64_t db = make_smem_desc_sw128(sb, 1024, 16);
+    if (A8 && u < nunits8) {                     // warp-uniform
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+    }
     wgmma_commit();
     // group u stays in flight; group u - 1 has retired, so its slot goes back to the producer
     wgmma_wait<1>();
@@ -195,7 +228,12 @@ conv_gemm_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ 
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!ok[i]) continue;
-        float v0 = acc[4 * j + 2 * i] + b.x, v1 = acc[4 * j + 2 * i + 1] + b.y;
+        float v0, v1;
+        if (A8) {
+          v0 = fmaf(acc[4 * j + 2 * i], p.acc_scale, b.x); v1 = fmaf(acc[4 * j + 2 * i + 1], p.acc_scale, b.y);
+        } else {
+          v0 = acc[4 * j + 2 * i] + b.x; v1 = acc[4 * j + 2 * i + 1] + b.y;
+        }
         if (p.out_mode == 2) {
           const uint32_t hw = static_cast<uint32_t>(p.H) * p.W, n = pix[i] / hw;
           float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(n) * p.Cout + c) * hw + (pix[i] - n * hw);

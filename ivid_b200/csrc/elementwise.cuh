@@ -107,7 +107,32 @@ struct GnApplyParams {
                                         // of a two-term split of the activation (operand of the split-precision output conv)
   __half* out_raw16;                    // optional fp16 raw copy (same-resolution only) [N][H][W][C]
   float* out_raw32;                     // optional fp32 raw (resampled) [N][Ho][Wo][C]
+  uint8_t* out_act8;                    // the kF8 kernels write the activation here instead, as e4m3 [N][Ho][Wo][C]
 };
+
+// 8 activations of one work item as the operand the next conv reads: fp16 (16 bytes) or, kF8, e4m3 (8 bytes, satfinite)
+template <bool kF8> struct Act8 { using T = uint4; };
+template <> struct Act8<true> { using T = uint2; };
+template <bool kF8>
+__device__ __forceinline__ typename Act8<kF8>::T pack_act8(const float (&a)[8]) {
+  if constexpr (kF8) {
+    uint2 pk;
+    pk.x = pack_e4m3x2(a[0], a[1]) | (static_cast<uint32_t>(pack_e4m3x2(a[2], a[3])) << 16);
+    pk.y = pack_e4m3x2(a[4], a[5]) | (static_cast<uint32_t>(pack_e4m3x2(a[6], a[7])) << 16);
+    return pk;
+  } else {
+    uint4 pk;
+    pk.x = pack_h2(a[0], a[1]); pk.y = pack_h2(a[2], a[3]);
+    pk.z = pack_h2(a[4], a[5]); pk.w = pack_h2(a[6], a[7]);
+    return pk;
+  }
+}
+// element offset o of the activation output
+template <bool kF8>
+__device__ __forceinline__ void store_act8(const GnApplyParams& p, size_t o, const typename Act8<kF8>::T& v) {
+  if constexpr (kF8) *reinterpret_cast<uint2*>(p.out_act8 + o) = v;
+  else *reinterpret_cast<uint4*>(p.out_act + o) = v;
+}
 
 __device__ __forceinline__ void load8(const GnApplyParams& p, int n, int h, int w, int c, float (&v)[8]) {
   if (p.x0h != nullptr) {
@@ -241,6 +266,7 @@ __device__ __forceinline__ void gn_prologue(const GnApplyParams& p, float* s_ab,
 
 }
 
+template <bool kF8 = false>
 __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p) {
   extern __shared__ float s_ab[];        // A then B, each stored [c % 8][c / 8] so a warp's reads are conflict-free
   __shared__ float s_mean[64], s_rstd[64];
@@ -269,16 +295,14 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
         if (p.silu) y = silu_f(y);
         act[j] = y;
       }
-      uint4 pk;
-      pk.x = pack_h2(act[0], act[1]); pk.y = pack_h2(act[2], act[3]);
-      pk.z = pack_h2(act[4], act[5]); pk.w = pack_h2(act[6], act[7]);
+      const auto pk = pack_act8<kF8>(act);
       const float4 r0 = make_float4(raw[0], raw[1], raw[2], raw[3]), r1 = make_float4(raw[4], raw[5], raw[6], raw[7]);
 #pragma unroll
       for (int dy = 0; dy < 2; ++dy)
 #pragma unroll
         for (int dx = 0; dx < 2; ++dx) {
           const size_t o = ((static_cast<size_t>(n) * Ho + 2 * hs + dy) * Wo + 2 * ws + dx) * C + cg * 8;
-          *reinterpret_cast<uint4*>(p.out_act + o) = pk;
+          store_act8<kF8>(p, o, pk);
           if (p.out_raw32 != nullptr) { stg_f4(p.out_raw32 + o, r0); stg_f4(p.out_raw32 + o + 4, r1); }
         }
     };
@@ -330,10 +354,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
           if (p.silu) y = silu_f(y);
           act[j] = y;
         }
-        uint4 pk;
-        pk.x = pack_h2(act[0], act[1]); pk.y = pack_h2(act[2], act[3]);
-        pk.z = pack_h2(act[4], act[5]); pk.w = pack_h2(act[6], act[7]);
-        *reinterpret_cast<uint4*>(p.out_act + o) = pk;
+        store_act8<kF8>(p, o, pack_act8<kF8>(act));
         if (p.out_raw16 != nullptr) {
           uint4 pr;
           pr.x = pack_h2(raw[u][0], raw[u][1]); pr.y = pack_h2(raw[u][2], raw[u][3]);
@@ -387,10 +408,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const GnApplyParams p)
       }
     }
     const size_t o = ((static_cast<size_t>(n) * Ho + ho) * Wo + wo) * C + c;
-    uint4 pk;
-    pk.x = pack_h2(act[0], act[1]); pk.y = pack_h2(act[2], act[3]);
-    pk.z = pack_h2(act[4], act[5]); pk.w = pack_h2(act[6], act[7]);
-    *reinterpret_cast<uint4*>(p.out_act + o) = pk;
+    store_act8<kF8>(p, o, pack_act8<kF8>(act));
     if (p.out_raw16 != nullptr) {
       uint4 pr;
       pr.x = pack_h2(raw[0], raw[1]); pr.y = pack_h2(raw[2], raw[3]);
@@ -474,7 +492,8 @@ __global__ void __launch_bounds__(256) resample_f32_kernel(const float* __restri
 // (4 registers each) until consumed, so a thread has 128 bytes of reads in flight although an item is only 16 bytes.
 // kHoist: the channel-group count divides the block size, so a thread keeps the same 8 channels on every trip and its 16
 // coefficients live in registers (saves 16 shared-memory loads per 16-byte item).
-template <bool kHoist, bool kLo = false>
+// kF8: the activation is written as e4m3 to out_act8 (same element offsets).
+template <bool kHoist, bool kLo = false, bool kF8 = false>
 __global__ void __launch_bounds__(256, 3) gn_apply_h16_kernel(const GnApplyParams p) {
   extern __shared__ float s_ab[];
   __shared__ float s_mean[64], s_rstd[64];
@@ -496,6 +515,7 @@ __global__ void __launch_bounds__(256, 3) gn_apply_h16_kernel(const GnApplyParam
   auto apply8 = [&](const uint4& rawv, int cg, __half* dst) {
     const __half2* h2 = reinterpret_cast<const __half2*>(&rawv);
     uint32_t pk[4], pl[4];
+    uint16_t p8[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 f = __half22float2(h2[j]);
@@ -508,11 +528,17 @@ __global__ void __launch_bounds__(256, 3) gn_apply_h16_kernel(const GnApplyParam
         y1 = fmaf(f.y, s_ab[(2 * j + 1) * c8 + cg], s_ab[C + (2 * j + 1) * c8 + cg]);
       }
       if (p.silu) { y0 = silu_f(y0); y1 = silu_f(y1); }
+      if (kF8) { p8[j] = pack_e4m3x2(y0, y1); continue; }
       pk[j] = pack_h2(y0, y1);
       if (kLo) {
         const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&pk[j]));
         pl[j] = pack_h2(y0 - hi.x, y1 - hi.y);
       }
+    }
+    if (kF8) {
+      *reinterpret_cast<uint2*>(p.out_act8 + (dst - p.out_act)) =
+          make_uint2(p8[0] | (static_cast<uint32_t>(p8[1]) << 16), p8[2] | (static_cast<uint32_t>(p8[3]) << 16));
+      return;
     }
     *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
     if (kLo) *reinterpret_cast<uint4*>(p.out_lo + (dst - p.out_act)) = make_uint4(pl[0], pl[1], pl[2], pl[3]);

@@ -1,5 +1,6 @@
 #include "host_util.h"
 
+#include <cmath>
 #include <cstring>
 #include <mutex>
 
@@ -45,22 +46,25 @@ CUtensorMap make_tensor_map(CUtensorMapDataType dtype, int rank, void* base, con
   return m;
 }
 
-CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN) {
+static uint64_t elem_bytes(CUtensorMapDataType dtype) { return dtype == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 2; }
+
+CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN, CUtensorMapDataType dtype) {
+  const uint64_t es = elem_bytes(dtype);
   const uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(W), static_cast<uint64_t>(H),
                             static_cast<uint64_t>(N)};
-  const uint64_t str[3] = {static_cast<uint64_t>(C) * 2, static_cast<uint64_t>(W) * C * 2,
-                           static_cast<uint64_t>(H) * W * C * 2};
-  const uint32_t box[4] = {64, static_cast<uint32_t>(TW), static_cast<uint32_t>(TH), static_cast<uint32_t>(TN)};
-  return make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, str, box,
-                         CU_TENSOR_MAP_SWIZZLE_128B);
+  const uint64_t str[3] = {static_cast<uint64_t>(C) * es, static_cast<uint64_t>(W) * C * es,
+                           static_cast<uint64_t>(H) * W * C * es};
+  const uint32_t box[4] = {static_cast<uint32_t>(128 / es), static_cast<uint32_t>(TW), static_cast<uint32_t>(TH),
+                           static_cast<uint32_t>(TN)};
+  return make_tensor_map(dtype, 4, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-CUtensorMap make_weight_map(const void* base, int rows, int K, int box_rows) {
+CUtensorMap make_weight_map(const void* base, int rows, int K, int box_rows, CUtensorMapDataType dtype) {
+  const uint64_t es = elem_bytes(dtype);
   const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(rows)};
-  const uint64_t str[1] = {static_cast<uint64_t>(K) * 2};
-  const uint32_t box[2] = {64, static_cast<uint32_t>(box_rows)};
-  return make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, str, box,
-                         CU_TENSOR_MAP_SWIZZLE_128B);
+  const uint64_t str[1] = {static_cast<uint64_t>(K) * es};
+  const uint32_t box[2] = {static_cast<uint32_t>(128 / es), static_cast<uint32_t>(box_rows)};
+  return make_tensor_map(dtype, 2, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 int sm_count() {
@@ -73,6 +77,40 @@ int sm_count() {
     n = prop.multiProcessorCount;
   }
   return n;
+}
+
+uint8_t fp8_e4m3_from_float(float v) {
+  uint32_t bits;
+  std::memcpy(&bits, &v, 4);
+  const uint8_t sign = static_cast<uint8_t>((bits >> 24) & 0x80u);
+  if ((bits & 0x7FFFFFFFu) > 0x7F800000u) return sign | 0x7F;
+  const double a = std::fabs(static_cast<double>(v));
+  if (a >= 448.0) return sign | 0x7E;
+  if (a < 0.015625) {                                   // below 2^-6: subnormals in steps of 2^-9 (8 rounds up to 2^-6)
+    return sign | static_cast<uint8_t>(std::nearbyint(a * 512.0));
+  }
+  int k;
+  const double f = std::frexp(a, &k);                   // a = f * 2^k, f in [0.5, 1): exponent E = k - 1 in [-6, 8]
+  int E = k - 1;
+  int m = static_cast<int>(std::nearbyint((f * 2.0 - 1.0) * 8.0));   // 3 mantissa bits, ties to even
+  if (m == 8) { m = 0; ++E; }
+  const int code = ((E + 7) << 3) | m;
+  return sign | static_cast<uint8_t>(code > 0x7E ? 0x7E : code);
+}
+
+float fp8_e4m3_to_float(uint8_t q) {
+  const int e = (q >> 3) & 0xF, m = q & 7;
+  if (e == 0xF && m == 7) return std::nanf("");
+  const float v = e == 0 ? std::ldexp(static_cast<float>(m), -9) : std::ldexp(1.0f + m / 8.0f, e - 7);
+  return (q & 0x80) ? -v : v;
+}
+
+int fp8_weight_exponent(float max_abs) {
+  if (!(max_abs > 0.f)) return 0;
+  int k;
+  const double f = std::frexp(static_cast<double>(max_abs), &k);   // max_abs = f * 2^k, f in [0.5, 1)
+  // 448 = 0.875 * 2^9: f <= 0.875 scales to f * 2^9 in [256, 448], f > 0.875 to f * 2^8 in (224, 256)
+  return (f <= 0.875 ? 9 : 8) - k;
 }
 
 }  // namespace ivid

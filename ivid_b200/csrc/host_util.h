@@ -41,11 +41,21 @@ CUtensorMap make_tensor_map(CUtensorMapDataType dtype, int rank, void* base, con
                             const uint64_t* strides_bytes /* rank-1 entries, dim0 is dense */, const uint32_t* box,
                             CUtensorMapSwizzle swizzle);
 
-// NHWC fp16 activation [N][H][W][C] viewed as (C, W, H, N); box = (64, TW, TH, TN), 128B swizzle.
-CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN);
-// fp16 weight matrix [rows][K] (K contiguous); box = (64, box_rows), 128B swizzle.
-CUtensorMap make_weight_map(const void* base, int rows, int K, int box_rows);
+// NHWC activation [N][H][W][C] viewed as (C, W, H, N); box = (128 bytes of channels, TW, TH, TN), 128B swizzle.  dtype
+// FLOAT16 (64-channel box) or UINT8 (e4m3 operands, 128-channel box).
+CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN,
+                         CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+// weight matrix [rows][K] (K contiguous); box = (128 bytes of K, box_rows), 128B swizzle; dtype as for make_act_map.
+CUtensorMap make_weight_map(const void* base, int rows, int K, int box_rows,
+                            CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
 
 int sm_count();
+
+// fp32 -> e4m3 (OCP FP8 E4M3FN) on the host: round to nearest even, saturated to +-448, NaN -> 0x7F | sign.  The device
+// conversion of the fp8 mode (cvt.rn.satfinite.e4m3x2.f32) gives the same bytes for every non-NaN input.
+uint8_t fp8_e4m3_from_float(float v);
+float fp8_e4m3_to_float(uint8_t q);
+// Power-of-two weight scale of the fp8 mode: the e with max|w| * 2^e in (224, 448]; 0 for max|w| == 0.
+int fp8_weight_exponent(float max_abs);
 
 }  // namespace ivid

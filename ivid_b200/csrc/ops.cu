@@ -17,9 +17,10 @@ namespace ivid {
 // conv implicit GEMM
 // --------------------------------------------------------------------------------------------------
 struct ConvLaunch {
-  ConvMaps maps;
+  ConvMaps8 maps;              // b8 is used by the A8 kernels only
   ConvGemmParams p;
   int BN;
+  bool a8;
   int grid;
 };
 
@@ -59,6 +60,7 @@ int conv_pick_bn(int cout_pad) {
 bool conv_can_res_up(int W, int cout) { return W >= 16 && cout % 8 == 0; }
 bool conv_can_out16(int cout) { return cout % 8 == 0; }
 int conv_pad_k(int c) { return ((c + 63) / 64) * 64; }
+int conv_pad_k8(int c) { return ((c + 127) / 128) * 128; }
 
 ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.C0 > 0 && d.C0 % 8 == 0, "conv: segment-0 channels must be a positive multiple of 8");
@@ -68,7 +70,10 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.C2 % 8 == 0 && (d.taps2 == 9 || d.taps2 == 1), "conv: segment 2 must be a multiple of 8 channels, 3x3 or 1x1");
   IVID_REQUIRE(d.N > 0 && static_cast<int64_t>(d.N) * d.H * d.W < (int64_t{1} << 31),
                "conv: N*H*W must be below 2^31 (32-bit pixel indices in the epilogue)");
+  const bool a8 = d.weight8 != nullptr;
+  IVID_REQUIRE(!a8 || d.C0 % 16 == 0, "conv: an e4m3 segment 0 needs a multiple of 16 channels (16-byte TMA rows)");
   auto* l = new ConvLaunch();
+  l->a8 = a8;
   ConvGemmParams& p = l->p;
   p.N = d.N; p.H = d.H; p.W = d.W;
   conv_tile(d.H, d.W, &p.TW, &p.TH, &p.TN);
@@ -77,7 +82,8 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   p.tiles_n = (d.N + p.TN - 1) / p.TN;
   l->BN = conv_pick_bn(d.cout_pad);
   p.n_blocks = d.cout_pad / l->BN;
-  p.seg_chunks[0] = conv_pad_k(d.C0) / 64; p.seg_taps[0] = d.taps0;
+  p.seg_chunks[0] = a8 ? conv_pad_k8(d.C0) / 128 : conv_pad_k(d.C0) / 64; p.seg_taps[0] = d.taps0;
+  p.acc_scale = d.acc_scale;
   p.seg_chunks[1] = conv_pad_k(d.C1) / 64; p.seg_taps[1] = d.C1 > 0 ? d.taps1 : 0;
   p.seg_chunks[2] = conv_pad_k(d.C2) / 64; p.seg_taps[2] = d.C2 > 0 ? d.taps2 : 0;
   p.Cout = d.cout; p.ldc = d.ldc; p.ldr = d.ldr; p.out_mode = d.out_mode;
@@ -98,26 +104,36 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   }
   // packed weight columns: every segment padded to whole 64-channel chunks per tap (zero columns); the activation maps keep
   // the real channel extent, so TMA zero-fills the missing channels of a segment's last chunk
-  const int Ktot = d.taps0 * conv_pad_k(d.C0) + (d.C1 > 0 ? d.taps1 * conv_pad_k(d.C1) : 0) + (d.C2 > 0 ? d.taps2 * conv_pad_k(d.C2) : 0);
-  ConvMaps& M = l->maps;
-  M.a[0] = make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN);
+  // (fp8 mode: segment 0's columns live in weight8, so the fp16 matrix holds the skip segments only)
+  const int Kskip = (d.C1 > 0 ? d.taps1 * conv_pad_k(d.C1) : 0) + (d.C2 > 0 ? d.taps2 * conv_pad_k(d.C2) : 0);
+  const int Ktot = (a8 ? 0 : d.taps0 * conv_pad_k(d.C0)) + Kskip;
+  ConvMaps8& M = l->maps;
+  M.a[0] = a8 ? make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN, CU_TENSOR_MAP_DATA_TYPE_UINT8)
+              : make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN);
   M.a[1] = d.C1 > 0 ? make_act_map(d.act1, d.N, d.H, d.W, d.C1, p.TW, p.TH, p.TN) : M.a[0];
   M.a[2] = d.C2 > 0 ? make_act_map(d.act2, d.N, d.H, d.W, d.C2, p.TW, p.TH, p.TN) : M.a[0];
-  M.b = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN);
+  if (a8) {
+    M.b8 = make_weight_map(d.weight8, d.cout_pad, d.taps0 * conv_pad_k8(d.C0), l->BN, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+    M.b = Ktot > 0 ? make_weight_map(d.weight, d.cout_pad, Ktot, l->BN) : M.b8;    // no skip segment: b is never read
+  } else {
+    M.b = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN);
+  }
   l->grid = p.tiles_w * p.tiles_h * p.tiles_n * p.n_blocks;     // one CTA per (pixel tile, column block)
   return l;
 }
 void conv_launch_destroy(ConvLaunch* l) { delete l; }
 int conv_launch_bn(const ConvLaunch* l) { return l->BN; }
+bool conv_launch_a8(const ConvLaunch* l) { return l->a8; }
 
-template <int BN>
+template <int BN, bool A8>
 static void run_conv(const ConvLaunch* l, cudaStream_t s) {
   using Cfg = ConvGemmCfg<BN>;
   static std::once_flag once;
   std::call_once(once, [] {
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, A8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   });
-  conv_gemm_kernel<BN><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
+  if constexpr (A8) conv_gemm_kernel<BN, true><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
+  else conv_gemm_kernel<BN, false><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(static_cast<const ConvMaps&>(l->maps), l->p);
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
@@ -126,10 +142,18 @@ void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
   conv_launch_run(&tmp, s);
 }
 void conv_launch_run(const ConvLaunch* l, cudaStream_t s) {
+  if (l->a8) {
+    switch (l->BN) {
+      case 128: run_conv<128, true>(l, s); break;
+      case 64: run_conv<64, true>(l, s); break;
+      default: run_conv<16, true>(l, s); break;
+    }
+    return;
+  }
   switch (l->BN) {
-    case 128: run_conv<128>(l, s); break;
-    case 64: run_conv<64>(l, s); break;
-    default: run_conv<16>(l, s); break;
+    case 128: run_conv<128, false>(l, s); break;
+    case 64: run_conv<64, false>(l, s); break;
+    default: run_conv<16, false>(l, s); break;
   }
 }
 
@@ -251,10 +275,12 @@ void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s) {
   p.eps = d.eps; p.gamma = d.gamma; p.beta = d.beta; p.film = d.film; p.film_ld = d.film_ld; p.film_off = d.film_off;
   p.film_add = d.film_add ? 1 : 0;
   p.out_act = reinterpret_cast<__half*>(d.out_act); p.out_raw16 = reinterpret_cast<__half*>(d.out_raw16);
+  p.out_act8 = d.out_e4m3 ? reinterpret_cast<uint8_t*>(d.out_act) : nullptr;
   p.out_raw32 = d.out_raw32;
   p.out_lo = reinterpret_cast<__half*>(d.out_lo);
   IVID_REQUIRE(d.out_lo == nullptr || (d.mode == 0 && d.x0_half && d.out_raw16 == nullptr && d.out_raw32 == nullptr),
                "gn_apply: the split (hi/lo) output exists on the same-resolution fp16-source path only");
+  IVID_REQUIRE(!d.out_e4m3 || (d.out_lo == nullptr && C % 16 == 0), "gn_apply: an e4m3 output needs C % 16 == 0 and no split output");
   const int Ho = d.mode == 1 ? d.H * 2 : (d.mode == 2 ? d.H / 2 : d.H);
   const int Wo = d.mode == 1 ? d.W * 2 : (d.mode == 2 ? d.W / 2 : d.W);
   // One wave of blocks (3 resident per SM) split evenly over the samples, so the statistics -> coefficient prologue is
@@ -278,10 +304,15 @@ void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s) {
     if (p.out_lo != nullptr) {        // output head only: also emits the low half of the two-term split
       if (hoist) gn_apply_h16_kernel<true, true><<<grid, 256, smem, s>>>(p);
       else gn_apply_h16_kernel<false, true><<<grid, 256, smem, s>>>(p);
+    } else if (d.out_e4m3) {
+      if (hoist) gn_apply_h16_kernel<true, false, true><<<grid, 256, smem, s>>>(p);
+      else gn_apply_h16_kernel<false, false, true><<<grid, 256, smem, s>>>(p);
     } else if (hoist) gn_apply_h16_kernel<true><<<grid, 256, smem, s>>>(p);
     else gn_apply_h16_kernel<false><<<grid, 256, smem, s>>>(p);
+  } else if (d.out_e4m3) {
+    gn_apply_kernel<true><<<grid, 256, smem, s>>>(p);
   } else {
-    gn_apply_kernel<<<grid, 256, smem, s>>>(p);
+    gn_apply_kernel<><<<grid, 256, smem, s>>>(p);
   }
   IVID_CHECK_CUDA(cudaGetLastError());
 }

@@ -19,6 +19,11 @@ struct ConvDesc {
   const void* act2 = nullptr; int C2 = 0; int taps2 = 1;   // optional segment 2 (second half of a virtual concat)
   void* out16 = nullptr;                                   // optional fp16 NHWC copy of an fp32 output (same ldc)
   const void* weight = nullptr;                            // fp16 [cout_pad][Ktot], Ktot = sum of taps*conv_pad_k(C) over segments
+  // fp8 operand mode: act0 is e4m3 NHWC (C0 % 16 == 0) and weight8 its e4m3 weights [cout_pad][taps0*conv_pad_k8(C0)],
+  // scaled by 2^e; `weight` then holds only the skip segments' columns (fp16, scaled by the same 2^e; may be null without
+  // skip segments), and acc_scale = 2^-e
+  const void* weight8 = nullptr;
+  float acc_scale = 1.f;
   int cout_pad = 0;
   int cout = 0;                                            // valid output channels
   const float* bias = nullptr;                             // [cout_pad]
@@ -34,6 +39,7 @@ ConvLaunch* conv_launch_create(const ConvDesc& d);
 void conv_launch_destroy(ConvLaunch* l);
 void conv_launch_run(const ConvLaunch* l, cudaStream_t s);
 int conv_launch_bn(const ConvLaunch* l);
+bool conv_launch_a8(const ConvLaunch* l);                  // segment 0 runs as e4m3 (ConvDesc::weight8)
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s);   // same launch, output pointer overridden
 int conv_pick_bn(int cout_pad);
 // whether a conv with this many (unpadded) output channels can also emit the fp16 copy of its fp32 NHWC output
@@ -46,6 +52,8 @@ bool conv_can_fuse_stats(int H, int W);                    // epilogue statistic
 int conv_pad_cout(int cout);
 // packed weight columns per tap of a K segment of c channels (c % 8 == 0): whole 64-channel chunks, zero columns at the pad
 int conv_pad_k(int c);
+// the same for an e4m3 segment 0 (c % 16 == 0): whole 128-channel chunks
+int conv_pad_k8(int c);
 
 // head_ch = 64: attention_kernel; any other multiple of 64: attention_hd_kernel (kErrNotImplemented otherwise)
 AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out);
@@ -64,6 +72,7 @@ struct GnApplyDesc {
   bool film_add = false;                                            // table holds ONE row per channel, added before the norm
   void* out_act = nullptr; void* out_raw16 = nullptr; float* out_raw32 = nullptr;
   void* out_lo = nullptr;      // optional low half of a two-term fp16 split of the output (fp16-source same-resolution path only)
+  bool out_e4m3 = false;       // out_act is e4m3 (one byte per element, satfinite round-to-nearest-even) instead of fp16
 };
 void launch_gn_apply(const GnApplyDesc& d, cudaStream_t s);
 // eps[n][c][h][w] = bias[c] + sum_tap Y[n][h+dy][w+dx][tap*Co + c]  (output head, see eps_gather_kernel)

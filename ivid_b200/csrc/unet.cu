@@ -309,6 +309,11 @@ void pack_out_rows(__half* dst, int C, int Cp, const float* w, int co_n) {
 }
 }  // namespace
 
+void Unet::set_precision(int precision) {
+  IVID_REQUIRE(precision == 0 || precision == 1, "precision must be 0 (fp16) or 1 (fp8 ResBlock convs)");
+  precision_ = precision;
+}
+
 void Unet::finalize(int device) {
   IVID_CHECK_CUDA(cudaSetDevice(device));
   for (const auto& p : params_)
@@ -349,6 +354,55 @@ void Unet::finalize(int device) {
       const float* w2 = P(skip_w).host.data();
       pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, kmain, w2, cout, cin2, 0, s0, s0, 1);
       if (s1 > 0) pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, kmain + conv_pad_k(s0), w2, cout, cin2, s0, s1, s1, 1);
+      const auto& b2 = P(skip_b).host;
+      for (int i = 0; i < cout; ++i) bias[i] += b2[i];
+    }
+    cw.b_off = put_f32(bias);
+    return cw;
+  };
+  // fp8 form of a ResBlock 3x3 conv (DESIGN.md §2): e4m3(w * 2^e) over the cin channels of segment 0, then the 1x1 skip
+  // columns as fp16(w_skip * 2^e) in the layout pack_conv gives them.  The conv stays fp16 (pack_conv) when its operand
+  // rows are not 16-byte multiples, or when the scaled skip weights would overflow fp16 or fall into its subnormals where
+  // the unscaled ones do not.
+  auto pack_res_conv = [&](const std::string& wname, const std::string& bname, int cout, int cin, const std::string& skip_w,
+                           const std::string& skip_b, int cin2, int cin2a = 0) {
+    const auto& w = P(wname).host;
+    float mx = 0.f;
+    for (float v : w) mx = std::max(mx, std::fabs(v));
+    const int e = fp8_weight_exponent(mx);
+    const float scale = std::ldexp(1.0f, e);
+    bool fp8 = precision_ == 1 && cin % 16 == 0 && e >= -100 && e <= 100;
+    std::vector<float> w2s;
+    if (fp8 && cin2 > 0) {
+      const float kMinNormal16 = std::ldexp(1.0f, -14);
+      for (float v : P(skip_w).host) {
+        const float sv = std::fabs(v) * scale;
+        if (sv > 65504.f || (std::fabs(v) >= kMinNormal16 && sv < kMinNormal16)) { fp8 = false; break; }
+        w2s.push_back(v * scale);
+      }
+    }
+    if (!fp8) return pack_conv(wname, bname, cout, cin, conv_pad_k(cin), 3, skip_w, skip_b, cin2, cin2a);
+    ConvW cw;
+    cw.cout = cout;
+    cw.cout_pad = conv_pad_cout(cout);
+    cw.fp8 = true;
+    cw.e8 = e;
+    const int cp8 = conv_pad_k8(cin), K8 = 9 * cp8;
+    cw.w8_off = ab.alloc(static_cast<size_t>(cw.cout_pad) * K8);
+    uint8_t* w8 = ab.at<uint8_t>(cw.w8_off);
+    for (int co = 0; co < cout; ++co)
+      for (int tap = 0; tap < 9; ++tap)
+        for (int ci = 0; ci < cin; ++ci)
+          w8[static_cast<size_t>(co) * K8 + tap * cp8 + ci] = fp8_e4m3_from_float(w[(static_cast<size_t>(co) * cin + ci) * 9 + tap] * scale);
+    std::vector<float> bias(cw.cout_pad, 0.f);
+    const auto& b = P(bname).host;
+    for (int i = 0; i < cout; ++i) bias[i] = b[i];
+    const int s0 = cin2a > 0 ? cin2a : cin2, s1 = cin2 - s0;
+    cw.K = cin2 > 0 ? conv_pad_k(s0) + conv_pad_k(s1) : 0;
+    if (cin2 > 0) {
+      cw.w_off = ab.alloc(static_cast<size_t>(cw.cout_pad) * cw.K * 2);
+      pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, 0, w2s.data(), cout, cin2, 0, s0, s0, 1);
+      if (s1 > 0) pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, conv_pad_k(s0), w2s.data(), cout, cin2, s0, s1, s1, 1);
       const auto& b2 = P(skip_b).host;
       for (int i = 0; i < cout; ++i) bias[i] += b2[i];
     }
@@ -402,10 +456,10 @@ void Unet::finalize(int device) {
     }
   for (auto& r : res_) {
     r.gn1 = pack_gn(r.pfx + ".in_layers.0", r.cin);
-    r.conv1 = pack_conv(r.pfx + ".in_layers.2.weight", r.pfx + ".in_layers.2.bias", r.cout, r.cin, conv_pad_k(r.cin), 3, "", "", 0);
+    r.conv1 = pack_res_conv(r.pfx + ".in_layers.2.weight", r.pfx + ".in_layers.2.bias", r.cout, r.cin, "", "", 0);
     r.gn2 = pack_gn(r.pfx + ".out_layers.0", r.cout);
-    r.conv2 = pack_conv(r.pfx + ".out_layers.3.weight", r.pfx + ".out_layers.3.bias", r.cout, r.cout, conv_pad_k(r.cout), 3,
-                        r.pfx + ".skip_connection.weight", r.pfx + ".skip_connection.bias", r.skip_conv ? r.cin : 0, r.cat0);
+    r.conv2 = pack_res_conv(r.pfx + ".out_layers.3.weight", r.pfx + ".out_layers.3.bias", r.cout, r.cout,
+                            r.pfx + ".skip_connection.weight", r.pfx + ".skip_connection.bias", r.skip_conv ? r.cin : 0, r.cat0);
   }
   for (auto& a : attn_) {
     a.gn = pack_gn(a.pfx + ".norm", a.C);
@@ -573,6 +627,8 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     // N x H x W x C elements of a slot
     auto s16 = [&](Slot s, int H, int Wd, int C) { return scratch(s, static_cast<size_t>(N) * H * Wd * C * 2); };
     auto s32 = [&](Slot s, int H, int Wd, int C) { return static_cast<float*>(scratch(s, static_cast<size_t>(N) * H * Wd * C * 4)); };
+    // conv operand: fp16, or e4m3 (one byte per element) for a conv packed fp8
+    auto sop = [&](Slot s, int H, int Wd, int C, bool e4m3) { return scratch(s, static_cast<size_t>(N) * H * Wd * C * (e4m3 ? 1 : 2)); };
     size_t soff = 0;
     auto take_stats = [&](int C) -> double* {
       const size_t o = soff;
@@ -627,10 +683,14 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
                        (d.C2 > 0 ? static_cast<double>(d.taps2) * d.C2 : 0.0);
       const double M = static_cast<double>(d.N) * d.H * d.W;
       const double Nalg = n_alg > 0.0 ? n_alg : static_cast<double>(d.cout);
-      static const char* names[] = {"conv_gemm<16>", "conv_gemm<64>", "conv_gemm<128>"};
+      static const char* names[2][3] = {{"conv_gemm<16>", "conv_gemm<64>", "conv_gemm<128>"},
+                                        {"conv_gemm<16,e4m3>", "conv_gemm<64,e4m3>", "conv_gemm<128,e4m3>"}};
       const int bn = conv_launch_bn(l);
-      pl->add_op(names[bn == 128 ? 2 : bn == 64 ? 1 : 0], 2.0 * M * K * Nalg,
-                 M * (d.C0 + d.C1 + d.C2) * 2 + M * d.cout * ((d.out_mode == 1 ? 2 : 4) + (d.out16 ? 2 : 0) + (d.residual ? 4 : 0)) + K * d.cout_pad * 2,
+      const bool a8 = conv_launch_a8(l);
+      const double K0 = static_cast<double>(d.taps0) * d.C0;     // bytes per element of segment 0's operands: 1 under a8
+      pl->add_op(names[a8 ? 1 : 0][bn == 128 ? 2 : bn == 64 ? 1 : 0], 2.0 * M * K * Nalg,
+                 M * (d.C0 * (a8 ? 1 : 2) + (d.C1 + d.C2) * 2) + M * d.cout * ((d.out_mode == 1 ? 2 : 4) + (d.out16 ? 2 : 0) + (d.residual ? 4 : 0)) +
+                     (a8 ? K0 + 2 * (K - K0) : 2 * K) * d.cout_pad,
                  std::to_string(d.H) + "x" + std::to_string(d.W) + " " + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") + (d.C2 ? "+" + std::to_string(d.C2) : "") +
                      "->" + std::to_string(d.cout) + " k" + std::to_string(d.taps0) + (d.residual ? " res" : "") + (d.stats ? " stats" : "") +
                      (d.out_mode == 1 ? " f16" : "") + (d.out16 ? " +f16" : ""),
@@ -682,9 +742,10 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       const int Wo = d.mode == 1 ? d.W * 2 : (d.mode == 2 ? d.W / 2 : d.W);
       const double in_el = static_cast<double>(d.N) * d.H * d.W * (d.C0 + d.C1);
       const double out_el = static_cast<double>(d.N) * Ho * Wo * (d.C0 + d.C1);
-      pl->add_op("gn_apply", 0, in_el * (d.x0_half ? 2 : 4) + out_el * 2 + (d.out_raw16 ? out_el * 2 : 0) + (d.out_raw32 ? out_el * 4 : 0),
+      pl->add_op("gn_apply", 0, in_el * (d.x0_half ? 2 : 4) + out_el * (d.out_e4m3 ? 1 : 2) + (d.out_raw16 ? out_el * 2 : 0) + (d.out_raw32 ? out_el * 4 : 0),
                  std::to_string(d.H) + "x" + std::to_string(d.W) + " C" + std::to_string(d.C0) + (d.C1 ? "+" + std::to_string(d.C1) : "") +
-                     " m" + std::to_string(d.mode) + (d.x0_half ? " h16" : "") + (d.out_raw16 ? " raw16" : "") + (d.out_raw32 ? " raw32" : ""),
+                     " m" + std::to_string(d.mode) + (d.x0_half ? " h16" : "") + (d.out_raw16 ? " raw16" : "") + (d.out_raw32 ? " raw32" : "") +
+                     (d.out_e4m3 ? " e4m3" : ""),
                  [d](cudaStream_t s) { launch_gn_apply(d, s); });
     };
 
@@ -739,10 +800,10 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       g1.C0 = x0.C; g1.C1 = x1 ? x1->C : 0;
       g1.N = N; g1.H = H; g1.W = Wd; g1.mode = r.mode; g1.silu = 1;
       IVID_REQUIRE(!(r.skip_conv && r.mode != 0), "internal: up/down ResBlocks keep the channel count");
-      void* a1 = s16(kA1, Ho, Wo, r.cin);
+      void* a1 = sop(kA1, Ho, Wo, r.cin, r.conv1.fp8);
       void* xh = r.skip_conv && !use16 ? s16(kXh, H, Wd, r.cin) : nullptr;
       float* xr = need_xr ? s32(kXr, Ho, Wo, r.cin) : nullptr;
-      g1.out_act = a1; g1.out_raw16 = xh; g1.out_raw32 = xr;
+      g1.out_act = a1; g1.out_raw16 = xh; g1.out_raw32 = xr; g1.out_e4m3 = r.conv1.fp8;
       add_gn(g1, x0, x1, r.gn1, -1);
       // conv1 -> h ; stats.  The hidden tensor only feeds GroupNorm 2: stored as fp16 (half the epilogue and GN traffic);
       // its statistics are taken from the rounded values in the conv epilogue.  Tiny feature maps keep the fp32 +
@@ -755,14 +816,15 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
         ConvDesc d;
         d.act0 = a1; d.C0 = r.cin; d.taps0 = 9;
         d.weight = W8(r.conv1.w_off); d.cout_pad = r.conv1.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv1.b_off);
+        if (r.conv1.fp8) { d.weight8 = W8(r.conv1.w8_off); d.weight = nullptr; d.acc_scale = std::ldexp(1.0f, -r.conv1.e8); }
         d.out = h.data; d.ldc = r.cout; d.out_mode = h_half ? 1 : 0; d.N = N; d.H = Ho; d.W = Wo;
         add_conv(d, &h);
       }
       // GN2 * (1+scale) + shift, SiLU -> a2
-      void* a2 = s16(kA2, Ho, Wo, r.cout);
+      void* a2 = sop(kA2, Ho, Wo, r.cout, r.conv2.fp8);
       GnApplyDesc g2;
       g2.x0 = h.data; g2.x0_half = h_half; g2.C0 = r.cout; g2.N = N; g2.H = Ho; g2.W = Wo; g2.mode = 0; g2.silu = 1;
-      g2.out_act = a2;
+      g2.out_act = a2; g2.out_e4m3 = r.conv2.fp8;
       add_gn(g2, h, nullptr, r.gn2, r.film_off);
       // conv2 (+ 1x1 skip as extra K) + residual -> out
       Act out = new_act(r.cout, Ho, Wo, !identity);
@@ -779,6 +841,11 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
           d.act1 = xh; d.C1 = r.cin; d.taps1 = 1;
         }
         d.weight = W8(r.conv2.w_off); d.cout_pad = r.conv2.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv2.b_off);
+        if (r.conv2.fp8) {
+          d.weight8 = W8(r.conv2.w8_off);
+          if (r.conv2.K == 0) d.weight = nullptr;
+          d.acc_scale = std::ldexp(1.0f, -r.conv2.e8);
+        }
         if (identity) { d.residual = need_xr ? xr : use32(x0); d.ldr = r.cout; d.residual_up = res_up; }
         write_to(d, out);
         add_conv(d, &out);

@@ -39,7 +39,9 @@ struct ParamSpec {
   size_t numel() const { size_t n = 1; for (auto d : shape) n *= static_cast<size_t>(d); return n; }
 };
 
-struct ConvW { int cout = 0, cout_pad = 0, K = 0; size_t w_off = 0, b_off = 0; };
+// fp8: segment 0 runs as e4m3 (see Unet::finalize): w8_off holds its e4m3 columns [cout_pad][taps * conv_pad_k8(cin)],
+// and w_off / K only the fp16 skip columns, all scaled by 2^e8
+struct ConvW { int cout = 0, cout_pad = 0, K = 0; size_t w_off = 0, b_off = 0; bool fp8 = false; int e8 = 0; size_t w8_off = 0; };
 struct GnW { int C = 0; size_t g_off = 0, b_off = 0; };
 struct LinW { int O = 0, K = 0; size_t w_off = 0, b_off = 0; };
 
@@ -91,6 +93,9 @@ class Unet {
   const std::vector<ParamSpec>& params() const { return params_; }
   void set_param(const std::string& name, const float* data, const int64_t* shape, int ndim);
   void finalize(int device);
+  // 0 = fp16 operands everywhere (default), 1 = e4m3 operands for the ResBlock 3x3 convs (DESIGN.md §2); takes effect at
+  // the next finalize
+  void set_precision(int precision);
   bool finalized() const { return arena_ != nullptr; }
   void* arena() const { return arena_; }
   size_t arena_bytes() const { return arena_bytes_; }
@@ -130,6 +135,7 @@ class Unet {
   int film_total_ = 0;
   int in_ch_stem_ = 0;               // channels after the input conv
   int final_ch_ = 0;
+  int precision_ = 0;
 
   // packed weights
   ConvW in_conv_, out_conv_;

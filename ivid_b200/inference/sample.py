@@ -59,11 +59,16 @@ def build_modelviews(viewset, num_samples, rng=None):
 
 @torch.no_grad()
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
-               far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim"):
+               far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
+               precision="fp16"):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
-    (DPM-Solver++(2M)) wherever the reference runs DdimSampler; DDPM at steps_uncond >= 1000 is kept."""
+    (DPM-Solver++(2M)) wherever the reference runs DdimSampler; DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
+    runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision)."""
     assert solver in ("ddim", "dpmpp"), f"solver must be 'ddim' or 'dpmpp', got {solver!r}"
+    for fw in (framework_uncond, framework_cond):
+        if fw is not None and fw.backbone.precision != precision:
+            fw.backbone.set_precision(precision)
     ode = samplers.DdimSampler if solver == "ddim" else samplers.DpmSolverSampler
     sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
@@ -231,14 +236,16 @@ def main(rank, world_size, opt):
     idx = list(range(num))[rank::world_size]
     mvs_r = shard(mvs, rank, world_size) if isinstance(mvs[0], list) else mvs
     solver = getattr(opt, "solver", "ddim")
+    precision = getattr(opt, "precision", "fp16")
     out_dir = os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
-                           + ("" if solver == "ddim" else f"_{solver}"))
+                           + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}"))
     for sub in ("results", "grids", "conds", "scenes"):                 # sample.py:283-286
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
     save_cfg = edict(output_dir=out_dir, viewset=opt.viewset)
     gen = sample_all(fw_u, fw_c, seeds_r if seeds_r is not None else len(idx), opt.steps_uncond, opt.steps_cond, mvs_r, classes=classes_r,
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
-                     rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver)
+                     rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
+                     precision=precision)
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -274,6 +281,8 @@ if __name__ == "__main__":
     ap.add_argument("--solver", choices=["ddim", "dpmpp"], default="ddim",
                     help="ODE sampler of the DDIM-step views: 'ddim' as the reference, 'dpmpp' DPM-Solver++(2M), which needs fewer "
                          "steps for the same convergence (DDPM at --steps_uncond >= 1000 is unchanged)")
+    ap.add_argument("--precision", choices=["fp16", "fp8"], default="fp16",
+                    help="operands of the ResBlock convs: 'fp16' (default) or 'fp8' (e4m3, faster, changes the numbers; DESIGN.md §2)")
     o = ap.parse_args()
     n = torch.cuda.device_count()
     if n <= 1:
