@@ -288,7 +288,9 @@ int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const floa
                    const float* residual_dev, void* out_dev, int out_fp16, void* stream);
 /* The fp8 twin of ivid_op_conv2d: act_dev e4m3 NHWC [N,H,W,Cin] (Cin % 16 == 0); w_host fp32, quantized as the packer
  * does (e4m3(w * 2^e), the e of ivid_fp8_weight_exponent, written to *e_out when e_out is not NULL); the optional fp16
- * 1x1 skip segment is packed as fp16(w2 * 2^e); out = acc * 2^-e + bias (+ residual). */
+ * 1x1 skip segment is packed as fp16(w2 * 2^e); out = acc * 2^-e + bias (+ residual).  Returns IVID_ERR_INVALID_ARGUMENT
+ * wherever the UNet's fp8 mode keeps a conv fp16: Cin % 16 != 0, |e| > 100, or skip weights that overflow fp16 or become
+ * fp16 subnormals once scaled by 2^e. */
 int ivid_op_conv2d_e4m3(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
                         int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
                         const float* residual_dev, void* out_dev, int out_fp16, int* e_out, void* stream);

@@ -229,99 +229,55 @@ int ivid_sampler_run(ivid_sampler_t* s, ivid_unet_t* unet, float* x_inout_dev, i
 // ------------------------------------------------------------------------------------------------------------------
 namespace {
 struct DevBuf {
-  void* p = nullptr;
-  explicit DevBuf(size_t bytes) { IVID_CHECK_CUDA(cudaMalloc(&p, bytes)); }
+  void* p = nullptr;                                 // stays null for zero bytes
+  explicit DevBuf(size_t bytes) { if (bytes > 0) IVID_CHECK_CUDA(cudaMalloc(&p, bytes)); }
   ~DevBuf() { if (p) cudaFree(p); }
   DevBuf(const DevBuf&) = delete;
 };
 }  // namespace
 
-int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
-                   int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
-                   const float* residual_dev, void* out_dev, int out_fp16, void* stream) {
+// one conv, packed by conv_pack; e4m3: segment 0 in e4m3, and its weight exponent goes to e_out
+static int op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host, int Cout,
+                     int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
+                     const float* residual_dev, void* out_dev, int out_fp16, bool e4m3, int* e_out, void* stream) {
   return guarded([&] {
     IVID_NOT_NULL(act_dev); IVID_NOT_NULL(w_host); IVID_NOT_NULL(out_dev);
     IVID_REQUIRE(ksize == 3 || ksize == 1, "conv: kernel size must be 3 or 1");
     IVID_REQUIRE(Cin > 0 && Cin % 8 == 0 && Cin2 % 8 == 0, "conv: channels must be multiples of 8");
+    IVID_REQUIRE(act2_dev == nullptr || w2_host != nullptr, "conv: a skip input (act2_dev) needs its weights (w2_host)");
+    const ConvPack pk = conv_pack(w_host, bias_host, Cout, Cin, ksize, conv_pad_k(Cin), act2_dev ? w2_host : nullptr,
+                                  act2_dev ? bias2_host : nullptr, act2_dev ? Cin2 : 0, 0, e4m3);
+    if (pk.refused != nullptr) throw Error(kErrInvalidArgument, std::string("conv: no e4m3 form: ") + pk.refused);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int taps = ksize * ksize;
-    const int cout_pad = conv_pad_cout(Cout);
-    const int cp = conv_pad_k(Cin);                // per-tap column pitch: whole 64-channel chunks, zero columns at the pad
-    const int K = taps * cp + (act2_dev ? conv_pad_k(Cin2) : 0);
-    std::vector<__half> wp(static_cast<size_t>(cout_pad) * K, __float2half_rn(0.f));
-    for (int co = 0; co < Cout; ++co) {
-      for (int tap = 0; tap < taps; ++tap)
-        for (int ci = 0; ci < Cin; ++ci)
-          wp[static_cast<size_t>(co) * K + tap * cp + ci] = __float2half_rn(w_host[(static_cast<size_t>(co) * Cin + ci) * taps + tap]);
-      if (act2_dev)
-        for (int ci = 0; ci < Cin2; ++ci)
-          wp[static_cast<size_t>(co) * K + taps * cp + ci] = __float2half_rn(w2_host[static_cast<size_t>(co) * Cin2 + ci]);
-    }
-    std::vector<float> bias(cout_pad, 0.f);
-    for (int i = 0; i < Cout; ++i) bias[i] = (bias_host ? bias_host[i] : 0.f) + ((act2_dev && bias2_host) ? bias2_host[i] : 0.f);
-    DevBuf dw(wp.size() * 2), db(bias.size() * 4);
-    IVID_CHECK_CUDA(cudaMemcpyAsync(dw.p, wp.data(), wp.size() * 2, cudaMemcpyHostToDevice, st));
-    IVID_CHECK_CUDA(cudaMemcpyAsync(db.p, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice, st));
+    DevBuf dw8(pk.w8.size()), dw(pk.w16.size() * 2), db(pk.bias.size() * 4);
+    if (pk.e4m3) IVID_CHECK_CUDA(cudaMemcpyAsync(dw8.p, pk.w8.data(), pk.w8.size(), cudaMemcpyHostToDevice, st));
+    if (pk.K > 0) IVID_CHECK_CUDA(cudaMemcpyAsync(dw.p, pk.w16.data(), pk.w16.size() * 2, cudaMemcpyHostToDevice, st));
+    IVID_CHECK_CUDA(cudaMemcpyAsync(db.p, pk.bias.data(), pk.bias.size() * 4, cudaMemcpyHostToDevice, st));
     ConvDesc d;
-    d.act0 = act_dev; d.C0 = Cin; d.taps0 = taps;
+    d.act0 = act_dev; d.C0 = Cin; d.taps0 = ksize * ksize;
     if (act2_dev) { d.act1 = act2_dev; d.C1 = Cin2; d.taps1 = 1; }
-    d.weight = dw.p; d.cout_pad = cout_pad; d.cout = Cout; d.bias = static_cast<const float*>(db.p);
+    d.weight = dw.p; d.weight8 = dw8.p; d.acc_scale = std::ldexp(1.0f, -pk.e);
+    d.cout_pad = pk.cout_pad; d.cout = Cout; d.bias = static_cast<const float*>(db.p);
     d.residual = residual_dev; d.ldr = Cout; d.out = out_dev; d.ldc = Cout; d.out_mode = out_fp16 ? 1 : 0;
     d.N = N; d.H = H; d.W = W;
     std::unique_ptr<ConvLaunch, void (*)(ConvLaunch*)> l(conv_launch_create(d), conv_launch_destroy);
     conv_launch_run(l.get(), st);
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+    if (e_out) *e_out = pk.e;
   });
 }
 
+int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
+                   int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
+                   const float* residual_dev, void* out_dev, int out_fp16, void* stream) {
+  return op_conv2d(act_dev, N, H, W, Cin, w_host, bias_host, Cout, ksize, act2_dev, Cin2, w2_host, bias2_host, residual_dev,
+                   out_dev, out_fp16, false, nullptr, stream);
+}
 int ivid_op_conv2d_e4m3(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
                         int Cout, int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
                         const float* residual_dev, void* out_dev, int out_fp16, int* e_out, void* stream) {
-  return guarded([&] {
-    IVID_NOT_NULL(act_dev); IVID_NOT_NULL(w_host); IVID_NOT_NULL(out_dev);
-    IVID_REQUIRE(ksize == 3 || ksize == 1, "conv: kernel size must be 3 or 1");
-    IVID_REQUIRE(Cin > 0 && Cin % 16 == 0, "conv: an e4m3 operand needs a multiple of 16 channels");
-    IVID_REQUIRE(Cin2 % 8 == 0 && (act2_dev == nullptr || w2_host != nullptr), "conv: skip channels must be a multiple of 8");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int taps = ksize * ksize;
-    const int cout_pad = conv_pad_cout(Cout);
-    const size_t nw = static_cast<size_t>(Cout) * Cin * taps;
-    float mx = 0.f;
-    for (size_t i = 0; i < nw; ++i) mx = std::max(mx, std::fabs(w_host[i]));
-    const int e = fp8_weight_exponent(mx);
-    const float scale = std::ldexp(1.0f, e);
-    const int cp8 = conv_pad_k8(Cin), K8 = taps * cp8;
-    std::vector<uint8_t> w8(static_cast<size_t>(cout_pad) * K8, 0);
-    for (int co = 0; co < Cout; ++co)
-      for (int tap = 0; tap < taps; ++tap)
-        for (int ci = 0; ci < Cin; ++ci)
-          w8[static_cast<size_t>(co) * K8 + tap * cp8 + ci] = fp8_e4m3_from_float(w_host[(static_cast<size_t>(co) * Cin + ci) * taps + tap] * scale);
-    const int K = act2_dev ? conv_pad_k(Cin2) : 0;
-    std::vector<__half> wp(static_cast<size_t>(cout_pad) * std::max(K, 1), __float2half_rn(0.f));
-    for (int co = 0; co < Cout && act2_dev; ++co)
-      for (int ci = 0; ci < Cin2; ++ci) {
-        const float v = w2_host[static_cast<size_t>(co) * Cin2 + ci] * scale;
-        IVID_REQUIRE(std::fabs(v) <= 65504.f, "conv: skip weights times 2^e leave the fp16 range");
-        wp[static_cast<size_t>(co) * K + ci] = __float2half_rn(v);
-      }
-    std::vector<float> bias(cout_pad, 0.f);
-    for (int i = 0; i < Cout; ++i) bias[i] = (bias_host ? bias_host[i] : 0.f) + ((act2_dev && bias2_host) ? bias2_host[i] : 0.f);
-    DevBuf dw8(w8.size()), dw(wp.size() * 2), db(bias.size() * 4);
-    IVID_CHECK_CUDA(cudaMemcpyAsync(dw8.p, w8.data(), w8.size(), cudaMemcpyHostToDevice, st));
-    IVID_CHECK_CUDA(cudaMemcpyAsync(dw.p, wp.data(), wp.size() * 2, cudaMemcpyHostToDevice, st));
-    IVID_CHECK_CUDA(cudaMemcpyAsync(db.p, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice, st));
-    ConvDesc d;
-    d.act0 = act_dev; d.C0 = Cin; d.taps0 = taps;
-    if (act2_dev) { d.act1 = act2_dev; d.C1 = Cin2; d.taps1 = 1; }
-    d.weight8 = dw8.p; d.weight = act2_dev ? dw.p : nullptr; d.acc_scale = std::ldexp(1.0f, -e);
-    d.cout_pad = cout_pad; d.cout = Cout; d.bias = static_cast<const float*>(db.p);
-    d.residual = residual_dev; d.ldr = Cout; d.out = out_dev; d.ldc = Cout; d.out_mode = out_fp16 ? 1 : 0;
-    d.N = N; d.H = H; d.W = W;
-    std::unique_ptr<ConvLaunch, void (*)(ConvLaunch*)> l(conv_launch_create(d), conv_launch_destroy);
-    conv_launch_run(l.get(), st);
-    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
-    if (e_out) *e_out = e;
-  });
+  return op_conv2d(act_dev, N, H, W, Cin, w_host, bias_host, Cout, ksize, act2_dev, Cin2, w2_host, bias2_host, residual_dev,
+                   out_dev, out_fp16, true, e_out, stream);
 }
 
 static int op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,

@@ -10,7 +10,7 @@
 //   pixels) at the tap-shifted coordinate; TMA's out-of-bounds zero fill implements the conv zero padding.  Further
 //   "segments" let a 1x1 skip convolution over a different tensor (raw x) accumulate into the same tile as extra K slabs
 //   (SURVEY K2), so  skip(x) + conv(h)  is one kernel.
-//   B (weights) is packed [Cout_pad][K] fp16, K-major, loaded by 2-D TMA.
+//   B (weights) is packed [Cout_pad][K] fp16, K-major, by conv_pack (ops.cu) on the host, and loaded by 2-D TMA.
 //   Segments of C % 64 != 0 channels (C % 8 == 0) run ceil(C/64) chunks: the activation map keeps the real channel extent, so
 //   TMA zero-fills the channels past C of the last box, and the packed weights hold zero columns there.  Out-of-bounds
 //   elements still count toward the transaction bytes, so every stage expects the full box.
@@ -30,7 +30,7 @@
 // shared-memory layout, TMA bytes and wgmma descriptors of an fp16 one; only the instruction differs (k32 e4m3 for k16
 // f16) and a chunk covers 128 channels.  Its weights come from a second map (b8) over e4m3 columns pre-scaled by 2^e; the
 // fp16 skip segments keep the b map with columns pre-scaled by the same 2^e, so all of K sums into one accumulator, and
-// the epilogue takes v = acc * 2^-e + bias.
+// the epilogue takes v = acc * 2^-e + bias.  conv_pack writes both and decides which convs qualify.
 #pragma once
 #include <type_traits>
 

@@ -61,6 +61,55 @@ bool conv_can_res_up(int W, int cout) { return W >= 16 && cout % 8 == 0; }
 bool conv_can_out16(int cout) { return cout % 8 == 0; }
 int conv_pad_k(int c) { return ((c + 63) / 64) * 64; }
 int conv_pad_k8(int c) { return ((c + 127) / 128) * 128; }
+int conv_seg_cols(int taps, int c) { return taps * conv_pad_k(c); }
+
+ConvPack conv_pack(const float* w, const float* b, int cout, int cin, int ksz, int pitch, const float* w2, const float* b2,
+                   int cin2, int cin2a, bool e4m3) {
+  ConvPack pk;
+  const int taps = ksz * ksz;
+  pk.cout_pad = conv_pad_cout(cout);
+  // e4m3: a power-of-two scale with max|w| * 2^e in (224, 448], shared by the fp16 skip columns
+  float scale = 1.f;
+  if (e4m3) {
+    IVID_REQUIRE(pitch == conv_pad_k(cin), "internal: an e4m3 segment 0 is an ordinary 3x3 or 1x1 conv");
+    float mx = 0.f;
+    for (size_t i = 0; i < static_cast<size_t>(cout) * cin * taps; ++i) mx = std::max(mx, std::fabs(w[i]));
+    const int e = fp8_weight_exponent(mx);
+    const float kMinNormal16 = std::ldexp(1.0f, -14);
+    if (cin % 16 != 0) pk.refused = "its input channels are not a multiple of 16";
+    else if (e < -100 || e > 100) pk.refused = "its weight exponent is outside [-100, 100]";
+    for (size_t i = 0; pk.refused == nullptr && i < static_cast<size_t>(cout) * cin2; ++i) {
+      const float v = std::fabs(w2[i]), sv = v * std::ldexp(1.0f, e);
+      if (sv > 65504.f) pk.refused = "its skip weights times 2^e overflow fp16";
+      else if (v >= kMinNormal16 && sv < kMinNormal16) pk.refused = "its skip weights times 2^e become fp16 subnormals";
+    }
+    pk.e4m3 = pk.refused == nullptr;
+    if (pk.e4m3) { pk.e = e; scale = std::ldexp(1.0f, e); }
+  }
+  const int s0 = cin2a > 0 ? cin2a : cin2, s1 = cin2 - s0;
+  const int k0 = pk.e4m3 ? 0 : conv_seg_cols(1, taps * pitch);     // segment 0 padded once, at its end
+  pk.K = k0 + conv_seg_cols(1, s0) + conv_seg_cols(1, s1);
+  pk.w16.assign(static_cast<size_t>(pk.cout_pad) * pk.K, __float2half_rn(0.f));
+  const int cp8 = conv_pad_k8(cin), K8 = pk.e4m3 ? taps * cp8 : 0;
+  pk.w8.assign(static_cast<size_t>(pk.cout_pad) * K8, 0);
+  for (int co = 0; co < cout; ++co) {
+    __half* row = pk.w16.data() + static_cast<size_t>(co) * pk.K;
+    for (int tap = 0; tap < taps; ++tap)
+      for (int ci = 0; ci < cin; ++ci) {
+        const float v = w[(static_cast<size_t>(co) * cin + ci) * taps + tap];
+        if (pk.e4m3) pk.w8[static_cast<size_t>(co) * K8 + tap * cp8 + ci] = fp8_e4m3_from_float(v * scale);
+        else row[tap * pitch + ci] = __float2half_rn(v);
+      }
+    for (int ci = 0; ci < cin2; ++ci)
+      row[k0 + (ci < s0 ? ci : conv_pad_k(s0) + ci - s0)] = __float2half_rn(w2[static_cast<size_t>(co) * cin2 + ci] * scale);
+  }
+  pk.bias.assign(pk.cout_pad, 0.f);
+  for (int i = 0; i < cout; ++i) {
+    if (b != nullptr) pk.bias[i] = b[i];
+    if (b2 != nullptr) pk.bias[i] += b2[i];
+  }
+  return pk;
+}
 
 ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.C0 > 0 && d.C0 % 8 == 0, "conv: segment-0 channels must be a positive multiple of 8");
@@ -105,8 +154,7 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   // packed weight columns: every segment padded to whole 64-channel chunks per tap (zero columns); the activation maps keep
   // the real channel extent, so TMA zero-fills the missing channels of a segment's last chunk
   // (fp8 mode: segment 0's columns live in weight8, so the fp16 matrix holds the skip segments only)
-  const int Kskip = (d.C1 > 0 ? d.taps1 * conv_pad_k(d.C1) : 0) + (d.C2 > 0 ? d.taps2 * conv_pad_k(d.C2) : 0);
-  const int Ktot = (a8 ? 0 : d.taps0 * conv_pad_k(d.C0)) + Kskip;
+  const int Ktot = (a8 ? 0 : conv_seg_cols(d.taps0, d.C0)) + conv_seg_cols(d.taps1, d.C1) + conv_seg_cols(d.taps2, d.C2);
   ConvMaps8& M = l->maps;
   M.a[0] = a8 ? make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN, CU_TENSOR_MAP_DATA_TYPE_UINT8)
               : make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN);

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "host_util.h"
 
 namespace ivid {
@@ -18,10 +20,11 @@ struct ConvDesc {
   const void* act1 = nullptr; int C1 = 0; int taps1 = 1;   // optional segment 1 (1x1 skip over another tensor)
   const void* act2 = nullptr; int C2 = 0; int taps2 = 1;   // optional segment 2 (second half of a virtual concat)
   void* out16 = nullptr;                                   // optional fp16 NHWC copy of an fp32 output (same ldc)
-  const void* weight = nullptr;                            // fp16 [cout_pad][Ktot], Ktot = sum of taps*conv_pad_k(C) over segments
+  // weights and bias as conv_pack writes them (the stem and the split output head write their own columns in this layout)
+  const void* weight = nullptr;                            // fp16 [cout_pad][Ktot], Ktot = sum of conv_seg_cols over segments
   // fp8 operand mode: act0 is e4m3 NHWC (C0 % 16 == 0) and weight8 its e4m3 weights [cout_pad][taps0*conv_pad_k8(C0)],
-  // scaled by 2^e; `weight` then holds only the skip segments' columns (fp16, scaled by the same 2^e; may be null without
-  // skip segments), and acc_scale = 2^-e
+  // scaled by 2^e; `weight` then holds only the skip segments' columns (fp16, scaled by the same 2^e; null without skip
+  // segments), and acc_scale = 2^-e
   const void* weight8 = nullptr;
   float acc_scale = 1.f;
   int cout_pad = 0;
@@ -54,6 +57,27 @@ int conv_pad_cout(int cout);
 int conv_pad_k(int c);
 // the same for an e4m3 segment 0 (c % 16 == 0): whole 128-channel chunks
 int conv_pad_k8(int c);
+// fp16 weight columns of a K segment of c channels over `taps` taps (0 for c == 0)
+int conv_seg_cols(int taps, int c);
+
+// Host-packed operands of one conv, in the layout conv_launch_create reads.
+struct ConvPack {
+  std::vector<__half> w16;     // [cout_pad][K]: segment 0 (unless e4m3), then the 1x1 skip segments
+  std::vector<uint8_t> w8;     // e4m3 only: segment 0 as e4m3(w * 2^e), [cout_pad][taps * conv_pad_k8(cin)]
+  std::vector<float> bias;     // [cout_pad]: b + b2
+  int cout_pad = 0, K = 0;     // K == 0: an e4m3 conv without skip segments (no fp16 columns)
+  bool e4m3 = false;
+  int e = 0;                   // weight exponent of an e4m3 segment 0 (0 otherwise); the skip columns hold fp16(w2 * 2^e)
+  const char* refused = nullptr;   // why an e4m3 segment 0 was requested but not packed (everything is fp16 then)
+};
+// Packs w [cout][cin][ksz][ksz] (+ bias b; null: zero) as segment 0 at `pitch` columns per tap: conv_pad_k(cin) for an
+// ordinary conv, 64 for the stem, cin for the im2col stride-2 conv (whose taps * cin columns are padded once at the end).
+// An optional 1x1 skip conv w2 [cout][cin2] follows as one K segment per part of a concatenated input (the first cin2a
+// channels, then the rest; cin2a = 0: one segment); its bias b2 (if not null) is folded into the bias.
+// e4m3 asks for segment 0 in e4m3 (DESIGN.md §2), which is refused, leaving the conv fp16, when cin % 16 != 0, when
+// |e| > 100, or when a scaled skip weight would overflow fp16 or turn a normal fp16 weight into a subnormal.
+ConvPack conv_pack(const float* w, const float* b, int cout, int cin, int ksz, int pitch, const float* w2, const float* b2,
+                   int cin2, int cin2a, bool e4m3);
 
 // head_ch = 64: attention_kernel; any other multiple of 64: attention_hd_kernel (kErrNotImplemented otherwise)
 AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out);

@@ -267,16 +267,6 @@ struct ArenaBuilder {
   template <class T> T* at(size_t off) { return reinterpret_cast<T*>(buf.data() + off); }
 };
 
-// [Cout][Cin][k][k] fp32, input channels [ci0, ci0 + cn) -> rows of [taps][cn_pad] fp16 written at column `kcol0` of a
-// [cout_pad][Ktot] matrix (columns past cn in each tap stay zero)
-void pack_conv_rows(__half* dst, int Ktot, int kcol0, const float* w, int cout, int cin, int ci0, int cn, int cn_pad, int ksz) {
-  const int taps = ksz * ksz;
-  for (int co = 0; co < cout; ++co)
-    for (int tap = 0; tap < taps; ++tap)
-      for (int ci = 0; ci < cn; ++ci)
-        dst[static_cast<size_t>(co) * Ktot + kcol0 + tap * cn_pad + ci] =
-            __float2half_rn(w[(static_cast<size_t>(co) * cin + ci0 + ci) * taps + tap]);
-}
 // Stem: the 64 operand channels of the packed network input are  hi | lo | hi  of a two-term fp16 split of x
 // (pack_input_kernel); the matching weight columns are  Wh | Wh | Wl  with W = Wh + Wl, so that the fp16 tensor-core
 // product reproduces x*W to ~2^-21 (the lo*Wl term is dropped).
@@ -334,79 +324,24 @@ void Unet::finalize(int device) {
     g.b_off = put_f32(P(pfx + ".bias").host);
     return g;
   };
-  // generic conv: main weight (ksz x ksz over cin, channel-padded to cin_pad per tap, the whole main part to 64-channel
-  // chunks) + optional 1x1 skip weight over cin2 channels, one K segment per part of a concatenated input (cin2a | rest;
-  // cin2a = 0: one segment), each padded to 64-channel chunks as conv_launch_create expects
-  auto pack_conv = [&](const std::string& wname, const std::string& bname, int cout, int cin, int cin_pad, int ksz,
-                       const std::string& skip_w, const std::string& skip_b, int cin2, int cin2a = 0) {
+  // conv_pack over the named parameters (other arguments as there), placed as e4m3 columns, fp16 columns, bias
+  auto put_conv = [&](const std::string& wname, const std::string& bname, int cout, int cin, int pitch, int ksz,
+                       const std::string& skip_w = "", const std::string& skip_b = "", int cin2 = 0, int cin2a = 0,
+                       bool e4m3 = false) {
+    const ConvPack pk = conv_pack(P(wname).host.data(), P(bname).host.data(), cout, cin, ksz, pitch,
+                                  cin2 > 0 ? P(skip_w).host.data() : nullptr, cin2 > 0 ? P(skip_b).host.data() : nullptr,
+                                  cin2, cin2a, e4m3);
     ConvW cw;
-    cw.cout = cout;
-    cw.cout_pad = conv_pad_cout(cout);
-    const int kmain = conv_pad_k(ksz * ksz * cin_pad);
-    const int s0 = cin2a > 0 ? cin2a : cin2, s1 = cin2 - s0;
-    cw.K = kmain + conv_pad_k(s0) + conv_pad_k(s1);
-    cw.w_off = ab.alloc(static_cast<size_t>(cw.cout_pad) * cw.K * 2);
-    pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, 0, P(wname).host.data(), cout, cin, 0, cin, cin_pad, ksz);
-    std::vector<float> bias(cw.cout_pad, 0.f);
-    const auto& b = P(bname).host;
-    for (int i = 0; i < cout; ++i) bias[i] = b[i];
-    if (cin2 > 0) {
-      const float* w2 = P(skip_w).host.data();
-      pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, kmain, w2, cout, cin2, 0, s0, s0, 1);
-      if (s1 > 0) pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, kmain + conv_pad_k(s0), w2, cout, cin2, s0, s1, s1, 1);
-      const auto& b2 = P(skip_b).host;
-      for (int i = 0; i < cout; ++i) bias[i] += b2[i];
+    cw.cout = cout; cw.cout_pad = pk.cout_pad; cw.K = pk.K; cw.fp8 = pk.e4m3; cw.e8 = pk.e;
+    if (pk.e4m3) {
+      cw.w8_off = ab.alloc(pk.w8.size());
+      std::memcpy(ab.at<uint8_t>(cw.w8_off), pk.w8.data(), pk.w8.size());
     }
-    cw.b_off = put_f32(bias);
-    return cw;
-  };
-  // fp8 form of a ResBlock 3x3 conv (DESIGN.md §2): e4m3(w * 2^e) over the cin channels of segment 0, then the 1x1 skip
-  // columns as fp16(w_skip * 2^e) in the layout pack_conv gives them.  The conv stays fp16 (pack_conv) when its operand
-  // rows are not 16-byte multiples, or when the scaled skip weights would overflow fp16 or fall into its subnormals where
-  // the unscaled ones do not.
-  auto pack_res_conv = [&](const std::string& wname, const std::string& bname, int cout, int cin, const std::string& skip_w,
-                           const std::string& skip_b, int cin2, int cin2a = 0) {
-    const auto& w = P(wname).host;
-    float mx = 0.f;
-    for (float v : w) mx = std::max(mx, std::fabs(v));
-    const int e = fp8_weight_exponent(mx);
-    const float scale = std::ldexp(1.0f, e);
-    bool fp8 = precision_ == 1 && cin % 16 == 0 && e >= -100 && e <= 100;
-    std::vector<float> w2s;
-    if (fp8 && cin2 > 0) {
-      const float kMinNormal16 = std::ldexp(1.0f, -14);
-      for (float v : P(skip_w).host) {
-        const float sv = std::fabs(v) * scale;
-        if (sv > 65504.f || (std::fabs(v) >= kMinNormal16 && sv < kMinNormal16)) { fp8 = false; break; }
-        w2s.push_back(v * scale);
-      }
+    if (pk.K > 0) {
+      cw.w_off = ab.alloc(pk.w16.size() * 2);
+      std::memcpy(ab.at<__half>(cw.w_off), pk.w16.data(), pk.w16.size() * 2);
     }
-    if (!fp8) return pack_conv(wname, bname, cout, cin, conv_pad_k(cin), 3, skip_w, skip_b, cin2, cin2a);
-    ConvW cw;
-    cw.cout = cout;
-    cw.cout_pad = conv_pad_cout(cout);
-    cw.fp8 = true;
-    cw.e8 = e;
-    const int cp8 = conv_pad_k8(cin), K8 = 9 * cp8;
-    cw.w8_off = ab.alloc(static_cast<size_t>(cw.cout_pad) * K8);
-    uint8_t* w8 = ab.at<uint8_t>(cw.w8_off);
-    for (int co = 0; co < cout; ++co)
-      for (int tap = 0; tap < 9; ++tap)
-        for (int ci = 0; ci < cin; ++ci)
-          w8[static_cast<size_t>(co) * K8 + tap * cp8 + ci] = fp8_e4m3_from_float(w[(static_cast<size_t>(co) * cin + ci) * 9 + tap] * scale);
-    std::vector<float> bias(cw.cout_pad, 0.f);
-    const auto& b = P(bname).host;
-    for (int i = 0; i < cout; ++i) bias[i] = b[i];
-    const int s0 = cin2a > 0 ? cin2a : cin2, s1 = cin2 - s0;
-    cw.K = cin2 > 0 ? conv_pad_k(s0) + conv_pad_k(s1) : 0;
-    if (cin2 > 0) {
-      cw.w_off = ab.alloc(static_cast<size_t>(cw.cout_pad) * cw.K * 2);
-      pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, 0, w2s.data(), cout, cin2, 0, s0, s0, 1);
-      if (s1 > 0) pack_conv_rows(ab.at<__half>(cw.w_off), cw.K, conv_pad_k(s0), w2s.data(), cout, cin2, s0, s1, s1, 1);
-      const auto& b2 = P(skip_b).host;
-      for (int i = 0; i < cout; ++i) bias[i] += b2[i];
-    }
-    cw.b_off = put_f32(bias);
+    cw.b_off = put_f32(pk.bias);
     return cw;
   };
   auto pack_lin = [&](const std::string& pfx) {
@@ -444,7 +379,7 @@ void Unet::finalize(int device) {
       std::memcpy(ab.at<float>(film_.b_off) + r.film_off, b.data(), b.size() * 4);
     }
   }
-  in_conv_ = pack_conv("input_blocks.0.0.weight", "input_blocks.0.0.bias", in_ch_stem_, cfg_.in_channels, 64, 3, "", "", 0);
+  in_conv_ = put_conv("input_blocks.0.0.weight", "input_blocks.0.0.bias", in_ch_stem_, cfg_.in_channels, 64, 3);
   IVID_REQUIRE(3 * cfg_.in_channels <= 64, "in_channels must be <= 21 (two-term input split inside 64 operand channels)");
   pack_stem_rows(ab.at<__half>(in_conv_.w_off), in_conv_.K, P("input_blocks.0.0.weight").host.data(), in_ch_stem_, cfg_.in_channels, 64);
   for (auto& r : resample_)
@@ -452,22 +387,24 @@ void Unet::finalize(int device) {
       const std::string sub = r.mode == 2 ? ".op" : ".conv";
       // the stride-2 conv runs as a 1x1 GEMM over the 9C im2col channels (one segment, padded at its end); the upsample
       // conv is an ordinary 3x3 conv over C channels
-      r.w = pack_conv(r.pfx + sub + ".weight", r.pfx + sub + ".bias", r.C, r.C, r.mode == 2 ? r.C : conv_pad_k(r.C), 3, "", "", 0);
+      r.w = put_conv(r.pfx + sub + ".weight", r.pfx + sub + ".bias", r.C, r.C, r.mode == 2 ? r.C : conv_pad_k(r.C), 3);
     }
   for (auto& r : res_) {
     r.gn1 = pack_gn(r.pfx + ".in_layers.0", r.cin);
-    r.conv1 = pack_res_conv(r.pfx + ".in_layers.2.weight", r.pfx + ".in_layers.2.bias", r.cout, r.cin, "", "", 0);
+    r.conv1 = put_conv(r.pfx + ".in_layers.2.weight", r.pfx + ".in_layers.2.bias", r.cout, r.cin, conv_pad_k(r.cin), 3,
+                       "", "", 0, 0, precision_ == 1);
     r.gn2 = pack_gn(r.pfx + ".out_layers.0", r.cout);
-    r.conv2 = pack_res_conv(r.pfx + ".out_layers.3.weight", r.pfx + ".out_layers.3.bias", r.cout, r.cout,
-                            r.pfx + ".skip_connection.weight", r.pfx + ".skip_connection.bias", r.skip_conv ? r.cin : 0, r.cat0);
+    r.conv2 = put_conv(r.pfx + ".out_layers.3.weight", r.pfx + ".out_layers.3.bias", r.cout, r.cout, conv_pad_k(r.cout), 3,
+                       r.pfx + ".skip_connection.weight", r.pfx + ".skip_connection.bias", r.skip_conv ? r.cin : 0, r.cat0,
+                       precision_ == 1);
   }
   for (auto& a : attn_) {
     a.gn = pack_gn(a.pfx + ".norm", a.C);
-    a.qkv = pack_conv(a.pfx + ".qkv.weight", a.pfx + ".qkv.bias", 3 * a.C, a.C, conv_pad_k(a.C), 1, "", "", 0);
-    a.proj = pack_conv(a.pfx + ".proj_out.weight", a.pfx + ".proj_out.bias", a.C, a.C, conv_pad_k(a.C), 1, "", "", 0);
+    a.qkv = put_conv(a.pfx + ".qkv.weight", a.pfx + ".qkv.bias", 3 * a.C, a.C, conv_pad_k(a.C), 1);
+    a.proj = put_conv(a.pfx + ".proj_out.weight", a.pfx + ".proj_out.bias", a.C, a.C, conv_pad_k(a.C), 1);
   }
   out_gn_ = pack_gn("out.0", final_ch_);
-  out_conv_ = pack_conv("out.2.weight", "out.2.bias", cfg_.out_channels, final_ch_, conv_pad_k(final_ch_), 3, "", "", 0);
+  out_conv_ = put_conv("out.2.weight", "out.2.bias", cfg_.out_channels, final_ch_, conv_pad_k(final_ch_), 3);
   // split-precision 1x1 form of the same conv (see pack_out_rows); bias is added by eps_gather_kernel
   out_split_ = 9 * cfg_.out_channels <= 64 && getenv("IVID_NO_OUTSPLIT") == nullptr;
   if (out_split_) {
@@ -609,6 +546,13 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
   const float eps = 1e-5f;
   auto W8 = [&](size_t off) { return arena_ + off; };
   auto Wf = [&](size_t off) { return reinterpret_cast<const float*>(arena_ + off); };
+  // a packed conv's operands (Unet::finalize) as a ConvDesc's weights, output width and bias
+  auto bind = [&](ConvDesc& d, const ConvW& w) {
+    d.weight = w.K > 0 ? W8(w.w_off) : nullptr;
+    d.weight8 = w.fp8 ? W8(w.w8_off) : nullptr;
+    d.acc_scale = std::ldexp(1.0f, -w.e8);
+    d.cout_pad = w.cout_pad; d.cout = w.cout; d.bias = Wf(w.b_off);
+  };
 
   // One walk over the topology, run twice.  The sizing pass (base == nullptr) creates no ops: it records the largest
   // request made of each scratch slot, the shape and storage needs of each block output, and the statistics bytes.  The
@@ -770,7 +714,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     {
       ConvDesc d;
       d.act0 = s_in; d.C0 = 64; d.taps0 = 9;
-      d.weight = W8(in_conv_.w_off); d.cout_pad = in_conv_.cout_pad; d.cout = in_conv_.cout; d.bias = Wf(in_conv_.b_off);
+      bind(d, in_conv_);
       write_to(d, cur);
       add_conv(d, &cur, 9.0 * cfg_.in_channels);
       if (create) pl->taps.push_back({"input_blocks.0.0", cur.data, cur.d16, cur.C, cur.H, cur.W});
@@ -815,8 +759,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       {
         ConvDesc d;
         d.act0 = a1; d.C0 = r.cin; d.taps0 = 9;
-        d.weight = W8(r.conv1.w_off); d.cout_pad = r.conv1.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv1.b_off);
-        if (r.conv1.fp8) { d.weight8 = W8(r.conv1.w8_off); d.weight = nullptr; d.acc_scale = std::ldexp(1.0f, -r.conv1.e8); }
+        bind(d, r.conv1);
         d.out = h.data; d.ldc = r.cout; d.out_mode = h_half ? 1 : 0; d.N = N; d.H = Ho; d.W = Wo;
         add_conv(d, &h);
       }
@@ -840,12 +783,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
           IVID_REQUIRE(r.cat0 % 64 == 0, "internal: raw-copy skip conv over a concat whose first part is not a multiple of 64");
           d.act1 = xh; d.C1 = r.cin; d.taps1 = 1;
         }
-        d.weight = W8(r.conv2.w_off); d.cout_pad = r.conv2.cout_pad; d.cout = r.cout; d.bias = Wf(r.conv2.b_off);
-        if (r.conv2.fp8) {
-          d.weight8 = W8(r.conv2.w8_off);
-          if (r.conv2.K == 0) d.weight = nullptr;
-          d.acc_scale = std::ldexp(1.0f, -r.conv2.e8);
-        }
+        bind(d, r.conv2);
         if (identity) { d.residual = need_xr ? xr : use32(x0); d.ldr = r.cout; d.residual_up = res_up; }
         write_to(d, out);
         add_conv(d, &out);
@@ -866,7 +804,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       {
         ConvDesc d;
         d.act0 = a1; d.C0 = a.C; d.taps0 = 1;
-        d.weight = W8(a.qkv.w_off); d.cout_pad = a.qkv.cout_pad; d.cout = 3 * a.C; d.bias = Wf(a.qkv.b_off);
+        bind(d, a.qkv);
         d.out = qkv; d.ldc = 3 * a.C; d.out_mode = 1; d.N = N; d.H = x.H; d.W = x.W;
         add_conv(d);
       }
@@ -881,7 +819,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       {
         ConvDesc d;
         d.act0 = a2; d.C0 = a.C; d.taps0 = 1;
-        d.weight = W8(a.proj.w_off); d.cout_pad = a.proj.cout_pad; d.cout = a.C; d.bias = Wf(a.proj.b_off);
+        bind(d, a.proj);
         d.residual = use32(x); d.ldr = a.C;
         write_to(d, out);
         add_conv(d, &out);
@@ -913,7 +851,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
                        [=](cudaStream_t s) { launch_upsample2x_h16(x16, up, N, H, Wd, C, s); });
           d.act0 = up; d.C0 = C; d.taps0 = 9;
         }
-        d.weight = W8(r.w.w_off); d.cout_pad = r.w.cout_pad; d.cout = C; d.bias = Wf(r.w.b_off);
+        bind(d, r.w);
         write_to(d, out);
         add_conv(d, &out, 9.0 * C);
       } else {
@@ -970,7 +908,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       d.act0 = a1; d.C0 = cur.C; d.taps0 = 1;
       d.act1 = a2; d.C1 = cur.C; d.taps1 = 1;
       d.act2 = a1; d.C2 = cur.C; d.taps2 = 1;
-      d.weight = W8(out1x1_.w_off); d.cout_pad = 64; d.cout = 64; d.bias = Wf(out1x1_.b_off);
+      bind(d, out1x1_);
       d.out = Y; d.ldc = 64; d.out_mode = 0; d.N = N; d.H = SH; d.W = SW;
       add_conv(d, nullptr, 9.0 * cur.C, static_cast<double>(cfg_.out_channels));
       if (create) {
@@ -984,7 +922,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     } else if (create) {
       ConvDesc d;
       d.act0 = a1; d.C0 = cur.C; d.taps0 = 9;
-      d.weight = W8(out_conv_.w_off); d.cout_pad = out_conv_.cout_pad; d.cout = cfg_.out_channels; d.bias = Wf(out_conv_.b_off);
+      bind(d, out_conv_);
       d.out = nullptr; d.ldc = 0; d.out_mode = 2; d.N = N; d.H = SH; d.W = SW;
       ConvLaunch* l = conv_launch_create(d);
       pl->convs.push_back(l);

@@ -39,8 +39,9 @@ struct ParamSpec {
   size_t numel() const { size_t n = 1; for (auto d : shape) n *= static_cast<size_t>(d); return n; }
 };
 
-// fp8: segment 0 runs as e4m3 (see Unet::finalize): w8_off holds its e4m3 columns [cout_pad][taps * conv_pad_k8(cin)],
-// and w_off / K only the fp16 skip columns, all scaled by 2^e8
+// A conv's operands in the weight arena, as conv_pack lays them out: fp16 columns [cout_pad][K] at w_off (none when K == 0)
+// and the bias at b_off.  fp8: segment 0 runs as e4m3 from its columns at w8_off, and the fp16 columns are only the skip
+// segments', all scaled by 2^e8.  Unet::build_plan binds them to a ConvDesc.
 struct ConvW { int cout = 0, cout_pad = 0, K = 0; size_t w_off = 0, b_off = 0; bool fp8 = false; int e8 = 0; size_t w8_off = 0; };
 struct GnW { int C = 0; size_t g_off = 0, b_off = 0; };
 struct LinW { int O = 0, K = 0; size_t w_off = 0, b_off = 0; };

@@ -72,6 +72,41 @@ def test_fp8_entry_points_exported():
         assert hasattr(L, name)
 
 
+def _conv_op_status(e4m3, Cin, w, w2=None, act2=False):
+    """Status and message of a conv op call whose device pointers are dummies, so it is only meaningful for arguments that
+    are rejected before any CUDA call."""
+    L = _lib.lib()
+    dev = 0x1000                                          # never dereferenced
+    Cout, k = w.shape[0], w.shape[-1]
+    w = np.ascontiguousarray(w, dtype=np.float32)
+    b = np.zeros(Cout, dtype=np.float32)
+    w2 = None if w2 is None else np.ascontiguousarray(w2, dtype=np.float32)
+    Cin2 = 64 if act2 else 0
+    args = (dev, 1, 16, 16, Cin, w.ctypes.data, b.ctypes.data, Cout, k, dev if act2 else None, Cin2,
+            None if w2 is None else w2.ctypes.data, None, None, dev, 0)
+    rc = L.ivid_op_conv2d_e4m3(*args, None, None) if e4m3 else L.ivid_op_conv2d(*args, None)
+    return rc, _lib.last_error()
+
+
+def test_conv_ops_reject_before_any_cuda_call():
+    w = np.random.default_rng(0).standard_normal((64, 64, 3, 3)).astype(np.float32) * 0.05
+    # a skip input without its weights, for both entries
+    for e4m3 in (False, True):
+        rc, msg = _conv_op_status(e4m3, 64, w, act2=True)
+        assert rc == _lib.IVID_ERR_INVALID_ARGUMENT and "w2_host" in msg, (e4m3, msg)
+    # e4m3 only where the network's fp8 mode would run the conv in e4m3
+    rc, msg = _conv_op_status(True, 40, w[:, :40])
+    assert rc == _lib.IVID_ERR_INVALID_ARGUMENT and "multiple of 16" in msg, msg
+    rc, msg = _conv_op_status(True, 64, w * 1e-36)                     # e > 100
+    assert rc == _lib.IVID_ERR_INVALID_ARGUMENT and "exponent" in msg, msg
+    w_small = w / np.abs(w).max() * 1e-3                               # e = 18: a skip weight of 1 scales to 2^18
+    rc, msg = _conv_op_status(True, 64, w_small, np.full((64, 64), 1.0), act2=True)
+    assert rc == _lib.IVID_ERR_INVALID_ARGUMENT and "overflow" in msg, msg
+    w_large = w / np.abs(w).max() * 1e3                                # e = -2: 1e-4 (a normal fp16) scales to 2.5e-5
+    rc, msg = _conv_op_status(True, 64, w_large, np.full((64, 64), 1e-4), act2=True)
+    assert rc == _lib.IVID_ERR_INVALID_ARGUMENT and "subnormal" in msg, msg
+
+
 def test_set_precision_rejects_unknown_values():
     import pytest
     import ivid_b200.backbones as backbones
