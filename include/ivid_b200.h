@@ -302,6 +302,49 @@ int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1,
 int ivid_op_group_norm_e4m3(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
                             float eps, const float* gamma_host, const float* beta_host, const float* film_dev,
                             int silu, int mode, void* out_e4m3_dev, void* stream);
+/* One conv with every epilogue form the UNet uses (ivid_op_conv2d and ivid_op_conv2d_e4m3 are this call with a subset):
+ *   segment 0: act0_dev fp16 NHWC [N,H,W,C0] (e4m3 = 1: e4m3, C0 % 16 == 0, quantized as ivid_op_conv2d_e4m3 does; the
+ *              weight exponent goes to *e_out when e_out is not NULL), w0_host fp32 [Cout,C0,k,k], b0_host [Cout] or NULL;
+ *   optional 1x1 skip over act1_dev [N,H,W,C1], or over the virtual concat of act1_dev and act2_dev [N,H,W,C2]:
+ *              wskip_host fp32 [Cout,C1+C2], bskip_host [Cout] or NULL (C1, C2 % 8 == 0);
+ *   residual_dev fp32 NHWC [N,H,W,Cout], or with residual_up = 1 [N,H/2,W/2,Cout] added through a nearest-2x upsample;
+ *   out_mode 0: out_dev fp32 NHWC [N,H,W,Cout]; 1: fp16 NHWC; 2: fp32 NCHW [N,Cout,H,W];
+ *   out16_dev: optional fp16 NHWC copy of an fp32 NHWC output;
+ *   stats_dev: optional fp64 [N,Cout,2] per-(sample, channel) sum and sum of squares of the output (of the fp16 values for
+ *              out_mode 1, of the fp32 values after the residual otherwise).  The kernel adds to it: zero it first.
+ * Returns IVID_ERR_INVALID_ARGUMENT where the network never runs a combination: statistics when the conv tile holds fewer
+ * than 32 pixels of one sample (ivid_conv_tile's fused_stats = 0) or with an NCHW output, residual_up at W < 16, out16
+ * without an fp32 NHWC output, a residual with an NCHW output. */
+typedef struct {
+  const void* act0_dev; int C0; int ksize; const float* w0_host; const float* b0_host;
+  int e4m3; int* e_out;
+  const void* act1_dev; int C1; const void* act2_dev; int C2; const float* wskip_host; const float* bskip_host;
+  const float* residual_dev; int residual_up;
+  int N, H, W, Cout;
+  void* out_dev; int out_mode; void* out16_dev; double* stats_dev;
+} ivid_op_conv_t;
+int ivid_op_conv2d_ex(const ivid_op_conv_t* args, void* stream);
+/* GroupNorm apply with every option the UNet uses (ivid_op_group_norm and ivid_op_group_norm_e4m3 are this call with a
+ * subset): y = [SiLU](GN(x) [* (1 + scale) + shift]) over the virtual concat of x0_dev [N,H,W,C0] and x1_dev [N,H,W,C1]
+ * (NHWC, fp32, or fp16 with x_fp16 = 1);
+ *   stats0_dev / stats1_dev: fp64 [N,C0,2] / [N,C1,2] per-channel sum and sum of squares of each source over H*W; NULL:
+ *              computed here (fp32 sources only);
+ *   film_dev:  optional [N,film_ld] table; scale = film[n][film_off + c], shift = film[n][film_off + C + c]; film_add = 1
+ *              (use_scale_shift_norm=False): y = GN(x + film[n][film_off + c]) instead;
+ *   mode 0 same resolution, 1 nearest-2x upsample, 2 2x2 average pool (fp32 sources);
+ *   out_dev fp16 NHWC at the output resolution (out_e4m3 = 1: e4m3, C0 + C1 a multiple of 16);
+ *   out_lo_dev: optional fp16 low half of the two-term split fp16(y - hi) (mode 0, fp16 sources, no raw outputs);
+ *   out_raw16_dev: optional fp16 copy of x (mode 0, fp32 sources); out_raw32_dev: optional fp32 x resampled as y is. */
+typedef struct {
+  const void* x0_dev; int C0; const void* x1_dev; int C1; int x_fp16;
+  const double* stats0_dev; const double* stats1_dev;
+  int N, H, W, groups; float eps;
+  const float* gamma_host; const float* beta_host;
+  const float* film_dev; int film_ld; int film_off; int film_add;
+  int silu, mode;
+  void* out_dev; int out_e4m3; void* out_lo_dev; void* out_raw16_dev; float* out_raw32_dev;
+} ivid_op_gn_t;
+int ivid_op_group_norm_apply(const ivid_op_gn_t* args, void* stream);
 /* QKVAttention (adm.py:233-253): qkv fp16 [N,T,3C] (legacy head-major q|k|v order) -> fp16 [N,T,C]. */
 int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, void* stream);
 /* The same with head width head_channels = C / heads (a multiple of 64, dividing C): qkv fp16 [N,T,3C] in the order

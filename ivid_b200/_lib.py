@@ -60,6 +60,31 @@ class StepArgsT(Structure):
     ]
 
 
+class OpConvT(Structure):
+    _fields_ = [
+        ("act0_dev", c_void_p), ("C0", c_int), ("ksize", c_int), ("w0_host", c_void_p), ("b0_host", c_void_p),
+        ("e4m3", c_int), ("e_out", POINTER(c_int)),
+        ("act1_dev", c_void_p), ("C1", c_int), ("act2_dev", c_void_p), ("C2", c_int), ("wskip_host", c_void_p),
+        ("bskip_host", c_void_p),
+        ("residual_dev", c_void_p), ("residual_up", c_int),
+        ("N", c_int), ("H", c_int), ("W", c_int), ("Cout", c_int),
+        ("out_dev", c_void_p), ("out_mode", c_int), ("out16_dev", c_void_p), ("stats_dev", c_void_p),
+    ]
+
+
+class OpGnT(Structure):
+    _fields_ = [
+        ("x0_dev", c_void_p), ("C0", c_int), ("x1_dev", c_void_p), ("C1", c_int), ("x_fp16", c_int),
+        ("stats0_dev", c_void_p), ("stats1_dev", c_void_p),
+        ("N", c_int), ("H", c_int), ("W", c_int), ("groups", c_int), ("eps", c_float),
+        ("gamma_host", c_void_p), ("beta_host", c_void_p),
+        ("film_dev", c_void_p), ("film_ld", c_int), ("film_off", c_int), ("film_add", c_int),
+        ("silu", c_int), ("mode", c_int),
+        ("out_dev", c_void_p), ("out_e4m3", c_int), ("out_lo_dev", c_void_p), ("out_raw16_dev", c_void_p),
+        ("out_raw32_dev", c_void_p),
+    ]
+
+
 class WarpParamsT(Structure):
     _fields_ = [("fov_deg", c_double), ("near", c_double), ("far", c_double), ("atol", c_double), ("rtol", c_double),
                 ("erode_rgb", c_int), ("padding", c_double)]
@@ -103,6 +128,8 @@ SIGNATURES = {
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), c_void_p]),
     "ivid_op_group_norm_e4m3": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                         c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "ivid_op_conv2d_ex": (c_int, [POINTER(OpConvT), c_void_p]),
+    "ivid_op_group_norm_apply": (c_int, [POINTER(OpGnT), c_void_p]),
     "ivid_op_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention_heads": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_warp_create": (c_int, [c_int, c_int, c_int, c_int, c_double, c_double, c_int, POINTER(c_void_p)]),

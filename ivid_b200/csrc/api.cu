@@ -236,17 +236,20 @@ struct DevBuf {
 };
 }  // namespace
 
-// one conv, packed by conv_pack; e4m3: segment 0 in e4m3, and its weight exponent goes to e_out
-static int op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host, int Cout,
-                     int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
-                     const float* residual_dev, void* out_dev, int out_fp16, bool e4m3, int* e_out, void* stream) {
+// One conv as the network builds it: packed by conv_pack (cin2a = C1 for a skip over two tensors), every ConvDesc field the
+// network sets taken from the arguments, and conv_launch_create left to reject the combinations it does not run.
+int ivid_op_conv2d_ex(const ivid_op_conv_t* a, void* stream) {
   return guarded([&] {
-    IVID_NOT_NULL(act_dev); IVID_NOT_NULL(w_host); IVID_NOT_NULL(out_dev);
-    IVID_REQUIRE(ksize == 3 || ksize == 1, "conv: kernel size must be 3 or 1");
-    IVID_REQUIRE(Cin > 0 && Cin % 8 == 0 && Cin2 % 8 == 0, "conv: channels must be multiples of 8");
-    IVID_REQUIRE(act2_dev == nullptr || w2_host != nullptr, "conv: a skip input (act2_dev) needs its weights (w2_host)");
-    const ConvPack pk = conv_pack(w_host, bias_host, Cout, Cin, ksize, conv_pad_k(Cin), act2_dev ? w2_host : nullptr,
-                                  act2_dev ? bias2_host : nullptr, act2_dev ? Cin2 : 0, 0, e4m3);
+    IVID_NOT_NULL(a);
+    IVID_NOT_NULL(a->act0_dev); IVID_NOT_NULL(a->w0_host); IVID_NOT_NULL(a->out_dev);
+    IVID_REQUIRE(a->ksize == 3 || a->ksize == 1, "conv: kernel size must be 3 or 1");
+    IVID_REQUIRE(a->C0 > 0 && a->C0 % 8 == 0 && a->C1 % 8 == 0 && a->C2 % 8 == 0, "conv: channels must be multiples of 8");
+    IVID_REQUIRE(a->act1_dev == nullptr || a->wskip_host != nullptr, "conv: a skip input needs its weights (w2_host; wskip_host of ivid_op_conv2d_ex)");
+    IVID_REQUIRE(a->act2_dev == nullptr || (a->act1_dev != nullptr && a->C2 > 0), "conv: act2_dev is the second part of a skip over act1_dev");
+    IVID_REQUIRE(a->out_mode >= 0 && a->out_mode <= 2, "conv: out_mode must be 0, 1 or 2");
+    const int C1 = a->act1_dev ? a->C1 : 0, C2 = a->act2_dev ? a->C2 : 0;
+    const ConvPack pk = conv_pack(a->w0_host, a->b0_host, a->Cout, a->C0, a->ksize, conv_pad_k(a->C0), C1 ? a->wskip_host : nullptr,
+                                  C1 ? a->bskip_host : nullptr, C1 + C2, C2 ? C1 : 0, a->e4m3 != 0);
     if (pk.refused != nullptr) throw Error(kErrInvalidArgument, std::string("conv: no e4m3 form: ") + pk.refused);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     DevBuf dw8(pk.w8.size()), dw(pk.w16.size() * 2), db(pk.bias.size() * 4);
@@ -254,17 +257,32 @@ static int op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const fl
     if (pk.K > 0) IVID_CHECK_CUDA(cudaMemcpyAsync(dw.p, pk.w16.data(), pk.w16.size() * 2, cudaMemcpyHostToDevice, st));
     IVID_CHECK_CUDA(cudaMemcpyAsync(db.p, pk.bias.data(), pk.bias.size() * 4, cudaMemcpyHostToDevice, st));
     ConvDesc d;
-    d.act0 = act_dev; d.C0 = Cin; d.taps0 = ksize * ksize;
-    if (act2_dev) { d.act1 = act2_dev; d.C1 = Cin2; d.taps1 = 1; }
+    d.act0 = a->act0_dev; d.C0 = a->C0; d.taps0 = a->ksize * a->ksize;
+    if (C1) { d.act1 = a->act1_dev; d.C1 = C1; d.taps1 = 1; }
+    if (C2) { d.act2 = a->act2_dev; d.C2 = C2; d.taps2 = 1; }
     d.weight = dw.p; d.weight8 = dw8.p; d.acc_scale = std::ldexp(1.0f, -pk.e);
-    d.cout_pad = pk.cout_pad; d.cout = Cout; d.bias = static_cast<const float*>(db.p);
-    d.residual = residual_dev; d.ldr = Cout; d.out = out_dev; d.ldc = Cout; d.out_mode = out_fp16 ? 1 : 0;
-    d.N = N; d.H = H; d.W = W;
+    d.cout_pad = pk.cout_pad; d.cout = a->Cout; d.bias = static_cast<const float*>(db.p);
+    d.residual = a->residual_dev; d.ldr = a->Cout; d.residual_up = a->residual_up != 0;
+    d.out = a->out_dev; d.ldc = a->Cout; d.out_mode = a->out_mode; d.out16 = a->out16_dev; d.stats = a->stats_dev;
+    d.N = a->N; d.H = a->H; d.W = a->W;
     std::unique_ptr<ConvLaunch, void (*)(ConvLaunch*)> l(conv_launch_create(d), conv_launch_destroy);
     conv_launch_run(l.get(), st);
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
-    if (e_out) *e_out = pk.e;
+    if (a->e_out) *a->e_out = pk.e;
   });
+}
+
+static int op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host, int Cout,
+                     int ksize, const void* act2_dev, int Cin2, const float* w2_host, const float* bias2_host,
+                     const float* residual_dev, void* out_dev, int out_fp16, bool e4m3, int* e_out, void* stream) {
+  ivid_op_conv_t a{};
+  a.act0_dev = act_dev; a.C0 = Cin; a.ksize = ksize; a.w0_host = w_host; a.b0_host = bias_host;
+  a.e4m3 = e4m3 ? 1 : 0; a.e_out = e_out;
+  a.act1_dev = act2_dev; a.C1 = act2_dev ? Cin2 : 0; a.wskip_host = w2_host; a.bskip_host = bias2_host;
+  a.residual_dev = residual_dev;
+  a.N = N; a.H = H; a.W = W; a.Cout = Cout;
+  a.out_dev = out_dev; a.out_mode = out_fp16 ? 1 : 0;
+  return ivid_op_conv2d_ex(&a, stream);
 }
 
 int ivid_op_conv2d(const void* act_dev, int N, int H, int W, int Cin, const float* w_host, const float* bias_host,
@@ -280,30 +298,53 @@ int ivid_op_conv2d_e4m3(const void* act_dev, int N, int H, int W, int Cin, const
                    out_dev, out_fp16, true, e_out, stream);
 }
 
-static int op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
-                         float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
-                         int mode, void* out_fp16_dev, bool e4m3, void* stream) {
+// One GroupNorm apply as the network launches it; statistics a caller does not supply are taken here by gn_stats (fp32
+// sources).  launch_gn_apply rejects the combinations the network does not run.
+int ivid_op_group_norm_apply(const ivid_op_gn_t* a, void* stream) {
   return guarded([&] {
-    IVID_NOT_NULL(x0_dev); IVID_NOT_NULL(gamma_host); IVID_NOT_NULL(beta_host); IVID_NOT_NULL(out_fp16_dev);
+    IVID_NOT_NULL(a);
+    IVID_NOT_NULL(a->x0_dev); IVID_NOT_NULL(a->gamma_host); IVID_NOT_NULL(a->beta_host); IVID_NOT_NULL(a->out_dev);
+    const int N = a->N, HW = a->H * a->W, C0 = a->C0, C1 = a->x1_dev ? a->C1 : 0, C = C0 + C1;
+    IVID_REQUIRE(N > 0 && HW > 0 && C0 > 0, "group norm: empty tensor");
+    IVID_REQUIRE(a->film_dev == nullptr || a->film_ld >= a->film_off + (a->film_add ? C : 2 * C),
+                 "group norm: the FiLM row (film_off + C, or + 2C with a shift) must fit film_ld");
+    const bool need0 = a->stats0_dev == nullptr, need1 = C1 > 0 && a->stats1_dev == nullptr;
+    IVID_REQUIRE(!(need0 || need1) || !a->x_fp16, "group norm: statistics of fp16 sources must be supplied");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int C = C0 + (x1_dev ? C1 : 0);
-    if (!x1_dev) C1 = 0;
-    DevBuf dg(C * 4), dbt(C * 4), st0(static_cast<size_t>(N) * C0 * 16), st1(static_cast<size_t>(N) * std::max(C1, 1) * 16);
-    IVID_CHECK_CUDA(cudaMemcpyAsync(dg.p, gamma_host, C * 4, cudaMemcpyHostToDevice, st));
-    IVID_CHECK_CUDA(cudaMemcpyAsync(dbt.p, beta_host, C * 4, cudaMemcpyHostToDevice, st));
-    IVID_CHECK_CUDA(cudaMemsetAsync(st0.p, 0, static_cast<size_t>(N) * C0 * 16, st));
-    IVID_CHECK_CUDA(cudaMemsetAsync(st1.p, 0, static_cast<size_t>(N) * std::max(C1, 1) * 16, st));
-    launch_gn_stats(x0_dev, static_cast<double*>(st0.p), N, H * W, C0, st);
-    if (C1 > 0) launch_gn_stats(x1_dev, static_cast<double*>(st1.p), N, H * W, C1, st);
+    DevBuf dg(C * 4), dbt(C * 4), st0(need0 ? static_cast<size_t>(N) * C0 * 16 : 0), st1(need1 ? static_cast<size_t>(N) * C1 * 16 : 0);
+    IVID_CHECK_CUDA(cudaMemcpyAsync(dg.p, a->gamma_host, C * 4, cudaMemcpyHostToDevice, st));
+    IVID_CHECK_CUDA(cudaMemcpyAsync(dbt.p, a->beta_host, C * 4, cudaMemcpyHostToDevice, st));
+    if (need0) {
+      IVID_CHECK_CUDA(cudaMemsetAsync(st0.p, 0, static_cast<size_t>(N) * C0 * 16, st));
+      launch_gn_stats(static_cast<const float*>(a->x0_dev), static_cast<double*>(st0.p), N, HW, C0, st);
+    }
+    if (need1) {
+      IVID_CHECK_CUDA(cudaMemsetAsync(st1.p, 0, static_cast<size_t>(N) * C1 * 16, st));
+      launch_gn_stats(static_cast<const float*>(a->x1_dev), static_cast<double*>(st1.p), N, HW, C1, st);
+    }
     GnApplyDesc g;
-    g.x0 = x0_dev; g.x1 = C1 > 0 ? x1_dev : nullptr; g.C0 = C0; g.C1 = C1; g.N = N; g.H = H; g.W = W; g.mode = mode;
-    g.silu = silu; g.out_act = out_fp16_dev; g.out_e4m3 = e4m3;
-    g.stats0 = static_cast<double*>(st0.p); g.stats1 = C1 > 0 ? static_cast<double*>(st1.p) : nullptr;
-    g.groups = groups; g.eps = eps; g.gamma = static_cast<float*>(dg.p); g.beta = static_cast<float*>(dbt.p);
-    g.film = film_dev; g.film_ld = 2 * C; g.film_off = 0;
+    g.x0 = a->x0_dev; g.x1 = C1 > 0 ? a->x1_dev : nullptr; g.C0 = C0; g.C1 = C1; g.x0_half = a->x_fp16 != 0;
+    g.N = N; g.H = a->H; g.W = a->W; g.mode = a->mode; g.silu = a->silu;
+    g.stats0 = need0 ? static_cast<const double*>(st0.p) : a->stats0_dev;
+    g.stats1 = C1 == 0 ? nullptr : (need1 ? static_cast<const double*>(st1.p) : a->stats1_dev);
+    g.groups = a->groups; g.eps = a->eps; g.gamma = static_cast<float*>(dg.p); g.beta = static_cast<float*>(dbt.p);
+    g.film = a->film_dev; g.film_ld = a->film_ld; g.film_off = a->film_off; g.film_add = a->film_add != 0;
+    g.out_act = a->out_dev; g.out_e4m3 = a->out_e4m3 != 0; g.out_lo = a->out_lo_dev;
+    g.out_raw16 = a->out_raw16_dev; g.out_raw32 = a->out_raw32_dev;
     launch_gn_apply(g, st);
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
   });
+}
+
+static int op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
+                         float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
+                         int mode, void* out_dev, bool e4m3, void* stream) {
+  ivid_op_gn_t a{};
+  a.x0_dev = x0_dev; a.C0 = C0; a.x1_dev = x1_dev; a.C1 = x1_dev ? C1 : 0;
+  a.N = N; a.H = H; a.W = W; a.groups = groups; a.eps = eps; a.gamma_host = gamma_host; a.beta_host = beta_host;
+  a.film_dev = film_dev; a.film_ld = 2 * (a.C0 + a.C1); a.film_off = 0;
+  a.silu = silu; a.mode = mode; a.out_dev = out_dev; a.out_e4m3 = e4m3 ? 1 : 0;
+  return ivid_op_group_norm_apply(&a, stream);
 }
 
 int ivid_op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
