@@ -57,6 +57,7 @@ class StepArgsT(Structure):
         ("order", c_int),             # kind 2 (DPM-Solver++): 1 or 2 (0 = 2)
         ("prev_x0_dev", c_void_p),    # kind 2, single step: the previous step's pred_x0 (NULL = first order)
         ("t_last", c_int),            # kind 2, single step: the previous step's t
+        ("sde", c_int),               # kind 2: 1 = the stochastic (SDE) update, which reads step noise
     ]
 
 

@@ -66,12 +66,13 @@ struct GuideParams {           // DDIM multiview guidance (all maps fp32 NCHW, n
 constexpr int kStepDdpm = 0, kStepDdim = 1, kStepDpm = 2;
 
 // DPM-Solver++ per-step scalars, computed in double by the step-state kernel and rounded to fp32 (sampler.cu):
-//   x_p = c_xt * x_t - c_d * D,  D = D0 (order 1) or w0 * D0 + w1 * D_{-1} (order 2)
+//   x_p = c_xt * x_t - c_d * D (+ c_z * z),  D = D0 (order 1) or w0 * D0 + w1 * D_{-1} (order 2)
 struct DpmStep {
-  float c_xt;                  // sigma_p / sigma_s
-  float c_d;                   // alpha_p * (exp(-h) - 1)
+  float c_xt;                  // ODE: sigma_p / sigma_s;             SDE: sigma_p / sigma_s * exp(-h)
+  float c_d;                   // ODE: alpha_p * (exp(-h) - 1);       SDE: alpha_p * (exp(-2h) - 1)
   float w0, w1;                // 1 + 1/(2r), -1/(2r)
   int order;                   // 1 or 2
+  float c_z;                   // ODE: 0;                             SDE: sigma_p * sqrt(1 - exp(-2h)), 0 on the final step
 };
 
 struct StepParams {
@@ -131,10 +132,10 @@ struct StepScalars {
   DpmStep d;                   // DPM-Solver++
   uint32_t stream;
 };
-// whether the step draws N(0,1) noise (DPM-Solver++ is deterministic)
+// whether the step draws N(0,1) noise (DPM-Solver++: only the SDE variant, and not on its final step)
 template <int kKind>
 __device__ __forceinline__ bool step_draws_noise(const StepScalars& s) {
-  return kKind == kStepDdpm || (kKind == kStepDdim && s.sigma != 0.0f);
+  return kKind == kStepDdpm || (kKind == kStepDdim && s.sigma != 0.0f) || (kKind == kStepDpm && s.d.c_z != 0.0f);
 }
 template <int kKind>
 __device__ __forceinline__ StepScalars step_scalars(const StepParams& p) {
@@ -162,7 +163,8 @@ __device__ __forceinline__ StepScalars step_scalars(const StepParams& p) {
   return s;
 }
 // x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, the (already guidance-mixed) eps and the N(0,1) draw z.
-// DPM-Solver++: z is unused, dprev is D_{-1} of the element (read only at order 2) and x0o the guided D0.
+// DPM-Solver++: z is read only by the SDE variant (c_z != 0), dprev is D_{-1} of the element (read only at order 2) and x0o the
+// guided D0.
 template <int kKind>
 __device__ __forceinline__ void step_element(const StepParams& p, const StepScalars& s, int n, int c, size_t pix, float xt, float e, float z,
                                              float dprev, float& xo, float& x0o) {
@@ -197,6 +199,7 @@ __device__ __forceinline__ void step_element(const StepParams& p, const StepScal
     // D_{-1} is not read at order 1: the history may hold anything (first step of a run)
     const float d = s.d.order == 2 ? add(mul(s.d.w0, x0), mul(s.d.w1, dprev)) : x0;
     xo = sub(mul(s.d.c_xt, xt), mul(s.d.c_d, d));
+    if (s.d.c_z != 0.0f) xo = add(xo, mul(s.d.c_z, z));    // SDE noise; the ODE expression above keeps its bits
     x0o = x0;
     return;
   }

@@ -63,15 +63,17 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                precision="fp16"):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
-    (DPM-Solver++(2M)) wherever the reference runs DdimSampler; DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
+    (DPM-Solver++(2M)) wherever the reference runs DdimSampler, and solver="dpmpp_sde" its stochastic variant
+    (SDE-DPM-Solver++(2M)); DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
     runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision)."""
-    assert solver in ("ddim", "dpmpp"), f"solver must be 'ddim' or 'dpmpp', got {solver!r}"
+    assert solver in ("ddim", "dpmpp", "dpmpp_sde"), f"solver must be 'ddim', 'dpmpp' or 'dpmpp_sde', got {solver!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
             fw.backbone.set_precision(precision)
     ode = samplers.DdimSampler if solver == "ddim" else samplers.DpmSolverSampler
     sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
+    sde_kw = dict(sde=True) if solver == "dpmpp_sde" else {}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
     net = framework_uncond.backbone
@@ -106,6 +108,8 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
             mv_j = [views_of(k)[j] for k in range(bs)] if per_sample_views else views_of(0)[j]
             if j == 0:
                 kw = dict(strength=guidance) if cfg_u else {}
+                if steps_uncond < 1000:
+                    kw.update(sde_kw)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
             else:
                 cond = warp.aggregate(mv_j, **wparams)                   # [bs,7,S,S] in [0,1]
@@ -116,6 +120,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
                 kw = dict(strength=guidance) if cfg_u else {}
+                kw.update(sde_kw)
                 res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
             samples.append(res.samples)
             if warp is not None:
@@ -278,9 +283,10 @@ if __name__ == "__main__":
     ap.add_argument("--rng", choices=["philox", "torch"], default="philox",
                     help="per-step noise: 'philox' draws in-kernel (fast, default); 'torch' draws with the torch generator exactly "
                          "where the reference does (seed-for-seed reproduction of the reference's images needs this)")
-    ap.add_argument("--solver", choices=["ddim", "dpmpp"], default="ddim",
-                    help="ODE sampler of the DDIM-step views: 'ddim' as the reference, 'dpmpp' DPM-Solver++(2M), which needs fewer "
-                         "steps for the same convergence (DDPM at --steps_uncond >= 1000 is unchanged)")
+    ap.add_argument("--solver", choices=["ddim", "dpmpp", "dpmpp_sde"], default="ddim",
+                    help="sampler of the DDIM-step views: 'ddim' as the reference, 'dpmpp' DPM-Solver++(2M), which needs fewer "
+                         "steps for the same convergence, 'dpmpp_sde' its stochastic variant SDE-DPM-Solver++(2M) "
+                         "(DDPM at --steps_uncond >= 1000 is unchanged)")
     ap.add_argument("--precision", choices=["fp16", "fp8"], default="fp16",
                     help="operands of the ResBlock convs: 'fp16' (default) or 'fp8' (e4m3, faster, changes the numbers; DESIGN.md §2)")
     o = ap.parse_args()

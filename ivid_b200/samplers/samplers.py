@@ -66,7 +66,7 @@ class _NativeSampler:
 
     # ------------------------------------------------------------------------------------------------------------
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None):
+                   order=0, prev=None, sde=False):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -120,6 +120,7 @@ class _NativeSampler:
             t_last, x0_last = prev
             a.t_last = int(t_last[0]) if torch.is_tensor(t_last) and t_last.dim() > 0 else int(t_last)
             a.prev_x0_dev = P(x0_last)
+        a.sde = 1 if sde else 0
         return a, keep
 
     def _net(self):
@@ -127,12 +128,13 @@ class _NativeSampler:
         net._ensure_packed()
         return net
 
-    def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None):
+    def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
+                     sde=False):
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         with torch.cuda.device(dev):
@@ -142,13 +144,14 @@ class _NativeSampler:
         del keep
         return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
 
-    def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None):
+    def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
+                         sde=False):
         """Same step with the timestep taken on the device from the [N] tensors the caller passed (no host sync)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde)
         td = t.to(device=dev, dtype=torch.int64).contiguous()
         tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
         x_prev = torch.empty_like(x_t)
@@ -170,7 +173,8 @@ class _NativeSampler:
             cond_noise = torch.cat([n_rgb, n_d], dim=1)
         return torch.randn_like(x_t), cond_noise
 
-    def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0):
+    def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
+             sde=False):
         net = self._net()
         net.eval()
         if image_size is None:
@@ -200,9 +204,9 @@ class _NativeSampler:
                     cond_noise = torch.cat([torch.randn_like(y[:, :3]), torch.randn_like(y[:, 3:])], dim=1)
                 z = torch.randn_like(img)
                 if self.KIND == 2:
-                    # deterministic: z is drawn only to consume the torch RNG as DdimSampler does
-                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, None, cond_noise, order=order,
-                                            prev=prev if order != 1 else None)
+                    # the SDE update uses z; the ODE update draws it only to consume the torch RNG as DdimSampler does
+                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if sde else None, cond_noise,
+                                            order=order, prev=prev if order != 1 else None, sde=sde)
                     prev = (t, out.pred_x_0)
                 else:
                     out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise)
@@ -212,7 +216,7 @@ class _NativeSampler:
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order)
+            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde)
             traj0 = trajt = None
             if return_trajectory:
                 traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
@@ -293,34 +297,42 @@ class DdimSampler(_NativeSampler):
 
 
 class DpmSolverSampler(_NativeSampler):
-    """DPM-Solver++(2M) (Lu et al. 2022), the second-order multistep ODE solver in data-prediction form, on DdimSampler's
+    """DPM-Solver++(2M) (Lu et al. 2022), the second-order multistep solver in data-prediction form, on DdimSampler's
     time grid (jump = T // steps, model called at t - 1) with the same guidance (classifier-free mix, multiview replace /
-    constrain applied to x_0 exactly as DdimSampler.sample_once applies it).  Order 1 is DDIM with eta = 0.  Deterministic:
-    no step noise.  The update is fused into the output head like the DDPM / DDIM steps (include/ivid_b200.h, kind 2)."""
+    constrain applied to x_0 exactly as DdimSampler.sample_once applies it).  The update is fused into the output head like
+    the DDPM / DDIM steps (include/ivid_b200.h, kind 2).
+
+    With alpha = sqrt(alphas_cumprod), sigma = sqrt(1 - alphas_cumprod) at t - 1 (s) and t_prev - 1 (p), h = lambda_p -
+    lambda_s for lambda = log(alpha / sigma), and D the guided x_0 (order 1) or (1 + 1/(2r)) D0 - 1/(2r) D_{-1} (order 2):
+      sde=False (ODE, deterministic):  x_p = sigma_p/sigma_s x_t + alpha_p (1 - e^-h) D;          order 1 = DDIM, eta = 0
+      sde=True  (SDE-DPM-Solver++(2M)): x_p = sigma_p/sigma_s e^-h x_t + alpha_p (1 - e^-2h) D
+                                              + sigma_p sqrt(1 - e^-2h) z,  z ~ N(0, 1);        order 1 = DDIM, eta = 1"""
     KIND = 2
 
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
-                    constrain_depth=None, noise=None, **kwargs):
+                    constrain_depth=None, noise=None, sde=False, **kwargs):
         """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
-        `noise` is not used by the update: when it is None the torch RNG is consumed exactly as DdimSampler.sample_once
-        consumes it (InpaintCFG hole noise, then one randn_like(x_t)); `cond_noise` injects the hole noise."""
+        With sde=True `noise` is the injected z of the update; with sde=False the update does not use it.  When it is None
+        the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
+        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise."""
         B = x_t.shape[0]
         assert t.shape == (B,) and t_prev.shape == (B,)
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         if noise is None:
-            _, cond_noise = self._draw_step_noise(x_t, kw)
+            noise, cond_noise = self._draw_step_noise(x_t, kw)
         else:
             cond_noise = kw.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, None, cond_noise,
-                                     order=2 if prev is not None else 1, prev=prev)
+        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise if sde else None, cond_noise,
+                                     order=2 if prev is not None else 1, prev=prev, sde=sde)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
-               rng="philox", return_trajectory=False, **kwargs):
-        """Run `steps` DPM-Solver++ steps of order `order` (1 or 2).  The first step and the final step (to t_prev = 0,
-        which returns x_0 as DDIM does) are first order.  Same return dict as DdimSampler.sample."""
+               rng="philox", return_trajectory=False, sde=False, **kwargs):
+        """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
+        final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
+        is drawn where DdimSampler draws it (`rng`).  Same return dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         order=order)
+                         order=order, sde=bool(sde))
