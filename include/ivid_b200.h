@@ -144,12 +144,14 @@ int ivid_sampler_table(const ivid_sampler_t* s, int which, double* out, int coun
  *   sde = 1 (SDE-DPM-Solver++(2M); step_noise_dev / noise_all_dev or Philox (seed, step) as for DDIM supply z):
  *        x_prev = (sigma_p / sigma_s) * exp(-h) * x_t + alpha_p * (1 - exp(-2h)) * D
  *                 + sigma_p * sqrt(1 - exp(-2h)) * z                                  (order 1 = DDIM with eta = 1).
- * The step to t_prev = 0 is always first order, returns D0 and draws no noise.  The trailing fields below are read
- * only for kind 2; zero keeps the behaviour of kinds 0 and 1 unchanged. */
+ * The step to t_prev = 0 is always first order, returns D0 and draws no noise.  The fields order to sde below are read
+ * only for kind 2; zero keeps the behaviour of kinds 0 and 1 unchanged.  The guidance-interval fields after them apply to
+ * every kind; zero means guidance at every step. */
 typedef struct {
   int kind;                 /* 0 = DDPM ancestral (ddpm.py:111-131), 1 = DDIM (ddim.py:48-103), 2 = DPM-Solver++ (above) */
   int use_cfg;              /* 1: (1+strength)*eps(c) - strength*eps(null), both halves in ONE batch-2N forward */
-  float strength;           /* <= 0: ONE forward, eps scaled by (1+strength) when classes are given (classifier_free_guidance.py:40-41) */
+  float strength;           /* <= 0: ONE forward, eps scaled by (1+strength) when classes are given (classifier_free_guidance.py:40-41);
+                               guidance_interval (below) restricts use_cfg / strength to a range of model times */
   int clip_denoised;
   float eta;
   const int64_t* classes_dev;   /* [N] or NULL */
@@ -174,6 +176,17 @@ typedef struct {
   int t_last;                          /* single-step entry points, with prev_x0_dev: the previous step's t, t < t_last <= T */
   int sde;                             /* 0: ODE update; 1: SDE update, valid with kind 2 only (any other value, or 1 with
                                           kind 0 / 1, is IVID_ERR_INVALID_ARGUMENT) */
+  /* Guidance interval (Kynkaenniemi et al. 2024, arXiv:2404.07724), every kind.  guidance_interval = 0: guidance at every
+   * step (use_cfg / strength above).  1: a step is guided only when its model time (the t the network receives: t for
+   * DDPM, t - 1 for DDIM and DPM-Solver++) lies in [guidance_t_lo, guidance_t_hi]; every other step is the same step at
+   * strength 0, eps = eps(x, t, classes).  0 <= guidance_t_lo <= guidance_t_hi < T, and guidance_interval 0 or 1, else
+   * IVID_ERR_INVALID_ARGUMENT.  No effect without classes_dev or with use_cfg = 0 (one forward either way).
+   *   ivid_sampler_step / ivid_sampler_run: an unguided step runs ONE batch-N forward (about half the work of a guided
+   *   step).  ivid_sampler_step_dev reads t on the device, so it keeps the batch-2N forward and the step kernel drops the
+   *   null-class half: the same bits, not faster. */
+  int guidance_interval;
+  int guidance_t_lo;
+  int guidance_t_hi;
 } ivid_step_args_t;
 
 /* sample_once: x_prev = f(x_t, t[, t_prev]).  `t` follows the reference's convention of each sampler:

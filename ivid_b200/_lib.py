@@ -58,6 +58,9 @@ class StepArgsT(Structure):
         ("prev_x0_dev", c_void_p),    # kind 2, single step: the previous step's pred_x0 (NULL = first order)
         ("t_last", c_int),            # kind 2, single step: the previous step's t
         ("sde", c_int),               # kind 2: 1 = the stochastic (SDE) update, which reads step noise
+        ("guidance_interval", c_int), # 1: guide only steps whose model time is in [guidance_t_lo, guidance_t_hi]
+        ("guidance_t_lo", c_int),
+        ("guidance_t_hi", c_int),
     ]
 
 

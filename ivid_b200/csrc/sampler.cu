@@ -17,7 +17,7 @@ struct StepState {
   int t_index;       // coefficient-table row of the model timestep
   int t_prev;        // DDIM / DPM: previous actual step
   int stream;        // Philox stream (step counter)
-  int pad;
+  int guided;        // 0: the step lies outside the guidance interval (StepParams::guided)
   DpmStep dpm;       // DPM-Solver++ scalars of this step
 };
 
@@ -51,12 +51,14 @@ __device__ void dpm_step_state(DpmStep* d, const double* acp, int t, int t_prev,
 }
 
 // acp != nullptr: DPM-Solver++ step t_index + 1 -> t_prev (order / t_last / sde as in dpm_step_state)
+// guided: whether the step lies inside the guidance interval (the host route decides it and sizes the forward by it)
 __global__ void set_step_kernel(StepState* st, int64_t* t_model, int N, int t_index, int t_prev, int stream, const double* acp,
-                                int t_last, int order, int sde) {
+                                int t_last, int order, int sde, int guided) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     st->t_index = t_index;
     st->t_prev = t_prev;
     st->stream = stream;
+    st->guided = guided;
     if (acp != nullptr) dpm_step_state(&st->dpm, acp, t_index + 1, t_prev, t_last, order, sde);
   }
   for (int i = threadIdx.x; i < N; i += blockDim.x) t_model[i] = t_index;
@@ -64,9 +66,11 @@ __global__ void set_step_kernel(StepState* st, int64_t* t_model, int N, int t_in
 
 // same, with the step read from the caller's device tensors (sample_once(x_t, t[, t_prev]) of the reference passes [N]
 // tensors; reading element 0 here removes the device->host sync an int(t[0]) would cost).  Out-of-range steps are
-// clamped into the table (the host path raises instead); a DPM-Solver++ step is first order unless t_last > t.
+// clamped into the table (the host path raises instead); a DPM-Solver++ step is first order unless t_last > t.  The step is
+// guided unless an interval is given (interval != 0) and the clamped model time lies outside [t_lo, t_hi].
 __global__ void set_step_dev_kernel(StepState* st, int64_t* t_model, int N, const int64_t* t_dev, const int64_t* t_prev_dev,
-                                    int ddim, int T, const double* acp, int t_last, int order, int sde) {
+                                    int ddim, int T, const double* acp, int t_last, int order, int sde, int interval, int t_lo,
+                                    int t_hi) {
   long long t = t_dev[0];
   long long ti = ddim ? t - 1 : t;
   ti = ti < 0 ? 0 : (ti > T - 1 ? T - 1 : ti);
@@ -76,6 +80,7 @@ __global__ void set_step_dev_kernel(StepState* st, int64_t* t_model, int N, cons
     st->t_index = static_cast<int>(ti);
     st->t_prev = static_cast<int>(tp);
     st->stream = static_cast<int>(t);
+    st->guided = (!interval || (ti >= t_lo && ti <= t_hi)) ? 1 : 0;
     if (acp != nullptr) dpm_step_state(&st->dpm, acp, static_cast<int>(ti) + 1, static_cast<int>(tp), t_last, order, sde);
   }
   for (int i = threadIdx.x; i < N; i += blockDim.x) t_model[i] = ti;
@@ -211,6 +216,13 @@ static void require_sde(const ivid_step_args_t& a) {
   IVID_REQUIRE(a.sde == 0 || a.kind == kStepDpm, "sde = 1 needs kind 2 (DPM-Solver++)");
 }
 
+// guidance interval in model times: 0 <= t_lo <= t_hi < T
+static void require_interval(const ivid_step_args_t& a, int T) {
+  IVID_REQUIRE(a.guidance_interval == 0 || a.guidance_interval == 1, "guidance_interval must be 0 or 1");
+  IVID_REQUIRE(a.guidance_interval == 0 || (a.guidance_t_lo >= 0 && a.guidance_t_lo <= a.guidance_t_hi && a.guidance_t_hi < T),
+               "guidance interval must satisfy 0 <= t_lo <= t_hi < T");
+}
+
 void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, int t, int t_prev,
                    const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
                    const int64_t* t_prev_dev) {
@@ -222,6 +234,7 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
   IVID_REQUIRE(a.kind == kStepDdpm || a.kind == kStepDdim || a.kind == kStepDpm,
                "sampler kind must be 0 (DDPM), 1 (DDIM) or 2 (DPM-Solver++)");
   require_sde(a);
+  require_interval(a, T_);
   const int kind = a.kind;
   const bool ddim = kind != kStepDdpm;      // DDIM's step convention: actual steps t / t_prev (DPM-Solver++ shares it)
   const bool dpm = kind == kStepDpm;
@@ -236,11 +249,16 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
   IVID_REQUIRE(!dpm2 || t_dev != nullptr || a.t_last > t, "the previous step t_last must come before t (t_last > t)");
   // classifier-free guidance: one batch-2N forward when strength > 0 and the model is class conditional
   const bool has_classes = a.classes_dev != nullptr;
-  const bool cfg_two = a.use_cfg && has_classes && a.strength > 0.0f;
+  // guidance interval: a step whose model time lies outside it is the step at strength 0, eps = eps_c of one forward.  The
+  // host-int route knows t and runs that step as a batch-N forward; the device route keeps the batch-2N forward and the step
+  // kernel reads the guided flag set_step_dev_kernel writes.  Without classes (or use_cfg) only one forward runs anyway.
+  const bool gated = a.guidance_interval != 0 && a.use_cfg && has_classes;
+  const bool guided = !gated || t_dev != nullptr || (t_index >= a.guidance_t_lo && t_index <= a.guidance_t_hi);
+  const bool cfg_two = a.use_cfg && has_classes && a.strength > 0.0f && guided;
   // inpaint_cfg.py:77-78 / sr_cfg.py:53-54: classes None -> single null-class forward, no (1+s) scaling
   // strength < 0: (1 + strength) * eps of ONE forward (classifier_free_guidance.py:40-41); the conditional frameworks skip even
   // that when classes is None
-  const bool scale_only = a.use_cfg && a.strength < 0.0f && (has_classes || a.cond.kind == 0);
+  const bool scale_only = a.use_cfg && a.strength < 0.0f && (has_classes || a.cond.kind == 0) && guided;
   const int Nf = cfg_two ? 2 * N : N;
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));      // before any allocation: a direct C-ABI caller may be on another device
   ensure_device(Nf, static_cast<size_t>(Nf) * C * HW);
@@ -256,10 +274,10 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
   const int order = dpm2 ? 2 : 1;
   if (t_dev != nullptr)
     set_step_dev_kernel<<<1, 128, 0, stream>>>(reinterpret_cast<StepState*>(d_state_), d_t_, Nf, t_dev, t_prev_dev, ddim ? 1 : 0, T_,
-                                               acp, a.t_last, order, a.sde);
+                                               acp, a.t_last, order, a.sde, gated ? 1 : 0, a.guidance_t_lo, a.guidance_t_hi);
   else
     set_step_kernel<<<1, 128, 0, stream>>>(reinterpret_cast<StepState*>(d_state_), d_t_, Nf, t_index, t_prev, stream_id, acp,
-                                           a.t_last, order, a.sde);
+                                           a.t_last, order, a.sde, guided ? 1 : 0);
   IVID_CHECK_CUDA(cudaGetLastError());
   const int64_t* cls = nullptr;
   if (has_classes) {
@@ -295,6 +313,8 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
     p.dpm = &reinterpret_cast<StepState*>(d_state_)->dpm;
     p.hist = d_hist_;
   }
+  // the host route has folded the interval into cfg already; nullptr keeps the step kernels' arithmetic of a run without one
+  if (gated && t_dev != nullptr) p.guided = &reinterpret_cast<StepState*>(d_state_)->guided;
   GuideParams& g = p.g;
   g.rgb = a.replace_rgb_dev; g.rgb_mask = a.replace_rgb_mask_dev;
   g.depth = a.replace_depth_dev; g.depth_mask = a.replace_depth_mask_dev; g.convex = a.constrain_depth_dev;
@@ -319,7 +339,9 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
     hp.sp = p; hp.H = H; hp.W = W;
     HeadHook hook;
     // FNV-1a over everything the launcher bakes in
-    // (sde: the SDE and ODE steps differ only in device state, but an ODE and an SDE run never share a captured graph)
+    // (sde: the SDE and ODE steps differ only in device state, but an ODE and an SDE run never share a captured graph;
+    // on the host route a guided and an unguided step differ in p.cfg (and in the plan); on the device route they share one
+    // graph and differ only in the flag p.guided points to)
     uint64_t h = 1469598103934665603ull ^ (kind == kStepDdim ? 0x9E37ull : kind == kStepDpm ? 0x7F4Aull : 0ull) ^
                  (a.sde ? 0x5DE00000ull : 0ull);
     const unsigned char* bytes = reinterpret_cast<const unsigned char*>(&p);
@@ -361,6 +383,7 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   IVID_REQUIRE(steps >= 1 && steps <= T_, "steps out of range");
   IVID_REQUIRE(!dpm || (a.order >= 0 && a.order <= 2), "DPM-Solver++ order must be 1 or 2");
   require_sde(a);
+  require_interval(a, T_);
   const int jump = T_ / steps;                     // ddim.py:153
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));
   ensure_device(2 * N, 2 * img);
@@ -369,7 +392,8 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   float* bufs[2] = {x, d_xtmp_};                   // ping-pong; the result is copied back to x if it ends in d_xtmp_
   int cur = 0;
   // per denoising step the host then issues three calls: the step-state kernel, ONE CUDA-graph launch (the whole batch-2N
-  // forward) and the fused guidance-mix + x_{t-1} update
+  // forward, batch-N for a step outside the guidance interval: each batch has its own plan and graphs) and the fused
+  // guidance-mix + x_{t-1} update
   struct Ready { Sampler* s; ~Ready() { s->classes2_ready_ = false; s->no_fuse_ = false; } } ready_guard{this};
   no_fuse_ = noise_all != nullptr || cond_noise_all != nullptr || traj_x0 != nullptr || traj_xt != nullptr;
   if (a.use_cfg && a.classes_dev != nullptr && a.strength > 0.0f) {

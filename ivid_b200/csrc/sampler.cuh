@@ -96,6 +96,9 @@ struct StepParams {
   // DPM-Solver++ only (appended, so the DDPM / DDIM layout is unchanged)
   const DpmStep* dpm;          // device step state
   float* hist;                 // [N,C,H,W] D_{-1} on entry (order 2), overwritten in place with this step's D0
+  // guidance interval on the device-timestep route (appended): device flag, 0 = this step is unguided, so eps = eps_c
+  // whatever cfg says (the null-class rows are ignored); nullptr = always guided
+  const int* guided;
 };
 
 // (1 + strength) * eps_c - strength * eps_u (only evaluated with strength > 0).  Every product / sum of the step arithmetic is
@@ -104,10 +107,12 @@ struct StepParams {
 __device__ __forceinline__ float cfg_mix(float ec, float eu, float strength) {
   return __fsub_rn(__fmul_rn(__fadd_rn(1.0f, strength), ec), __fmul_rn(strength, eu));
 }
-__device__ __forceinline__ float mix_eps(const StepParams& p, size_t i, size_t total) {
+// cfg of this step: p.cfg, or 0 when the device flag says the step lies outside the guidance interval
+__device__ __forceinline__ int step_cfg(const StepParams& p) { return (p.guided != nullptr && *p.guided == 0) ? 0 : p.cfg; }
+__device__ __forceinline__ float mix_eps(const StepParams& p, int cfg, size_t i, size_t total) {
   const float ec = p.eps[i];
-  if (!p.cfg) return ec;
-  if (p.cfg == 2) return __fmul_rn(__fadd_rn(1.0f, p.strength), ec);
+  if (!cfg) return ec;
+  if (cfg == 2) return __fmul_rn(__fadd_rn(1.0f, p.strength), ec);
   return cfg_mix(ec, p.eps[total + i], p.strength);
 }
 
@@ -235,6 +240,7 @@ template <int kKind>
 __global__ void __launch_bounds__(256) step_kernel(const StepParams p) {
   const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
   const StepScalars s = step_scalars<kKind>(p);
+  const int cfg = step_cfg(p);
   for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
        i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const size_t i = i4 * 4;
@@ -246,7 +252,7 @@ __global__ void __launch_bounds__(256) step_kernel(const StepParams p) {
     hist_load4<kKind>(p, s, i, hp);
     float xo[4], x0o[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) step_element<kKind>(p, s, n, c, pix + j, p.x_t[i + j], mix_eps(p, i + j, total), z[j], hp[j], xo[j], x0o[j]);
+    for (int j = 0; j < 4; ++j) step_element<kKind>(p, s, n, c, pix + j, p.x_t[i + j], mix_eps(p, cfg, i + j, total), z[j], hp[j], xo[j], x0o[j]);
     stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
     if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
     hist_store4<kKind>(p, i, x0o);
@@ -279,6 +285,7 @@ template <int kKind>
 __global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) {
   const StepParams& p = h.sp;
   const StepScalars s = step_scalars<kKind>(p);
+  const int cfg = step_cfg(p);
   const int w4 = h.W / 4;
   const size_t groups = static_cast<size_t>(p.N) * h.H * w4;
   for (size_t g = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; g < groups; g += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -290,12 +297,12 @@ __global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) 
     for (int j = 0; j < 4; ++j) {
       float ec[4];
       head_eps4(h, n, y, xg * 4 + j, ec);
-      if (p.cfg == 1) {
+      if (cfg == 1) {
         float eu[4];
         head_eps4(h, n + p.N, y, xg * 4 + j, eu);
 #pragma unroll
         for (int c = 0; c < 4; ++c) ec[c] = cfg_mix(ec[c], eu[c], p.strength);
-      } else if (p.cfg == 2) {
+      } else if (cfg == 2) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) ec[c] = __fmul_rn(__fadd_rn(1.0f, p.strength), ec[c]);
       }

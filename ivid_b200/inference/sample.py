@@ -60,12 +60,14 @@ def build_modelviews(viewset, num_samples, rng=None):
 @torch.no_grad()
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
-               precision="fp16"):
+               precision="fp16", guidance_interval=None):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, and solver="dpmpp_sde" its stochastic variant
     (SDE-DPM-Solver++(2M)); DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
-    runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision)."""
+    runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision).  guidance_interval=(t_lo, t_hi)
+    guides only the steps of both networks whose model time lies in [t_lo, t_hi] (the samplers' `guidance_interval`);
+    the other steps run at strength 0 with one batch-N forward."""
     assert solver in ("ddim", "dpmpp", "dpmpp_sde"), f"solver must be 'ddim', 'dpmpp' or 'dpmpp_sde', got {solver!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
@@ -74,6 +76,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
     sde_kw = dict(sde=True) if solver == "dpmpp_sde" else {}
+    gi_kw = dict(guidance_interval=tuple(guidance_interval)) if guidance_interval is not None else {}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
     net = framework_uncond.backbone
@@ -107,7 +110,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
         for j in range(n_views):
             mv_j = [views_of(k)[j] for k in range(bs)] if per_sample_views else views_of(0)[j]
             if j == 0:
-                kw = dict(strength=guidance) if cfg_u else {}
+                kw = dict(strength=guidance, **gi_kw) if cfg_u else {}
                 if steps_uncond < 1000:
                     kw.update(sde_kw)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
@@ -119,7 +122,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 cond_depth.append(cond[:, 3:4] * 2 - 1)
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
-                kw = dict(strength=guidance) if cfg_u else {}
+                kw = dict(strength=guidance, **gi_kw) if cfg_u else {}
                 kw.update(sde_kw)
                 res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
             samples.append(res.samples)
@@ -242,15 +245,17 @@ def main(rank, world_size, opt):
     mvs_r = shard(mvs, rank, world_size) if isinstance(mvs[0], list) else mvs
     solver = getattr(opt, "solver", "ddim")
     precision = getattr(opt, "precision", "fp16")
+    interval = getattr(opt, "guidance_interval", None)
     out_dir = os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
-                           + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}"))
+                           + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}")
+                           + ("" if interval is None else f"_interval{interval[0]}-{interval[1]}"))
     for sub in ("results", "grids", "conds", "scenes"):                 # sample.py:283-286
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
     save_cfg = edict(output_dir=out_dir, viewset=opt.viewset)
     gen = sample_all(fw_u, fw_c, seeds_r if seeds_r is not None else len(idx), opt.steps_uncond, opt.steps_cond, mvs_r, classes=classes_r,
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
                      rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
-                     precision=precision)
+                     precision=precision, guidance_interval=interval)
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -259,7 +264,21 @@ def main(rank, world_size, opt):
         th.join()
 
 
-if __name__ == "__main__":
+def parse_interval(s):
+    """'LO,HI' -> (LO, HI), the inclusive model-time bounds of --guidance_interval."""
+    parts = s.split(",")
+    if len(parts) != 2:
+        raise argparse.ArgumentTypeError(f"expected LO,HI, got {s!r}")
+    try:
+        lo, hi = int(parts[0]), int(parts[1])
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected two integers LO,HI, got {s!r}") from None
+    if not 0 <= lo <= hi:
+        raise argparse.ArgumentTypeError(f"expected 0 <= LO <= HI, got {s!r}")
+    return lo, hi
+
+
+def build_arg_parser():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config_uncond", default="configs/rgbd_imagenet_adm_128_large_cfg.json")
     ap.add_argument("--config_cond", default="configs/rgbd_imagenet_adm_128_large_cond.json")
@@ -289,7 +308,14 @@ if __name__ == "__main__":
                          "(DDPM at --steps_uncond >= 1000 is unchanged)")
     ap.add_argument("--precision", choices=["fp16", "fp8"], default="fp16",
                     help="operands of the ResBlock convs: 'fp16' (default) or 'fp8' (e4m3, faster, changes the numbers; DESIGN.md §2)")
-    o = ap.parse_args()
+    ap.add_argument("--guidance_interval", type=parse_interval, default=None, metavar="LO,HI",
+                    help="apply classifier-free guidance only at the steps whose model time t (0 <= t < T, the t the network "
+                         "receives) lies in [LO, HI]; the other steps run unguided with half the network work (default: every step)")
+    return ap
+
+
+if __name__ == "__main__":
+    o = build_arg_parser().parse_args()
     n = torch.cuda.device_count()
     if n <= 1:
         main(0, 1, o)

@@ -34,6 +34,16 @@ def _f32(t, device):
     return None if t is None else t.to(device=device, dtype=torch.float32).contiguous()
 
 
+def _check_interval(guidance_interval, T):
+    """(t_lo, t_hi) as ints, or None.  Both bounds are inclusive model times (the t the network receives), 0 <= t_lo <= t_hi < T."""
+    if guidance_interval is None:
+        return None
+    assert len(guidance_interval) == 2, f"guidance_interval must be (t_lo, t_hi), got {guidance_interval!r}"
+    lo, hi = (int(v) for v in guidance_interval)
+    assert 0 <= lo <= hi < T, f"guidance_interval must satisfy 0 <= t_lo <= t_hi < {T}, got ({lo}, {hi})"
+    return lo, hi
+
+
 class _NativeSampler:
     KIND = 0
 
@@ -66,7 +76,7 @@ class _NativeSampler:
 
     # ------------------------------------------------------------------------------------------------------------
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None, sde=False):
+                   order=0, prev=None, sde=False, interval=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -121,6 +131,10 @@ class _NativeSampler:
             a.t_last = int(t_last[0]) if torch.is_tensor(t_last) and t_last.dim() > 0 else int(t_last)
             a.prev_x0_dev = P(x0_last)
         a.sde = 1 if sde else 0
+        interval = _check_interval(interval, len(fw.betas))
+        if interval is not None:
+            a.guidance_interval = 1
+            a.guidance_t_lo, a.guidance_t_hi = interval
         return a, keep
 
     def _net(self):
@@ -129,12 +143,12 @@ class _NativeSampler:
         return net
 
     def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                     sde=False):
+                     sde=False, interval=None):
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         with torch.cuda.device(dev):
@@ -145,13 +159,13 @@ class _NativeSampler:
         return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
 
     def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                         sde=False):
+                         sde=False, interval=None):
         """Same step with the timestep taken on the device from the [N] tensors the caller passed (no host sync)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval)
         td = t.to(device=dev, dtype=torch.int64).contiguous()
         tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
         x_prev = torch.empty_like(x_t)
@@ -174,7 +188,8 @@ class _NativeSampler:
         return torch.randn_like(x_t), cond_noise
 
     def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
-             sde=False):
+             sde=False, interval=None):
+        interval = _check_interval(interval, len(self.framework.betas))   # before any device work
         net = self._net()
         net.eval()
         if image_size is None:
@@ -206,17 +221,18 @@ class _NativeSampler:
                 if self.KIND == 2:
                     # the SDE update uses z; the ODE update draws it only to consume the torch RNG as DdimSampler does
                     out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if sde else None, cond_noise,
-                                            order=order, prev=prev if order != 1 else None, sde=sde)
+                                            order=order, prev=prev if order != 1 else None, sde=sde, interval=interval)
                     prev = (t, out.pred_x_0)
                 else:
-                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise)
+                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise, interval=interval)
                 img = out.pred_x_prev
                 if return_trajectory:
                     ret.pred_x_t.append(out.pred_x_prev)
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde)
+            a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
+                                      interval=interval)
             traj0 = trajt = None
             if return_trajectory:
                 traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
@@ -249,26 +265,35 @@ class DdpmSampler(_NativeSampler):
         self.posterior_mean_coef2 = (1.0 - self.alphas_cumprod_prev) * np.sqrt(alphas) / (1.0 - self.alphas_cumprod)
 
     @torch.no_grad()
-    def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, **kwargs):
+    def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, guidance_interval=None, **kwargs):
         """x_{t-1} from x_t (ddpm.py:111-131).  `t` is the [N] tensor of steps minus 1 (all equal).
-        `noise` (extension) injects the randn_like draw; default draws it with torch like the reference."""
+        `noise` (extension) injects the randn_like draw; default draws it with torch like the reference.
+        `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`)."""
         B = x_t.shape[0]
         assert t.shape == (B,), "t must be a 1D tensor of shape (B,)"
+        _check_interval(guidance_interval, len(self.framework.betas))
         # all samples of a batch share the timestep (both reference samplers are driven that way: ddpm.py:177-179);
         # element 0 is read on the device, so this call does not synchronise with the host
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kwargs)
         else:
             cond_noise = kwargs.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, cond_noise)
+        return self._native_step_dev(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, cond_noise,
+                                     interval=guidance_interval)
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
-               rng="philox", return_trajectory=False, **kwargs):
+               rng="philox", return_trajectory=False, guidance_interval=None, **kwargs):
         """Run the full reverse process (ddpm.py:134-187).  `steps` is accepted and ignored exactly as in the reference.
         pred_x_t / pred_x_0 are only materialised with return_trajectory=True (the reference keeps 2x1000 tensors alive;
-        its callers read `.samples` only: inference/sample.py:82)."""
-        return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs)
+        its callers read `.samples` only: inference/sample.py:82).
+
+        guidance_interval=(t_lo, t_hi) (extension; Kynkaanniemi et al. 2024, arXiv:2404.07724): classifier-free guidance
+        only at the steps whose model time t (the t the network receives) lies in [t_lo, t_hi], 0 <= t_lo <= t_hi < T;
+        every other step is the same step at strength 0 and runs one batch-N forward instead of the batch-2N one.  None
+        (default) guides every step.  No effect without classes."""
+        return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
+                         interval=guidance_interval)
 
 
 class DdimSampler(_NativeSampler):
@@ -277,23 +302,27 @@ class DdimSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, eta=0.0, replace_rgb=None,
-                    replace_depth=None, constrain_depth=None, noise=None, **kwargs):
-        """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step)."""
+                    replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, **kwargs):
+        """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step).
+        `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi]."""
         B = x_t.shape[0]
         assert t.shape == (B,) and t_prev.shape == (B,)
+        _check_interval(guidance_interval, len(self.framework.betas))
         # element 0 of t / t_prev is read on the device (all samples share the step, ddim.py:154-158): no host sync
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kw)
         else:
             cond_noise = kw.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, cond_noise)
+        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, cond_noise, interval=guidance_interval)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
-               verbose=True, rng="philox", return_trajectory=False, **kwargs):
-        """Run `steps` DDIM steps (ddim.py:106-165)."""
-        return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs)
+               verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, **kwargs):
+        """Run `steps` DDIM steps (ddim.py:106-165).  `guidance_interval=(t_lo, t_hi)` as in DdpmSampler.sample, on the model
+        time t - 1 of each step."""
+        return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
+                         interval=guidance_interval)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -311,28 +340,31 @@ class DpmSolverSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
-                    constrain_depth=None, noise=None, sde=False, **kwargs):
+                    constrain_depth=None, noise=None, sde=False, guidance_interval=None, **kwargs):
         """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
         With sde=True `noise` is the injected z of the update; with sde=False the update does not use it.  When it is None
         the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
-        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise."""
+        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval` as for
+        DdimSampler.sample_once."""
         B = x_t.shape[0]
         assert t.shape == (B,) and t_prev.shape == (B,)
+        _check_interval(guidance_interval, len(self.framework.betas))
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kw)
         else:
             cond_noise = kw.pop("cond_noise", None)
         return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise if sde else None, cond_noise,
-                                     order=2 if prev is not None else 1, prev=prev, sde=sde)
+                                     order=2 if prev is not None else 1, prev=prev, sde=sde, interval=guidance_interval)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
-               rng="philox", return_trajectory=False, sde=False, **kwargs):
+               rng="philox", return_trajectory=False, sde=False, guidance_interval=None, **kwargs):
         """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
         final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
-        is drawn where DdimSampler draws it (`rng`).  Same return dict as DdimSampler.sample."""
+        is drawn where DdimSampler draws it (`rng`).  `guidance_interval` as in DdimSampler.sample; the history D_{-1} of a
+        step after an unguided one is that step's unguided D0.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         order=order, sde=bool(sde))
+                         order=order, sde=bool(sde), interval=guidance_interval)
