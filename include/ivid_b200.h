@@ -82,7 +82,8 @@ int ivid_conv_tile(int H, int W, int* tw, int* th, int* tn, int* fused_stats);
 /* Parity aid (per-layer taps, tests/test_gpu_unet.py): output of the module `layer` (reference module path such as
  * "input_blocks.3.0", "middle_block.1", "output_blocks.14.0"; the stem is "input_blocks.0.0"; "emb" = time + class embedding
  * [N, 4*model_channels, 1, 1]; "film" = the stacked emb_layers outputs of all ResBlocks) of the LAST forward of batch
- * N, as fp32 NCHW on the host.  host_out == NULL only queries the shape.  Synchronises the device. */
+ * N, as fp32 NCHW on the host.  host_out == NULL only queries the shape.  Synchronises the device.  After a reuse forward
+ * (ivid_unet_forward_reuse) the layers it skipped still show the tensors of the plan's last full forward. */
 int ivid_unet_debug_tap(ivid_unet_t* h, int N, const char* layer, float* host_out, uint64_t capacity, int* C, int* H, int* W);
 
 /* Profiling aid (bench.py roofline): between begin/end every kernel launch of ivid_unet_forward is bracketed by CUDA
@@ -116,6 +117,24 @@ int ivid_unet_forward_cond(ivid_unet_t* h, const float* x_dev, int Nx, const ivi
  * H = W = image_size.  Execution plans are cached per (N, H, W). */
 int ivid_unet_forward_hw(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
                          const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, void* stream);
+
+/* Feature reuse between denoising steps (DeepCache, Ma, Fang, Wang, CVPR 2024, arXiv:2312.00858; no reference counterpart).
+ * L = the number of output blocks (15 for the shipped configs).  Output block L-1-j pairs with input block j (it reads
+ * input block j's output as its skip tensor).
+ *   A full forward is ivid_unet_forward_hw.
+ *   A reuse forward at branch b runs only the embeddings (time, class, FiLM table), the input packing, input blocks 0..b,
+ *   output blocks L-1-b..L-1 and the output head.  Output block L-1-b takes as its h input the output of output block
+ *   L-2-b stored by the last full forward of the same execution plan (the same N, H and W), with its fp16 copy and its
+ *   GroupNorm statistics.  Every skip tensor it reads is one it has just recomputed.
+ * Valid branches are 0 <= b <= num_res_blocks, the blocks of the top level; any other value is IVID_ERR_INVALID_ARGUMENT.
+ * A plan holds a valid cache once a full forward has been enqueued on it.  A new plan holds none, including one rebuilt after
+ * eviction (more than four (N, H, W) in use) or after ivid_unet_finalize; a reuse forward on it is IVID_ERR_STATE.  Full and
+ * reuse forwards replay separate CUDA graphs; a reuse forward allocates nothing.  The sampler entry points use it through
+ * the cache_* fields of ivid_step_args_t.
+ * ivid_unet_forward_reuse is ivid_unet_forward_hw as a reuse forward at branch cache_branch. */
+int ivid_unet_forward_reuse(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
+                            const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, int cache_branch,
+                            void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Samplers — replace diffusion.samplers.DdpmSampler / DdimSampler (samplers/ddpm.py:12-187, samplers/ddim.py:12-165)
@@ -187,6 +206,20 @@ typedef struct {
   int guidance_interval;
   int guidance_t_lo;
   int guidance_t_hi;
+  /* Feature reuse (ivid_unet_forward_reuse), every kind; zero means off.  The step's update, the DPM-Solver++ history and
+   * all noise are those of a step without reuse; only eps changes.
+   *   cache_interval: ivid_sampler_run.  0 or 1: every step runs a full forward.  N > 1: step i runs a full forward when
+   *     i == 0, when the previous step ran on the other plan (the guidance interval switched the forward between batch 2N
+   *     and batch N), or when N steps have passed since the last full step; every other step is a reuse forward.  A
+   *     negative value is IVID_ERR_INVALID_ARGUMENT.
+   *   cache_branch: the branch b of the reuse forwards, 0 <= b <= num_res_blocks (IVID_ERR_INVALID_ARGUMENT otherwise).
+   *   cache_reuse: ivid_sampler_step / ivid_sampler_step_dev.  1: this step's forward is a reuse forward (IVID_ERR_STATE
+   *     before any full forward on its plan); 0 or 1, else IVID_ERR_INVALID_ARGUMENT.  ivid_sampler_run ignores it.
+   *     ivid_sampler_step_dev always runs the batch-2N plan of a guided run, so its cache stays valid across the guidance
+   *     interval. */
+  int cache_interval;
+  int cache_branch;
+  int cache_reuse;
 } ivid_step_args_t;
 
 /* sample_once: x_prev = f(x_t, t[, t_prev]).  `t` follows the reference's convention of each sampler:

@@ -61,6 +61,9 @@ class StepArgsT(Structure):
         ("guidance_interval", c_int), # 1: guide only steps whose model time is in [guidance_t_lo, guidance_t_hi]
         ("guidance_t_lo", c_int),
         ("guidance_t_hi", c_int),
+        ("cache_interval", c_int),    # ivid_sampler_run: a full forward every cache_interval steps, reuse forwards between
+        ("cache_branch", c_int),      # branch b of the reuse forwards, 0 <= b <= num_res_blocks
+        ("cache_reuse", c_int),       # single step: 1 = this step's forward is a reuse forward
     ]
 
 
@@ -113,6 +116,8 @@ SIGNATURES = {
     "ivid_unet_forward_cond": (c_int, [c_void_p, c_void_p, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "ivid_unet_forward_hw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p, c_int,
                                      c_void_p]),
+    "ivid_unet_forward_reuse": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p,
+                                        c_int, c_int, c_void_p]),
     "ivid_conv_tile": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "ivid_unet_debug_tap": (c_int, [c_void_p, c_int, c_char_p, c_void_p, c_uint64, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "ivid_unet_profile_begin": (c_int, [c_void_p]),

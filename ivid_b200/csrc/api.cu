@@ -131,6 +131,16 @@ int ivid_unet_forward_hw(ivid_unet_t* h, const float* x_dev, int Nx, int H, int 
     h->impl->forward(x_dev, Nx, H, W, cond, t_dev, classes_dev, eps_dev, N, static_cast<cudaStream_t>(stream));
   });
 }
+int ivid_unet_forward_reuse(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
+                            const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, int cache_branch,
+                            void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(h); IVID_NOT_NULL(x_dev); IVID_NOT_NULL(t_dev); IVID_NOT_NULL(eps_dev);
+    IVID_REQUIRE(cache_branch >= 0, "cache_branch must be in [0, num_res_blocks]");
+    h->impl->forward(x_dev, Nx, H, W, cond, t_dev, classes_dev, eps_dev, N, static_cast<cudaStream_t>(stream), nullptr,
+                     cache_branch);
+  });
+}
 // the square forwards at the backbone's image_size
 int ivid_unet_forward(ivid_unet_t* h, const float* x_dev, int Nx, const int64_t* t_dev, const int64_t* classes_dev,
                       float* eps_dev, int N, void* stream) {

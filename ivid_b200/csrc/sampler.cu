@@ -223,6 +223,14 @@ static void require_interval(const ivid_step_args_t& a, int T) {
                "guidance interval must satisfy 0 <= t_lo <= t_hi < T");
 }
 
+// feature reuse: cache_interval >= 0, cache_branch one of the top-level blocks, cache_reuse a flag
+static void require_cache(const ivid_step_args_t& a, const Unet& unet) {
+  IVID_REQUIRE(a.cache_interval >= 0, "cache_interval must be >= 0");
+  IVID_REQUIRE(a.cache_branch >= 0 && a.cache_branch <= unet.cfg().num_res_blocks,
+               "cache_branch must be in [0, num_res_blocks] = [0, " + std::to_string(unet.cfg().num_res_blocks) + "]");
+  IVID_REQUIRE(a.cache_reuse == 0 || a.cache_reuse == 1, "cache_reuse must be 0 or 1");
+}
+
 void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, int t, int t_prev,
                    const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
                    const int64_t* t_prev_dev) {
@@ -235,6 +243,8 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
                "sampler kind must be 0 (DDPM), 1 (DDIM) or 2 (DPM-Solver++)");
   require_sde(a);
   require_interval(a, T_);
+  require_cache(a, unet);
+  const int cache_branch = a.cache_reuse ? a.cache_branch : -1;
   const int kind = a.kind;
   const bool ddim = kind != kStepDdpm;      // DDIM's step convention: actual steps t / t_prev (DPM-Solver++ shares it)
   const bool dpm = kind == kStepDpm;
@@ -358,11 +368,11 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
       else head_step_kernel<kStepDdpm><<<std::max(grid, 1), 256, 0, st>>>(q);
       IVID_CHECK_CUDA(cudaGetLastError());
     };
-    unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, Nf, stream, &hook);
+    unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, Nf, stream, &hook, cache_branch);
     unet.set_cond_stream_dev(nullptr);
     return;
   }
-  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, Nf, stream);
+  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, Nf, stream, nullptr, cache_branch);
   unet.set_cond_stream_dev(nullptr);
   const size_t total4 = static_cast<size_t>(N) * C * HW / 4;
   const int grid = static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8));
@@ -384,6 +394,7 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   IVID_REQUIRE(!dpm || (a.order >= 0 && a.order <= 2), "DPM-Solver++ order must be 1 or 2");
   require_sde(a);
   require_interval(a, T_);
+  require_cache(a, unet);
   const int jump = T_ / steps;                     // ddim.py:153
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));
   ensure_device(2 * N, 2 * img);
@@ -401,11 +412,24 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
     IVID_CHECK_CUDA(cudaGetLastError());
     classes2_ready_ = true; classes2_src_ = a.classes_dev; classes2_n_ = N;
   }
+  // feature reuse: a full forward at step 0, at a switch between the batch-2N and batch-N plans, and every cache_interval
+  // steps after the last full one; reuse forwards in between
+  const bool gated = a.guidance_interval != 0 && a.use_cfg && a.classes_dev != nullptr;
+  int last_full = 0;
+  bool last_two = false;
   for (int i = 0; i < steps; ++i) {
     int t, t_prev;
     if (ddim) { t = jump * (steps - i); t_prev = jump * (steps - 1 - i); }   // ddim.py:154
     else { t = T_ - 1 - i; t_prev = 0; }                                      // ddpm.py:177
     ivid_step_args_t ai = a;
+    const int t_model = ddim ? t - 1 : t;
+    // the plan step() runs this step's forward on: batch 2N exactly when it is a guided classifier-free step
+    const bool two = a.use_cfg && a.classes_dev != nullptr && a.strength > 0.0f &&
+                     (!gated || (t_model >= a.guidance_t_lo && t_model <= a.guidance_t_hi));
+    const bool full = a.cache_interval <= 1 || i == 0 || two != last_two || i - last_full >= a.cache_interval;
+    if (full) last_full = i;
+    last_two = two;
+    ai.cache_reuse = full ? 0 : 1;
     ai.step_noise_dev = noise_all ? noise_all + static_cast<size_t>(i) * img : nullptr;
     if (dpm) {
       // multistep history: from the second step on, D_{-1} is the previous step's D0, already in the sampler's buffer

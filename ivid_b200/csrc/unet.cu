@@ -442,18 +442,40 @@ struct Plan {
     double bytes;           // algorithmic HBM bytes of this launch (memory-bound ops)
     std::string note;       // shape description (per-op profile dump)
     std::function<void(cudaStream_t)> fn;
+    int block;              // index into Unet::blocks_ of the block the op belongs to; -1: embeddings, input packing, head
   };
   std::vector<OpRec> ops;
+  int op_block = -1;        // block of the ops the walk adds next
   void add_op(const char* label, double flops, double bytes, std::string note, std::function<void(cudaStream_t)> fn) {
-    ops.push_back(OpRec{label, flops, bytes, std::move(note), std::move(fn)});
+    ops.push_back(OpRec{label, flops, bytes, std::move(note), std::move(fn), op_block});
   }
-  // One forward: zero the statistics arena, then enqueue every op on s.  With `ev` (ops.size() + 1 events), ev[i] and
-  // ev[i + 1] bracket op i.
-  void run(cudaStream_t s, cudaEvent_t* ev = nullptr) const {
-    IVID_CHECK_CUDA(cudaMemsetAsync(stats_base, 0, stats_bytes, s));
+  // Feature reuse (DeepCache).  A reuse forward at branch b runs the ops of input blocks 0..b and output blocks L-1-b..L-1
+  // (blocks_ indices >= n_blocks - 1 - b) and those of no block.  It reads the output of output block L-2-b, with its fp16
+  // copy and its statistics, as the plan's last full forward left them.  The walk takes statistics block by block, so the
+  // kept blocks' statistics are the arena's head [0, block_stats[b + 1]) and tail [block_stats[n_blocks - 1 - b], end): a
+  // reuse forward zeroes only those, and the statistics of every skipped block, the cached tensor's among them, stay as the
+  // last full forward left them, whatever branches ran in between.
+  int n_blocks = 0;
+  std::vector<size_t> block_stats;   // arena offset of the first statistics each block takes
+  bool cache_valid = false;          // a full forward has been enqueued on this plan
+  bool kept(int block, int branch) const {
+    return branch < 0 || block < 0 || block <= branch || block >= n_blocks - 1 - branch;
+  }
+  // One forward: zero the statistics arena, then enqueue every op on s; branch >= 0: the reuse forward at that branch, which
+  // zeroes the kept blocks' statistics and runs the kept ops only.  With `ev` (ops.size() + 1 events), ev[i] and ev[i + 1]
+  // bracket op i (nothing in between for an op the reuse forward skips).
+  void run(cudaStream_t s, cudaEvent_t* ev = nullptr, int branch = -1) const {
+    if (branch < 0) {
+      IVID_CHECK_CUDA(cudaMemsetAsync(stats_base, 0, stats_bytes, s));
+    } else {
+      uint8_t* base = reinterpret_cast<uint8_t*>(stats_base);
+      const size_t head = block_stats[branch + 1], tail = block_stats[n_blocks - 1 - branch];
+      IVID_CHECK_CUDA(cudaMemsetAsync(base, 0, head, s));
+      if (tail < stats_bytes) IVID_CHECK_CUDA(cudaMemsetAsync(base + tail, 0, stats_bytes - tail, s));
+    }
     if (ev) IVID_CHECK_CUDA(cudaEventRecord(ev[0], s));
     for (size_t i = 0; i < ops.size(); ++i) {
-      ops[i].fn(s);
+      if (kept(ops[i].block, branch)) ops[i].fn(s);
       if (ev) IVID_CHECK_CUDA(cudaEventRecord(ev[i + 1], s));
     }
   }
@@ -472,8 +494,9 @@ struct Plan {
     const void* stream_dev;
     uint64_t hook_key;
     int sr_scale;
+    int cache_branch;        // -1: full forward; b: reuse forward at branch b
     bool operator==(const GraphKey& o) const {
-      return hook_key == o.hook_key && sr_scale == o.sr_scale && x == o.x && Nx == o.Nx && t == o.t && classes == o.classes && eps == o.eps && kind == o.kind && y == o.y && mask == o.mask &&
+      return hook_key == o.hook_key && sr_scale == o.sr_scale && cache_branch == o.cache_branch && x == o.x && Nx == o.Nx && t == o.t && classes == o.classes && eps == o.eps && kind == o.kind && y == o.y && mask == o.mask &&
              mask_rgb == o.mask_rgb && noise == o.noise && seed == o.seed && stream_id == o.stream_id && stream_dev == o.stream_dev;
     }
   };
@@ -541,6 +564,8 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
   std::unique_ptr<Plan> plan(new Plan());
   plan->N = N;
   plan->H = SH; plan->W = SW;
+  plan->n_blocks = static_cast<int>(blocks_.size());
+  plan->block_stats.assign(blocks_.size(), 0);      // block 0, the stem, takes the first statistics
   Plan* pl = plan.get();
   const int G = cfg_.num_groups;
   const float eps = 1e-5f;
@@ -648,6 +673,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     };
 
     // ---- embeddings ----
+    pl->op_block = -1;
     float* s_pe = s32(kPe, 1, 1, cfg_.model_channels);
     float* s_e1 = s32(kE1, 1, 1, embed_dim_);
     float* s_emb = s32(kEmb, 1, 1, embed_dim_);
@@ -710,6 +736,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
         }
       });
     }
+    pl->op_block = 0;
     Act cur = new_act(in_ch_stem_, SH, SW, true);
     {
       ConvDesc d;
@@ -870,6 +897,8 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
 
     for (size_t bi = 1; bi < blocks_.size(); ++bi) {
       const BlockDef& b = blocks_[bi];
+      if (create) pl->block_stats[bi] = soff;
+      pl->op_block = static_cast<int>(bi);
       bool first = true;
       for (const auto& l : b.layers) {
         switch (l.kind) {
@@ -892,6 +921,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
     IVID_REQUIRE(skips.empty(), "internal: skip stack not consumed");
 
     // ---- output head: GN + SiLU + conv3x3 -> eps (fp32 NCHW) ----
+    pl->op_block = -1;
     keep32(cur);
     const bool split_head = out_split_ && cur.has16;
     void* a1 = s16(kA1, SH, SW, cur.C);
@@ -963,8 +993,10 @@ bool Unet::can_fuse_head(int W) const {
 }
 
 void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes,
-                   float* eps, int N, cudaStream_t stream, const HeadHook* hook) {
+                   float* eps, int N, cudaStream_t stream, const HeadHook* hook, int cache_branch) {
   if (!finalized()) throw Error(kErrState, "AdmUnet2d: forward before .cuda()/finalize");
+  IVID_REQUIRE(cache_branch >= -1 && cache_branch <= cfg_.num_res_blocks,
+               "cache_branch must be in [0, num_res_blocks] = [0, " + std::to_string(cfg_.num_res_blocks) + "]");
   check_geometry(H, W);
   IVID_REQUIRE(N >= 1 && Nx >= 1 && N % Nx == 0, "forward: N must be a positive multiple of Nx");
   // reference: "this model is not class-conditioned" (adm.py:540)
@@ -979,10 +1011,13 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
   IVID_REQUIRE(hook != nullptr || eps != nullptr, "forward: eps output missing");
 
   Plan* pl = get_plan(N, H, W);
+  if (cache_branch >= 0 && !pl->cache_valid)
+    throw Error(kErrState, "reuse forward: no full forward of this batch size and input size has run since the plan was built");
   pl->x = x; pl->Nx = Nx; pl->t = t; pl->classes = classes; pl->eps = eps;
   pl->cond = cnd;
   pl->cond_stream_dev = cond_stream_dev_;
   pl->hook = hook;
+  if (cache_branch < 0) pl->cache_valid = true;      // the full forward is enqueued below
   if (!profile_) {
     // The first call of a plan runs eagerly (one-time function attributes, module loading); from the second call on the
     // forward is ONE cudaGraphLaunch.  Graphs are captured on a private stream (the caller's may be the legacy default
@@ -992,7 +1027,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
     if (graphs_on && pl->runs > 1) {
       const Plan::GraphKey key{x, Nx, t, classes, eps, cnd.kind, cnd.y_dev, cnd.mask_dev, cnd.mask_rgb_dev, cnd.noise_dev,
                                cnd.kind != 0 ? cnd.seed : 0ull, cnd.kind != 0 ? cnd.stream_id : 0u, cond_stream_dev_,
-                               hook ? hook->key : 0ull, cnd.kind == 2 ? cnd.sr_scale : 0};
+                               hook ? hook->key : 0ull, cnd.kind == 2 ? cnd.sr_scale : 0, cache_branch};
       for (auto& g : pl->graphs)
         if (g.key == key) {
           g.last_use = pl->runs;
@@ -1004,7 +1039,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
       // hands fresh buffers to every call (e.g. a Python loop that keeps every x_{t-1}): replay the launches on the stream
       const bool thrash = pl->graph_captures >= 32 && pl->graph_hits < pl->graph_captures;
       if (thrash) {
-        pl->run(stream);
+        pl->run(stream, nullptr, cache_branch);
         return;
       }
       ++pl->graph_captures;
@@ -1012,7 +1047,7 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
       cudaGraph_t graph = nullptr;
       IVID_CHECK_CUDA(cudaStreamBeginCapture(cap_stream_, cudaStreamCaptureModeRelaxed));
       try {
-        pl->run(cap_stream_);
+        pl->run(cap_stream_, nullptr, cache_branch);
       } catch (...) {
         cudaStreamEndCapture(cap_stream_, &graph);
         if (graph) cudaGraphDestroy(graph);
@@ -1035,16 +1070,17 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
       IVID_CHECK_CUDA(cudaGraphLaunch(exec, stream));
       return;
     }
-    pl->run(stream);
+    pl->run(stream, nullptr, cache_branch);
     return;
   }
   // profiling pass: every launch bracketed by CUDA events on the launching stream (serialised; shares, not absolutes)
   std::vector<cudaEvent_t> ev(pl->ops.size() + 1);
   for (auto& e : ev) IVID_CHECK_CUDA(cudaEventCreate(&e));
-  pl->run(stream, ev.data());
+  pl->run(stream, ev.data(), cache_branch);
   IVID_CHECK_CUDA(cudaStreamSynchronize(stream));
   for (size_t i = 0; i < pl->ops.size(); ++i) {
     const Plan::OpRec& op = pl->ops[i];
+    if (!pl->kept(op.block, cache_branch)) continue;
     float ms = 0.f;
     IVID_CHECK_CUDA(cudaEventElapsedTime(&ms, ev[i], ev[i + 1]));
     auto& agg = profile_acc_[op.label];

@@ -102,9 +102,13 @@ class Unet {
   size_t arena_bytes() const { return arena_bytes_; }
   int device() const { return device_; }
 
-  // forward over a batch of N samples of H x W pixels; x rows are read modulo Nx (CFG halves share x)
+  // forward over a batch of N samples of H x W pixels; x rows are read modulo Nx (CFG halves share x).
+  // cache_branch = -1: the full forward.  0 <= cache_branch <= num_res_blocks: the reuse forward at that branch (DeepCache,
+  // include/ivid_b200.h), which runs the embeddings, input packing, input blocks 0..b, output blocks L-1-b..L-1 and the head,
+  // and reads the output of output block L-2-b that the plan's last full forward left in place; kErrState before any full
+  // forward of the plan.
   void forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes,
-               float* eps, int N, cudaStream_t stream, const HeadHook* hook = nullptr);
+               float* eps, int N, cudaStream_t stream, const HeadHook* hook = nullptr, int cache_branch = -1);
   // whether the output head of an H x W forward runs as the tap-column GEMM whose last kernel a HeadHook can replace
   bool can_fuse_head(int W) const;
   // inputs the network accepts: H and W positive multiples of 2^(levels - 1), as in the reference (its skip concatenations

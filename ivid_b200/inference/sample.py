@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from .. import backbones, frameworks, samplers
+from ..samplers.samplers import _check_cache
 from ..rgbd_3d import DeviceWarp, glm_compat as glm
 from ..rgbd_3d import utils as rgbd_utils
 from ..utils import edict
@@ -60,14 +61,18 @@ def build_modelviews(viewset, num_samples, rng=None):
 @torch.no_grad()
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
-               precision="fp16", guidance_interval=None):
+               precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, and solver="dpmpp_sde" its stochastic variant
     (SDE-DPM-Solver++(2M)); DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
     runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision).  guidance_interval=(t_lo, t_hi)
     guides only the steps of both networks whose model time lies in [t_lo, t_hi] (the samplers' `guidance_interval`);
-    the other steps run at strength 0 with one batch-N forward."""
+    the other steps run at strength 0 with one batch-N forward.  cache_interval=N, cache_branch=b reuse the deep features of
+    both networks between full forwards every N steps (the samplers' `cache_interval` / `cache_branch`; None: no reuse)."""
+    for fw in (framework_uncond, framework_cond):          # before any device work
+        if fw is not None:
+            _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
     assert solver in ("ddim", "dpmpp", "dpmpp_sde"), f"solver must be 'ddim', 'dpmpp' or 'dpmpp_sde', got {solver!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
@@ -77,6 +82,8 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
     sde_kw = dict(sde=True) if solver == "dpmpp_sde" else {}
     gi_kw = dict(guidance_interval=tuple(guidance_interval)) if guidance_interval is not None else {}
+    if cache_interval is not None:
+        gi_kw.update(cache_interval=cache_interval, cache_branch=cache_branch)
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
     net = framework_uncond.backbone
@@ -110,7 +117,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
         for j in range(n_views):
             mv_j = [views_of(k)[j] for k in range(bs)] if per_sample_views else views_of(0)[j]
             if j == 0:
-                kw = dict(strength=guidance, **gi_kw) if cfg_u else {}
+                kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
                 if steps_uncond < 1000:
                     kw.update(sde_kw)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
@@ -122,7 +129,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 cond_depth.append(cond[:, 3:4] * 2 - 1)
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
-                kw = dict(strength=guidance, **gi_kw) if cfg_u else {}
+                kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
                 kw.update(sde_kw)
                 res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
             samples.append(res.samples)
@@ -246,22 +253,45 @@ def main(rank, world_size, opt):
     solver = getattr(opt, "solver", "ddim")
     precision = getattr(opt, "precision", "fp16")
     interval = getattr(opt, "guidance_interval", None)
-    out_dir = os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
-                           + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}")
-                           + ("" if interval is None else f"_interval{interval[0]}-{interval[1]}"))
+    cache_interval, cache_branch = getattr(opt, "cache_interval", None), getattr(opt, "cache_branch", 0)
+    out_dir = output_dir_name(opt)
     for sub in ("results", "grids", "conds", "scenes"):                 # sample.py:283-286
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
     save_cfg = edict(output_dir=out_dir, viewset=opt.viewset)
     gen = sample_all(fw_u, fw_c, seeds_r if seeds_r is not None else len(idx), opt.steps_uncond, opt.steps_cond, mvs_r, classes=classes_r,
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
                      rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
-                     precision=precision, guidance_interval=interval)
+                     precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch)
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
         threads.append(async_save(meshes, colors, samples, conds, tag, save_cfg))
     for th in threads:
         th.join()
+
+
+def output_dir_name(opt):
+    """Output directory of a run: the reference's name, with a suffix for every extension that changes the samples."""
+    solver = getattr(opt, "solver", "ddim")
+    precision = getattr(opt, "precision", "fp16")
+    interval = getattr(opt, "guidance_interval", None)
+    cache_interval = getattr(opt, "cache_interval", None)
+    return os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
+                        + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}")
+                        + ("" if interval is None else f"_interval{interval[0]}-{interval[1]}")
+                        + ("" if cache_interval is None else f"_cache{cache_interval}b{getattr(opt, 'cache_branch', 0)}"))
+
+
+def _int_at_least(lo):
+    def parse(s):
+        try:
+            v = int(s)
+        except ValueError:
+            raise argparse.ArgumentTypeError(f"expected an integer, got {s!r}") from None
+        if v < lo:
+            raise argparse.ArgumentTypeError(f"expected an integer >= {lo}, got {s!r}")
+        return v
+    return parse
 
 
 def parse_interval(s):
@@ -311,6 +341,12 @@ def build_arg_parser():
     ap.add_argument("--guidance_interval", type=parse_interval, default=None, metavar="LO,HI",
                     help="apply classifier-free guidance only at the steps whose model time t (0 <= t < T, the t the network "
                          "receives) lies in [LO, HI]; the other steps run unguided with half the network work (default: every step)")
+    ap.add_argument("--cache_interval", type=_int_at_least(1), default=None, metavar="N",
+                    help="reuse the deep UNet features between denoising steps (DeepCache): a full forward every N steps, shallow "
+                         "forwards in between; approximates the samples (default: every forward in full)")
+    ap.add_argument("--cache_branch", type=_int_at_least(0), default=0, metavar="B",
+                    help="with --cache_interval: the shallow forwards recompute input blocks 0..B and the last B+1 output blocks, "
+                         "0 <= B <= num_res_blocks (default 0, the cheapest)")
     return ap
 
 

@@ -15,6 +15,7 @@ the torch RNG stream consumption identical to the reference.
 from __future__ import annotations
 
 import ctypes
+import numbers
 
 import numpy as np
 import torch
@@ -42,6 +43,17 @@ def _check_interval(guidance_interval, T):
     lo, hi = (int(v) for v in guidance_interval)
     assert 0 <= lo <= hi < T, f"guidance_interval must satisfy 0 <= t_lo <= t_hi < {T}, got ({lo}, {hi})"
     return lo, hi
+
+
+def _check_cache(cache_interval, cache_branch, num_res_blocks):
+    """Feature reuse (DeepCache) arguments: cache_interval None (no reuse) or an int >= 1, and cache_branch an int in
+    [0, num_res_blocks], one of the top-level blocks.  Returns cache_interval as an int, 0 for None."""
+    if cache_interval is not None:
+        assert isinstance(cache_interval, numbers.Integral) and cache_interval >= 1, \
+            f"cache_interval must be None or an integer >= 1, got {cache_interval!r}"
+    assert isinstance(cache_branch, numbers.Integral) and 0 <= cache_branch <= num_res_blocks, \
+        f"cache_branch must be an integer in [0, num_res_blocks] = [0, {num_res_blocks}], got {cache_branch!r}"
+    return int(cache_interval) if cache_interval is not None else 0
 
 
 class _NativeSampler:
@@ -76,7 +88,7 @@ class _NativeSampler:
 
     # ------------------------------------------------------------------------------------------------------------
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None, sde=False, interval=None):
+                   order=0, prev=None, sde=False, interval=None, cache=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -135,6 +147,8 @@ class _NativeSampler:
         if interval is not None:
             a.guidance_interval = 1
             a.guidance_t_lo, a.guidance_t_hi = interval
+        if cache is not None:
+            a.cache_interval, a.cache_branch, a.cache_reuse = (int(v) for v in cache)
         return a, keep
 
     def _net(self):
@@ -142,13 +156,16 @@ class _NativeSampler:
         net._ensure_packed()
         return net
 
+    def _num_res_blocks(self):
+        return _unwrap(self.framework.backbone).num_res_blocks
+
     def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                     sde=False, interval=None):
+                     sde=False, interval=None, cache=None):
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         with torch.cuda.device(dev):
@@ -159,13 +176,13 @@ class _NativeSampler:
         return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
 
     def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                         sde=False, interval=None):
+                         sde=False, interval=None, cache=None):
         """Same step with the timestep taken on the device from the [N] tensors the caller passed (no host sync)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache)
         td = t.to(device=dev, dtype=torch.int64).contiguous()
         tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
         x_prev = torch.empty_like(x_t)
@@ -187,9 +204,26 @@ class _NativeSampler:
             cond_noise = torch.cat([n_rgb, n_d], dim=1)
         return torch.randn_like(x_t), cond_noise
 
+    def _reuse_schedule(self, model_times, classes, kwargs, interval, cache_interval):
+        """Whether each step of a run reuses the cached features, by ivid_sampler_run's rule: a full forward at the first
+        step, where the forward switches between the guided batch-2N and the unguided batch-N plan, and cache_interval steps
+        after the last full one."""
+        uses_cfg = isinstance(self.framework, (ClassifierFreeGuidance, InpaintCFG, SuperResCFG))
+        strength = float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
+        reuse, last_full, last_two = [], 0, False
+        for i, tm in enumerate(model_times):
+            two = uses_cfg and classes is not None and strength > 0 and (interval is None or interval[0] <= tm <= interval[1])
+            full = cache_interval <= 1 or i == 0 or two != last_two or i - last_full >= cache_interval
+            if full:
+                last_full = i
+            last_two = two
+            reuse.append(not full)
+        return reuse
+
     def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
-             sde=False, interval=None):
+             sde=False, interval=None, cache_interval=None, cache_branch=0):
         interval = _check_interval(interval, len(self.framework.betas))   # before any device work
+        cache_interval = _check_cache(cache_interval, cache_branch, self._num_res_blocks())
         net = self._net()
         net.eval()
         if image_size is None:
@@ -211,7 +245,10 @@ class _NativeSampler:
                 jump = T // nsteps
                 sched = [(jump * (i + 1), jump * i) for i in reversed(range(nsteps))]
             prev = None
-            for (t, t_prev) in sched:
+            reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
+                                         cache_interval)
+            for i, (t, t_prev) in enumerate(sched):
+                cache = (0, cache_branch, reuse[i])
                 # the reference draws the model-input noise first (inside model_inference), then randn_like(x_t)
                 cond_noise = None
                 if isinstance(self.framework, InpaintCFG):
@@ -221,10 +258,12 @@ class _NativeSampler:
                 if self.KIND == 2:
                     # the SDE update uses z; the ODE update draws it only to consume the torch RNG as DdimSampler does
                     out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if sde else None, cond_noise,
-                                            order=order, prev=prev if order != 1 else None, sde=sde, interval=interval)
+                                            order=order, prev=prev if order != 1 else None, sde=sde, interval=interval,
+                                            cache=cache)
                     prev = (t, out.pred_x_0)
                 else:
-                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise, interval=interval)
+                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise, interval=interval,
+                                            cache=cache)
                 img = out.pred_x_prev
                 if return_trajectory:
                     ret.pred_x_t.append(out.pred_x_prev)
@@ -232,7 +271,7 @@ class _NativeSampler:
         elif rng == "philox":
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
             a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
-                                      interval=interval)
+                                      interval=interval, cache=(cache_interval, cache_branch, 0))
             traj0 = trajt = None
             if return_trajectory:
                 traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
@@ -265,13 +304,17 @@ class DdpmSampler(_NativeSampler):
         self.posterior_mean_coef2 = (1.0 - self.alphas_cumprod_prev) * np.sqrt(alphas) / (1.0 - self.alphas_cumprod)
 
     @torch.no_grad()
-    def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, guidance_interval=None, **kwargs):
+    def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, guidance_interval=None, reuse_features=False,
+                    cache_branch=0, **kwargs):
         """x_{t-1} from x_t (ddpm.py:111-131).  `t` is the [N] tensor of steps minus 1 (all equal).
         `noise` (extension) injects the randn_like draw; default draws it with torch like the reference.
-        `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`)."""
+        `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`).
+        `reuse_features=True` (extension): the step's forward reuses the deep features of the last full forward of the same
+        batch and size at branch `cache_branch` (see `sample`); RuntimeError if no full forward has run on it."""
         B = x_t.shape[0]
         assert t.shape == (B,), "t must be a 1D tensor of shape (B,)"
         _check_interval(guidance_interval, len(self.framework.betas))
+        _check_cache(None, cache_branch, self._num_res_blocks())
         # all samples of a batch share the timestep (both reference samplers are driven that way: ddpm.py:177-179);
         # element 0 is read on the device, so this call does not synchronise with the host
         if noise is None:
@@ -279,11 +322,11 @@ class DdpmSampler(_NativeSampler):
         else:
             cond_noise = kwargs.pop("cond_noise", None)
         return self._native_step_dev(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, cond_noise,
-                                     interval=guidance_interval)
+                                     interval=guidance_interval, cache=(0, cache_branch, bool(reuse_features)))
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
-               rng="philox", return_trajectory=False, guidance_interval=None, **kwargs):
+               rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0, **kwargs):
         """Run the full reverse process (ddpm.py:134-187).  `steps` is accepted and ignored exactly as in the reference.
         pred_x_t / pred_x_0 are only materialised with return_trajectory=True (the reference keeps 2x1000 tensors alive;
         its callers read `.samples` only: inference/sample.py:82).
@@ -291,9 +334,16 @@ class DdpmSampler(_NativeSampler):
         guidance_interval=(t_lo, t_hi) (extension; Kynkaanniemi et al. 2024, arXiv:2404.07724): classifier-free guidance
         only at the steps whose model time t (the t the network receives) lies in [t_lo, t_hi], 0 <= t_lo <= t_hi < T;
         every other step is the same step at strength 0 and runs one batch-N forward instead of the batch-2N one.  None
-        (default) guides every step.  No effect without classes."""
+        (default) guides every step.  No effect without classes.
+
+        cache_interval=N, cache_branch=b (extension; DeepCache, Ma, Fang, Wang, CVPR 2024, arXiv:2312.00858): a full network
+        forward every N steps; the steps in between recompute only the shallow branch b (the stem, input blocks 0..b, the
+        last b + 1 output blocks and the head) and reuse the deeper up-path features of the last full forward.  A step where
+        the guidance interval switches between the guided and the unguided forward is always full.  0 <= b <=
+        num_res_blocks; b = 0 is the cheapest.  None (default) or 1 runs every forward in full.  The update, the noise and the
+        torch RNG consumption are those of a run without reuse; eps is an approximation."""
         return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         interval=guidance_interval)
+                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch)
 
 
 class DdimSampler(_NativeSampler):
@@ -302,27 +352,32 @@ class DdimSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, eta=0.0, replace_rgb=None,
-                    replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, **kwargs):
+                    replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
+                    cache_branch=0, **kwargs):
         """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step).
-        `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi]."""
+        `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi].
+        `reuse_features` / `cache_branch` as in DdpmSampler.sample_once."""
         B = x_t.shape[0]
         assert t.shape == (B,) and t_prev.shape == (B,)
         _check_interval(guidance_interval, len(self.framework.betas))
+        _check_cache(None, cache_branch, self._num_res_blocks())
         # element 0 of t / t_prev is read on the device (all samples share the step, ddim.py:154-158): no host sync
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kw)
         else:
             cond_noise = kw.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, cond_noise, interval=guidance_interval)
+        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, cond_noise, interval=guidance_interval,
+                                     cache=(0, cache_branch, bool(reuse_features)))
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
-               verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, **kwargs):
+               verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
+               **kwargs):
         """Run `steps` DDIM steps (ddim.py:106-165).  `guidance_interval=(t_lo, t_hi)` as in DdpmSampler.sample, on the model
-        time t - 1 of each step."""
+        time t - 1 of each step; `cache_interval` / `cache_branch` as in DdpmSampler.sample."""
         return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
-                         interval=guidance_interval)
+                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -340,31 +395,37 @@ class DpmSolverSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
-                    constrain_depth=None, noise=None, sde=False, guidance_interval=None, **kwargs):
+                    constrain_depth=None, noise=None, sde=False, guidance_interval=None, reuse_features=False, cache_branch=0,
+                    **kwargs):
         """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
         With sde=True `noise` is the injected z of the update; with sde=False the update does not use it.  When it is None
         the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
-        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval` as for
-        DdimSampler.sample_once."""
+        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval`, `reuse_features`
+        and `cache_branch` as for DdimSampler.sample_once."""
         B = x_t.shape[0]
         assert t.shape == (B,) and t_prev.shape == (B,)
         _check_interval(guidance_interval, len(self.framework.betas))
+        _check_cache(None, cache_branch, self._num_res_blocks())
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kw)
         else:
             cond_noise = kw.pop("cond_noise", None)
         return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise if sde else None, cond_noise,
-                                     order=2 if prev is not None else 1, prev=prev, sde=sde, interval=guidance_interval)
+                                     order=2 if prev is not None else 1, prev=prev, sde=sde, interval=guidance_interval,
+                                     cache=(0, cache_branch, bool(reuse_features)))
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
-               rng="philox", return_trajectory=False, sde=False, guidance_interval=None, **kwargs):
+               rng="philox", return_trajectory=False, sde=False, guidance_interval=None, cache_interval=None, cache_branch=0,
+               **kwargs):
         """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
         final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
         is drawn where DdimSampler draws it (`rng`).  `guidance_interval` as in DdimSampler.sample; the history D_{-1} of a
-        step after an unguided one is that step's unguided D0.  Same return dict as DdimSampler.sample."""
+        step after an unguided one is that step's unguided D0.  `cache_interval` / `cache_branch` as in DdpmSampler.sample;
+        the history D_{-1} of a step is that step's D0, from whichever forward ran.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         order=order, sde=bool(sde), interval=guidance_interval)
+                         order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
+                         cache_branch=cache_branch)
