@@ -278,7 +278,7 @@ void attn_launch_run(const AttnLaunch* l, cudaStream_t s) {
       case 5: run_attn_hd<2, true>(l, s); break;
       case 7: run_attn_hd<3, true>(l, s); break;
       case 9: run_attn_hd<4, true>(l, s); break;
-      case 4: run_attn_hd<2, false>(l, s); break;
+      // nv = 2 only at k <= 4 chunks, where Q is always resident: there is no <2, false>
       case 6: run_attn_hd<3, false>(l, s); break;
       case 8: run_attn_hd<4, false>(l, s); break;
       default: throw Error(kErrState, "internal: attention slice width " + std::to_string(l->nv));
