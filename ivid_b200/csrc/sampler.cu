@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 
 #include "sampler.cuh"
 
@@ -50,37 +51,29 @@ __device__ void dpm_step_state(DpmStep* d, const double* acp, int t, int t_prev,
   }
 }
 
-// acp != nullptr: DPM-Solver++ step t_index + 1 -> t_prev (order / t_last / sde as in dpm_step_state)
-// guided: whether the step lies inside the guidance interval (the host route decides it and sizes the forward by it)
-__global__ void set_step_kernel(StepState* st, int64_t* t_model, int N, int t_index, int t_prev, int stream, const double* acp,
-                                int t_last, int order, int sde, int guided) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    st->t_index = t_index;
-    st->t_prev = t_prev;
-    st->stream = stream;
-    st->guided = guided;
-    if (acp != nullptr) dpm_step_state(&st->dpm, acp, t_index + 1, t_prev, t_last, order, sde);
+// The step state, and the model time of every row of the forward.  Host route (t_dev == nullptr): the host ints t_index /
+// t_prev, already range-checked, and Philox stream stream_id.  Device route: the step is read from element 0 of the
+// caller's tensors (sample_once(x_t, t[, t_prev]) of the reference passes [N] tensors; reading it here removes the
+// device->host sync an int(t[0]) would cost), out-of-range steps are clamped into the table (the host route raises
+// instead), and the Philox stream is t.  acp != nullptr: DPM-Solver++ step t_index + 1 -> t_prev (order / t_last / sde as
+// in dpm_step_state; a device-route step is first order unless t_last > t).  The step is guided unless an interval applies
+// (gated != 0) and the model time lies outside [t_lo, t_hi].
+__global__ void set_step_kernel(StepState* st, int64_t* t_model, int N, int t_index, int t_prev, int stream_id,
+                                const int64_t* t_dev, const int64_t* t_prev_dev, int ddim, int T, const double* acp, int t_last,
+                                int order, int sde, int gated, int t_lo, int t_hi) {
+  long long ti = t_index, tp = t_prev, stream = stream_id;
+  if (t_dev != nullptr) {
+    stream = t_dev[0];
+    ti = ddim ? stream - 1 : stream;
+    ti = ti < 0 ? 0 : (ti > T - 1 ? T - 1 : ti);
+    tp = (ddim && t_prev_dev != nullptr) ? t_prev_dev[0] : 0;
+    tp = tp < 0 ? 0 : (tp > T ? T : tp);
   }
-  for (int i = threadIdx.x; i < N; i += blockDim.x) t_model[i] = t_index;
-}
-
-// same, with the step read from the caller's device tensors (sample_once(x_t, t[, t_prev]) of the reference passes [N]
-// tensors; reading element 0 here removes the device->host sync an int(t[0]) would cost).  Out-of-range steps are
-// clamped into the table (the host path raises instead); a DPM-Solver++ step is first order unless t_last > t.  The step is
-// guided unless an interval is given (interval != 0) and the clamped model time lies outside [t_lo, t_hi].
-__global__ void set_step_dev_kernel(StepState* st, int64_t* t_model, int N, const int64_t* t_dev, const int64_t* t_prev_dev,
-                                    int ddim, int T, const double* acp, int t_last, int order, int sde, int interval, int t_lo,
-                                    int t_hi) {
-  long long t = t_dev[0];
-  long long ti = ddim ? t - 1 : t;
-  ti = ti < 0 ? 0 : (ti > T - 1 ? T - 1 : ti);
-  long long tp = (ddim && t_prev_dev != nullptr) ? t_prev_dev[0] : 0;
-  tp = tp < 0 ? 0 : (tp > T ? T : tp);
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     st->t_index = static_cast<int>(ti);
     st->t_prev = static_cast<int>(tp);
-    st->stream = static_cast<int>(t);
-    st->guided = (!interval || (ti >= t_lo && ti <= t_hi)) ? 1 : 0;
+    st->stream = static_cast<int>(stream);
+    st->guided = (!gated || (ti >= t_lo && ti <= t_hi)) ? 1 : 0;
     if (acp != nullptr) dpm_step_state(&st->dpm, acp, static_cast<int>(ti) + 1, static_cast<int>(tp), t_last, order, sde);
   }
   for (int i = threadIdx.x; i < N; i += blockDim.x) t_model[i] = ti;
@@ -210,97 +203,127 @@ void Sampler::ensure_hist(size_t elems) {
   cap_hist_ = elems;
 }
 
-// sde selects the stochastic DPM-Solver++ update; it is a flag of kind 2 only
-static void require_sde(const ivid_step_args_t& a) {
+// sample size H x W: 0 means the backbone's image_size
+static int sample_dim(int v, const Unet& unet) { return v > 0 ? v : unet.cfg().image_size; }
+
+// The checks of everything a step and a run share: the single step calls this once, the run once before its loop.  Nothing
+// here touches the device.
+void Sampler::check_step_args(const ivid_step_args_t& a, const Unet& unet, int N) const {
+  IVID_REQUIRE(N >= 1, "batch must be positive");
+  IVID_REQUIRE(sample_dim(a.height, unet) * sample_dim(a.width, unet) % 4 == 0, "image size");
+  IVID_REQUIRE(a.kind == kStepDdpm || a.kind == kStepDdim || a.kind == kStepDpm,
+               "sampler kind must be 0 (DDPM), 1 (DDIM) or 2 (DPM-Solver++)");
+  // DPM-Solver++: second order when the previous step's data prediction is given, unless order = 1 forces first order
+  IVID_REQUIRE(a.kind != kStepDpm || (a.order >= 0 && a.order <= 2), "DPM-Solver++ order must be 1 or 2");
+  // sde selects the stochastic DPM-Solver++ update; it is a flag of kind 2 only
   IVID_REQUIRE(a.sde == 0 || a.sde == 1, "sde must be 0 or 1");
   IVID_REQUIRE(a.sde == 0 || a.kind == kStepDpm, "sde = 1 needs kind 2 (DPM-Solver++)");
-}
-
-// guidance interval in model times: 0 <= t_lo <= t_hi < T
-static void require_interval(const ivid_step_args_t& a, int T) {
+  // guidance interval in model times: 0 <= t_lo <= t_hi < T
   IVID_REQUIRE(a.guidance_interval == 0 || a.guidance_interval == 1, "guidance_interval must be 0 or 1");
-  IVID_REQUIRE(a.guidance_interval == 0 || (a.guidance_t_lo >= 0 && a.guidance_t_lo <= a.guidance_t_hi && a.guidance_t_hi < T),
+  IVID_REQUIRE(a.guidance_interval == 0 || (a.guidance_t_lo >= 0 && a.guidance_t_lo <= a.guidance_t_hi && a.guidance_t_hi < T_),
                "guidance interval must satisfy 0 <= t_lo <= t_hi < T");
-}
-
-// feature reuse: cache_interval >= 0, cache_branch one of the top-level blocks, cache_reuse a flag
-static void require_cache(const ivid_step_args_t& a, const Unet& unet) {
+  // feature reuse: cache_interval >= 0, cache_branch one of the top-level blocks, cache_reuse a flag
   IVID_REQUIRE(a.cache_interval >= 0, "cache_interval must be >= 0");
   IVID_REQUIRE(a.cache_branch >= 0 && a.cache_branch <= unet.cfg().num_res_blocks,
                "cache_branch must be in [0, num_res_blocks] = [0, " + std::to_string(unet.cfg().num_res_blocks) + "]");
   IVID_REQUIRE(a.cache_reuse == 0 || a.cache_reuse == 1, "cache_reuse must be 0 or 1");
+  IVID_REQUIRE(a.replace_rgb_dev == nullptr || a.replace_rgb_mask_dev != nullptr, "replace_rgb needs its mask");
+  IVID_REQUIRE(a.replace_depth_dev == nullptr || a.replace_depth_mask_dev != nullptr, "replace_depth needs its mask");
+  IVID_REQUIRE(a.constrain_depth_dev == nullptr || a.replace_depth_dev != nullptr,
+               "constrain_depth is applied inside replace_depth (ddim.py:90-95)");
+  IVID_REQUIRE(a.kind != kStepDdpm || (a.replace_rgb_dev == nullptr && a.replace_depth_dev == nullptr),
+               "replace/constrain guidance is DDIM / DPM-Solver++ only");
+}
+
+// What one step runs, decided in one place from the arguments and the step.
+struct StepPlan {
+  int t_index;        // table row of the model time: t for DDPM, t - 1 for DDIM / DPM-Solver++ (ddim.py:81)
+  int t_prev;         // DDIM / DPM-Solver++: the previous actual step
+  bool gated;         // a guidance interval applies: use_cfg, classes and an interval
+  bool guided;        // host route: the model time lies inside the interval (or none applies); the device route sets true
+  int cfg;            // StepParams::cfg
+  int Nf;             // the forward's batch: 2N exactly when cfg == 1
+  int order;          // DPM-Solver++ order of the update: 2 with a previous data prediction unless order = 1, else 1
+  int cache_branch;   // branch of a reuse forward, -1 for a full forward
+};
+
+// t_on_device: the step is read on the device (t / t_prev are not known here)
+static StepPlan plan_step(const ivid_step_args_t& a, int N, int t, int t_prev, bool t_on_device) {
+  StepPlan sp;
+  sp.t_index = a.kind != kStepDdpm ? t - 1 : t;
+  sp.t_prev = t_prev;
+  const bool has_classes = a.classes_dev != nullptr;
+  // guidance interval: a step whose model time lies outside it is the step at strength 0, eps = eps_c of one forward.  The
+  // host route knows t and runs that step as a batch-N forward; the device route keeps the batch-2N forward and the step
+  // kernel reads the guided flag set_step_kernel writes.  Without classes (or use_cfg) only one forward runs anyway.
+  sp.gated = a.guidance_interval != 0 && a.use_cfg && has_classes;
+  sp.guided = !sp.gated || t_on_device || (sp.t_index >= a.guidance_t_lo && sp.t_index <= a.guidance_t_hi);
+  // classifier-free guidance: one batch-2N forward when strength > 0 and the model is class conditional (cfg 1).
+  // inpaint_cfg.py:77-78 / sr_cfg.py:53-54: classes None -> single null-class forward, no (1+s) scaling.
+  // strength < 0: (1 + strength) * eps of ONE forward (classifier_free_guidance.py:40-41, cfg 2); the conditional
+  // frameworks skip even that when classes is None
+  const bool two = a.use_cfg && has_classes && a.strength > 0.0f && sp.guided;
+  const bool scale_only = a.use_cfg && a.strength < 0.0f && (has_classes || a.cond.kind == 0) && sp.guided;
+  sp.cfg = two ? 1 : (scale_only ? 2 : 0);
+  sp.Nf = two ? 2 * N : N;
+  sp.order = (a.kind == kStepDpm && a.prev_x0_dev != nullptr && a.order != 1) ? 2 : 1;
+  sp.cache_branch = a.cache_reuse ? a.cache_branch : -1;
+  return sp;
+}
+
+// f(std::integral_constant<int, kind>()): the step kind as the step kernels' template argument
+template <typename F>
+static void with_step_kind(int kind, F&& f) {
+  if (kind == kStepDdim) f(std::integral_constant<int, kStepDdim>());
+  else if (kind == kStepDpm) f(std::integral_constant<int, kStepDpm>());
+  else f(std::integral_constant<int, kStepDdpm>());
 }
 
 void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, int t, int t_prev,
                    const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
                    const int64_t* t_prev_dev) {
-  const UnetConfig& uc = unet.cfg();
-  const int C = uc.out_channels, H = a.height > 0 ? a.height : uc.image_size, W = a.width > 0 ? a.width : uc.image_size;
+  check_step_args(a, unet, N);
+  const StepPlan sp = plan_step(a, N, t, t_prev, t_dev != nullptr);
+  if (t_dev == nullptr) {                   // the device route clamps the step instead
+    IVID_REQUIRE(sp.t_index >= 0 && sp.t_index < T_, "t out of range");
+    IVID_REQUIRE(a.kind == kStepDdpm || (t_prev >= 0 && t_prev <= T_), "t_prev out of range");
+    IVID_REQUIRE(a.kind != kStepDpm || t_prev < t, "DPM-Solver++ step needs t_prev < t");
+  }
+  IVID_REQUIRE(sp.order == 1 || (a.t_last >= 1 && a.t_last <= T_), "t_last out of range");
+  IVID_REQUIRE(sp.order == 1 || t_dev != nullptr || a.t_last > t, "the previous step t_last must come before t (t_last > t)");
+  step_impl(unet, x_t, x_prev, pred_x0, N, sp, a, stream_id, stream, t_dev, t_prev_dev, true, false);
+}
+
+void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, const StepPlan& sp,
+                        const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
+                        const int64_t* t_prev_dev, bool allow_fuse, bool classes2_filled) {
+  const int C = unet.cfg().out_channels, H = sample_dim(a.height, unet), W = sample_dim(a.width, unet);
   const int HW = H * W;
-  IVID_REQUIRE(N >= 1, "batch must be positive");
-  IVID_REQUIRE(HW % 4 == 0, "image size");
-  IVID_REQUIRE(a.kind == kStepDdpm || a.kind == kStepDdim || a.kind == kStepDpm,
-               "sampler kind must be 0 (DDPM), 1 (DDIM) or 2 (DPM-Solver++)");
-  require_sde(a);
-  require_interval(a, T_);
-  require_cache(a, unet);
-  const int cache_branch = a.cache_reuse ? a.cache_branch : -1;
   const int kind = a.kind;
-  const bool ddim = kind != kStepDdpm;      // DDIM's step convention: actual steps t / t_prev (DPM-Solver++ shares it)
   const bool dpm = kind == kStepDpm;
-  const int t_index = ddim ? t - 1 : t;     // ddim.py:81 calls the model with t - 1
-  IVID_REQUIRE(t_dev != nullptr || (t_index >= 0 && t_index < T_), "t out of range");
-  IVID_REQUIRE(t_dev != nullptr || !ddim || (t_prev >= 0 && t_prev <= T_), "t_prev out of range");
-  // DPM-Solver++: second order when the previous step's data prediction is given, unless order = 1 forces first order
-  IVID_REQUIRE(!dpm || (a.order >= 0 && a.order <= 2), "DPM-Solver++ order must be 1 or 2");
-  IVID_REQUIRE(t_dev != nullptr || !dpm || t_prev < t, "DPM-Solver++ step needs t_prev < t");
-  const bool dpm2 = dpm && a.prev_x0_dev != nullptr && a.order != 1;
-  IVID_REQUIRE(!dpm2 || (a.t_last >= 1 && a.t_last <= T_), "t_last out of range");
-  IVID_REQUIRE(!dpm2 || t_dev != nullptr || a.t_last > t, "the previous step t_last must come before t (t_last > t)");
-  // classifier-free guidance: one batch-2N forward when strength > 0 and the model is class conditional
-  const bool has_classes = a.classes_dev != nullptr;
-  // guidance interval: a step whose model time lies outside it is the step at strength 0, eps = eps_c of one forward.  The
-  // host-int route knows t and runs that step as a batch-N forward; the device route keeps the batch-2N forward and the step
-  // kernel reads the guided flag set_step_dev_kernel writes.  Without classes (or use_cfg) only one forward runs anyway.
-  const bool gated = a.guidance_interval != 0 && a.use_cfg && has_classes;
-  const bool guided = !gated || t_dev != nullptr || (t_index >= a.guidance_t_lo && t_index <= a.guidance_t_hi);
-  const bool cfg_two = a.use_cfg && has_classes && a.strength > 0.0f && guided;
-  // inpaint_cfg.py:77-78 / sr_cfg.py:53-54: classes None -> single null-class forward, no (1+s) scaling
-  // strength < 0: (1 + strength) * eps of ONE forward (classifier_free_guidance.py:40-41); the conditional frameworks skip even
-  // that when classes is None
-  const bool scale_only = a.use_cfg && a.strength < 0.0f && (has_classes || a.cond.kind == 0) && guided;
-  const int Nf = cfg_two ? 2 * N : N;
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));      // before any allocation: a direct C-ABI caller may be on another device
-  ensure_device(Nf, static_cast<size_t>(Nf) * C * HW);
+  ensure_device(sp.Nf, static_cast<size_t>(sp.Nf) * C * HW);
   const size_t img = static_cast<size_t>(N) * C * HW;
   if (dpm) {
     // D_{-1} always lives in the sampler's own buffer (a fixed pointer: consecutive steps replay the same CUDA graph); run()
     // passes that buffer itself, a caller's previous data prediction is copied in
     ensure_hist(img);
-    if (dpm2 && a.prev_x0_dev != d_hist_)
+    if (sp.order == 2 && a.prev_x0_dev != d_hist_)
       IVID_CHECK_CUDA(cudaMemcpyAsync(d_hist_, a.prev_x0_dev, img * 4, cudaMemcpyDeviceToDevice, stream));
   }
-  const double* acp = dpm ? d_acp_ : nullptr;
-  const int order = dpm2 ? 2 : 1;
-  if (t_dev != nullptr)
-    set_step_dev_kernel<<<1, 128, 0, stream>>>(reinterpret_cast<StepState*>(d_state_), d_t_, Nf, t_dev, t_prev_dev, ddim ? 1 : 0, T_,
-                                               acp, a.t_last, order, a.sde, gated ? 1 : 0, a.guidance_t_lo, a.guidance_t_hi);
-  else
-    set_step_kernel<<<1, 128, 0, stream>>>(reinterpret_cast<StepState*>(d_state_), d_t_, Nf, t_index, t_prev, stream_id, acp,
-                                           a.t_last, order, a.sde, guided ? 1 : 0);
+  StepState* state = reinterpret_cast<StepState*>(d_state_);
+  set_step_kernel<<<1, 128, 0, stream>>>(state, d_t_, sp.Nf, sp.t_index, sp.t_prev, stream_id, t_dev, t_prev_dev,
+                                         kind != kStepDdpm ? 1 : 0, T_, dpm ? d_acp_ : nullptr, a.t_last, sp.order, a.sde,
+                                         sp.gated ? 1 : 0, a.guidance_t_lo, a.guidance_t_hi);
   IVID_CHECK_CUDA(cudaGetLastError());
-  const int64_t* cls = nullptr;
-  if (has_classes) {
-    if (cfg_two) {
-      // [classes, -1 ...] of the batch-2N forward; inside run() it is filled once for the whole reverse process
-      if (!(classes2_ready_ && classes2_src_ == a.classes_dev && classes2_n_ == N)) {
-        fill_classes_kernel<<<1, 256, 0, stream>>>(a.classes_dev, d_classes2_, N);
-        IVID_CHECK_CUDA(cudaGetLastError());
-      }
-      cls = d_classes2_;
-    } else {
-      cls = a.classes_dev;
+  const int64_t* cls = a.classes_dev;
+  if (sp.cfg == 1) {
+    // [classes, -1 ...] of the batch-2N forward
+    if (!classes2_filled) {
+      fill_classes_kernel<<<1, 256, 0, stream>>>(a.classes_dev, d_classes2_, N);
+      IVID_CHECK_CUDA(cudaGetLastError());
     }
+    cls = d_classes2_;
   }
   ivid_cond_t cond = a.cond;
   // in-kernel noise of the conditional inputs: Philox(seed', step) with the step read from the device-resident step state
@@ -311,37 +334,32 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
   std::memset(&p, 0, sizeof(p));         // padding bytes are part of the fused route's graph key
   p.x_t = x_t; p.eps = d_eps_; p.noise = a.step_noise_dev; p.x_prev = x_prev; p.pred_x0 = pred_x0;
   p.table = reinterpret_cast<const StepCoef*>(d_table_);
-  p.t_index = &reinterpret_cast<StepState*>(d_state_)->t_index;
-  p.t_prev = &reinterpret_cast<StepState*>(d_state_)->t_prev;
+  p.t_index = &state->t_index;
+  p.t_prev = &state->t_prev;
   p.N = N; p.C = C; p.HW = HW;
-  // strength <= 0 with classes: (1 + strength) * eps_c without the null-class forward (classifier_free_guidance.py:40-41)
-  p.cfg = cfg_two ? 1 : (scale_only ? 2 : 0);
+  p.cfg = sp.cfg;
   p.strength = a.strength;
   p.clip = a.clip_denoised; p.eta = a.eta; p.seed = a.seed; p.stream = 0;
-  p.stream_dev = &reinterpret_cast<StepState*>(d_state_)->stream;
+  p.stream_dev = &state->stream;
   if (dpm) {
-    p.dpm = &reinterpret_cast<StepState*>(d_state_)->dpm;
+    p.dpm = &state->dpm;
     p.hist = d_hist_;
   }
   // the host route has folded the interval into cfg already; nullptr keeps the step kernels' arithmetic of a run without one
-  if (gated && t_dev != nullptr) p.guided = &reinterpret_cast<StepState*>(d_state_)->guided;
+  if (sp.gated && t_dev != nullptr) p.guided = &state->guided;
   GuideParams& g = p.g;
   g.rgb = a.replace_rgb_dev; g.rgb_mask = a.replace_rgb_mask_dev;
   g.depth = a.replace_depth_dev; g.depth_mask = a.replace_depth_mask_dev; g.convex = a.constrain_depth_dev;
   g.w_rgb = static_cast<float>(a.replace_rgb_weight); g.w_rgb_c = static_cast<float>(1.0 - a.replace_rgb_weight);
   g.w_depth = static_cast<float>(a.replace_depth_weight); g.w_depth_c = static_cast<float>(1.0 - a.replace_depth_weight);
   g.w_convex = static_cast<float>(a.constrain_depth_weight); g.w_convex_c = static_cast<float>(1.0 - a.constrain_depth_weight);
-  IVID_REQUIRE(g.rgb == nullptr || g.rgb_mask != nullptr, "replace_rgb needs its mask");
-  IVID_REQUIRE(g.depth == nullptr || g.depth_mask != nullptr, "replace_depth needs its mask");
-  IVID_REQUIRE(g.convex == nullptr || g.depth != nullptr, "constrain_depth is applied inside replace_depth (ddim.py:90-95)");
-  IVID_REQUIRE(!ddim ? (g.rgb == nullptr && g.depth == nullptr) : true, "replace/constrain guidance is DDIM / DPM-Solver++ only");
 
-  unet.set_cond_stream_dev(cond.kind != 0 && cond.noise_dev == nullptr ? &reinterpret_cast<StepState*>(d_state_)->stream : nullptr);
+  unet.set_cond_stream_dev(cond.kind != 0 && cond.noise_dev == nullptr ? &state->stream : nullptr);
   // Fused route: the output head's last kernel IS the step (head_step_kernel): eps never reaches HBM and the update is the last
-  // node of the forward's CUDA graph.  Not taken when per-step pointers change every step (injected noise / trajectories inside
-  // run(): every step would need its own graph) or when the model has no tap-column head.
+  // node of the forward's CUDA graph.  Not taken when the caller does not allow it (per-step pointers that change every
+  // step inside run(): every step would need its own graph) or when the model has no tap-column head.
   static const bool fuse_ok = getenv("IVID_NO_FUSED_STEP") == nullptr;
-  const bool fuse = fuse_ok && !no_fuse_ && unet.can_fuse_head(W) && C == 4 && W % 4 == 0;
+  const bool fuse = fuse_ok && allow_fuse && unet.can_fuse_head(W) && C == 4 && W % 4 == 0;
   if (fuse) {
     p.eps = nullptr;
     HeadStepParams hp;
@@ -363,73 +381,51 @@ void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, 
       q.Y = Y; q.bias = bias; q.H = Hy; q.W = Wy; q.ldy = ldy;
       const size_t groups = static_cast<size_t>(q.sp.N) * Hy * (Wy / 4);
       const int grid = static_cast<int>(std::min<size_t>((groups + 255) / 256, static_cast<size_t>(sm_count()) * 8));
-      if (kind == kStepDdim) head_step_kernel<kStepDdim><<<std::max(grid, 1), 256, 0, st>>>(q);
-      else if (kind == kStepDpm) head_step_kernel<kStepDpm><<<std::max(grid, 1), 256, 0, st>>>(q);
-      else head_step_kernel<kStepDdpm><<<std::max(grid, 1), 256, 0, st>>>(q);
+      with_step_kind(kind, [&](auto k) { head_step_kernel<decltype(k)::value><<<std::max(grid, 1), 256, 0, st>>>(q); });
       IVID_CHECK_CUDA(cudaGetLastError());
     };
-    unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, Nf, stream, &hook, cache_branch);
+    unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, sp.Nf, stream, &hook, sp.cache_branch);
     unet.set_cond_stream_dev(nullptr);
     return;
   }
-  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, Nf, stream, nullptr, cache_branch);
+  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, sp.Nf, stream, nullptr, sp.cache_branch);
   unet.set_cond_stream_dev(nullptr);
   const size_t total4 = static_cast<size_t>(N) * C * HW / 4;
   const int grid = static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8));
-  if (kind == kStepDdim) step_kernel<kStepDdim><<<std::max(grid, 1), 256, 0, stream>>>(p);
-  else if (kind == kStepDpm) step_kernel<kStepDpm><<<std::max(grid, 1), 256, 0, stream>>>(p);
-  else step_kernel<kStepDdpm><<<std::max(grid, 1), 256, 0, stream>>>(p);
+  with_step_kind(kind, [&](auto k) { step_kernel<decltype(k)::value><<<std::max(grid, 1), 256, 0, stream>>>(p); });
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 
 void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t& a, const float* noise_all,
                   const float* cond_noise_all, float* traj_x0, float* traj_xt, cudaStream_t stream) {
-  const UnetConfig& uc = unet.cfg();
-  const size_t hw = static_cast<size_t>(a.height > 0 ? a.height : uc.image_size) * (a.width > 0 ? a.width : uc.image_size);
-  const size_t img = static_cast<size_t>(N) * uc.out_channels * hw;
+  check_step_args(a, unet, N);
+  const size_t hw = static_cast<size_t>(sample_dim(a.height, unet)) * sample_dim(a.width, unet);
+  const size_t img = static_cast<size_t>(N) * unet.cfg().out_channels * hw;
   const bool ddim = a.kind != kStepDdpm;           // DDIM and DPM-Solver++ share the DDIM time grid
   const bool dpm = a.kind == kStepDpm;
   if (!ddim) steps = T_;
   IVID_REQUIRE(steps >= 1 && steps <= T_, "steps out of range");
-  IVID_REQUIRE(!dpm || (a.order >= 0 && a.order <= 2), "DPM-Solver++ order must be 1 or 2");
-  require_sde(a);
-  require_interval(a, T_);
-  require_cache(a, unet);
   const int jump = T_ / steps;                     // ddim.py:153
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));
   ensure_device(2 * N, 2 * img);
   if (dpm) ensure_hist(img);                       // before the loop: the history must not move between steps
   if (dpm && !a.sde) noise_all = nullptr;          // the ODE solver draws no step noise
+  // the fused head step needs per-step pointers that stay the same from step to step
+  const bool allow_fuse = noise_all == nullptr && cond_noise_all == nullptr && traj_x0 == nullptr && traj_xt == nullptr;
   float* bufs[2] = {x, d_xtmp_};                   // ping-pong; the result is copied back to x if it ends in d_xtmp_
   int cur = 0;
   // per denoising step the host then issues three calls: the step-state kernel, ONE CUDA-graph launch (the whole batch-2N
   // forward, batch-N for a step outside the guidance interval: each batch has its own plan and graphs) and the fused
-  // guidance-mix + x_{t-1} update
-  struct Ready { Sampler* s; ~Ready() { s->classes2_ready_ = false; s->no_fuse_ = false; } } ready_guard{this};
-  no_fuse_ = noise_all != nullptr || cond_noise_all != nullptr || traj_x0 != nullptr || traj_xt != nullptr;
-  if (a.use_cfg && a.classes_dev != nullptr && a.strength > 0.0f) {
-    fill_classes_kernel<<<1, 256, 0, stream>>>(a.classes_dev, d_classes2_, N);
-    IVID_CHECK_CUDA(cudaGetLastError());
-    classes2_ready_ = true; classes2_src_ = a.classes_dev; classes2_n_ = N;
-  }
+  // guidance-mix + x_{t-1} update.  The first batch-2N step fills [classes, -1 ...] once for the whole reverse process.
   // feature reuse: a full forward at step 0, at a switch between the batch-2N and batch-N plans, and every cache_interval
   // steps after the last full one; reuse forwards in between
-  const bool gated = a.guidance_interval != 0 && a.use_cfg && a.classes_dev != nullptr;
   int last_full = 0;
-  bool last_two = false;
+  bool last_two = false, classes2_filled = false;
   for (int i = 0; i < steps; ++i) {
     int t, t_prev;
     if (ddim) { t = jump * (steps - i); t_prev = jump * (steps - 1 - i); }   // ddim.py:154
     else { t = T_ - 1 - i; t_prev = 0; }                                      // ddpm.py:177
     ivid_step_args_t ai = a;
-    const int t_model = ddim ? t - 1 : t;
-    // the plan step() runs this step's forward on: batch 2N exactly when it is a guided classifier-free step
-    const bool two = a.use_cfg && a.classes_dev != nullptr && a.strength > 0.0f &&
-                     (!gated || (t_model >= a.guidance_t_lo && t_model <= a.guidance_t_hi));
-    const bool full = a.cache_interval <= 1 || i == 0 || two != last_two || i - last_full >= a.cache_interval;
-    if (full) last_full = i;
-    last_two = two;
-    ai.cache_reuse = full ? 0 : 1;
     ai.step_noise_dev = noise_all ? noise_all + static_cast<size_t>(i) * img : nullptr;
     if (dpm) {
       // multistep history: from the second step on, D_{-1} is the previous step's D0, already in the sampler's buffer
@@ -438,11 +434,18 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
     }
     if (cond_noise_all && ai.cond.kind == 1)
       ai.cond.noise_dev = cond_noise_all + static_cast<size_t>(i) * N * 4 * hw;
+    const bool two = plan_step(ai, N, t, t_prev, false).Nf == 2 * N;
+    const bool full = a.cache_interval <= 1 || i == 0 || two != last_two || i - last_full >= a.cache_interval;
+    if (full) last_full = i;
+    last_two = two;
+    ai.cache_reuse = full ? 0 : 1;
     float* dst = traj_xt ? traj_xt + static_cast<size_t>(i) * img : bufs[cur ^ 1];
     float* x0 = traj_x0 ? traj_x0 + static_cast<size_t>(i) * img : nullptr;
     const float* src = (traj_xt && i > 0) ? traj_xt + static_cast<size_t>(i - 1) * img : bufs[cur];
     if (traj_xt && i == 0) src = x;
-    step(unet, src, dst, x0, N, t, t_prev, ai, i, stream);
+    step_impl(unet, src, dst, x0, N, plan_step(ai, N, t, t_prev, false), ai, i, stream, nullptr, nullptr, allow_fuse,
+              classes2_filled);
+    classes2_filled = classes2_filled || two;
     if (!traj_xt) cur ^= 1;
   }
   const float* last = traj_xt ? traj_xt + static_cast<size_t>(steps - 1) * img : bufs[cur];

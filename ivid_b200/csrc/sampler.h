@@ -6,6 +6,8 @@
 
 namespace ivid {
 
+struct StepPlan;   // what one step runs (sampler.cu)
+
 class Sampler {
  public:
   Sampler(const double* betas, int T);
@@ -23,6 +25,12 @@ class Sampler {
            const float* cond_noise_all, float* traj_x0, float* traj_xt, cudaStream_t stream);
 
  private:
+  void check_step_args(const ivid_step_args_t& a, const Unet& unet, int N) const;
+  // one step of checked arguments.  allow_fuse: the update may run as the output head's last kernel; classes2_filled:
+  // d_classes2_ already holds [classes, -1 ...] of a.classes_dev and N
+  void step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, const StepPlan& sp,
+                 const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
+                 const int64_t* t_prev_dev, bool allow_fuse, bool classes2_filled);
   void ensure_device(int N2, size_t eps_elems);
   void ensure_hist(size_t elems);
   int T_;
@@ -36,10 +44,6 @@ class Sampler {
   int64_t* d_classes2_ = nullptr;
   float* d_eps_ = nullptr;
   float* d_xtmp_ = nullptr;
-  bool no_fuse_ = false;                   // inside run() with per-step noise / trajectory pointers: keep the separate step kernel
-  bool classes2_ready_ = false;            // d_classes2_ already holds [classes, -1 ...] for (classes2_src_, classes2_n_)
-  const int64_t* classes2_src_ = nullptr;
-  int classes2_n_ = 0;
   int cap_n_ = 0;
   size_t cap_eps_ = 0;
 };

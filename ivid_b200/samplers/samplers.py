@@ -87,6 +87,12 @@ class _NativeSampler:
         return out
 
     # ------------------------------------------------------------------------------------------------------------
+    def _guidance(self, kwargs):
+        """(uses_cfg, strength): whether the framework mixes in a null-class forward, and model_inference's strength
+        (default 3.0); 0.0 for a framework without classifier-free guidance."""
+        uses_cfg = isinstance(self.framework, (ClassifierFreeGuidance, InpaintCFG, SuperResCFG))
+        return uses_cfg, float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
+
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
                    order=0, prev=None, sde=False, interval=None, cache=None):
         fw = self.framework
@@ -101,9 +107,8 @@ class _NativeSampler:
             return t.data_ptr()
 
         a.kind = self.KIND
-        uses_cfg = isinstance(fw, (ClassifierFreeGuidance, InpaintCFG, SuperResCFG))
+        uses_cfg, a.strength = self._guidance(kwargs)
         a.use_cfg = 1 if uses_cfg else 0
-        a.strength = float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
         a.clip_denoised = 1 if clip_denoised else 0
         a.eta = float(eta)
         if classes is not None:
@@ -159,8 +164,10 @@ class _NativeSampler:
     def _num_res_blocks(self):
         return _unwrap(self.framework.backbone).num_res_blocks
 
-    def _native_step(self, x_t, t_int, t_prev_int, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
+    def _native_step(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
                      sde=False, interval=None, cache=None):
+        """One step.  `t` / `t_prev` are host ints (ivid_sampler_step) or the [N] tensors sample_once receives
+        (ivid_sampler_step_dev: the step is read on the device, no host sync; t_prev None for DDPM)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
@@ -168,31 +175,37 @@ class _NativeSampler:
                                   hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
+        L = _lib.lib()
+        head = (self._handle, net._handle, _lib.ptr(x_t), _lib.ptr(x_prev), _lib.ptr(x0), x_t.shape[0])
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().ivid_sampler_step(self._handle, net._handle, _lib.ptr(x_t), _lib.ptr(x_prev), _lib.ptr(x0),
-                                                    x_t.shape[0], int(t_int), int(t_prev_int), ctypes.byref(a),
-                                                    _lib.cur_stream(dev)))
+            if torch.is_tensor(t):
+                td = t.to(device=dev, dtype=torch.int64).contiguous()
+                tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
+                rc = L.ivid_sampler_step_dev(*head, _lib.ptr(td), _lib.ptr(tp), ctypes.byref(a), _lib.cur_stream(dev))
+            else:
+                rc = L.ivid_sampler_step(*head, int(t), int(t_prev), ctypes.byref(a), _lib.cur_stream(dev))
+            _lib.check(rc)
         del keep
         return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
 
-    def _native_step_dev(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                         sde=False, interval=None, cache=None):
-        """Same step with the timestep taken on the device from the [N] tensors the caller passed (no host sync)."""
-        net = self._net()
-        dev = x_t.device
-        x_t = _f32(x_t, dev)
-        a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache)
-        td = t.to(device=dev, dtype=torch.int64).contiguous()
-        tp = t_prev.to(device=dev, dtype=torch.int64).contiguous() if t_prev is not None else None
-        x_prev = torch.empty_like(x_t)
-        x0 = torch.empty_like(x_t)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().ivid_sampler_step_dev(self._handle, net._handle, _lib.ptr(x_t), _lib.ptr(x_prev), _lib.ptr(x0),
-                                                        x_t.shape[0], _lib.ptr(td), _lib.ptr(tp), ctypes.byref(a),
-                                                        _lib.cur_stream(dev)))
-        del keep
-        return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
+    def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, interval, reuse_features, cache_branch,
+                     order=0, prev=None, sde=False):
+        """The body of every sample_once: the host checks before any device work or torch draw, the step noise (drawn as
+        the reference draws it, or the injected `noise` and kwargs' `cond_noise`), then the step with t / t_prev read on
+        the device (all samples of a batch share the step, ddpm.py:177-179, ddim.py:154-158: no host sync)."""
+        B = x_t.shape[0]
+        assert t.shape == (B,), "t must be a 1D tensor of shape (B,)"
+        assert self.KIND == 0 or t_prev.shape == (B,), "t_prev must be a 1D tensor of shape (B,)"
+        _check_interval(interval, len(self.framework.betas))
+        _check_cache(None, cache_branch, self._num_res_blocks())
+        if noise is None:
+            noise, cond_noise = self._draw_step_noise(x_t, kwargs)
+        else:
+            cond_noise = kwargs.pop("cond_noise", None)
+        # the DPM-Solver++ ODE update reads no step noise
+        return self._native_step(x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise if self.KIND != 2 or sde else None,
+                                 cond_noise, order=order, prev=prev, sde=sde, interval=interval,
+                                 cache=(0, cache_branch, bool(reuse_features)))
 
     def _draw_step_noise(self, x_t, kwargs):
         """torch draws in the reference's order: InpaintCFG rgb, depth (inside model_inference), then randn_like(x_t)."""
@@ -208,11 +221,10 @@ class _NativeSampler:
         """Whether each step of a run reuses the cached features, by ivid_sampler_run's rule: a full forward at the first
         step, where the forward switches between the guided batch-2N and the unguided batch-N plan, and cache_interval steps
         after the last full one."""
-        uses_cfg = isinstance(self.framework, (ClassifierFreeGuidance, InpaintCFG, SuperResCFG))
-        strength = float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
+        _, strength = self._guidance(kwargs)
         reuse, last_full, last_two = [], 0, False
         for i, tm in enumerate(model_times):
-            two = uses_cfg and classes is not None and strength > 0 and (interval is None or interval[0] <= tm <= interval[1])
+            two = classes is not None and strength > 0 and (interval is None or interval[0] <= tm <= interval[1])
             full = cache_interval <= 1 or i == 0 or two != last_two or i - last_full >= cache_interval
             if full:
                 last_full = i
@@ -248,22 +260,13 @@ class _NativeSampler:
             reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
                                          cache_interval)
             for i, (t, t_prev) in enumerate(sched):
-                cache = (0, cache_branch, reuse[i])
-                # the reference draws the model-input noise first (inside model_inference), then randn_like(x_t)
-                cond_noise = None
-                if isinstance(self.framework, InpaintCFG):
-                    y = kwargs["y"]
-                    cond_noise = torch.cat([torch.randn_like(y[:, :3]), torch.randn_like(y[:, 3:])], dim=1)
-                z = torch.randn_like(img)
-                if self.KIND == 2:
-                    # the SDE update uses z; the ODE update draws it only to consume the torch RNG as DdimSampler does
-                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if sde else None, cond_noise,
-                                            order=order, prev=prev if order != 1 else None, sde=sde, interval=interval,
-                                            cache=cache)
+                z, cond_noise = self._draw_step_noise(img, kwargs)
+                # the DPM-Solver++ ODE update draws z only to consume the torch RNG as DdimSampler does
+                out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if self.KIND != 2 or sde else None,
+                                        cond_noise, order=order, prev=prev, sde=sde, interval=interval,
+                                        cache=(0, cache_branch, reuse[i]))
+                if self.KIND == 2 and order != 1:
                     prev = (t, out.pred_x_0)
-                else:
-                    out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z, cond_noise, interval=interval,
-                                            cache=cache)
                 img = out.pred_x_prev
                 if return_trajectory:
                     ret.pred_x_t.append(out.pred_x_prev)
@@ -311,18 +314,8 @@ class DdpmSampler(_NativeSampler):
         `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`).
         `reuse_features=True` (extension): the step's forward reuses the deep features of the last full forward of the same
         batch and size at branch `cache_branch` (see `sample`); RuntimeError if no full forward has run on it."""
-        B = x_t.shape[0]
-        assert t.shape == (B,), "t must be a 1D tensor of shape (B,)"
-        _check_interval(guidance_interval, len(self.framework.betas))
-        _check_cache(None, cache_branch, self._num_res_blocks())
-        # all samples of a batch share the timestep (both reference samplers are driven that way: ddpm.py:177-179);
-        # element 0 is read on the device, so this call does not synchronise with the host
-        if noise is None:
-            noise, cond_noise = self._draw_step_noise(x_t, kwargs)
-        else:
-            cond_noise = kwargs.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, cond_noise,
-                                     interval=guidance_interval, cache=(0, cache_branch, bool(reuse_features)))
+        return self._sample_once(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, guidance_interval, reuse_features,
+                                 cache_branch)
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
@@ -357,18 +350,9 @@ class DdimSampler(_NativeSampler):
         """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step).
         `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi].
         `reuse_features` / `cache_branch` as in DdpmSampler.sample_once."""
-        B = x_t.shape[0]
-        assert t.shape == (B,) and t_prev.shape == (B,)
-        _check_interval(guidance_interval, len(self.framework.betas))
-        _check_cache(None, cache_branch, self._num_res_blocks())
-        # element 0 of t / t_prev is read on the device (all samples share the step, ddim.py:154-158): no host sync
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
-        if noise is None:
-            noise, cond_noise = self._draw_step_noise(x_t, kw)
-        else:
-            cond_noise = kw.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, cond_noise, interval=guidance_interval,
-                                     cache=(0, cache_branch, bool(reuse_features)))
+        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, guidance_interval, reuse_features,
+                                 cache_branch)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
@@ -403,18 +387,9 @@ class DpmSolverSampler(_NativeSampler):
         the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
         randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval`, `reuse_features`
         and `cache_branch` as for DdimSampler.sample_once."""
-        B = x_t.shape[0]
-        assert t.shape == (B,) and t_prev.shape == (B,)
-        _check_interval(guidance_interval, len(self.framework.betas))
-        _check_cache(None, cache_branch, self._num_res_blocks())
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
-        if noise is None:
-            noise, cond_noise = self._draw_step_noise(x_t, kw)
-        else:
-            cond_noise = kw.pop("cond_noise", None)
-        return self._native_step_dev(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise if sde else None, cond_noise,
-                                     order=2 if prev is not None else 1, prev=prev, sde=sde, interval=guidance_interval,
-                                     cache=(0, cache_branch, bool(reuse_features)))
+        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
+                                 cache_branch, order=2 if prev is not None else 1, prev=prev, sde=sde)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
