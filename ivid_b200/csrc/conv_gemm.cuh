@@ -26,6 +26,16 @@
 // The epilogue works on the accumulator fragments in place: bias, residual (optionally through a nearest-2x upsample),
 // fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.
 //
+// Slab mode (SLAB, chosen by conv_launch_create for tiles of one sample and TW >= 8): the three taps of a 3x3 segment that
+// differ only in dy read the same pixels shifted by one image row.  So the producer loads one (TH + 2)-row activation slab
+// per (chunk, dx), box (64 ch, TW, TH + 2, 1) at row h0 - 1, and the k-blocks of dy = -1, 0, 1 start their A descriptor 0,
+// TW*128 and 2*TW*128 bytes into it.  TW*128 is a whole number of 1024-byte swizzle atoms when TW >= 8, so a shifted start
+// sees exactly the layout of a box loaded at that row.  K runs chunk slow, then dx, then dy fastest; the packed weight
+// columns are the same as per tap.  The slabs have a ring of their own (2 slots, released after the third dy's group has
+// retired); the weight boxes keep a per-k-block ring, 4 deep.  A 1x1 segment of a slab launch puts its one box per chunk in
+// a slab slot.  Per three k-blocks a CTA takes in TW*(TH+2)*128 + 3*BN*128 bytes instead of 3*(16 KB + BN*128).  The
+// epilogue's statistics scratch lies over the ring, which is idle once both warpgroups' last groups have retired.
+//
 // fp8 operand mode (A8): segment 0 is e4m3.  Its 128-byte box row is 128 channels, so an e4m3 k-block has exactly the
 // shared-memory layout, TMA bytes and wgmma descriptors of an fp16 one; only the instruction differs (k32 e4m3 for k16
 // f16) and a chunk covers 128 channels.  Its weights come from a second map (b8) over e4m3 columns pre-scaled by 2^e; the
@@ -69,17 +79,24 @@ struct ConvMaps8 : ConvMaps {
   CUtensorMap b8;
 };
 
-template <int BN>
+template <int BN, bool SLAB = false>
 struct ConvGemmCfg {
   static constexpr int BM = 128;
   static constexpr int BK = 64;
   static constexpr int A_BYTES = BM * BK * 2;                  // 16 KB
   static constexpr int B_BYTES = ((BN * BK * 2 + 1023) / 1024) * 1024;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = BN == 128 ? 3 : 4;
+  static constexpr int STAGES = BN == 128 && !SLAB ? 3 : 4;   // k-blocks in flight (SLAB: weight boxes)
+  // SLAB: the largest slab, TW * (TH + 2) pixels with TW * TH = 128 and TW >= 8 (16 x 10), in each of 2 slots.  Two CTAs
+  // of 2 slabs + 4 weight boxes (BN 128: 104 KB) fit one SM only with the statistics scratch over the ring; a third slab
+  // or a third weight box in its place measured slower.
+  static constexpr int SLAB_BYTES = 16 * 10 * 128;
+  static constexpr int SLAB_STAGES = 2;
+  static constexpr int RING_BYTES = SLAB ? SLAB_STAGES * SLAB_BYTES + STAGES * B_BYTES : STAGES * STAGE_BYTES;
   static constexpr int BAR_BYTES = 128;
   static constexpr int STAT_BYTES = 8 * 2 * BN * 4;            // [8 warps][sum|sumsq][BN] fp32
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + STAT_BYTES + 1024;   // +1024 alignment slack
+  static constexpr bool STATS_ON_RING = SLAB;                  // the epilogue's statistics scratch over the idle ring
+  static constexpr int SMEM_BYTES = RING_BYTES + BAR_BYTES + (STATS_ON_RING ? 0 : STAT_BYTES) + 1024;   // +1024 alignment slack
   static constexpr int CONSUMER_THREADS = 256;                 // two warpgroups: MMA and epilogue
   static constexpr int THREADS = CONSUMER_THREADS + 32;        // + one producer warp: TMA loads
 };
@@ -91,17 +108,22 @@ struct ConvKCursor {
 
 // p is read in place (__grid_constant__): the K cursor indexes seg_chunks / seg_taps at run time, and without it the compiler
 // may copy the whole struct to a local-memory stack frame to do so.
-template <int BN, bool A8 = false>
+template <int BN, bool A8 = false, bool SLAB = false>
 __global__ void __launch_bounds__(ConvGemmCfg<BN>::THREADS, 2)
 conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvMaps> maps, const __grid_constant__ ConvGemmParams p) {
-  using Cfg = ConvGemmCfg<BN>;
+  using Cfg = ConvGemmCfg<BN, SLAB>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int SLAB_STAGES = Cfg::SLAB_STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  float* stat_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES);
+  uint64_t* slab_full = empty_bar + STAGES;      // SLAB only
+  uint64_t* slab_empty = slab_full + SLAB_STAGES;
+  float* stat_smem = reinterpret_cast<float*>(Cfg::STATS_ON_RING ? smem : smem + Cfg::RING_BYTES + Cfg::BAR_BYTES);
+  uint8_t* const slab_ring = smem;               // SLAB: [SLAB_STAGES][SLAB_BYTES], then [STAGES][B_BYTES] weight boxes
+  uint8_t* const w_ring = smem + SLAB_STAGES * Cfg::SLAB_BYTES;
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
@@ -111,6 +133,12 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8u);              // one arrive per consumer warp
+    }
+    if constexpr (SLAB) {
+      for (int s = 0; s < SLAB_STAGES; ++s) {
+        mbar_init(&slab_full[s], 1);
+        mbar_init(&slab_empty[s], 8u);
+      }
     }
     fence_barrier_init();
   }
@@ -136,37 +164,74 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
       tma_prefetch_desc(&maps.a[0]);
       tma_prefetch_desc(&maps.b);
       if constexpr (A8) tma_prefetch_desc(&maps.b8);
-      ConvKCursor c;                             // units are issued strictly in order: segment, tap slow, chunk fast
-      while (p.seg_chunks[c.seg] == 0) ++c.seg;
+      if constexpr (SLAB) {
+        // per segment: chunk slow, dx, dy fast (3x3: one slab per (chunk, dx)); 1x1: one box per chunk
+        const uint32_t slab_bytes = static_cast<uint32_t>(p.TW * (p.TH + 2)) * 128u;
+        uint32_t u = 0, a = 0;                     // k-block, activation load
+        int base = 0;
 #pragma unroll 1
-      for (int u = 0; u < nunits; ++u) {
-        const uint32_t g = static_cast<uint32_t>(u);
-        const int s = static_cast<int>(g % STAGES);
-        if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
-        const int taps = p.seg_taps[c.seg], chunks = p.seg_chunks[c.seg];
-        uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
-        uint8_t* sb = sa + Cfg::A_BYTES;
-        const int dy = (taps == 9) ? (c.t / 3 - 1) : 0;
-        const int dx = (taps == 9) ? (c.t % 3 - 1) : 0;
-        mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
-        bool e4m3 = false;
-        if constexpr (A8) {
-          if (c.seg == 0) {                      // e4m3: 128 channels per box row; columns of b8 (c.base stays 0)
-            tma_load_4d(&maps.a[0], &full_bar[s], sa, c.ch * 128, w0 + dx, h0 + dy, n0);
-            tma_load_2d(&maps.b8, &full_bar[s], sb, (c.t * chunks + c.ch) * 128, colbase);
-            e4m3 = true;
+        for (int sg = 0; sg < 3; ++sg) {
+          const int chunks = p.seg_chunks[sg];
+          const int nx = p.seg_taps[sg] == 9 ? 3 : 1;
+          const bool e4m3 = A8 && sg == 0;         // 128 channels per box row; columns of b8 (base stays 0)
+#pragma unroll 1
+          for (int ch = 0; ch < chunks; ++ch) {
+#pragma unroll 1
+            for (int xi = 0; xi < nx; ++xi, ++a) {
+              const int sl = static_cast<int>(a % SLAB_STAGES);
+              if (a >= SLAB_STAGES) mbar_wait(&slab_empty[sl], ((a / SLAB_STAGES) - 1) & 1);
+              mbar_arrive_expect_tx(&slab_full[sl], nx == 3 ? slab_bytes : static_cast<uint32_t>(Cfg::A_BYTES));
+              tma_load_4d(&maps.a[sg], &slab_full[sl], slab_ring + sl * Cfg::SLAB_BYTES, ch * (e4m3 ? 128 : 64),
+                          w0 + (nx == 3 ? xi - 1 : 0), h0 - (nx == 3 ? 1 : 0), n0);
+#pragma unroll 1
+              for (int yi = 0; yi < nx; ++yi, ++u) {
+                const int s = static_cast<int>(u % STAGES);
+                if (u >= STAGES) mbar_wait(&empty_bar[s], ((u / STAGES) - 1) & 1);
+                mbar_arrive_expect_tx(&full_bar[s], BN * Cfg::BK * 2);
+                const int t = nx == 3 ? 3 * yi + xi : 0;
+                uint8_t* sb = w_ring + s * Cfg::B_BYTES;
+                if constexpr (A8) {
+                  if (e4m3) { tma_load_2d(&maps.b8, &full_bar[s], sb, (t * chunks + ch) * 128, colbase); continue; }
+                }
+                tma_load_2d(&maps.b, &full_bar[s], sb, base + (t * chunks + ch) * 64, colbase);
+              }
+            }
           }
+          if (!e4m3) base += p.seg_taps[sg] * chunks * 64;
         }
-        if (!e4m3) {
-          const int kcol = c.base + (c.t * chunks + c.ch) * 64;
-          tma_load_4d(&maps.a[c.seg], &full_bar[s], sa, c.ch * 64, w0 + dx, h0 + dy, n0);
-          tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
+      } else {
+        ConvKCursor c;                            // units are issued strictly in order: segment, tap slow, chunk fast
+        while (p.seg_chunks[c.seg] == 0) ++c.seg;
+#pragma unroll 1
+        for (int u = 0; u < nunits; ++u) {
+          const uint32_t g = static_cast<uint32_t>(u);
+          const int s = static_cast<int>(g % STAGES);
+          if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
+          const int taps = p.seg_taps[c.seg], chunks = p.seg_chunks[c.seg];
+          uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
+          uint8_t* sb = sa + Cfg::A_BYTES;
+          const int dy = (taps == 9) ? (c.t / 3 - 1) : 0;
+          const int dx = (taps == 9) ? (c.t % 3 - 1) : 0;
+          mbar_arrive_expect_tx(&full_bar[s], Cfg::A_BYTES + BN * Cfg::BK * 2);
+          bool e4m3 = false;
+          if constexpr (A8) {
+            if (c.seg == 0) {                      // e4m3: 128 channels per box row; columns of b8 (c.base stays 0)
+              tma_load_4d(&maps.a[0], &full_bar[s], sa, c.ch * 128, w0 + dx, h0 + dy, n0);
+              tma_load_2d(&maps.b8, &full_bar[s], sb, (c.t * chunks + c.ch) * 128, colbase);
+              e4m3 = true;
+            }
+          }
+          if (!e4m3) {
+            const int kcol = c.base + (c.t * chunks + c.ch) * 64;
+            tma_load_4d(&maps.a[c.seg], &full_bar[s], sa, c.ch * 64, w0 + dx, h0 + dy, n0);
+            tma_load_2d(&maps.b, &full_bar[s], sb, kcol, colbase);
+          }
+          if (++c.ch == chunks) {
+            c.ch = 0;
+            if (++c.t == taps) { c.t = 0; if (!A8 || c.seg != 0) c.base += taps * chunks * 64; ++c.seg; }
+          }
+          while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
         }
-        if (++c.ch == chunks) {
-          c.ch = 0;
-          if (++c.t == taps) { c.t = 0; if (!A8 || c.seg != 0) c.base += taps * chunks * 64; ++c.seg; }
-        }
-        while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
       }
     }
     return;                                      // the consumers' barriers below count 256 threads
@@ -177,31 +242,76 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
+  if constexpr (SLAB) {
+    // the producer's order; a slab is released once the group of its last k-block has retired, like a weight slot
+    const uint32_t row_bytes = static_cast<uint32_t>(p.TW) * 128u;    // one image row of the tile: dy + 1 rows into the slab
+    uint32_t u = 0, a = 0;
 #pragma unroll 1
-  for (int u = 0; u < nunits; ++u) {
-    const uint32_t g = static_cast<uint32_t>(u);
-    const int s = static_cast<int>(g % STAGES);
-    mbar_wait(&full_bar[s], (g / STAGES) & 1);
-    const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
-    const uint32_t sb = sa + Cfg::A_BYTES;
-    wgmma_fence();
-    const uint64_t da = make_smem_desc_sw128(sa + wg * 64 * 128, 1024, 16);
-    const uint64_t db = make_smem_desc_sw128(sb, 1024, 16);
-    if (A8 && u < nunits8) {                     // warp-uniform
+    for (int sg = 0; sg < 3; ++sg) {
+      const int nx = p.seg_taps[sg] == 9 ? 3 : 1;
+      const int loads = p.seg_chunks[sg] * nx;
+#pragma unroll 1
+      for (int l = 0; l < loads; ++l, ++a) {
+        const uint32_t sl = a % SLAB_STAGES;
+        mbar_wait(&slab_full[sl], (a / SLAB_STAGES) & 1);
+        const uint32_t sa = smem_u32(slab_ring + sl * Cfg::SLAB_BYTES) + wg * 64 * 128;
+#pragma unroll 1
+        for (int yi = 0; yi < nx; ++yi, ++u) {
+          const uint32_t s = u % STAGES;
+          mbar_wait(&full_bar[s], (u / STAGES) & 1);
+          wgmma_fence();
+          const uint64_t da = make_smem_desc_sw128(sa + yi * row_bytes, 1024, 16);
+          const uint64_t db = make_smem_desc_sw128(smem_u32(w_ring + s * Cfg::B_BYTES), 1024, 16);
+          if (A8 && sg == 0) {                   // warp-uniform
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
-    } else {
+            for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+          } else {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+            for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          // group u - 1 has retired: its weight slot, and at the first k-block of a load the previous load's slab, go back
+          wgmma_wait<1>();
+          if (u > 0 && lane == 0) {
+            mbar_arrive(&empty_bar[(u - 1) % STAGES]);
+            if (yi == 0) mbar_arrive(&slab_empty[(a - 1) % SLAB_STAGES]);
+          }
+        }
+      }
     }
-    wgmma_commit();
-    // group u stays in flight; group u - 1 has retired, so its slot goes back to the producer
-    wgmma_wait<1>();
-    if (u > 0 && lane == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (lane == 0) {
+      mbar_arrive(&empty_bar[(u - 1) % STAGES]);
+      mbar_arrive(&slab_empty[(a - 1) % SLAB_STAGES]);
+    }
+  } else {
+#pragma unroll 1
+    for (int u = 0; u < nunits; ++u) {
+      const uint32_t g = static_cast<uint32_t>(u);
+      const int s = static_cast<int>(g % STAGES);
+      mbar_wait(&full_bar[s], (g / STAGES) & 1);
+      const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
+      const uint32_t sb = sa + Cfg::A_BYTES;
+      wgmma_fence();
+      const uint64_t da = make_smem_desc_sw128(sa + wg * 64 * 128, 1024, 16);
+      const uint64_t db = make_smem_desc_sw128(sb, 1024, 16);
+      if (A8 && u < nunits8) {                     // warp-uniform
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss_e4m3<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      // group u stays in flight; group u - 1 has retired, so its slot goes back to the producer
+      wgmma_wait<1>();
+      if (u > 0 && lane == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[static_cast<uint32_t>(nunits - 1) % STAGES]);
   }
-  wgmma_wait<0>();
-  reg_fence(acc);
-  if (lane == 0) mbar_arrive(&empty_bar[static_cast<uint32_t>(nunits - 1) % STAGES]);
 
   // ===================================== epilogue =====================================
   const int wr = warp & 3;
@@ -219,6 +329,10 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
     rpix[i] = p.res_up ? (static_cast<uint32_t>(n) * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (x >> 1) : pix[i];
   }
   const bool do_stats = p.stats != nullptr;
+  // scratch over the ring: both warpgroups' wgmma have retired (every TMA write landed before its group was issued)
+  if constexpr (Cfg::STATS_ON_RING) {
+    if (do_stats) asm volatile("bar.sync 1, %0;\n" ::"n"(Cfg::CONSUMER_THREADS) : "memory");
+  }
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int c = colbase + 8 * j + 2 * quad;    // this thread's column pair

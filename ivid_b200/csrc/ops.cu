@@ -21,6 +21,7 @@ struct ConvLaunch {
   ConvGemmParams p;
   int BN;
   bool a8;
+  bool slab;                   // the 3x3 segments load one (TH + 2)-row slab per (chunk, dx): conv_gemm_kernel<BN, A8, true>
   int grid;
 };
 
@@ -129,6 +130,12 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   p.tiles_w = d.W / p.TW;
   p.tiles_h = d.H / p.TH;
   p.tiles_n = (d.N + p.TN - 1) / p.TN;
+  // The slab of a 3x3 segment spans TH + 2 rows of one sample, and its one-row shift of TW * 128 bytes must be a whole
+  // number of 1024-byte swizzle atoms: tiles of one sample (TN == 1, so TW * TH == 128 and TH + 2 <= 18 rows, within the
+  // 256-row TMA box limit) with TW >= 8: 16 x 8 tiles (W % 16 == 0, H % 8 == 0) and 8 x 16 tiles (W % 8 == 0, H % 16 == 0).
+  const bool any3x3 = d.taps0 == 9 || (d.C1 > 0 && d.taps1 == 9) || (d.C2 > 0 && d.taps2 == 9);
+  l->slab = any3x3 && p.TN == 1 && p.TW >= 8;
+  IVID_REQUIRE(!l->slab || p.TW * (p.TH + 2) * 128 <= (ConvGemmCfg<128, true>::SLAB_BYTES), "internal: conv slab larger than its slot");
   l->BN = conv_pick_bn(d.cout_pad);
   p.n_blocks = d.cout_pad / l->BN;
   p.seg_chunks[0] = a8 ? conv_pad_k8(d.C0) / 128 : conv_pad_k(d.C0) / 64; p.seg_taps[0] = d.taps0;
@@ -156,10 +163,12 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   // (fp8 mode: segment 0's columns live in weight8, so the fp16 matrix holds the skip segments only)
   const int Ktot = (a8 ? 0 : conv_seg_cols(d.taps0, d.C0)) + conv_seg_cols(d.taps1, d.C1) + conv_seg_cols(d.taps2, d.C2);
   ConvMaps8& M = l->maps;
-  M.a[0] = a8 ? make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN, CU_TENSOR_MAP_DATA_TYPE_UINT8)
-              : make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, p.TH, p.TN);
-  M.a[1] = d.C1 > 0 ? make_act_map(d.act1, d.N, d.H, d.W, d.C1, p.TW, p.TH, p.TN) : M.a[0];
-  M.a[2] = d.C2 > 0 ? make_act_map(d.act2, d.N, d.H, d.W, d.C2, p.TW, p.TH, p.TN) : M.a[0];
+  // a slab segment's box is TH + 2 rows, loaded from row h0 - 1 (TMA zero-fills the halo rows outside the image)
+  auto rows = [&](int taps) { return l->slab && taps == 9 ? p.TH + 2 : p.TH; };
+  M.a[0] = a8 ? make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, rows(d.taps0), p.TN, CU_TENSOR_MAP_DATA_TYPE_UINT8)
+              : make_act_map(d.act0, d.N, d.H, d.W, d.C0, p.TW, rows(d.taps0), p.TN);
+  M.a[1] = d.C1 > 0 ? make_act_map(d.act1, d.N, d.H, d.W, d.C1, p.TW, rows(d.taps1), p.TN) : M.a[0];
+  M.a[2] = d.C2 > 0 ? make_act_map(d.act2, d.N, d.H, d.W, d.C2, p.TW, rows(d.taps2), p.TN) : M.a[0];
   if (a8) {
     M.b8 = make_weight_map(d.weight8, d.cout_pad, d.taps0 * conv_pad_k8(d.C0), l->BN, CU_TENSOR_MAP_DATA_TYPE_UINT8);
     M.b = Ktot > 0 ? make_weight_map(d.weight, d.cout_pad, Ktot, l->BN) : M.b8;    // no skip segment: b is never read
@@ -173,16 +182,24 @@ void conv_launch_destroy(ConvLaunch* l) { delete l; }
 int conv_launch_bn(const ConvLaunch* l) { return l->BN; }
 bool conv_launch_a8(const ConvLaunch* l) { return l->a8; }
 
-template <int BN, bool A8>
+template <int BN, bool A8, bool SLAB>
 static void run_conv(const ConvLaunch* l, cudaStream_t s) {
-  using Cfg = ConvGemmCfg<BN>;
+  using Cfg = ConvGemmCfg<BN, SLAB>;
   static std::once_flag once;
   std::call_once(once, [] {
-    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, A8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    IVID_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, A8, SLAB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   });
-  if constexpr (A8) conv_gemm_kernel<BN, true><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
-  else conv_gemm_kernel<BN, false><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(static_cast<const ConvMaps&>(l->maps), l->p);
+  if constexpr (A8) conv_gemm_kernel<BN, true, SLAB><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(l->maps, l->p);
+  else conv_gemm_kernel<BN, false, SLAB><<<l->grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(static_cast<const ConvMaps&>(l->maps), l->p);
   IVID_CHECK_CUDA(cudaGetLastError());
+}
+template <bool A8, bool SLAB>
+static void run_conv_bn(const ConvLaunch* l, cudaStream_t s) {
+  switch (l->BN) {
+    case 128: run_conv<128, A8, SLAB>(l, s); break;
+    case 64: run_conv<64, A8, SLAB>(l, s); break;
+    default: run_conv<16, A8, SLAB>(l, s); break;
+  }
 }
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
   ConvLaunch tmp = *l;
@@ -191,17 +208,11 @@ void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
 }
 void conv_launch_run(const ConvLaunch* l, cudaStream_t s) {
   if (l->a8) {
-    switch (l->BN) {
-      case 128: run_conv<128, true>(l, s); break;
-      case 64: run_conv<64, true>(l, s); break;
-      default: run_conv<16, true>(l, s); break;
-    }
-    return;
-  }
-  switch (l->BN) {
-    case 128: run_conv<128, false>(l, s); break;
-    case 64: run_conv<64, false>(l, s); break;
-    default: run_conv<16, false>(l, s); break;
+    if (l->slab) run_conv_bn<true, true>(l, s);
+    else run_conv_bn<true, false>(l, s);
+  } else {
+    if (l->slab) run_conv_bn<false, true>(l, s);
+    else run_conv_bn<false, false>(l, s);
   }
 }
 

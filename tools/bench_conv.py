@@ -6,9 +6,12 @@
 kernel_ms: device time of the conv kernel per call (torch.profiler, CUDA activity, only the kernels whose name contains
 `conv_gemm`), warm, in a run of its own.  The C entry point (ivid_op_conv2d) packs the weights on the host and copies them
 to the device on every call; the profiler separates that from the kernel.  TFLOP/s are algorithmic, 2 M Cout K with the
-real channel counts.  l2_smem_TBs is the operand traffic the tiles imply, over kernel time: every CTA (128 pixels x BN
-columns) loads one 128 x 64 activation box and one BN x 64 weight box per k-block, so the bytes are
-CTAs * k-blocks * (16 KB + BN * 128 B).  Needs a GPU: there is no fallback."""
+real channel counts.  l2_smem_TBs is the operand traffic the tiles load, over kernel time.  Every CTA (128 pixels x BN
+columns) loads one BN x 64 weight box (BN * 128 B) per k-block.  Per-tap segments (k_order "tap"): one 128 x 64 activation
+box (16 KB) per k-block.  Slab segments (k_order "slab", the 3x3 segments of one-sample tiles with TW >= 8): one
+TW x (TH + 2) x 64 slab per (chunk, dx), serving the three dy k-blocks, so a 3x3 segment of `chunks` chunks loads
+chunks * 3 * TW * (TH + 2) * 128 B of activations; its 1x1 skip segment still loads 16 KB per k-block.  Needs a GPU: there
+is no fallback."""
 import argparse
 import ctypes
 import json
@@ -62,11 +65,15 @@ def _card():
 def _tile_bytes(H, W, Cin, Cout, k, Cin2):
     tw, th, tn, fused = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
     _lib.check(_lib.lib().ivid_conv_tile(H, W, ctypes.byref(tw), ctypes.byref(th), ctypes.byref(tn), ctypes.byref(fused)))
+    tw, th, tn = tw.value, th.value, tn.value
     cout_pad = -(-Cout // 64) * 64
     bn = 128 if cout_pad % 128 == 0 else 64
-    ctas = math.ceil(N / tn.value) * (H // th.value) * (W // tw.value) * (cout_pad // bn)
-    kblocks = k * k * math.ceil(Cin / 64) + math.ceil(Cin2 / 64)
-    return ctas, kblocks, ctas * kblocks * (128 * 64 * 2 + bn * 64 * 2)
+    ctas = math.ceil(N / tn) * (H // th) * (W // tw) * (cout_pad // bn)
+    chunks, chunks2 = math.ceil(Cin / 64), math.ceil(Cin2 / 64)
+    kblocks = k * k * chunks + chunks2
+    slab = k == 3 and tn == 1 and tw >= 8              # conv_launch_create's rule
+    act = chunks * 3 * tw * (th + 2) * 128 + chunks2 * 128 * 64 * 2 if slab else kblocks * 128 * 64 * 2
+    return ctas, kblocks, slab, ctas * (act + kblocks * bn * 64 * 2)
 
 
 def main():
@@ -96,9 +103,9 @@ def main():
             call()
         ms = _kernel_ms(call, a.reps)
         flop = 2.0 * N * H * W * Cout * (k * k * Cin + Cin2)
-        ctas, kblocks, tile_bytes = _tile_bytes(H, W, Cin, Cout, k, Cin2)
-        rows.append(dict(shape=tag, ctas=ctas, k_blocks=kblocks, kernel_ms=round(ms, 4), tflops=round(flop / ms / 1e9, 1),
-                         l2_smem_TBs=round(tile_bytes / ms / 1e9, 2)))
+        ctas, kblocks, slab, tile_bytes = _tile_bytes(H, W, Cin, Cout, k, Cin2)
+        rows.append(dict(shape=tag, ctas=ctas, k_blocks=kblocks, k_order="slab" if slab else "tap", kernel_ms=round(ms, 4),
+                         tflops=round(flop / ms / 1e9, 1), l2_smem_TBs=round(tile_bytes / ms / 1e9, 2)))
     print(json.dumps(dict(bench="conv", batch=N, card=_card(), reps=a.reps, rows=rows)))
 
 
