@@ -220,6 +220,21 @@ typedef struct {
   int cache_interval;
   int cache_branch;
   int cache_reuse;
+  /* Dynamic thresholding of x0 (Saharia et al. 2022, "Imagen", arXiv:2205.11487, sec. 2.3), every kind; zero means off.
+   * For every sample n, after the classifier-free guidance mix and x0 = sqrt(1/acp) * x_t - sqrt(1/acp - 1) * eps, where
+   * clip_denoised would clamp it:
+   *   a = |x0| over the M = C*H*W elements of sample n (fp32), v_0 <= ... <= v_{M-1} the same values sorted;
+   *   pos = threshold_ratio * (M - 1) in double, k = floor(pos), f = pos - k;
+   *   q = v_k + f * (v_{min(k+1, M-1)} - v_k) in double, rounded once to fp32 (numpy.quantile's "linear" method);
+   *   s = min(max(q, 1), s_max), s_max = threshold_max (threshold_max <= 0: no upper bound);
+   *   x0 <- clamp(x0, -s, s) / s in fp32.
+   * The replace / constrain guidance, the DDPM / DDIM / DPM-Solver++ updates, the DPM-Solver++ history and pred_x0 then read
+   * the thresholded x0.  threshold_max = 1 gives s = 1: the step of clip_denoised = 1, bit for bit.  s is exact and depends
+   * on sample n alone.  dynamic_threshold other than 0 / 1, threshold_ratio outside (0, 1], threshold_max in (0, 1) or NaN,
+   * or dynamic_threshold together with clip_denoised: IVID_ERR_INVALID_ARGUMENT. */
+  int dynamic_threshold;
+  double threshold_ratio;
+  double threshold_max;
 } ivid_step_args_t;
 
 /* sample_once: x_prev = f(x_t, t[, t_prev]).  `t` follows the reference's convention of each sampler:
@@ -235,6 +250,12 @@ int ivid_sampler_step(ivid_sampler_t* s, ivid_unet_t* unet, const float* x_t_dev
 int ivid_sampler_step_dev(ivid_sampler_t* s, ivid_unet_t* unet, const float* x_t_dev, float* x_prev_dev,
                           float* pred_x0_dev, int N, const int64_t* t_dev, const int64_t* t_prev_dev,
                           const ivid_step_args_t* args, void* stream);
+
+/* The dynamic thresholding of ivid_step_args_t alone, on the kernels the step runs (tests drive it with crafted data):
+ * x_dev fp32 [N][M]; s_out_dev [N] receives s of every sample and x_out_dev [N][M] clamp(x, -s, s) / s.  ratio and
+ * threshold_max as threshold_ratio and threshold_max there (IVID_ERR_INVALID_ARGUMENT outside them).  Synchronises the stream. */
+int ivid_op_dynamic_threshold(const float* x_dev, int N, int M, double ratio, double threshold_max, float* s_out_dev,
+                              float* x_out_dev, void* stream);
 
 /* ClassifierFreeGuidance.model_inference's mix alone (classifier_free_guidance.py:42): out = (1+s)*eps[0:count) -
  * s*eps[count:2*count) for the batch-2N forward's output (count = N*C*H*W, multiple of 4). */

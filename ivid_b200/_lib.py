@@ -64,6 +64,9 @@ class StepArgsT(Structure):
         ("cache_interval", c_int),    # ivid_sampler_run: a full forward every cache_interval steps, reuse forwards between
         ("cache_branch", c_int),      # branch b of the reuse forwards, 0 <= b <= num_res_blocks
         ("cache_reuse", c_int),       # single step: 1 = this step's forward is a reuse forward
+        ("dynamic_threshold", c_int), # 1: threshold x_0 at the threshold_ratio-quantile of |x_0| of each sample
+        ("threshold_ratio", c_double),
+        ("threshold_max", c_double),  # upper bound of the threshold; <= 0 = none
     ]
 
 
@@ -128,6 +131,7 @@ SIGNATURES = {
     "ivid_sampler_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(StepArgsT), c_void_p]),
     "ivid_sampler_step_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, POINTER(StepArgsT), c_void_p]),
     "ivid_cfg_mix": (c_int, [c_void_p, c_float, c_void_p, c_uint64, c_void_p]),
+    "ivid_op_dynamic_threshold": (c_int, [c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_void_p, c_void_p]),
     "ivid_sampler_run": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(StepArgsT), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ivid_op_conv2d": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int,
                                c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),

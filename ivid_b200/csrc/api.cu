@@ -224,6 +224,15 @@ int ivid_cfg_mix(const float* eps2n_dev, float strength, float* out_dev, uint64_
     launch_cfg_mix(eps2n_dev, out_dev, static_cast<size_t>(count), strength, static_cast<cudaStream_t>(stream));
   });
 }
+int ivid_op_dynamic_threshold(const float* x_dev, int N, int M, double ratio, double threshold_max, float* s_out_dev,
+                              float* x_out_dev, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(x_dev); IVID_NOT_NULL(s_out_dev); IVID_NOT_NULL(x_out_dev);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_dynamic_threshold(x_dev, N, M, ratio, threshold_max, s_out_dev, x_out_dev, st);
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+  });
+}
 int ivid_sampler_run(ivid_sampler_t* s, ivid_unet_t* unet, float* x_inout_dev, int N, int steps,
                      const ivid_step_args_t* args, const float* noise_all_dev, const float* cond_noise_all_dev,
                      float* traj_x0_dev, float* traj_xt_dev, void* stream) {

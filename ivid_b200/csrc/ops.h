@@ -115,6 +115,9 @@ struct CondPackDesc {
 };
 void launch_cond_pack(const CondPackDesc& d, cudaStream_t s);   // sampler.cu
 void launch_cfg_mix(const float* eps2, float* out, size_t count, float strength, cudaStream_t s);   // sampler.cu
+// dynamic thresholding of x [N][M] (sampler.cuh): s_out [N] and x_out = clamp(x, -s, s) / s; threshold_max <= 0: no upper bound
+void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double threshold_max, float* s_out, float* x_out,
+                              cudaStream_t s);   // sampler.cu
 
 void launch_posenc(const int64_t* t, int Nt, const float* freqs, int half, float* out, int N, cudaStream_t s);
 // FiLM table (all ResBlock emb_layers as one product): out = silu(emb) * Wp^T + bias, Wp in the swizzled K-chunk-major

@@ -93,6 +93,34 @@ void launch_cfg_mix(const float* eps2, float* out, size_t count, float strength,
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 
+// fp32 s_max of a dynamic threshold: threshold_max <= 0 means no upper bound
+static float threshold_max_f32(double m) { return m <= 0.0 ? INFINITY : static_cast<float>(m); }
+
+// The thresholded tail of a step on x_0 [N,C,H,W] before thresholding (sampler.cuh): s of every sample into s, then the update.
+template <typename Launch>
+static void launch_threshold_tail(const StepParams& p, const float* x0, float* s, double ratio, float s_max, Launch&& update,
+                                  cudaStream_t st) {
+  threshold_select_kernel<<<p.N, kSelectThreads, 0, st>>>(x0, p.C * p.HW, ratio, s_max, s);
+  IVID_CHECK_CUDA(cudaGetLastError());
+  const size_t total4 = static_cast<size_t>(p.N) * p.C * p.HW / 4;
+  update(std::max(static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8)), 1));
+  IVID_CHECK_CUDA(cudaGetLastError());
+}
+
+void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double threshold_max, float* s_out, float* x_out,
+                              cudaStream_t st) {
+  IVID_REQUIRE(N >= 1 && M >= 1, "dynamic threshold: N and M must be positive");
+  IVID_REQUIRE(ratio > 0.0 && ratio <= 1.0, "dynamic threshold: ratio must be in (0, 1]");
+  IVID_REQUIRE(!(threshold_max > 0.0 && threshold_max < 1.0) && !std::isnan(threshold_max),
+               "dynamic threshold: threshold_max must be >= 1 (or <= 0: no upper bound)");
+  threshold_select_kernel<<<N, kSelectThreads, 0, st>>>(x, M, ratio, threshold_max_f32(threshold_max), s_out);
+  IVID_CHECK_CUDA(cudaGetLastError());
+  const size_t total = static_cast<size_t>(N) * M;
+  const int grid = static_cast<int>(std::min<size_t>((total + 255) / 256, static_cast<size_t>(sm_count()) * 8));
+  threshold_apply_kernel<<<std::max(grid, 1), 256, 0, st>>>(x, s_out, x_out, static_cast<size_t>(M), total);
+  IVID_CHECK_CUDA(cudaGetLastError());
+}
+
 void launch_cond_pack(const CondPackDesc& d, cudaStream_t s) {
   CondPackParams cp;
   cp.x = d.x; cp.y = d.y; cp.mask = d.mask; cp.mask_rgb = d.mask_rgb; cp.noise = d.noise;
@@ -145,6 +173,7 @@ Sampler::~Sampler() {
   if (d_xtmp_) cudaFree(d_xtmp_);
   if (d_acp_) cudaFree(d_acp_);
   if (d_hist_) cudaFree(d_hist_);
+  if (d_thr_s_) cudaFree(d_thr_s_);
 }
 
 const std::vector<double>& Sampler::table(int which) const {
@@ -183,8 +212,10 @@ void Sampler::ensure_device(int N2, size_t eps_elems) {
   if (N2 > cap_n_) {
     if (d_t_) cudaFree(d_t_);
     if (d_classes2_) cudaFree(d_classes2_);
+    if (d_thr_s_) cudaFree(d_thr_s_);
     IVID_CHECK_CUDA(cudaMalloc(&d_t_, sizeof(int64_t) * N2));
     IVID_CHECK_CUDA(cudaMalloc(&d_classes2_, sizeof(int64_t) * N2));
+    IVID_CHECK_CUDA(cudaMalloc(&d_thr_s_, sizeof(float) * N2));
     cap_n_ = N2;
   }
   if (eps_elems > cap_eps_) {
@@ -227,6 +258,13 @@ void Sampler::check_step_args(const ivid_step_args_t& a, const Unet& unet, int N
   IVID_REQUIRE(a.cache_branch >= 0 && a.cache_branch <= unet.cfg().num_res_blocks,
                "cache_branch must be in [0, num_res_blocks] = [0, " + std::to_string(unet.cfg().num_res_blocks) + "]");
   IVID_REQUIRE(a.cache_reuse == 0 || a.cache_reuse == 1, "cache_reuse must be 0 or 1");
+  // dynamic thresholding: a flag, a ratio in (0, 1], threshold_max >= 1 or <= 0 (no upper bound), and not with the static clip
+  IVID_REQUIRE(a.dynamic_threshold == 0 || a.dynamic_threshold == 1, "dynamic_threshold must be 0 or 1");
+  IVID_REQUIRE(!a.dynamic_threshold || (a.threshold_ratio > 0.0 && a.threshold_ratio <= 1.0),
+               "dynamic threshold ratio must be in (0, 1]");
+  IVID_REQUIRE(!a.dynamic_threshold || (!(a.threshold_max > 0.0 && a.threshold_max < 1.0) && !std::isnan(a.threshold_max)),
+               "dynamic threshold_max must be >= 1 (or <= 0: no upper bound)");
+  IVID_REQUIRE(!a.dynamic_threshold || !a.clip_denoised, "clip_denoised and dynamic_threshold exclude each other");
   IVID_REQUIRE(a.replace_rgb_dev == nullptr || a.replace_rgb_mask_dev != nullptr, "replace_rgb needs its mask");
   IVID_REQUIRE(a.replace_depth_dev == nullptr || a.replace_depth_mask_dev != nullptr, "replace_depth needs its mask");
   IVID_REQUIRE(a.constrain_depth_dev == nullptr || a.replace_depth_dev != nullptr,
@@ -354,6 +392,14 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
   g.w_depth = static_cast<float>(a.replace_depth_weight); g.w_depth_c = static_cast<float>(1.0 - a.replace_depth_weight);
   g.w_convex = static_cast<float>(a.constrain_depth_weight); g.w_convex_c = static_cast<float>(1.0 - a.constrain_depth_weight);
 
+  // dynamic thresholding: x_0 before thresholding goes to d_eps_ (rows [0, N); the separate route overwrites eps in place) and
+  // s of every sample to d_thr_s_
+  const bool thr = a.dynamic_threshold != 0;
+  const double thr_ratio = a.threshold_ratio;
+  const float thr_max = threshold_max_f32(a.threshold_max);
+  float* const x0buf = d_eps_;
+  float* const sbuf = d_thr_s_;
+
   unet.set_cond_stream_dev(cond.kind != 0 && cond.noise_dev == nullptr ? &state->stream : nullptr);
   // Fused route: the output head's last kernel IS the step (head_step_kernel): eps never reaches HBM and the update is the last
   // node of the forward's CUDA graph.  Not taken when the caller does not allow it (per-step pointers that change every
@@ -372,15 +418,29 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
     // graph and differ only in the flag p.guided points to)
     uint64_t h = 1469598103934665603ull ^ (kind == kStepDdim ? 0x9E37ull : kind == kStepDpm ? 0x7F4Aull : 0ull) ^
                  (a.sde ? 0x5DE00000ull : 0ull);
-    const unsigned char* bytes = reinterpret_cast<const unsigned char*>(&p);
-    for (size_t i = 0; i < sizeof(StepParams); ++i) { h ^= bytes[i]; h *= 1099511628211ull; }
+    auto mix = [&h](const void* v, size_t n) {
+      for (size_t i = 0; i < n; ++i) { h ^= static_cast<const unsigned char*>(v)[i]; h *= 1099511628211ull; }
+    };
+    mix(&p, sizeof(StepParams));
+    if (thr) {     // the thresholded step also bakes in the ratio, s_max and its two buffers
+      mix(&thr_ratio, sizeof(thr_ratio)); mix(&thr_max, sizeof(thr_max)); mix(&x0buf, sizeof(x0buf)); mix(&sbuf, sizeof(sbuf));
+    }
     hook.key = h | 1ull;
-    hook.launch = [hp, kind](const float* Y, const float* bias, int, int Hy, int Wy, int Co, int ldy, cudaStream_t st) mutable {
+    hook.launch = [hp, kind, thr, thr_ratio, thr_max, x0buf, sbuf](const float* Y, const float* bias, int, int Hy, int Wy, int Co,
+                                                                     int ldy, cudaStream_t st) mutable {
       IVID_REQUIRE(Co == 4 && Wy % 4 == 0, "fused head step: 4 output channels, width % 4 == 0");
       HeadStepParams q = hp;
       q.Y = Y; q.bias = bias; q.H = Hy; q.W = Wy; q.ldy = ldy;
       const size_t groups = static_cast<size_t>(q.sp.N) * Hy * (Wy / 4);
       const int grid = static_cast<int>(std::min<size_t>((groups + 255) / 256, static_cast<size_t>(sm_count()) * 8));
+      if (thr) {
+        head_x0_kernel<<<std::max(grid, 1), 256, 0, st>>>(q, x0buf);
+        IVID_CHECK_CUDA(cudaGetLastError());
+        launch_threshold_tail(q.sp, x0buf, sbuf, thr_ratio, thr_max, [&](int g) {
+          with_step_kind(kind, [&](auto k) { threshold_step_kernel<decltype(k)::value><<<g, 256, 0, st>>>(q.sp, x0buf, sbuf); });
+        }, st);
+        return;
+      }
       with_step_kind(kind, [&](auto k) { head_step_kernel<decltype(k)::value><<<std::max(grid, 1), 256, 0, st>>>(q); });
       IVID_CHECK_CUDA(cudaGetLastError());
     };
@@ -392,6 +452,14 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
   unet.set_cond_stream_dev(nullptr);
   const size_t total4 = static_cast<size_t>(N) * C * HW / 4;
   const int grid = static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8));
+  if (thr) {
+    x0_kernel<<<std::max(grid, 1), 256, 0, stream>>>(p, x0buf);
+    IVID_CHECK_CUDA(cudaGetLastError());
+    launch_threshold_tail(p, x0buf, sbuf, thr_ratio, thr_max, [&](int g) {
+      with_step_kind(kind, [&](auto k) { threshold_step_kernel<decltype(k)::value><<<g, 256, 0, stream>>>(p, x0buf, sbuf); });
+    }, stream);
+    return;
+  }
   with_step_kind(kind, [&](auto k) { step_kernel<decltype(k)::value><<<std::max(grid, 1), 256, 0, stream>>>(p); });
   IVID_CHECK_CUDA(cudaGetLastError());
 }

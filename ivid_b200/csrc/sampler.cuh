@@ -167,18 +167,20 @@ __device__ __forceinline__ StepScalars step_scalars(const StepParams& p) {
   }
   return s;
 }
-// x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, the (already guidance-mixed) eps and the N(0,1) draw z.
-// DPM-Solver++: z is read only by the SDE variant (c_z != 0), dprev is D_{-1} of the element (read only at order 2) and x0o the
-// guided D0.
+// x_0 = sqrt(1/acp) * x_t - sqrt(1/acp - 1) * eps of one element (before clipping or thresholding)
+__device__ __forceinline__ float step_x0(const StepCoef& k, float xt, float e) {
+  return __fsub_rn(__fmul_rn(k.sqrt_recip_acp, xt), __fmul_rn(k.sqrt_recipm1_acp, e));
+}
+// x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, its x_0 after clipping or thresholding and the N(0,1)
+// draw z: the replace / constrain guidance, then the DDPM / DDIM / DPM-Solver++ update.  DPM-Solver++: z is read only by the SDE
+// variant (c_z != 0), dprev is D_{-1} of the element (read only at order 2) and x0o the guided D0.
 template <int kKind>
-__device__ __forceinline__ void step_element(const StepParams& p, const StepScalars& s, int n, int c, size_t pix, float xt, float e, float z,
-                                             float dprev, float& xo, float& x0o) {
+__device__ __forceinline__ void step_update(const StepParams& p, const StepScalars& s, int n, int c, size_t pix, float xt, float x0,
+                                            float z, float dprev, float& xo, float& x0o) {
   const StepCoef& k = s.k;
   auto mul = [](float a, float b) { return __fmul_rn(a, b); };
   auto add = [](float a, float b) { return __fadd_rn(a, b); };
   auto sub = [](float a, float b) { return __fsub_rn(a, b); };
-  float x0 = sub(mul(k.sqrt_recip_acp, xt), mul(k.sqrt_recipm1_acp, e));
-  if (p.clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
   if (kKind == kStepDdpm) {
     const float mean = add(mul(k.post_mean_coef1, x0), mul(k.post_mean_coef2, xt));
     xo = add(mean, mul(mul(s.nz, s.sd), z));
@@ -212,6 +214,14 @@ __device__ __forceinline__ void step_element(const StepParams& p, const StepScal
   const float mean = add(mul(s.c_x0, x0), mul(s.c_eps, e2));
   xo = add(mean, mul(mul(s.nz, s.sigma), z));
   x0o = x0;
+}
+// the whole step of one element from x_t and the (already guidance-mixed) eps, x_0 clipped to [-1, 1] when p.clip is set
+template <int kKind>
+__device__ __forceinline__ void step_element(const StepParams& p, const StepScalars& s, int n, int c, size_t pix, float xt, float e, float z,
+                                             float dprev, float& xo, float& x0o) {
+  float x0 = step_x0(s.k, xt, e);
+  if (p.clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
+  step_update<kKind>(p, s, n, c, pix, xt, x0, z, dprev, xo, x0o);
 }
 // the four N(0,1) draws of elements [i, i+4) of the flattened [N,C,H,W] tensor (i % 4 == 0): injected or Philox(seed, stream, i/4)
 __device__ __forceinline__ void step_noise4(const StepParams& p, const StepScalars& s, size_t i, bool needed, float (&z)[4]) {
@@ -326,6 +336,194 @@ __global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) 
       hist_store4<kKind>(p, i, x0o);
     }
   }
+}
+
+// ----------------------------------------------------------------------------------------------
+// Dynamic thresholding of x_0 (Saharia et al. 2022, arXiv:2205.11487, sec. 2.3), per sample n over its M = C*H*W elements:
+//   q = the ratio-quantile of |x_0| with linear interpolation (v_k + f * (v_{k+1} - v_k), pos = ratio * (M - 1) = k + f, in
+//       double, rounded once to fp32), s = min(max(q, 1), s_max), x_0 <- clamp(x_0, -s, s) / s.
+// A step in this mode runs three kernels: x_0 before thresholding into a [N,C,H,W] buffer (head_x0_kernel on the fused route,
+// x0_kernel from eps on the separate one), threshold_select_kernel (s of every sample) and threshold_step_kernel (step_kernel's
+// update on the thresholded x_0).  Both routes share the last two, so they agree bit for bit.
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ float threshold_x0(float x0, float s) { return __fdiv_rn(fminf(fmaxf(x0, -s), s), s); }
+
+// x0 may be p.eps itself: each element is read before it is overwritten, by the same thread
+__global__ void __launch_bounds__(256) x0_kernel(const StepParams p, float* x0) {
+  const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
+  const StepCoef k = p.table[*p.t_index];
+  const int cfg = step_cfg(p);
+  for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
+       i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t i = i4 * 4;
+    float v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = step_x0(k, p.x_t[i + j], mix_eps(p, cfg, i + j, total));
+    stg_f4(x0 + i, make_float4(v[0], v[1], v[2], v[3]));
+  }
+}
+
+// guidance-mixed eps of pixel (x, y) of sample n, all Co = 4 channels: the arithmetic of head_step_kernel
+__device__ __forceinline__ void head_mixed_eps4(const HeadStepParams& h, int cfg, int n, int y, int x, float (&ec)[4]) {
+  const StepParams& p = h.sp;
+  head_eps4(h, n, y, x, ec);
+  if (cfg == 1) {
+    float eu[4];
+    head_eps4(h, n + p.N, y, x, eu);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) ec[c] = cfg_mix(ec[c], eu[c], p.strength);
+  } else if (cfg == 2) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) ec[c] = __fmul_rn(__fadd_rn(1.0f, p.strength), ec[c]);
+  }
+}
+// head_step_kernel's eps, turned into x_0 and written to x0 [N,4,H,W] instead of being pushed through the update
+__global__ void __launch_bounds__(256) head_x0_kernel(const HeadStepParams h, float* __restrict__ x0) {
+  const StepParams& p = h.sp;
+  const StepCoef k = p.table[*p.t_index];
+  const int cfg = step_cfg(p);
+  const int w4 = h.W / 4;
+  const size_t groups = static_cast<size_t>(p.N) * h.H * w4;
+  for (size_t g = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; g < groups; g += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int xg = static_cast<int>(g % w4);
+    const int y = static_cast<int>((g / w4) % h.H);
+    const int n = static_cast<int>(g / (static_cast<size_t>(w4) * h.H));
+    float e[4][4];                  // [pixel][channel]
+#pragma unroll
+    for (int j = 0; j < 4; ++j) head_mixed_eps4(h, cfg, n, y, xg * 4 + j, e[j]);
+    const size_t pix = static_cast<size_t>(y) * h.W + xg * 4;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const size_t i = (static_cast<size_t>(n) * 4 + c) * p.HW + pix;
+      const float4 xt = ldg_f4(p.x_t + i);
+      stg_f4(x0 + i, make_float4(step_x0(k, xt.x, e[0][c]), step_x0(k, xt.y, e[1][c]), step_x0(k, xt.z, e[2][c]),
+                                 step_x0(k, xt.w, e[3][c])));
+    }
+  }
+}
+
+// Exact per-sample selection: one block per sample n of x [N][M] radix-selects the order statistic v_k of |x| over the fp32 bit
+// patterns (ordered like unsigned integers for non-negative floats) in three digit passes, bits 31..21, 20..10 and 9..0, each a
+// shared-memory histogram of the elements that share the digits found so far.  Integer counts make s exact and deterministic,
+// and a sample's s depends on its own elements only.  v_{k+1} comes from the last pass: v_k again while its bin holds more
+// elements, else the next non-empty bin, else the smallest element above the last pass's group.
+constexpr int kSelectThreads = 1024;
+// exclusive prefix sum of v over the block (kSelectThreads threads)
+__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* warp_sums) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sums[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    uint32_t w = warp_sums[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, w, o);
+      if (lane >= o) w += y;
+    }
+    warp_sums[lane] = w;
+  }
+  __syncthreads();
+  const uint32_t r = x - v + (warp > 0 ? warp_sums[warp - 1] : 0u);
+  __syncthreads();
+  return r;
+}
+__global__ void __launch_bounds__(kSelectThreads) threshold_select_kernel(const float* __restrict__ x, int M, double ratio,
+                                                                          float s_max, float* __restrict__ s_out) {
+  __shared__ uint32_t hist[2048];
+  __shared__ uint32_t warp_sums[32];
+  __shared__ uint32_t sh_bin, sh_rank, sh_next, sh_above;
+  const float* xs = x + static_cast<size_t>(blockIdx.x) * M;
+  const double pos = __dmul_rn(ratio, static_cast<double>(M - 1));
+  const double kd = floor(pos);
+  const double f = __dsub_rn(pos, kd);
+  uint32_t rank = static_cast<uint32_t>(kd);   // rank of v_k among the elements that share the digits found so far
+  uint32_t prefix = 0;                         // those digits
+  uint32_t above = 0xFFFFFFFFu;                // last pass: the smallest key above its group (|x| < 2^31: never a key)
+  if (threadIdx.x == 0) { sh_next = 0xFFFFFFFFu; sh_above = 0xFFFFFFFFu; }
+#pragma unroll
+  for (int pass = 0; pass < 3; ++pass) {
+    const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
+    const int bits = pass == 2 ? 10 : 11;
+    for (int b = threadIdx.x; b < 2048; b += kSelectThreads) hist[b] = 0u;
+    __syncthreads();
+    for (int i = threadIdx.x; i < M; i += kSelectThreads) {
+      const uint32_t key = __float_as_uint(fabsf(xs[i]));
+      if (pass == 0) {
+        atomicAdd(&hist[key >> shift], 1u);
+      } else {
+        const uint32_t hi = key >> (shift + bits);
+        if (hi == prefix) atomicAdd(&hist[(key >> shift) & ((1u << bits) - 1u)], 1u);
+        else if (pass == 2 && hi > prefix) above = min(above, key);
+      }
+    }
+    __syncthreads();
+    // the bin that holds rank: thread t owns bins 2t and 2t + 1
+    const uint32_t c0 = hist[2 * threadIdx.x], c1 = hist[2 * threadIdx.x + 1];
+    const uint32_t before = block_exclusive_scan(c0 + c1, warp_sums);
+    if (rank >= before && rank < before + c0 + c1) {
+      const bool lo = rank < before + c0;
+      sh_bin = 2 * threadIdx.x + (lo ? 0u : 1u);
+      sh_rank = rank - before - (lo ? 0u : c0);
+    }
+    __syncthreads();
+    rank = sh_rank;
+    prefix = (prefix << bits) | sh_bin;
+  }
+  const uint32_t bin = prefix & 0x3FFu;
+  for (int b = threadIdx.x; b < 1024; b += kSelectThreads)
+    if (b > static_cast<int>(bin) && hist[b] != 0u) atomicMin(&sh_next, static_cast<uint32_t>(b));
+  above = __reduce_min_sync(0xFFFFFFFFu, above);
+  if ((threadIdx.x & 31) == 0) atomicMin(&sh_above, above);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t next = prefix;                                          // k = M - 1: v_{min(k+1, M-1)} = v_k
+    if (rank + 1 < hist[bin]) next = prefix;
+    else if (sh_next != 0xFFFFFFFFu) next = (prefix & ~0x3FFu) | sh_next;
+    else if (sh_above != 0xFFFFFFFFu) next = sh_above;
+    const double vk = __uint_as_float(prefix), vk1 = __uint_as_float(next);
+    const float q = __double2float_rn(__dadd_rn(vk, __dmul_rn(f, __dsub_rn(vk1, vk))));
+    s_out[blockIdx.x] = fminf(fmaxf(q, 1.0f), s_max);
+  }
+}
+
+// step_kernel's update on the thresholded x_0: x0 [N,C,H,W] before thresholding, s [N] from threshold_select_kernel
+template <int kKind>
+__global__ void __launch_bounds__(256) threshold_step_kernel(const StepParams p, const float* __restrict__ x0, const float* __restrict__ s_n) {
+  const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
+  const StepScalars s = step_scalars<kKind>(p);
+  for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
+       i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t i = i4 * 4;
+    const int plane = static_cast<int>(i / p.HW);      // n*C + c
+    const int n = plane / p.C, c = plane % p.C;
+    const size_t pix = i - static_cast<size_t>(plane) * p.HW;
+    const float sn = s_n[n];
+    float z[4], hp[4];
+    step_noise4(p, s, i, step_draws_noise<kKind>(s), z);
+    hist_load4<kKind>(p, s, i, hp);
+    const float4 xv = ldg_f4(x0 + i);
+    const float x0v[4] = {xv.x, xv.y, xv.z, xv.w};
+    float xo[4], x0o[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      step_update<kKind>(p, s, n, c, pix + j, p.x_t[i + j], threshold_x0(x0v[j], sn), z[j], hp[j], xo[j], x0o[j]);
+    stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
+    if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
+    hist_store4<kKind>(p, i, x0o);
+  }
+}
+
+// the clamp / scale alone (ivid_op_dynamic_threshold): out = threshold_x0(x, s[i / M]) over x [N][M]
+__global__ void __launch_bounds__(256) threshold_apply_kernel(const float* __restrict__ x, const float* __restrict__ s_n, float* __restrict__ out,
+                                                              size_t M, size_t total) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    out[i] = threshold_x0(x[i], s_n[i / M]);
 }
 
 // ----------------------------------------------------------------------------------------------

@@ -42,6 +42,7 @@ class Sampler {
   size_t cap_hist_ = 0;
   int64_t* d_t_ = nullptr;
   int64_t* d_classes2_ = nullptr;
+  float* d_thr_s_ = nullptr;               // dynamic thresholding: s of every sample [cap_n_]
   float* d_eps_ = nullptr;
   float* d_xtmp_ = nullptr;
   int cap_n_ = 0;

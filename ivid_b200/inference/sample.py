@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from .. import backbones, frameworks, samplers
-from ..samplers.samplers import _check_cache
+from ..samplers.samplers import _check_cache, _check_threshold
 from ..rgbd_3d import DeviceWarp, glm_compat as glm
 from ..rgbd_3d import utils as rgbd_utils
 from ..utils import edict
@@ -61,7 +61,7 @@ def build_modelviews(viewset, num_samples, rng=None):
 @torch.no_grad()
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
-               precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0):
+               precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, and solver="dpmpp_sde" its stochastic variant
@@ -69,10 +69,13 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision).  guidance_interval=(t_lo, t_hi)
     guides only the steps of both networks whose model time lies in [t_lo, t_hi] (the samplers' `guidance_interval`);
     the other steps run at strength 0 with one batch-N forward.  cache_interval=N, cache_branch=b reuse the deep features of
-    both networks between full forwards every N steps (the samplers' `cache_interval` / `cache_branch`; None: no reuse)."""
+    both networks between full forwards every N steps (the samplers' `cache_interval` / `cache_branch`; None: no reuse).
+    dynamic_threshold=p or (p, s_max) thresholds x_0 dynamically at every step of both networks (the samplers'
+    `dynamic_threshold`)."""
     for fw in (framework_uncond, framework_cond):          # before any device work
         if fw is not None:
             _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
+    _check_threshold(dynamic_threshold, False)
     assert solver in ("ddim", "dpmpp", "dpmpp_sde"), f"solver must be 'ddim', 'dpmpp' or 'dpmpp_sde', got {solver!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
@@ -84,6 +87,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     gi_kw = dict(guidance_interval=tuple(guidance_interval)) if guidance_interval is not None else {}
     if cache_interval is not None:
         gi_kw.update(cache_interval=cache_interval, cache_branch=cache_branch)
+    th_kw = dict(dynamic_threshold=dynamic_threshold) if dynamic_threshold is not None else {}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
     net = framework_uncond.backbone
@@ -120,6 +124,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
                 if steps_uncond < 1000:
                     kw.update(sde_kw)
+                kw.update(th_kw)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
             else:
                 cond = warp.aggregate(mv_j, **wparams)                   # [bs,7,S,S] in [0,1]
@@ -130,7 +135,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
                 kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
-                kw.update(sde_kw)
+                kw.update(sde_kw, **th_kw)
                 res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
             samples.append(res.samples)
             if warp is not None:
@@ -254,6 +259,7 @@ def main(rank, world_size, opt):
     precision = getattr(opt, "precision", "fp16")
     interval = getattr(opt, "guidance_interval", None)
     cache_interval, cache_branch = getattr(opt, "cache_interval", None), getattr(opt, "cache_branch", 0)
+    dynamic_threshold = getattr(opt, "dynamic_threshold", None)
     out_dir = output_dir_name(opt)
     for sub in ("results", "grids", "conds", "scenes"):                 # sample.py:283-286
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
@@ -261,7 +267,8 @@ def main(rank, world_size, opt):
     gen = sample_all(fw_u, fw_c, seeds_r if seeds_r is not None else len(idx), opt.steps_uncond, opt.steps_cond, mvs_r, classes=classes_r,
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
                      rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
-                     precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch)
+                     precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch,
+                     dynamic_threshold=dynamic_threshold)
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -276,10 +283,12 @@ def output_dir_name(opt):
     precision = getattr(opt, "precision", "fp16")
     interval = getattr(opt, "guidance_interval", None)
     cache_interval = getattr(opt, "cache_interval", None)
+    dt = getattr(opt, "dynamic_threshold", None)
     return os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
                         + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}")
                         + ("" if interval is None else f"_interval{interval[0]}-{interval[1]}")
-                        + ("" if cache_interval is None else f"_cache{cache_interval}b{getattr(opt, 'cache_branch', 0)}"))
+                        + ("" if cache_interval is None else f"_cache{cache_interval}b{getattr(opt, 'cache_branch', 0)}")
+                        + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}"))
 
 
 def _int_at_least(lo):
@@ -306,6 +315,22 @@ def parse_interval(s):
     if not 0 <= lo <= hi:
         raise argparse.ArgumentTypeError(f"expected 0 <= LO <= HI, got {s!r}")
     return lo, hi
+
+
+def parse_threshold(s):
+    """'P' or 'P,MAX' -> P or (P, MAX) of --dynamic_threshold: the quantile ratio 0 < P <= 1 and the bound MAX >= 1."""
+    parts = s.split(",")
+    if len(parts) not in (1, 2):
+        raise argparse.ArgumentTypeError(f"expected P or P,MAX, got {s!r}")
+    try:
+        vals = [float(v) for v in parts]
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected numbers P[,MAX], got {s!r}") from None
+    if not 0.0 < vals[0] <= 1.0:
+        raise argparse.ArgumentTypeError(f"expected 0 < P <= 1, got {s!r}")
+    if len(vals) == 2 and not vals[1] >= 1.0:
+        raise argparse.ArgumentTypeError(f"expected MAX >= 1, got {s!r}")
+    return vals[0] if len(vals) == 1 else (vals[0], vals[1])
 
 
 def build_arg_parser():
@@ -347,6 +372,9 @@ def build_arg_parser():
     ap.add_argument("--cache_branch", type=_int_at_least(0), default=0, metavar="B",
                     help="with --cache_interval: the shallow forwards recompute input blocks 0..B and the last B+1 output blocks, "
                          "0 <= B <= num_res_blocks (default 0, the cheapest)")
+    ap.add_argument("--dynamic_threshold", type=parse_threshold, default=None, metavar="P[,MAX]",
+                    help="dynamic thresholding of the predicted x_0 (Imagen): clamp each sample's x_0 to [-s, s] and divide by s, "
+                         "s = min(max(P-quantile of |x_0|, 1), MAX); e.g. 0.995 (default: off; MAX defaults to no bound)")
     return ap
 
 

@@ -15,6 +15,7 @@ the torch RNG stream consumption identical to the reference.
 from __future__ import annotations
 
 import ctypes
+import math
 import numbers
 
 import numpy as np
@@ -56,6 +57,24 @@ def _check_cache(cache_interval, cache_branch, num_res_blocks):
     return int(cache_interval) if cache_interval is not None else 0
 
 
+def _check_threshold(dynamic_threshold, clip_denoised):
+    """Dynamic thresholding argument: None, a ratio p in (0, 1], or a pair (p, s_max) with s_max >= 1 (None: no upper bound).
+    It replaces clip_denoised, so the two exclude each other.  Returns (p, s_max) as floats, s_max = inf without a bound, or None."""
+    if dynamic_threshold is None:
+        return None
+    if isinstance(dynamic_threshold, (tuple, list)):
+        assert len(dynamic_threshold) == 2, f"dynamic_threshold must be p or (p, s_max), got {dynamic_threshold!r}"
+        p, s_max = dynamic_threshold
+    else:
+        p, s_max = dynamic_threshold, None
+    real = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool)
+    assert real(p) and 0.0 < float(p) <= 1.0, f"dynamic_threshold ratio p must be in (0, 1], got {p!r}"
+    s_max = math.inf if s_max is None else s_max
+    assert real(s_max) and float(s_max) >= 1.0, f"dynamic_threshold s_max must be >= 1, got {s_max!r}"
+    assert not clip_denoised, "clip_denoised and dynamic_threshold exclude each other"
+    return float(p), float(s_max)
+
+
 class _NativeSampler:
     KIND = 0
 
@@ -94,7 +113,7 @@ class _NativeSampler:
         return uses_cfg, float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
 
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None, sde=False, interval=None, cache=None):
+                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -154,6 +173,10 @@ class _NativeSampler:
             a.guidance_t_lo, a.guidance_t_hi = interval
         if cache is not None:
             a.cache_interval, a.cache_branch, a.cache_reuse = (int(v) for v in cache)
+        if threshold is not None:
+            a.dynamic_threshold = 1
+            a.threshold_ratio = threshold[0]
+            a.threshold_max = 0.0 if math.isinf(threshold[1]) else threshold[1]
         return a, keep
 
     def _net(self):
@@ -165,14 +188,15 @@ class _NativeSampler:
         return _unwrap(self.framework.backbone).num_res_blocks
 
     def _native_step(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                     sde=False, interval=None, cache=None):
+                     sde=False, interval=None, cache=None, threshold=None):
         """One step.  `t` / `t_prev` are host ints (ivid_sampler_step) or the [N] tensors sample_once receives
         (ivid_sampler_step_dev: the step is read on the device, no host sync; t_prev None for DDPM)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
-                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache)
+                                  hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache,
+                                  threshold=threshold)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         L = _lib.lib()
@@ -189,7 +213,7 @@ class _NativeSampler:
         return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
 
     def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, interval, reuse_features, cache_branch,
-                     order=0, prev=None, sde=False):
+                     order=0, prev=None, sde=False, dynamic_threshold=None):
         """The body of every sample_once: the host checks before any device work or torch draw, the step noise (drawn as
         the reference draws it, or the injected `noise` and kwargs' `cond_noise`), then the step with t / t_prev read on
         the device (all samples of a batch share the step, ddpm.py:177-179, ddim.py:154-158: no host sync)."""
@@ -198,6 +222,7 @@ class _NativeSampler:
         assert self.KIND == 0 or t_prev.shape == (B,), "t_prev must be a 1D tensor of shape (B,)"
         _check_interval(interval, len(self.framework.betas))
         _check_cache(None, cache_branch, self._num_res_blocks())
+        threshold = _check_threshold(dynamic_threshold, clip_denoised)
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kwargs)
         else:
@@ -205,7 +230,7 @@ class _NativeSampler:
         # the DPM-Solver++ ODE update reads no step noise
         return self._native_step(x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise if self.KIND != 2 or sde else None,
                                  cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                 cache=(0, cache_branch, bool(reuse_features)))
+                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold)
 
     def _draw_step_noise(self, x_t, kwargs):
         """torch draws in the reference's order: InpaintCFG rgb, depth (inside model_inference), then randn_like(x_t)."""
@@ -233,9 +258,10 @@ class _NativeSampler:
         return reuse
 
     def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
-             sde=False, interval=None, cache_interval=None, cache_branch=0):
+             sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None):
         interval = _check_interval(interval, len(self.framework.betas))   # before any device work
         cache_interval = _check_cache(cache_interval, cache_branch, self._num_res_blocks())
+        threshold = _check_threshold(dynamic_threshold, clip_denoised)
         net = self._net()
         net.eval()
         if image_size is None:
@@ -264,7 +290,7 @@ class _NativeSampler:
                 # the DPM-Solver++ ODE update draws z only to consume the torch RNG as DdimSampler does
                 out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if self.KIND != 2 or sde else None,
                                         cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                        cache=(0, cache_branch, reuse[i]))
+                                        cache=(0, cache_branch, reuse[i]), threshold=threshold)
                 if self.KIND == 2 and order != 1:
                     prev = (t, out.pred_x_0)
                 img = out.pred_x_prev
@@ -274,7 +300,7 @@ class _NativeSampler:
         elif rng == "philox":
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
             a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
-                                      interval=interval, cache=(cache_interval, cache_branch, 0))
+                                      interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold)
             traj0 = trajt = None
             if return_trajectory:
                 traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
@@ -308,18 +334,20 @@ class DdpmSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, **kwargs):
         """x_{t-1} from x_t (ddpm.py:111-131).  `t` is the [N] tensor of steps minus 1 (all equal).
         `noise` (extension) injects the randn_like draw; default draws it with torch like the reference.
         `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`).
         `reuse_features=True` (extension): the step's forward reuses the deep features of the last full forward of the same
-        batch and size at branch `cache_branch` (see `sample`); RuntimeError if no full forward has run on it."""
+        batch and size at branch `cache_branch` (see `sample`); RuntimeError if no full forward has run on it.
+        `dynamic_threshold=p` or `(p, s_max)` (extension): dynamic thresholding of x_0 (see `sample`)."""
         return self._sample_once(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, guidance_interval, reuse_features,
-                                 cache_branch)
+                                 cache_branch, dynamic_threshold=dynamic_threshold)
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
-               rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0, **kwargs):
+               rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
+               dynamic_threshold=None, **kwargs):
         """Run the full reverse process (ddpm.py:134-187).  `steps` is accepted and ignored exactly as in the reference.
         pred_x_t / pred_x_0 are only materialised with return_trajectory=True (the reference keeps 2x1000 tensors alive;
         its callers read `.samples` only: inference/sample.py:82).
@@ -334,9 +362,16 @@ class DdpmSampler(_NativeSampler):
         last b + 1 output blocks and the head) and reuse the deeper up-path features of the last full forward.  A step where
         the guidance interval switches between the guided and the unguided forward is always full.  0 <= b <=
         num_res_blocks; b = 0 is the cheapest.  None (default) or 1 runs every forward in full.  The update, the noise and the
-        torch RNG consumption are those of a run without reuse; eps is an approximation."""
+        torch RNG consumption are those of a run without reuse; eps is an approximation.
+
+        dynamic_threshold=p or (p, s_max) (extension; Saharia et al. 2022, arXiv:2205.11487, sec. 2.3): at every step, where
+        clip_denoised would clamp x_0, each sample's x_0 is clamped to [-s, s] and divided by s, s = min(max(q, 1), s_max) and q
+        the p-quantile of |x_0| over the sample (linear interpolation, as numpy.quantile); s_max defaults to no bound, p in
+        (0, 1], s_max >= 1.  The guidance and the update then read the thresholded x_0 (include/ivid_b200.h).  Excludes
+        clip_denoised; s_max = 1 is clip_denoised=True.  The noise and the torch RNG consumption are unchanged."""
         return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch)
+                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
+                         dynamic_threshold=dynamic_threshold)
 
 
 class DdimSampler(_NativeSampler):
@@ -346,22 +381,24 @@ class DdimSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, eta=0.0, replace_rgb=None,
                     replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, **kwargs):
         """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step).
         `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi].
-        `reuse_features` / `cache_branch` as in DdpmSampler.sample_once."""
+        `reuse_features` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch)
+                                 cache_branch, dynamic_threshold=dynamic_threshold)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
                verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               **kwargs):
+               dynamic_threshold=None, **kwargs):
         """Run `steps` DDIM steps (ddim.py:106-165).  `guidance_interval=(t_lo, t_hi)` as in DdpmSampler.sample, on the model
-        time t - 1 of each step; `cache_interval` / `cache_branch` as in DdpmSampler.sample."""
+        time t - 1 of each step; `cache_interval` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample (the replace /
+        constrain guidance acts on the thresholded x_0)."""
         return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
-                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch)
+                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
+                         dynamic_threshold=dynamic_threshold)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -380,27 +417,29 @@ class DpmSolverSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
                     constrain_depth=None, noise=None, sde=False, guidance_interval=None, reuse_features=False, cache_branch=0,
-                    **kwargs):
+                    dynamic_threshold=None, **kwargs):
         """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
         With sde=True `noise` is the injected z of the update; with sde=False the update does not use it.  When it is None
         the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
-        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval`, `reuse_features`
-        and `cache_branch` as for DdimSampler.sample_once."""
+        randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval`, `reuse_features`,
+        `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once (D0, and so pred_x_0, is thresholded)."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, order=2 if prev is not None else 1, prev=prev, sde=sde)
+                                 cache_branch, order=2 if prev is not None else 1, prev=prev, sde=sde,
+                                 dynamic_threshold=dynamic_threshold)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, sde=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               **kwargs):
+               dynamic_threshold=None, **kwargs):
         """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
         final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
         is drawn where DdimSampler draws it (`rng`).  `guidance_interval` as in DdimSampler.sample; the history D_{-1} of a
         step after an unguided one is that step's unguided D0.  `cache_interval` / `cache_branch` as in DdpmSampler.sample;
-        the history D_{-1} of a step is that step's D0, from whichever forward ran.  Same return dict as DdimSampler.sample."""
+        the history D_{-1} of a step is that step's D0, from whichever forward ran.  `dynamic_threshold` as in
+        DdpmSampler.sample: D0 is the thresholded, guided x_0, and so is the history.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
-                         cache_branch=cache_branch)
+                         cache_branch=cache_branch, dynamic_threshold=dynamic_threshold)
