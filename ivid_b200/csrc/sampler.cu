@@ -5,7 +5,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <type_traits>
 
 #include "sampler.cuh"
 
@@ -85,26 +84,52 @@ __global__ void fill_classes_kernel(const int64_t* classes, int64_t* out, int N)
     out[i] = i < N ? classes[i] : -1;
 }
 
+// blocks of 256 threads for a grid-stride loop over `units` work units: at most 8 per SM
+static int elementwise_grid(size_t units) {
+  return static_cast<int>(std::max<size_t>(std::min<size_t>((units + 255) / 256, static_cast<size_t>(sm_count()) * 8), 1));
+}
+
 void launch_cfg_mix(const float* eps2, float* out, size_t count, float strength, cudaStream_t s) {
   IVID_REQUIRE(count % 4 == 0, "cfg mix: element count must be a multiple of 4");
   const size_t n4 = count / 4;
-  const int grid = static_cast<int>(std::min<size_t>((n4 + 255) / 256, static_cast<size_t>(sm_count()) * 8));
-  cfg_mix_kernel<<<std::max(grid, 1), 256, 0, s>>>(eps2, out, n4, strength);
+  cfg_mix_kernel<<<elementwise_grid(n4), 256, 0, s>>>(eps2, out, n4, strength);
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 
 // fp32 s_max of a dynamic threshold: threshold_max <= 0 means no upper bound
 static float threshold_max_f32(double m) { return m <= 0.0 ? INFINITY : static_cast<float>(m); }
 
-// The thresholded tail of a step on x_0 [N,C,H,W] before thresholding (sampler.cuh): s of every sample into s, then the update.
-template <typename Launch>
-static void launch_threshold_tail(const StepParams& p, const float* x0, float* s, double ratio, float s_max, Launch&& update,
-                                  cudaStream_t st) {
-  threshold_select_kernel<<<p.N, kSelectThreads, 0, st>>>(x0, p.C * p.HW, ratio, s_max, s);
+// What the tail of a step takes besides StepParams: the step kind and the dynamic threshold (ratio, s_max, the buffer of x_0
+// before thresholding and s of every sample)
+struct StepTail {
+  int kind;
+  bool threshold;
+  double ratio;
+  float s_max;
+  float* x0;
+  float* s;
+};
+
+// The tail of a step from x_0 source src (sampler.cuh: EpsRows after the forward, HeadTaps as the forward's last node): the
+// update, or with a dynamic threshold x_0 into t.x0, s of every sample and the update on the thresholded x_0.
+template <typename Src>
+static void launch_step_tail(const StepParams& p, const Src& src, const StepTail& t, cudaStream_t st) {
+  auto update = [&](const auto& from) {
+    const int grid = elementwise_grid(from.units(p));
+    if (t.kind == kStepDdim) step_kernel<<<grid, 256, 0, st>>>(p, from, Update<kStepDdim>());
+    else if (t.kind == kStepDpm) step_kernel<<<grid, 256, 0, st>>>(p, from, Update<kStepDpm>());
+    else step_kernel<<<grid, 256, 0, st>>>(p, from, Update<kStepDdpm>());
+    IVID_CHECK_CUDA(cudaGetLastError());
+  };
+  if (!t.threshold) {
+    update(src);
+    return;
+  }
+  step_kernel<<<elementwise_grid(src.units(p)), 256, 0, st>>>(p, src, StoreX0{t.x0});
   IVID_CHECK_CUDA(cudaGetLastError());
-  const size_t total4 = static_cast<size_t>(p.N) * p.C * p.HW / 4;
-  update(std::max(static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8)), 1));
+  threshold_select_kernel<<<p.N, kSelectThreads, 0, st>>>(t.x0, p.C * p.HW, t.ratio, t.s_max, t.s);
   IVID_CHECK_CUDA(cudaGetLastError());
+  update(ThresholdedX0{t.x0, t.s});
 }
 
 void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double threshold_max, float* s_out, float* x_out,
@@ -116,8 +141,7 @@ void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double
   threshold_select_kernel<<<N, kSelectThreads, 0, st>>>(x, M, ratio, threshold_max_f32(threshold_max), s_out);
   IVID_CHECK_CUDA(cudaGetLastError());
   const size_t total = static_cast<size_t>(N) * M;
-  const int grid = static_cast<int>(std::min<size_t>((total + 255) / 256, static_cast<size_t>(sm_count()) * 8));
-  threshold_apply_kernel<<<std::max(grid, 1), 256, 0, st>>>(x, s_out, x_out, static_cast<size_t>(M), total);
+  threshold_apply_kernel<<<elementwise_grid(total), 256, 0, st>>>(x, s_out, x_out, static_cast<size_t>(M), total);
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 
@@ -309,14 +333,6 @@ static StepPlan plan_step(const ivid_step_args_t& a, int N, int t, int t_prev, b
   return sp;
 }
 
-// f(std::integral_constant<int, kind>()): the step kind as the step kernels' template argument
-template <typename F>
-static void with_step_kind(int kind, F&& f) {
-  if (kind == kStepDdim) f(std::integral_constant<int, kStepDdim>());
-  else if (kind == kStepDpm) f(std::integral_constant<int, kStepDpm>());
-  else f(std::integral_constant<int, kStepDdpm>());
-}
-
 void Sampler::step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, int t, int t_prev,
                    const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev,
                    const int64_t* t_prev_dev) {
@@ -370,7 +386,7 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
 
   StepParams p;
   std::memset(&p, 0, sizeof(p));         // padding bytes are part of the fused route's graph key
-  p.x_t = x_t; p.eps = d_eps_; p.noise = a.step_noise_dev; p.x_prev = x_prev; p.pred_x0 = pred_x0;
+  p.x_t = x_t; p.noise = a.step_noise_dev; p.x_prev = x_prev; p.pred_x0 = pred_x0;
   p.table = reinterpret_cast<const StepCoef*>(d_table_);
   p.t_index = &state->t_index;
   p.t_prev = &state->t_prev;
@@ -394,24 +410,16 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
 
   // dynamic thresholding: x_0 before thresholding goes to d_eps_ (rows [0, N); the separate route overwrites eps in place) and
   // s of every sample to d_thr_s_
-  const bool thr = a.dynamic_threshold != 0;
-  const double thr_ratio = a.threshold_ratio;
-  const float thr_max = threshold_max_f32(a.threshold_max);
-  float* const x0buf = d_eps_;
-  float* const sbuf = d_thr_s_;
+  const StepTail tail{kind, a.dynamic_threshold != 0, a.threshold_ratio, threshold_max_f32(a.threshold_max), d_eps_, d_thr_s_};
 
   unet.set_cond_stream_dev(cond.kind != 0 && cond.noise_dev == nullptr ? &state->stream : nullptr);
-  // Fused route: the output head's last kernel IS the step (head_step_kernel): eps never reaches HBM and the update is the last
-  // node of the forward's CUDA graph.  Not taken when the caller does not allow it (per-step pointers that change every
+  // Fused route: the output head's last kernel IS the step (step_kernel<HeadTaps, ...>): eps never reaches HBM and the update is
+  // the last node of the forward's CUDA graph.  Not taken when the caller does not allow it (per-step pointers that change every
   // step inside run(): every step would need its own graph) or when the model has no tap-column head.
   static const bool fuse_ok = getenv("IVID_NO_FUSED_STEP") == nullptr;
   const bool fuse = fuse_ok && allow_fuse && unet.can_fuse_head(W) && C == 4 && W % 4 == 0;
+  HeadHook hook;
   if (fuse) {
-    p.eps = nullptr;
-    HeadStepParams hp;
-    std::memset(&hp, 0, sizeof(hp));
-    hp.sp = p; hp.H = H; hp.W = W;
-    HeadHook hook;
     // FNV-1a over everything the launcher bakes in
     // (sde: the SDE and ODE steps differ only in device state, but an ODE and an SDE run never share a captured graph;
     // on the host route a guided and an unguided step differ in p.cfg (and in the plan); on the device route they share one
@@ -422,46 +430,20 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
       for (size_t i = 0; i < n; ++i) { h ^= static_cast<const unsigned char*>(v)[i]; h *= 1099511628211ull; }
     };
     mix(&p, sizeof(StepParams));
-    if (thr) {     // the thresholded step also bakes in the ratio, s_max and its two buffers
-      mix(&thr_ratio, sizeof(thr_ratio)); mix(&thr_max, sizeof(thr_max)); mix(&x0buf, sizeof(x0buf)); mix(&sbuf, sizeof(sbuf));
+    if (tail.threshold) {     // the thresholded step also bakes in the ratio, s_max and its two buffers
+      mix(&tail.ratio, sizeof(tail.ratio)); mix(&tail.s_max, sizeof(tail.s_max)); mix(&tail.x0, sizeof(tail.x0));
+      mix(&tail.s, sizeof(tail.s));
     }
     hook.key = h | 1ull;
-    hook.launch = [hp, kind, thr, thr_ratio, thr_max, x0buf, sbuf](const float* Y, const float* bias, int, int Hy, int Wy, int Co,
-                                                                     int ldy, cudaStream_t st) mutable {
+    hook.launch = [p, tail](const float* Y, const float* bias, int, int Hy, int Wy, int Co, int ldy, cudaStream_t st) {
       IVID_REQUIRE(Co == 4 && Wy % 4 == 0, "fused head step: 4 output channels, width % 4 == 0");
-      HeadStepParams q = hp;
-      q.Y = Y; q.bias = bias; q.H = Hy; q.W = Wy; q.ldy = ldy;
-      const size_t groups = static_cast<size_t>(q.sp.N) * Hy * (Wy / 4);
-      const int grid = static_cast<int>(std::min<size_t>((groups + 255) / 256, static_cast<size_t>(sm_count()) * 8));
-      if (thr) {
-        head_x0_kernel<<<std::max(grid, 1), 256, 0, st>>>(q, x0buf);
-        IVID_CHECK_CUDA(cudaGetLastError());
-        launch_threshold_tail(q.sp, x0buf, sbuf, thr_ratio, thr_max, [&](int g) {
-          with_step_kind(kind, [&](auto k) { threshold_step_kernel<decltype(k)::value><<<g, 256, 0, st>>>(q.sp, x0buf, sbuf); });
-        }, st);
-        return;
-      }
-      with_step_kind(kind, [&](auto k) { head_step_kernel<decltype(k)::value><<<std::max(grid, 1), 256, 0, st>>>(q); });
-      IVID_CHECK_CUDA(cudaGetLastError());
+      launch_step_tail(p, HeadTaps{Y, bias, Hy, Wy, ldy}, tail, st);
     };
-    unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, nullptr, sp.Nf, stream, &hook, sp.cache_branch);
-    unet.set_cond_stream_dev(nullptr);
-    return;
   }
-  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, d_eps_, sp.Nf, stream, nullptr, sp.cache_branch);
+  unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, fuse ? nullptr : d_eps_, sp.Nf, stream, fuse ? &hook : nullptr,
+               sp.cache_branch);
   unet.set_cond_stream_dev(nullptr);
-  const size_t total4 = static_cast<size_t>(N) * C * HW / 4;
-  const int grid = static_cast<int>(std::min<size_t>((total4 + 255) / 256, static_cast<size_t>(sm_count()) * 8));
-  if (thr) {
-    x0_kernel<<<std::max(grid, 1), 256, 0, stream>>>(p, x0buf);
-    IVID_CHECK_CUDA(cudaGetLastError());
-    launch_threshold_tail(p, x0buf, sbuf, thr_ratio, thr_max, [&](int g) {
-      with_step_kind(kind, [&](auto k) { threshold_step_kernel<decltype(k)::value><<<g, 256, 0, stream>>>(p, x0buf, sbuf); });
-    }, stream);
-    return;
-  }
-  with_step_kind(kind, [&](auto k) { step_kernel<decltype(k)::value><<<std::max(grid, 1), 256, 0, stream>>>(p); });
-  IVID_CHECK_CUDA(cudaGetLastError());
+  if (!fuse) launch_step_tail(p, EpsRows{d_eps_}, tail, stream);
 }
 
 void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t& a, const float* noise_all,

@@ -77,7 +77,6 @@ struct DpmStep {
 
 struct StepParams {
   const float* x_t;            // [N,C,H,W]
-  const float* eps;            // [2N or N,C,H,W]: rows [0,N) conditional, [N,2N) unconditional when cfg
   const float* noise;          // [N,C,H,W] injected N(0,1) or nullptr -> Philox
   float* x_prev;               // [N,C,H,W]
   float* pred_x0;              // optional
@@ -102,18 +101,27 @@ struct StepParams {
 };
 
 // (1 + strength) * eps_c - strength * eps_u (only evaluated with strength > 0).  Every product / sum of the step arithmetic is
-// written with explicit round-to-nearest intrinsics (no compiler-chosen FMA contraction), so that step_kernel and
-// head_step_kernel - the same formulas inlined into different kernels - produce identical bits.
+// written with explicit round-to-nearest intrinsics (no compiler-chosen FMA contraction), so that the instantiations of
+// step_kernel - the same formulas inlined behind different sources of eps - produce identical bits.
 __device__ __forceinline__ float cfg_mix(float ec, float eu, float strength) {
   return __fsub_rn(__fmul_rn(__fadd_rn(1.0f, strength), ec), __fmul_rn(strength, eu));
 }
 // cfg of this step: p.cfg, or 0 when the device flag says the step lies outside the guidance interval
 __device__ __forceinline__ int step_cfg(const StepParams& p) { return (p.guided != nullptr && *p.guided == 0) ? 0 : p.cfg; }
-__device__ __forceinline__ float mix_eps(const StepParams& p, int cfg, size_t i, size_t total) {
-  const float ec = p.eps[i];
-  if (!cfg) return ec;
-  if (cfg == 2) return __fmul_rn(__fadd_rn(1.0f, p.strength), ec);
-  return cfg_mix(ec, p.eps[total + i], p.strength);
+// the guidance-mixed eps of four elements, cfg = step_cfg(p): eps(false, e) loads the conditional eps, eps(true, e) the
+// unconditional one (called only when cfg == 1)
+template <typename Eps>
+__device__ __forceinline__ void mix_eps4(const StepParams& p, int cfg, Eps&& eps, float (&e)[4]) {
+  eps(false, e);
+  if (cfg == 1) {
+    float eu[4];
+    eps(true, eu);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) e[j] = cfg_mix(e[j], eu[j], p.strength);
+  } else if (cfg == 2) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) e[j] = __fmul_rn(__fadd_rn(1.0f, p.strength), e[j]);
+  }
 }
 
 // classifier-free-guidance mix alone (framework.model_inference): out = (1+s)*eps[0:n) - s*eps[n:2n)
@@ -171,6 +179,14 @@ __device__ __forceinline__ StepScalars step_scalars(const StepParams& p) {
 __device__ __forceinline__ float step_x0(const StepCoef& k, float xt, float e) {
   return __fsub_rn(__fmul_rn(k.sqrt_recip_acp, xt), __fmul_rn(k.sqrt_recipm1_acp, e));
 }
+// x_0 of one element from x_t and the (already guidance-mixed) eps, clipped to [-1, 1] when p.clip is set
+__device__ __forceinline__ float eps_x0(const StepParams& p, const StepCoef& k, float xt, float e) {
+  float x0 = step_x0(k, xt, e);
+  if (p.clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
+  return x0;
+}
+// dynamic thresholding of one element of x_0 with its sample's s (see threshold_select_kernel)
+__device__ __forceinline__ float threshold_x0(float x0, float s) { return __fdiv_rn(fminf(fmaxf(x0, -s), s), s); }
 // x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, its x_0 after clipping or thresholding and the N(0,1)
 // draw z: the replace / constrain guidance, then the DDPM / DDIM / DPM-Solver++ update.  DPM-Solver++: z is read only by the SDE
 // variant (c_z != 0), dprev is D_{-1} of the element (read only at order 2) and x0o the guided D0.
@@ -215,14 +231,6 @@ __device__ __forceinline__ void step_update(const StepParams& p, const StepScala
   xo = add(mean, mul(mul(s.nz, s.sigma), z));
   x0o = x0;
 }
-// the whole step of one element from x_t and the (already guidance-mixed) eps, x_0 clipped to [-1, 1] when p.clip is set
-template <int kKind>
-__device__ __forceinline__ void step_element(const StepParams& p, const StepScalars& s, int n, int c, size_t pix, float xt, float e, float z,
-                                             float dprev, float& xo, float& x0o) {
-  float x0 = step_x0(s.k, xt, e);
-  if (p.clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
-  step_update<kKind>(p, s, n, c, pix, xt, x0, z, dprev, xo, x0o);
-}
 // the four N(0,1) draws of elements [i, i+4) of the flattened [N,C,H,W] tensor (i % 4 == 0): injected or Philox(seed, stream, i/4)
 __device__ __forceinline__ void step_noise4(const StepParams& p, const StepScalars& s, size_t i, bool needed, float (&z)[4]) {
   z[0] = z[1] = z[2] = z[3] = 0.f;
@@ -245,162 +253,174 @@ __device__ __forceinline__ void hist_store4(const StepParams& p, size_t i, const
   if (kKind == kStepDpm) stg_f4(p.hist + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
 }
 
-// one thread = 4 consecutive pixels of one (n, c) plane
-template <int kKind>
-__global__ void __launch_bounds__(256) step_kernel(const StepParams p) {
-  const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
-  const StepScalars s = step_scalars<kKind>(p);
-  const int cfg = step_cfg(p);
-  for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
-       i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t i = i4 * 4;
-    const int plane = static_cast<int>(i / p.HW);      // n*C + c
-    const int n = plane / p.C, c = plane % p.C;
-    const size_t pix = i - static_cast<size_t>(plane) * p.HW;
-    float z[4], hp[4];
-    step_noise4(p, s, i, step_draws_noise<kKind>(s), z);
-    hist_load4<kKind>(p, s, i, hp);
-    float xo[4], x0o[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) step_element<kKind>(p, s, n, c, pix + j, p.x_t[i + j], mix_eps(p, cfg, i + j, total), z[j], hp[j], xo[j], x0o[j]);
-    stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
-    if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
-    hist_store4<kKind>(p, i, x0o);
-  }
+// ----------------------------------------------------------------------------------------------
+// The step kernel: a source (where x_0 comes from) feeding a sink (what the pass writes).  A source knows its grid-stride work
+// unit and, for each quad of the unit (four consecutive pixels of one (n, c) plane), calls f(q, load); load(xt, x0) yields the
+// quad's x_t and its guided x_0, clipped or thresholded.  Sinks call load after their loads that do not depend on it (noise,
+// history), so the inputs of x_0 do not occupy registers across the Philox draw.  step_kernel<Src, Update<kind>> is a whole
+// step; a thresholded step is step_kernel<Src, StoreX0>, threshold_select_kernel, step_kernel<ThresholdedX0, Update<kind>>.
+// All share the element arithmetic above, so every route gives the same bits.
+// ----------------------------------------------------------------------------------------------
+struct Quad {
+  size_t i;                    // flat index of the first element in [N,C,H,W] (i % 4 == 0): Philox index i >> 2
+  size_t pix;                  // its pixel in the plane
+  int n, c;
+};
+// quad u of the flattened [N,C,H,W] tensor
+__device__ __forceinline__ Quad flat_quad(const StepParams& p, size_t u) {
+  Quad q;
+  q.i = u * 4;
+  const int plane = static_cast<int>(q.i / p.HW);      // n*C + c
+  q.n = plane / p.C;
+  q.c = plane % p.C;
+  q.pix = q.i - static_cast<size_t>(plane) * p.HW;
+  return q;
 }
 
-// Output head + denoising step in ONE kernel (the last node of the forward's CUDA graph): eps of both guidance halves is formed
-// from the tap columns Y of the output head's 1x1 GEMM (the shift-and-add of eps_gather_kernel, same summation order), mixed, and
-// pushed through the DDPM / DDIM / DPM-Solver++ update without ever being written to HBM.  One thread = 4 consecutive pixels (one row segment)
-// of one sample, all Co = 4 channels; noise indices and arithmetic are those of step_kernel, so both routes agree bit for bit.
-struct HeadStepParams {
-  StepParams sp;
-  const float* Y;          // [2N or N][H][W][ldy] tap columns (tap*Co + c)
-  const float* bias;       // [Co]
-  int H, W, ldy;
-};
-__device__ __forceinline__ void head_eps4(const HeadStepParams& h, int n, int y, int x, float (&e)[4]) {
-  e[0] = e[1] = e[2] = e[3] = 0.f;
+// x_0 from the eps buffer [2N or N,C,H,W]: rows [0,N) conditional, [N,2N) unconditional when cfg == 1.  One quad per unit.
+struct EpsRows {
+  const float* eps;
+  __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * p.C * p.HW / 4; }
+  template <typename F>
+  __device__ __forceinline__ void quads(const StepParams& p, const StepCoef& k, int cfg, size_t u, F&& f) const {
+    const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
+    const Quad q = flat_quad(p, u);
+    f(q, [&](float (&xt)[4], float (&x0)[4]) {
+      float e[4];
+      mix_eps4(p, cfg, [&](bool uncond, float (&v)[4]) {
 #pragma unroll
-  for (int tap = 0; tap < 9; ++tap) {
-    const int hh = y + tap / 3 - 1, ww = x + tap % 3 - 1;
-    if (hh < 0 || hh >= h.H || ww < 0 || ww >= h.W) continue;
-    const float4 v = ldg_f4(h.Y + ((static_cast<size_t>(n) * h.H + hh) * h.W + ww) * h.ldy + tap * 4);
-    e[0] += v.x; e[1] += v.y; e[2] += v.z; e[3] += v.w;
+        for (int j = 0; j < 4; ++j) v[j] = eps[(uncond ? total : 0) + q.i + j];
+      }, e);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        xt[j] = p.x_t[q.i + j];
+        x0[j] = eps_x0(p, k, xt[j], e[j]);
+      }
+    });
   }
+};
+
+// x_0 from the tap columns Y of the output head's 1x1 GEMM: eps is the shift-and-add of eps_gather_kernel (same summation
+// order), never written to HBM.  One unit = 4 consecutive pixels (one row segment) of one sample, all Co = 4 channels: 4 quads.
+struct HeadTaps {
+  const float* Y;              // [2N or N][H][W][ldy] tap columns (tap*Co + c)
+  const float* bias;           // [Co]
+  int H, W, ldy;
+  __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * H * (W / 4); }
+  // eps of pixel (x, y) of sample n (n >= N: the unconditional half), all 4 channels
+  __device__ __forceinline__ void eps4(int n, int y, int x, float (&e)[4]) const {
+    e[0] = e[1] = e[2] = e[3] = 0.f;
 #pragma unroll
-  for (int c = 0; c < 4; ++c) e[c] += __ldg(h.bias + c);
-}
-template <int kKind>
-__global__ void __launch_bounds__(256) head_step_kernel(const HeadStepParams h) {
-  const StepParams& p = h.sp;
-  const StepScalars s = step_scalars<kKind>(p);
-  const int cfg = step_cfg(p);
-  const int w4 = h.W / 4;
-  const size_t groups = static_cast<size_t>(p.N) * h.H * w4;
-  for (size_t g = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; g < groups; g += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    for (int tap = 0; tap < 9; ++tap) {
+      const int hh = y + tap / 3 - 1, ww = x + tap % 3 - 1;
+      if (hh < 0 || hh >= H || ww < 0 || ww >= W) continue;
+      const float4 v = ldg_f4(Y + ((static_cast<size_t>(n) * H + hh) * W + ww) * ldy + tap * 4);
+      e[0] += v.x; e[1] += v.y; e[2] += v.z; e[3] += v.w;
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) e[c] += __ldg(bias + c);
+  }
+  template <typename F>
+  __device__ __forceinline__ void quads(const StepParams& p, const StepCoef& k, int cfg, size_t g, F&& f) const {
+    const int w4 = W / 4;
     const int xg = static_cast<int>(g % w4);
-    const int y = static_cast<int>((g / w4) % h.H);
-    const int n = static_cast<int>(g / (static_cast<size_t>(w4) * h.H));
+    const int y = static_cast<int>((g / w4) % H);
+    const int n = static_cast<int>(g / (static_cast<size_t>(w4) * H));
     float e[4][4];                  // [pixel][channel]
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float ec[4];
-      head_eps4(h, n, y, xg * 4 + j, ec);
-      if (cfg == 1) {
-        float eu[4];
-        head_eps4(h, n + p.N, y, xg * 4 + j, eu);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) ec[c] = cfg_mix(ec[c], eu[c], p.strength);
-      } else if (cfg == 2) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) ec[c] = __fmul_rn(__fadd_rn(1.0f, p.strength), ec[c]);
-      }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) e[j][c] = ec[c];
-    }
-    const size_t pix = static_cast<size_t>(y) * h.W + xg * 4;
+    for (int j = 0; j < 4; ++j)
+      mix_eps4(p, cfg, [&](bool uncond, float (&v)[4]) { eps4(uncond ? n + p.N : n, y, xg * 4 + j, v); }, e[j]);
+    const size_t pix = static_cast<size_t>(y) * W + xg * 4;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      const size_t i = (static_cast<size_t>(n) * 4 + c) * p.HW + pix;
-      float z[4], hp[4];
-      step_noise4(p, s, i, step_draws_noise<kKind>(s), z);
-      hist_load4<kKind>(p, s, i, hp);
-      const float4 xt = ldg_f4(p.x_t + i);
-      const float xtv[4] = {xt.x, xt.y, xt.z, xt.w};
-      float xo[4], x0o[4];
+      Quad q;
+      q.i = (static_cast<size_t>(n) * 4 + c) * p.HW + pix;
+      q.pix = pix;
+      q.n = n;
+      q.c = c;
+      f(q, [&](float (&xt)[4], float (&x0)[4]) {
+        const float4 v = ldg_f4(p.x_t + q.i);
+        xt[0] = v.x; xt[1] = v.y; xt[2] = v.z; xt[3] = v.w;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) step_element<kKind>(p, s, n, c, pix + j, xtv[j], e[j][c], z[j], hp[j], xo[j], x0o[j]);
-      stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
-      if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
-      hist_store4<kKind>(p, i, x0o);
+        for (int j = 0; j < 4; ++j) x0[j] = eps_x0(p, k, xt[j], e[j][c]);
+      });
     }
   }
+};
+
+// x_0 from a [N,C,H,W] buffer of x_0 before thresholding and s [N] from threshold_select_kernel.  One quad per unit.
+struct ThresholdedX0 {
+  const float* x0;
+  const float* s;
+  __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * p.C * p.HW / 4; }
+  template <typename F>
+  __device__ __forceinline__ void quads(const StepParams& p, const StepCoef&, int, size_t u, F&& f) const {
+    const Quad q = flat_quad(p, u);
+    const float sn = s[q.n];
+    f(q, [&](float (&xt)[4], float (&th)[4]) {
+      const float4 v = ldg_f4(x0 + q.i);
+      const float x0v[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        xt[j] = p.x_t[q.i + j];
+        th[j] = threshold_x0(x0v[j], sn);
+      }
+    });
+  }
+};
+
+// x_{t-1}, pred_x0 and the DPM-Solver++ history of a quad: the noise, the history read before it is overwritten (same thread)
+// and the replace / constrain guidance + update of step kind kKind
+template <int kKind>
+struct Update {
+  using Scalars = StepScalars;
+  __device__ __forceinline__ static StepScalars scalars(const StepParams& p) { return step_scalars<kKind>(p); }
+  template <typename Load>
+  __device__ __forceinline__ void operator()(const StepParams& p, const StepScalars& s, const Quad& q, Load&& load) const {
+    float z[4], hp[4];
+    step_noise4(p, s, q.i, step_draws_noise<kKind>(s), z);
+    hist_load4<kKind>(p, s, q.i, hp);
+    float xt[4], x0[4], xo[4], x0o[4];
+    load(xt, x0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) step_update<kKind>(p, s, q.n, q.c, q.pix + j, xt[j], x0[j], z[j], hp[j], xo[j], x0o[j]);
+    stg_f4(p.x_prev + q.i, make_float4(xo[0], xo[1], xo[2], xo[3]));
+    if (p.pred_x0) stg_f4(p.pred_x0 + q.i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
+    hist_store4<kKind>(p, q.i, x0o);
+  }
+};
+
+// x_0 of a quad into a [N,C,H,W] buffer.  x0 may be the eps buffer of an EpsRows source (rows [0,N)): each element is read
+// before it is overwritten, by the same thread, so neither pointer is __restrict__.
+struct StoreX0 {
+  float* x0;
+  struct Scalars { StepCoef k; };
+  __device__ __forceinline__ static Scalars scalars(const StepParams& p) { return {p.table[*p.t_index]}; }
+  template <typename Load>
+  __device__ __forceinline__ void operator()(const StepParams&, const Scalars&, const Quad& q, Load&& load) const {
+    float xt[4], v[4];
+    load(xt, v);
+    stg_f4(x0 + q.i, make_float4(v[0], v[1], v[2], v[3]));
+  }
+};
+
+template <typename Src, typename Sink>
+__global__ void __launch_bounds__(256) step_kernel(const StepParams p, const Src src, const Sink sink) {
+  const typename Sink::Scalars s = Sink::scalars(p);
+  const int cfg = step_cfg(p);
+  const size_t units = src.units(p);
+  for (size_t u = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; u < units; u += static_cast<size_t>(gridDim.x) * blockDim.x)
+    src.quads(p, s.k, cfg, u, [&](const Quad& q, auto&& load) { sink(p, s, q, load); });
 }
 
 // ----------------------------------------------------------------------------------------------
 // Dynamic thresholding of x_0 (Saharia et al. 2022, arXiv:2205.11487, sec. 2.3), per sample n over its M = C*H*W elements:
 //   q = the ratio-quantile of |x_0| with linear interpolation (v_k + f * (v_{k+1} - v_k), pos = ratio * (M - 1) = k + f, in
 //       double, rounded once to fp32), s = min(max(q, 1), s_max), x_0 <- clamp(x_0, -s, s) / s.
-// A step in this mode runs three kernels: x_0 before thresholding into a [N,C,H,W] buffer (head_x0_kernel on the fused route,
-// x0_kernel from eps on the separate one), threshold_select_kernel (s of every sample) and threshold_step_kernel (step_kernel's
-// update on the thresholded x_0).  Both routes share the last two, so they agree bit for bit.
+// A step in this mode runs three kernels: step_kernel<Src, StoreX0> (x_0 before thresholding into a [N,C,H,W] buffer, from
+// HeadTaps on the fused route and EpsRows on the separate one), threshold_select_kernel (s of every sample) and
+// step_kernel<ThresholdedX0, Update<kind>>.  Both routes share the last two, so they agree bit for bit.
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ float threshold_x0(float x0, float s) { return __fdiv_rn(fminf(fmaxf(x0, -s), s), s); }
-
-// x0 may be p.eps itself: each element is read before it is overwritten, by the same thread
-__global__ void __launch_bounds__(256) x0_kernel(const StepParams p, float* x0) {
-  const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
-  const StepCoef k = p.table[*p.t_index];
-  const int cfg = step_cfg(p);
-  for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
-       i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t i = i4 * 4;
-    float v[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = step_x0(k, p.x_t[i + j], mix_eps(p, cfg, i + j, total));
-    stg_f4(x0 + i, make_float4(v[0], v[1], v[2], v[3]));
-  }
-}
-
-// guidance-mixed eps of pixel (x, y) of sample n, all Co = 4 channels: the arithmetic of head_step_kernel
-__device__ __forceinline__ void head_mixed_eps4(const HeadStepParams& h, int cfg, int n, int y, int x, float (&ec)[4]) {
-  const StepParams& p = h.sp;
-  head_eps4(h, n, y, x, ec);
-  if (cfg == 1) {
-    float eu[4];
-    head_eps4(h, n + p.N, y, x, eu);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) ec[c] = cfg_mix(ec[c], eu[c], p.strength);
-  } else if (cfg == 2) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) ec[c] = __fmul_rn(__fadd_rn(1.0f, p.strength), ec[c]);
-  }
-}
-// head_step_kernel's eps, turned into x_0 and written to x0 [N,4,H,W] instead of being pushed through the update
-__global__ void __launch_bounds__(256) head_x0_kernel(const HeadStepParams h, float* __restrict__ x0) {
-  const StepParams& p = h.sp;
-  const StepCoef k = p.table[*p.t_index];
-  const int cfg = step_cfg(p);
-  const int w4 = h.W / 4;
-  const size_t groups = static_cast<size_t>(p.N) * h.H * w4;
-  for (size_t g = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; g < groups; g += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int xg = static_cast<int>(g % w4);
-    const int y = static_cast<int>((g / w4) % h.H);
-    const int n = static_cast<int>(g / (static_cast<size_t>(w4) * h.H));
-    float e[4][4];                  // [pixel][channel]
-#pragma unroll
-    for (int j = 0; j < 4; ++j) head_mixed_eps4(h, cfg, n, y, xg * 4 + j, e[j]);
-    const size_t pix = static_cast<size_t>(y) * h.W + xg * 4;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const size_t i = (static_cast<size_t>(n) * 4 + c) * p.HW + pix;
-      const float4 xt = ldg_f4(p.x_t + i);
-      stg_f4(x0 + i, make_float4(step_x0(k, xt.x, e[0][c]), step_x0(k, xt.y, e[1][c]), step_x0(k, xt.z, e[2][c]),
-                                 step_x0(k, xt.w, e[3][c])));
-    }
-  }
-}
 
 // Exact per-sample selection: one block per sample n of x [N][M] radix-selects the order statistic v_k of |x| over the fp32 bit
 // patterns (ordered like unsigned integers for non-negative floats) in three digit passes, bits 31..21, 20..10 and 9..0, each a
@@ -489,33 +509,6 @@ __global__ void __launch_bounds__(kSelectThreads) threshold_select_kernel(const 
     const double vk = __uint_as_float(prefix), vk1 = __uint_as_float(next);
     const float q = __double2float_rn(__dadd_rn(vk, __dmul_rn(f, __dsub_rn(vk1, vk))));
     s_out[blockIdx.x] = fminf(fmaxf(q, 1.0f), s_max);
-  }
-}
-
-// step_kernel's update on the thresholded x_0: x0 [N,C,H,W] before thresholding, s [N] from threshold_select_kernel
-template <int kKind>
-__global__ void __launch_bounds__(256) threshold_step_kernel(const StepParams p, const float* __restrict__ x0, const float* __restrict__ s_n) {
-  const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
-  const StepScalars s = step_scalars<kKind>(p);
-  for (size_t i4 = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i4 * 4 < total;
-       i4 += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t i = i4 * 4;
-    const int plane = static_cast<int>(i / p.HW);      // n*C + c
-    const int n = plane / p.C, c = plane % p.C;
-    const size_t pix = i - static_cast<size_t>(plane) * p.HW;
-    const float sn = s_n[n];
-    float z[4], hp[4];
-    step_noise4(p, s, i, step_draws_noise<kKind>(s), z);
-    hist_load4<kKind>(p, s, i, hp);
-    const float4 xv = ldg_f4(x0 + i);
-    const float x0v[4] = {xv.x, xv.y, xv.z, xv.w};
-    float xo[4], x0o[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      step_update<kKind>(p, s, n, c, pix + j, p.x_t[i + j], threshold_x0(x0v[j], sn), z[j], hp[j], xo[j], x0o[j]);
-    stg_f4(p.x_prev + i, make_float4(xo[0], xo[1], xo[2], xo[3]));
-    if (p.pred_x0) stg_f4(p.pred_x0 + i, make_float4(x0o[0], x0o[1], x0o[2], x0o[3]));
-    hist_store4<kKind>(p, i, x0o);
   }
 }
 

@@ -77,7 +77,7 @@ struct BlockDef { std::vector<LayerRef> layers; bool is_input = false; bool is_o
 struct Plan;
 
 // Optional replacement of the output head's last kernel (eps_gather_kernel): the sampler hands the forward a launcher that
-// consumes the tap columns Y directly (head_step_kernel: eps of both guidance halves -> mix -> x_{t-1}), so that eps never
+// consumes the tap columns Y directly (step_kernel<HeadTaps, ...>: eps of both guidance halves -> mix -> x_{t-1}), so that eps never
 // goes to HBM and the update is the last node of the forward's CUDA graph.  `key` must change whenever anything the launcher
 // bakes in (pointers, scalars) changes: it is part of the graph-cache key.
 struct HeadHook {

@@ -219,7 +219,7 @@ def test_device_route_equals_host_route(golden):
 
 
 def test_device_route_equals_host_route_separate_kernel():
-    """The separate eps_gather_kernel + step_kernel pair (IVID_NO_FUSED_STEP=1 is read once per process: a fresh one)."""
+    """The separate eps_gather_kernel + step_kernel<EpsRows, ...> pair (IVID_NO_FUSED_STEP=1 is read once per process: a fresh one)."""
     code = ("import sys, json, os; sys.path[:0] = [sys.argv[1], sys.argv[2]]\n"
             "import numpy as np, test_gpu_guidance_interval as m\n"
             "golden = {k: v for i in (0, 1) for k, v in\n"

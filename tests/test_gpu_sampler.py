@@ -150,9 +150,9 @@ def test_superres_ddim_step_vs_oracle(golden):
 
 
 def test_fused_head_step_equals_separate_step_kernel(golden):
-    """The production loop ends every forward in head_step_kernel (output-head shift-and-add + guidance mix + x_{t-1} update,
-    last node of the forward's CUDA graph); with return_trajectory=True the per-step pointers change every step and the loop
-    falls back to eps_gather_kernel + step_kernel.  Same Philox draws (same torch seed) -> the two routes must agree."""
+    """The production loop ends every forward in step_kernel<HeadTaps, Update<kind>> (output-head shift-and-add + guidance
+    mix + x_{t-1} update, last node of the forward's CUDA graph); with return_trajectory=True the per-step pointers change every
+    step and the loop falls back to eps_gather_kernel + step_kernel<EpsRows, Update<kind>>.  Same Philox draws (same torch seed) -> the two routes must agree."""
     cfg = _cfg(golden, "tiny")
     fw = frameworks.ClassifierFreeGuidance(_net(cfg, 1234), timesteps=1000, beta_schedule="linear")
     rng = np.random.default_rng(2)

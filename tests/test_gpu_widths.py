@@ -218,8 +218,9 @@ def _kernel_names(fn):
 
 
 def test_fused_head_step_at_final_width_96(wid):
-    """Final width 96 keeps the tap-column output head, so the production loop ends every forward in head_step_kernel; with
-    return_trajectory=True it takes eps_gather_kernel + step_kernel instead.  Same Philox draws -> the same bits."""
+    """Final width 96 keeps the tap-column output head, so the production loop ends every forward in
+    step_kernel<HeadTaps, Update<kind>>; with return_trajectory=True it takes eps_gather_kernel + step_kernel<EpsRows, ...>
+    instead.  Same Philox draws -> the same bits."""
     cfg = _cfg(wid, "mc96")
     fw = frameworks.ClassifierFreeGuidance(_load(cfg, unet_ref.make_synthetic_state_dict(cfg, seed=77)), timesteps=1000,
                                            beta_schedule="linear")
@@ -233,8 +234,8 @@ def test_fused_head_step_at_final_width_96(wid):
         torch.manual_seed(5)
         b, separate = _kernel_names(lambda: s.sample(2, noise=x, classes=classes, strength=0.5, verbose=False,
                                                      return_trajectory=True, **kw))
-        assert any("head_step_kernel" in n for n in fused), "the fused head step is not active at final width 96"
-        assert not any("head_step_kernel" in n for n in separate)
+        assert any("step_kernel<ivid::HeadTaps" in n for n in fused), "the fused head step is not active at final width 96"
+        assert not any("step_kernel<ivid::HeadTaps" in n for n in separate)
         assert any("eps_gather_kernel" in n for n in separate)
         G.report(f"{type(s).__name__}: fused head+step vs separate kernels at width 96", a, b.samples)
         assert torch.isfinite(a).all()

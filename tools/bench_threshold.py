@@ -6,8 +6,9 @@ as bench.py builds it; batch 16, guidance 0.5 and 3.0) and on config 5 (rgbd_ima
 
 - ms per step with and without thresholding: CUDA events around whole `sample()` calls (production path, fused route),
   DPM-Solver++ 25 steps and DDIM 50 steps, the two settings alternated, best of `repeat` rounds after a warm-up round.
-- device time of the added kernels (x_0 out of the head, selection, update) against the default head-step kernel, from
-  torch.profiler in a separate run of 5 DPM-Solver++ steps each.
+- device time of the step's kernels, from torch.profiler in a separate run of 5 DPM-Solver++ steps each: the fused head step
+  step_kernel<HeadTaps, Update<2>> without thresholding; with it step_kernel<HeadTaps, StoreX0> (x_0 out of the head),
+  threshold_select_kernel and step_kernel<ThresholdedX0, Update<2>> (the update).
 - the relative L2 distance and the largest |x| of the final samples with and without thresholding.  Diagnostic drift on random
   weights, not a statement about sample quality.
 Needs a GPU: there is no fallback."""
@@ -26,7 +27,8 @@ import ivid_b200.frameworks as frameworks         # noqa: E402
 import ivid_b200.samplers as samplers             # noqa: E402
 from oracle import unet_ref                       # noqa: E402
 
-ADDED = ("head_x0_kernel", "threshold_select_kernel", "threshold_step_kernel", "x0_kernel")
+# every instantiation of step_kernel<Source, Sink> (not set_step_kernel), and the selection of a thresholded step
+STEP_KERNELS = ("step_kernel<", "threshold_select_kernel")
 
 
 def _card():
@@ -127,7 +129,7 @@ def main():
     for th in (None, args.ratio):
         times = _profile(lambda: dpm.sample(B, noise=x_T, classes=classes, steps=5, strength=bench.GUIDANCE, verbose=False,
                                             dynamic_threshold=th), args.profile_dir)
-        sel = {k: v for k, v in times.items() if any(a in k for a in ADDED) or "head_step_kernel" in k}
+        sel = {k: v for k, v in times.items() if any(a in k for a in STEP_KERNELS)}
         prof_rows["threshold" if th else "plain"] = {k: dict(ms_total=round(v[0], 4), calls=v[1]) for k, v in sel.items()}
     print("device time, 5 DPM-Solver++ steps (torch.profiler):")
     for mode, sel in prof_rows.items():
