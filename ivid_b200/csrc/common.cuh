@@ -109,6 +109,23 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// warm L2 with a 4-D box that a later tma_load_4d reads; no shared memory or barrier involved
+__device__ __forceinline__ void tma_prefetch_l2_4d(const CUtensorMap* m, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];\n" ::"l"(reinterpret_cast<uint64_t>(m)),
+               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+// shared -> global 4-D box store; elements outside the tensor's extent are not written.  Completion through the bulk group:
+// the source must stay untouched until tma_store_wait_read, and the fence_proxy_async_smem of the writers comes first.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];\n" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+// every committed store has read its shared-memory source (the global writes may still be in flight)
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA, sm_90a): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 inputs, fp32 accumulators in registers.

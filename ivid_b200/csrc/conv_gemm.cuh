@@ -23,8 +23,10 @@
 // flight: it issues the group of k-block u, waits for group u - 1 to retire and only then releases u - 1's slot, so its
 // tensor work never stops for a refill.  Two CTAs fit one SM (BN <= 128), so one CTA's epilogue overlaps the other's main
 // loop.
-// The epilogue works on the accumulator fragments in place: bias, residual (optionally through a nearest-2x upsample),
-// fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.
+// The epilogue adds bias and residual (optionally through a nearest-2x upsample) to the accumulator fragments and writes
+// fp32 / fp16 / NCHW output, an optional fp16 copy and the per-(sample, channel) GroupNorm statistics of the output.  The
+// ring is idle by then, so it holds the staged NHWC tile (ConvGemmCfg): the residual's boxes arrive in it by TMA as extra
+// k-blocks behind the last operand loads, and the outputs leave it by TMA box stores, issued by one thread.
 //
 // Slab mode (SLAB, chosen by conv_launch_create for tiles of one sample and TW >= 8): the three taps of a 3x3 segment that
 // differ only in dy read the same pixels shifted by one image row.  So the producer loads one (TH + 2)-row activation slab
@@ -34,7 +36,7 @@
 // columns are the same as per tap.  The slabs have a ring of their own (2 slots, released after the third dy's group has
 // retired); the weight boxes keep a per-k-block ring, 4 deep.  A 1x1 segment of a slab launch puts its one box per chunk in
 // a slab slot.  Per three k-blocks a CTA takes in TW*(TH+2)*128 + 3*BN*128 bytes instead of 3*(16 KB + BN*128).  The
-// epilogue's statistics scratch lies over the ring, which is idle once both warpgroups' last groups have retired.
+// epilogue's staging and statistics scratch lie over the ring, which is idle once both warpgroups' last groups have retired.
 //
 // fp8 operand mode (A8): segment 0 is e4m3.  Its 128-byte box row is 128 channels, so an e4m3 k-block has exactly the
 // shared-memory layout, TMA bytes and wgmma descriptors of an fp16 one; only the instruction differs (k32 e4m3 for k16
@@ -73,6 +75,9 @@ struct ConvGemmParams {
 struct ConvMaps {
   CUtensorMap a[3];            // activation segments (fp16 NHWC)
   CUtensorMap b;               // packed weights
+  CUtensorMap r;               // fp32 residual, box (F32_CH, TW, TH, TN); under res_up the half-size source tile
+  CUtensorMap o;               // fp32 NHWC output, box (F32_CH, TW, TH, TN)
+  CUtensorMap o16;             // fp16 NHWC output or copy, box (F16_CH, TW, TH, TN)
 };
 // the A8 kernels' maps: also the e4m3 weight columns of segment 0
 struct ConvMaps8 : ConvMaps {
@@ -99,6 +104,25 @@ struct ConvGemmCfg {
   static constexpr int SMEM_BYTES = RING_BYTES + BAR_BYTES + (STATS_ON_RING ? 0 : STAT_BYTES) + 1024;   // +1024 alignment slack
   static constexpr int CONSUMER_THREADS = 256;                 // two warpgroups: MMA and epilogue
   static constexpr int THREADS = CONSUMER_THREADS + 32;        // + one producer warp: TMA loads
+
+  // Epilogue staging over the idle ring.  The fp32 tile is UNITS units of UNIT_BOXES boxes (F32_CH channels x 128 pixels,
+  // one F32_CH * 4-byte row per pixel, swizzled over that row); the residual's units arrive as k-blocks nunits, nunits + 1,
+  // ... in the slots those take.  SLAB: a unit is a weight slot (F32_CH = BN / 4) and there are STAGES of them, so unit q
+  // is the one k-block nunits + i with (nunits + i) % STAGES == q brings into slot q; the fp16 tile and the statistics
+  // lie over the slab slots.  Per tap: unit u is the front of stage (nunits + u) % STAGES, and the fp16 tile fills stage
+  // (nunits + UNITS) % STAGES.
+  static constexpr int F32_CH = SLAB ? BN / 4 : (BN < 32 ? BN : 32);
+  static constexpr int F32_BOX = BM * F32_CH * 4;
+  static constexpr int UNIT_BOXES = !SLAB && BN == 128 ? 2 : 1;
+  static constexpr int UNIT_CH = F32_CH * UNIT_BOXES;
+  static constexpr int UNITS = BN / UNIT_CH;
+  static constexpr int UNIT_STRIDE = SLAB ? B_BYTES : STAGE_BYTES;
+  static constexpr int F16_CH = BN < 64 ? BN : 64;             // fp16 tile: BN / F16_CH boxes of F16_CH channels
+  static constexpr int F16_BOX = BM * F16_CH * 2;
+  static constexpr int F16_TILE = BM * BN * 2;
+  static_assert(UNIT_BOXES * F32_BOX <= UNIT_STRIDE, "an fp32 unit must fit its ring slot");
+  static_assert(SLAB ? UNITS == STAGES : UNITS < STAGES && F16_TILE <= STAGE_BYTES, "fp32 units and the fp16 tile must fit the ring");
+  static_assert(!SLAB || F16_TILE + STAT_BYTES <= SLAB_STAGES * SLAB_BYTES, "the fp16 tile and statistics must fit the slab slots");
 };
 
 // position in the K loop: segment, tap, 64-channel chunk, and the first packed weight column of the segment
@@ -121,7 +145,7 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* slab_full = empty_bar + STAGES;      // SLAB only
   uint64_t* slab_empty = slab_full + SLAB_STAGES;
-  float* stat_smem = reinterpret_cast<float*>(Cfg::STATS_ON_RING ? smem : smem + Cfg::RING_BYTES + Cfg::BAR_BYTES);
+  float* stat_smem = reinterpret_cast<float*>(Cfg::STATS_ON_RING ? smem + Cfg::F16_TILE : smem + Cfg::RING_BYTES + Cfg::BAR_BYTES);
   uint8_t* const slab_ring = smem;               // SLAB: [SLAB_STAGES][SLAB_BYTES], then [STAGES][B_BYTES] weight boxes
   uint8_t* const w_ring = smem + SLAB_STAGES * Cfg::SLAB_BYTES;
 
@@ -157,13 +181,21 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
   const int th = rem / p.tiles_w;
   const int tw = rem - th * p.tiles_w;
   const int n0 = tn * p.TN, h0 = th * p.TH, w0 = tw * p.TW;
+  uint8_t* const unit_ring = SLAB ? w_ring : smem;                  // the epilogue's fp32 units
 
   // ===================================== producer warp =====================================
   if (warp == Cfg::CONSUMER_THREADS / 32) {
     if (lane == 0) {
+      // residual box origin: under res_up the nearest-2x source tile at half the coordinates
+      const int rw0 = p.res_up ? w0 >> 1 : w0, rh0 = p.res_up ? h0 >> 1 : h0;
       tma_prefetch_desc(&maps.a[0]);
       tma_prefetch_desc(&maps.b);
       if constexpr (A8) tma_prefetch_desc(&maps.b8);
+      // the residual is read only after the main loop: start it towards L2 now
+      if (p.residual != nullptr) {
+#pragma unroll
+        for (int q = 0; q < Cfg::UNITS * Cfg::UNIT_BOXES; ++q) tma_prefetch_l2_4d(&maps.r, colbase + q * Cfg::F32_CH, rw0, rh0, n0);
+      }
       if constexpr (SLAB) {
         // per segment: chunk slow, dx, dy fast (3x3: one slab per (chunk, dx)); 1x1: one box per chunk
         const uint32_t slab_bytes = static_cast<uint32_t>(p.TW * (p.TH + 2)) * 128u;
@@ -231,6 +263,23 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
             if (++c.t == taps) { c.t = 0; if (!A8 || c.seg != 0) c.base += taps * chunks * 64; ++c.seg; }
           }
           while (c.seg < 3 && p.seg_chunks[c.seg] == 0) ++c.seg;
+        }
+      }
+      // the residual's units as k-blocks nunits, nunits + 1, ...: each goes into its slot as soon as the main loop
+      // releases it, so only the last units can arrive after the last wgmma group
+      if (p.residual != nullptr) {
+        const uint32_t bytes = static_cast<uint32_t>(Cfg::UNIT_BOXES * Cfg::F32_BOX) >> (p.res_up ? 2 : 0);
+#pragma unroll 1
+        for (int i = 0; i < Cfg::UNITS; ++i) {
+          const uint32_t g = static_cast<uint32_t>(nunits + i);
+          const int s = static_cast<int>(g % STAGES);
+          const int q = SLAB ? s : i;            // SLAB: every slot holds a unit, so unit q stays in slot q
+          if (g >= STAGES) mbar_wait(&empty_bar[s], ((g / STAGES) - 1) & 1);
+          mbar_arrive_expect_tx(&full_bar[s], bytes);
+#pragma unroll
+          for (int k = 0; k < Cfg::UNIT_BOXES; ++k)
+            tma_load_4d(&maps.r, &full_bar[s], unit_ring + s * Cfg::UNIT_STRIDE + k * Cfg::F32_BOX,
+                        colbase + q * Cfg::UNIT_CH + k * Cfg::F32_CH, rw0, rh0, n0);
         }
       }
     }
@@ -314,60 +363,127 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
   }
 
   // ===================================== epilogue =====================================
+  // Every NHWC value is staged in shared memory (Cfg: fp32 units over the ring, the fp16 tile beside them) and leaves by
+  // TMA box stores, which clip at the tensor's extent: the batch tail (n >= N) and the padded columns past Cout are never
+  // written.  NCHW (out_mode 2) keeps direct stores.
   const int wr = warp & 3;
   const int quad = lane & 3;
-  // 32-bit pixel indices (conv_launch_create requires N*H*W < 2^31): with the producer warp in the CTA, two CTAs per SM
-  // leave 96 registers per thread, and the 64 accumulators plus 64-bit row coordinates would spill
-  uint32_t pix[2], rpix[2];                      // output pixel, residual pixel (the 2x-upsample source under res_up)
+  // Staged addresses are 32-bit shared-window offsets: with the producer warp in the CTA, two CTAs per SM leave 96
+  // registers per thread, and the 64 accumulators plus 64-bit addresses would spill.  A box row of RB bytes is swizzled by
+  // XOR-ing (row bits) << 4 into its 16-byte chunk index, and the column's byte offset shares no bits with the row's
+  // offset, so an element's offset is (row base ^ row swizzle ^ thread column) ^ (column group's bytes).
+  constexpr int RB32 = Cfg::F32_CH * 4, RB16 = Cfg::F16_CH * 2;
+  const uint32_t s_res = static_cast<uint32_t>(nunits) % STAGES;   // per tap: the stage of unit 0
+  auto row_base = [](uint32_t r, int rb) {
+    const uint32_t m = rb >= 128 ? 7u : rb == 64 ? 3u : rb == 32 ? 1u : 0u;
+    return r * rb ^ ((((r * rb) >> 7) & m) << 4);
+  };
+  const uint32_t units_u32 = smem_u32(unit_ring);
+  auto unit_at = [&](int u) { return units_u32 + (SLAB ? u : (s_res + u) % STAGES) * Cfg::UNIT_STRIDE; };
+  // column group j (8 channels) of the thread's pair: unit, box in the unit and the group's bytes in the row
+  auto f32_at = [&](int j, uint32_t t) {
+    if constexpr (Cfg::F32_CH >= 8) {
+      const int cl = 8 * j;
+      return unit_at(cl / Cfg::UNIT_CH) + (cl % Cfg::UNIT_CH) / Cfg::F32_CH * Cfg::F32_BOX + (t ^ (cl % Cfg::F32_CH) * 4);
+    } else {                                     // 4-channel units (SLAB, BN 16): the pair's unit depends on quad
+      return unit_at(2 * j + (quad >> 1)) + t;
+    }
+  };
+  const int rows_per_n = p.TW * p.TH;
   bool ok[2];
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
-    const int n = n0 + row / (p.TW * p.TH), h = h0 + (row / p.TW) % p.TH, x = w0 + row % p.TW;
-    ok[i] = n < p.N;                             // rows of the batch tail (TMA zero fill) are not written
-    pix[i] = (static_cast<uint32_t>(n) * p.H + h) * p.W + x;
-    rpix[i] = p.res_up ? (static_cast<uint32_t>(n) * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (x >> 1) : pix[i];
+  for (int i = 0; i < 2; ++i) ok[i] = n0 + (wg * 64 + wr * 16 + (lane >> 2) + 8 * i) / rows_per_n < p.N;
+
+  // bias and residual, into the accumulators
+  if (p.residual != nullptr) {
+#pragma unroll 1
+    for (int q = 0; q < Cfg::UNITS; ++q) {
+      const uint32_t g = static_cast<uint32_t>(nunits + q);
+      mbar_wait(&full_bar[g % STAGES], (g / STAGES) & 1);
+    }
   }
-  const bool do_stats = p.stats != nullptr;
-  // scratch over the ring: both warpgroups' wgmma have retired (every TMA write landed before its group was issued)
-  if constexpr (Cfg::STATS_ON_RING) {
-    if (do_stats) asm volatile("bar.sync 1, %0;\n" ::"n"(Cfg::CONSUMER_THREADS) : "memory");
-  }
+  {
+    uint32_t tr[2];                              // residual box row (under res_up the 2x-upsample source row)
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int c = colbase + 8 * j + 2 * quad;    // this thread's column pair
-    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-    if (c < p.Cout) {
-      const float2 b = make_float2(__ldg(p.bias + c), __ldg(p.bias + c + 1));
+    for (int i = 0; i < 2; ++i) {
+      const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
+      const int nl = row / rows_per_n, hl = (row / p.TW) % p.TH, xl = row % p.TW;
+      const uint32_t rr = p.res_up ? (nl * (p.TH >> 1) + (hl >> 1)) * (p.TW >> 1) + (xl >> 1) : row;
+      tr[i] = row_base(rr, RB32) ^ ((8 * quad) % RB32);
+    }
+    const float* bias = p.bias + colbase + 2 * quad;   // columns < Cout_pad, the bias' extent
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const float2 b = make_float2(__ldg(bias + 8 * j), __ldg(bias + 8 * j + 1));
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        if (!ok[i]) continue;
         float v0, v1;
         if (A8) {
           v0 = fmaf(acc[4 * j + 2 * i], p.acc_scale, b.x); v1 = fmaf(acc[4 * j + 2 * i + 1], p.acc_scale, b.y);
         } else {
           v0 = acc[4 * j + 2 * i] + b.x; v1 = acc[4 * j + 2 * i + 1] + b.y;
         }
-        if (p.out_mode == 2) {
-          const uint32_t hw = static_cast<uint32_t>(p.H) * p.W, n = pix[i] / hw;
-          float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(n) * p.Cout + c) * hw + (pix[i] - n * hw);
-          o[0] = v0;
-          if (c + 1 < p.Cout) o[hw] = v1;
-          continue;
-        }
         if (p.residual != nullptr) {
-          const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + static_cast<size_t>(rpix[i]) * p.ldr + c));
-          v0 += r.x; v1 += r.y;
+          float r0, r1;
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];\n" : "=f"(r0), "=f"(r1) : "r"(f32_at(j, tr[i])) : "memory");
+          v0 += r0; v1 += r1;
         }
-        if (p.out_mode == 0) {
-          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + static_cast<size_t>(pix[i]) * p.ldc + c) = make_float2(v0, v1);
-          if (p.out16 != nullptr) *reinterpret_cast<uint32_t*>(p.out16 + static_cast<size_t>(pix[i]) * p.ldc + c) = pack_h2(v0, v1);
-        } else {
-          const __half2 hv = __floats2half2_rn(v0, v1);
-          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + static_cast<size_t>(pix[i]) * p.ldc + c) = hv;
-          const float2 r = __half22float2(hv);
-          v0 = r.x; v1 = r.y;
-        }
+        acc[4 * j + 2 * i] = v0; acc[4 * j + 2 * i + 1] = v1;
+      }
+    }
+  }
+
+  if (p.out_mode == 2) {                         // NCHW: planes of Cout channels, no statistics
+    const uint32_t hw = static_cast<uint32_t>(p.H) * p.W;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if (!ok[i]) continue;
+      const int row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
+      const int nl = row / rows_per_n, hl = (row / p.TW) % p.TH, xl = row % p.TW;
+      float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(n0 + nl) * p.Cout + colbase + 2 * quad) * hw +
+                 static_cast<uint32_t>(h0 + hl) * p.W + (w0 + xl);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j, o += 8 * static_cast<size_t>(hw)) {
+        const int c = colbase + 8 * j + 2 * quad;
+        if (c >= p.Cout) continue;
+        o[0] = acc[4 * j + 2 * i];
+        if (c + 1 < p.Cout) o[hw] = acc[4 * j + 2 * i + 1];
+      }
+    }
+    return;
+  }
+  // both warpgroups' last groups have retired (the staging overwrites their operands), and every residual element has been
+  // read (under res_up the outputs overwrite source rows that other threads read)
+  asm volatile("bar.sync 1, %0;\n" ::"n"(Cfg::CONSUMER_THREADS) : "memory");
+
+  const uint32_t f16_u32 = SLAB ? smem_u32(slab_ring) : smem_u32(smem) + ((s_res + Cfg::UNITS) % STAGES) * Cfg::STAGE_BYTES;
+  uint32_t t32[2], t16[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const uint32_t row = wg * 64 + wr * 16 + (lane >> 2) + 8 * i;
+    t32[i] = row_base(row, RB32) ^ ((8 * quad) % RB32);
+    t16[i] = row_base(row, RB16) ^ (4 * quad);
+  }
+  const bool do_stats = p.stats != nullptr;
+  const int c_left = p.Cout - (colbase + 2 * quad);           // column 8j + 2 quad of the tile is valid while 8j < c_left
+  const uint32_t st_u32 = smem_u32(stat_smem) + (warp * 2 * BN + 2 * quad) * 4;   // [warp][sum|sumsq][column]
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+      const uint32_t a16 = f16_u32 + (8 * j) / Cfg::F16_CH * Cfg::F16_BOX + (t16[i] ^ ((8 * j) % Cfg::F16_CH) * 2);
+      if (p.out_mode == 0) {
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(f32_at(j, t32[i])), "f"(v0), "f"(v1) : "memory");
+        if (p.out16 != nullptr) asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(a16), "r"(pack_h2(v0, v1)) : "memory");
+      } else {
+        const __half2 hv = __floats2half2_rn(v0, v1);
+        asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(a16), "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
+        const float2 r = __half22float2(hv);
+        v0 = r.x; v1 = r.y;
+      }
+      if (ok[i] && 8 * j < c_left) {
         s0 += v0; s1 += v1;
         q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
       }
@@ -382,17 +498,38 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
         q1 += __shfl_xor_sync(0xffffffffu, q1, off);
       }
       if (lane < 4) {
-        float* st = stat_smem + warp * 2 * BN + 8 * j + 2 * quad;
-        st[0] = s0; st[1] = s1; st[BN] = q0; st[BN + 1] = q1;
+        const uint32_t st = st_u32 + 32 * j;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(st), "f"(s0), "f"(s1) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(st + 4 * BN), "f"(q0), "f"(q1) : "memory");
       }
     }
+  }
+  // the staged tile (and the statistics scratch) is complete: one thread hands the boxes to TMA
+  fence_proxy_async_smem();
+  asm volatile("bar.sync 1, %0;\n" ::"n"(Cfg::CONSUMER_THREADS) : "memory");
+  if (tid == 0) {
+    if (p.out_mode == 0) {
+#pragma unroll
+      for (int q = 0; q < Cfg::UNITS * Cfg::UNIT_BOXES; ++q) {
+        const int u = q / Cfg::UNIT_BOXES, k = q % Cfg::UNIT_BOXES;
+        const int col = colbase + q * Cfg::F32_CH;
+        if (col < p.Cout)
+          tma_store_4d(&maps.o, unit_ring + (SLAB ? u : (s_res + u) % STAGES) * Cfg::UNIT_STRIDE + k * Cfg::F32_BOX, col, w0, h0, n0);
+      }
+    }
+    if (p.out_mode == 1 || p.out16 != nullptr) {
+#pragma unroll
+      for (int q = 0; q < BN / Cfg::F16_CH; ++q) {
+        const int col = colbase + q * Cfg::F16_CH;
+        if (col < p.Cout) tma_store_4d(&maps.o16, (SLAB ? slab_ring : smem + ((s_res + Cfg::UNITS) % STAGES) * Cfg::STAGE_BYTES) + q * Cfg::F16_BOX, col, w0, h0, n0);
+      }
+    }
+    tma_store_commit();
   }
   if (do_stats) {
     // a warp's 16 rows belong to one sample (TW*TH >= 32); the warps of each sample are combined in a fixed order, so the
     // statistics are reproducible bit for bit, and one fp64 atomic pair per (sample, channel) and tile goes to global memory.
-    // Named barrier 1 over the consumer warps only: the producer warp has exited.
-    asm volatile("bar.sync 1, %0;\n" ::"n"(Cfg::CONSUMER_THREADS) : "memory");
-    const int rows_per_n = p.TW * p.TH;
+    // They run while the stores are in flight.
     const int n_tile = (128 + rows_per_n - 1) / rows_per_n;
     for (int e = tid; e < n_tile * BN; e += Cfg::CONSUMER_THREADS) {
       const int sn = e / BN, c = e - sn * BN;
@@ -409,6 +546,8 @@ conv_gemm_kernel(const __grid_constant__ std::conditional_t<A8, ConvMaps8, ConvM
       atomicAdd(st + 1, static_cast<double>(qsum));
     }
   }
+  // the shared memory the stores read must outlive them
+  if (tid == 0) tma_store_wait_read();
 }
 
 }  // namespace ivid

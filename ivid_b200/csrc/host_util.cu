@@ -46,17 +46,26 @@ CUtensorMap make_tensor_map(CUtensorMapDataType dtype, int rank, void* base, con
   return m;
 }
 
-static uint64_t elem_bytes(CUtensorMapDataType dtype) { return dtype == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 2; }
+static uint64_t elem_bytes(CUtensorMapDataType dtype) {
+  return dtype == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : dtype == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2;
+}
 
-CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN, CUtensorMapDataType dtype) {
+CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN, CUtensorMapDataType dtype,
+                         int pitch, int box_c) {
   const uint64_t es = elem_bytes(dtype);
+  const uint64_t ld = static_cast<uint64_t>(pitch > 0 ? pitch : C);
+  if (box_c <= 0) box_c = static_cast<int>(128 / es);
   const uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(W), static_cast<uint64_t>(H),
                             static_cast<uint64_t>(N)};
-  const uint64_t str[3] = {static_cast<uint64_t>(C) * es, static_cast<uint64_t>(W) * C * es,
-                           static_cast<uint64_t>(H) * W * C * es};
-  const uint32_t box[4] = {static_cast<uint32_t>(128 / es), static_cast<uint32_t>(TW), static_cast<uint32_t>(TH),
+  const uint64_t str[3] = {ld * es, static_cast<uint64_t>(W) * ld * es, static_cast<uint64_t>(H) * W * ld * es};
+  const uint32_t box[4] = {static_cast<uint32_t>(box_c), static_cast<uint32_t>(TW), static_cast<uint32_t>(TH),
                            static_cast<uint32_t>(TN)};
-  return make_tensor_map(dtype, 4, const_cast<void*>(base), dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  const uint64_t row = static_cast<uint64_t>(box_c) * es;
+  const CUtensorMapSwizzle sw = row == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                : row == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                : row == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                            : CU_TENSOR_MAP_SWIZZLE_NONE;
+  return make_tensor_map(dtype, 4, const_cast<void*>(base), dims, str, box, sw);
 }
 
 CUtensorMap make_weight_map(const void* base, int rows, int K, int box_rows, CUtensorMapDataType dtype) {

@@ -41,10 +41,11 @@ CUtensorMap make_tensor_map(CUtensorMapDataType dtype, int rank, void* base, con
                             const uint64_t* strides_bytes /* rank-1 entries, dim0 is dense */, const uint32_t* box,
                             CUtensorMapSwizzle swizzle);
 
-// NHWC activation [N][H][W][C] viewed as (C, W, H, N); box = (128 bytes of channels, TW, TH, TN), 128B swizzle.  dtype
-// FLOAT16 (64-channel box) or UINT8 (e4m3 operands, 128-channel box).
+// NHWC activation [N][H][W][pitch] viewed as (C, W, H, N), C <= pitch (0: pitch = C); box = (box_c channels, TW, TH, TN),
+// box_c 0 meaning 128 bytes of channels.  The swizzle spans the box row: 128, 64 or 32 bytes, none at 16.  dtype FLOAT16
+// (64-channel box), UINT8 (e4m3 operands, 128-channel box) or FLOAT32 (the conv epilogue's residual and outputs).
 CUtensorMap make_act_map(const void* base, int N, int H, int W, int C, int TW, int TH, int TN,
-                         CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+                         CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16, int pitch = 0, int box_c = 0);
 // weight matrix [rows][K] (K contiguous); box = (128 bytes of K, box_rows), 128B swizzle; dtype as for make_act_map.
 CUtensorMap make_weight_map(const void* base, int rows, int K, int box_rows,
                             CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);

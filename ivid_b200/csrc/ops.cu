@@ -58,7 +58,7 @@ int conv_pick_bn(int cout_pad) {
 
 // The epilogue writes channel pairs (c, c + 1) under c < Cout: an NHWC output of Cout % 8 == 0 channels (the 16-byte row
 // pitch of the fp16 tensors that TMA reads next) keeps every pair inside the row and every 4- / 8-byte access aligned.
-bool conv_can_res_up(int W, int cout) { return W >= 16 && cout % 8 == 0; }
+bool conv_can_res_up(int W, int cout) { return W >= 16 && W % 2 == 0 && cout % 8 == 0; }
 bool conv_can_out16(int cout) { return cout % 8 == 0; }
 int conv_pad_k(int c) { return ((c + 63) / 64) * 64; }
 int conv_pad_k8(int c) { return ((c + 127) / 128) * 128; }
@@ -112,6 +112,19 @@ ConvPack conv_pack(const float* w, const float* b, int cout, int cin, int ksz, i
   return pk;
 }
 
+template <int BN, bool SLAB>
+static void epilogue_box_channels(int* f32_ch, int* f16_ch) {
+  *f32_ch = ConvGemmCfg<BN, SLAB>::F32_CH;
+  *f16_ch = ConvGemmCfg<BN, SLAB>::F16_CH;
+}
+static void epilogue_box_channels(int BN, bool slab, int* f32_ch, int* f16_ch) {
+  switch (BN) {
+    case 128: slab ? epilogue_box_channels<128, true>(f32_ch, f16_ch) : epilogue_box_channels<128, false>(f32_ch, f16_ch); break;
+    case 64: slab ? epilogue_box_channels<64, true>(f32_ch, f16_ch) : epilogue_box_channels<64, false>(f32_ch, f16_ch); break;
+    default: slab ? epilogue_box_channels<16, true>(f32_ch, f16_ch) : epilogue_box_channels<16, false>(f32_ch, f16_ch); break;
+  }
+}
+
 ConvLaunch* conv_launch_create(const ConvDesc& d) {
   IVID_REQUIRE(d.C0 > 0 && d.C0 % 8 == 0, "conv: segment-0 channels must be a positive multiple of 8");
   IVID_REQUIRE(d.C1 % 8 == 0, "conv: segment-1 channels must be a multiple of 8");
@@ -147,12 +160,17 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   p.stats = (d.stats != nullptr && conv_can_fuse_stats(d.H, d.W) && d.out_mode != 2) ? d.stats : nullptr;
   IVID_REQUIRE(d.stats == nullptr || p.stats != nullptr, "conv: fused statistics need >= 32 pixels per sample per warp");
   IVID_REQUIRE(d.out_mode == 2 || (d.cout % 8 == 0 && d.ldc % 8 == 0), "conv: NHWC output needs Cout % 8 == 0");
-  IVID_REQUIRE(d.residual == nullptr || (d.out_mode != 2 && d.ldr % 2 == 0), "conv: residual needs an NHWC output and an even row pitch");
+  IVID_REQUIRE(d.residual == nullptr || (d.out_mode != 2 && d.ldr % 4 == 0 && d.ldr >= d.cout),
+               "conv: residual needs an NHWC output and a row pitch of >= Cout, a multiple of 4 elements");
   p.res_up = 0;
   if (d.residual != nullptr && d.residual_up) {
-    IVID_REQUIRE(conv_can_res_up(d.W, d.cout) && d.H % 2 == 0, "conv: upsampled residual needs W >= 16 and Cout % 8 == 0");
+    IVID_REQUIRE(conv_can_res_up(d.W, d.cout) && d.H % 2 == 0, "conv: upsampled residual needs an even W >= 16 and Cout % 8 == 0");
     p.res_up = 1;
   }
+  // the epilogue's TMA boxes: 16-byte aligned tensors
+  auto aligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
+  IVID_REQUIRE(d.out_mode == 2 || (aligned(d.out) && aligned(d.out16) && aligned(d.residual)),
+               "conv: NHWC output, fp16 copy and residual must be 16-byte aligned");
   p.out16 = nullptr;
   if (d.out16 != nullptr) {
     IVID_REQUIRE(d.out_mode == 0 && conv_can_out16(d.cout), "conv: fp16 output copy needs an fp32 NHWC output and Cout % 8 == 0");
@@ -175,6 +193,18 @@ ConvLaunch* conv_launch_create(const ConvDesc& d) {
   } else {
     M.b = make_weight_map(d.weight, d.cout_pad, Ktot, l->BN);
   }
+  // epilogue: fp32 boxes of F32_CH channels and fp16 boxes of F16_CH, as the kernel stages them (ConvGemmCfg)
+  int f32_ch = 0, f16_ch = 0;
+  epilogue_box_channels(l->BN, l->slab, &f32_ch, &f16_ch);
+  const auto f32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  M.r = M.o = M.o16 = M.a[0];                                     // placeholders of the maps a launch does not read
+  if (d.residual != nullptr) {
+    const int up = p.res_up ? 1 : 0;
+    M.r = make_act_map(d.residual, d.N, d.H >> up, d.W >> up, d.cout, p.TW >> up, p.TH >> up, p.TN, f32, d.ldr, f32_ch);
+  }
+  if (d.out_mode == 0) M.o = make_act_map(d.out, d.N, d.H, d.W, d.cout, p.TW, p.TH, p.TN, f32, d.ldc, f32_ch);
+  const void* o16 = d.out_mode == 1 ? d.out : d.out_mode == 0 ? d.out16 : nullptr;
+  if (o16 != nullptr) M.o16 = make_act_map(o16, d.N, d.H, d.W, d.cout, p.TW, p.TH, p.TN, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, d.ldc, f16_ch);
   l->grid = p.tiles_w * p.tiles_h * p.tiles_n * p.n_blocks;     // one CTA per (pixel tile, column block)
   return l;
 }
@@ -202,6 +232,7 @@ static void run_conv_bn(const ConvLaunch* l, cudaStream_t s) {
   }
 }
 void conv_launch_run_out(const ConvLaunch* l, void* out, cudaStream_t s) {
+  IVID_REQUIRE(l->p.out_mode == 2, "internal: only an NCHW conv output is patched at run time (NHWC outputs are in tensor maps)");
   ConvLaunch tmp = *l;
   tmp.p.out = out;
   conv_launch_run(&tmp, s);
