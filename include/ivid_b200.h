@@ -220,6 +220,37 @@ typedef struct {
   int cache_interval;
   int cache_branch;
   int cache_reuse;
+  /* UniPC (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework for Fast Sampling of Diffusion Models",
+   * arXiv:2302.04867; data prediction, B(h) = e^h - 1, "bh2"), a variant of kind 2 selected by unipc = 1; zero keeps
+   * DPM-Solver++.  Same time grid, alpha, sigma, lambda and guided D0 as kind 2.  For one stage from s (data prediction m0 at
+   * s, history D_{-j} at t_j) to p:
+   *   h = lambda_p - lambda_s, hh = -h, phi1 = B = expm1(hh), r_j = (lambda_{t_j} - lambda_s) / h, Delta_j = (D_{-j} - m0) / r_j,
+   *   g_1 = phi1 / hh - 1, g_{k+1} = g_k / hh - 1/(k+1)!, b_k = g_k * k! / B, R[k][j] = r_j^k (last column r = 1).
+   *   Predictor UniP of order q (m0 = D0, history D_{-1} .. D_{-(q-1)}):
+   *     x_p = (sigma_p / sigma_s) x_s - alpha_p phi1 D0 - alpha_p B sum_j rho_j Delta_j,
+   *     q = 1: no sum; q = 2: rho = [1/2]; q = 3: R[:2,:2] rho = b[:2].  At q <= 2 this is the DPM-Solver++ update.
+   *   Corrector UniC of order q_c, at step i once the network has returned D_i at the predicted x_i: from s = t_{i-1}, base =
+   *   the corrected x at t_{i-1}, m0 = D_{i-1}, history D_{i-2} ..., q_c = the previous step's predictor order:
+   *     x_i^c = (sigma_i / sigma_s) base - alpha_i phi1 D_{i-1} - alpha_i B (sum_{j<q_c} rho^c_j Delta_j + rho^c_{q_c} (D_i - D_{i-1})),
+   *     q_c = 1: rho^c = [1/2]; otherwise R[:q_c,:q_c] rho^c = b[:q_c].
+   * A step corrects x_i to x_i^c, then predicts from x_i^c with D_i; the network always sees the uncorrected predictor output,
+   * so the corrector costs no network evaluation.  Step i of ivid_sampler_run (0-based) predicts at order min(order, i + 1)
+   * and corrects at the previous step's order; the first step has no corrector; the final step to t_prev = 0 is first order
+   * and returns D0.  The single-step entry points take the history newest first: prev_x0_dev / t_last, prev2_x0_dev /
+   * t_last2, prev3_x0_dev / t_last3 (each needs the one before it; T >= t_last3 > t_last2 > t_last > t) and the base
+   * prev_xt_dev, required with prev_x0_dev.  With n of them given (at most order), the step corrects at order min(order, n)
+   * (n >= 1) and predicts at order min(order, n + 1).  ivid_sampler_step_dev uses the longest prefix whose times lie above t.
+   * The history is copied into the sampler before the step.  pred_x0_dev receives D0, x_prev_dev the predictor output and
+   * corrected_xt_dev (optional) x_i^c, the base of the next step (x_t itself on a step without corrector).
+   * IVID_ERR_INVALID_ARGUMENT: unipc other than 0 / 1, unipc = 1 with a kind other than 2 or with sde = 1, order outside
+   * 1..3, history times out of order or range, prev_xt_dev missing. */
+  int unipc;
+  const float* prev2_x0_dev;
+  int t_last2;
+  const float* prev3_x0_dev;
+  int t_last3;
+  const float* prev_xt_dev;
+  float* corrected_xt_dev;
   /* Dynamic thresholding of x0 (Saharia et al. 2022, "Imagen", arXiv:2205.11487, sec. 2.3), every kind; zero means off.
    * For every sample n, after the classifier-free guidance mix and x0 = sqrt(1/acp) * x_t - sqrt(1/acp - 1) * eps, where
    * clip_denoised would clamp it:

@@ -64,6 +64,13 @@ class StepArgsT(Structure):
         ("cache_interval", c_int),    # ivid_sampler_run: a full forward every cache_interval steps, reuse forwards between
         ("cache_branch", c_int),      # branch b of the reuse forwards, 0 <= b <= num_res_blocks
         ("cache_reuse", c_int),       # single step: 1 = this step's forward is a reuse forward
+        ("unipc", c_int),             # kind 2: 1 = the UniPC predictor-corrector update (order 1..3)
+        ("prev2_x0_dev", c_void_p),   # UniPC, single step: the older history D_{-2} / D_{-3} and their t
+        ("t_last2", c_int),
+        ("prev3_x0_dev", c_void_p),
+        ("t_last3", c_int),
+        ("prev_xt_dev", c_void_p),    # UniPC, single step: the corrector's base, the corrected x at t_last
+        ("corrected_xt_dev", c_void_p),  # UniPC, optional output: this step's corrected x_t
         ("dynamic_threshold", c_int), # 1: threshold x_0 at the threshold_ratio-quantile of |x_0| of each sample
         ("threshold_ratio", c_double),
         ("threshold_max", c_double),  # upper bound of the threshold; <= 0 = none

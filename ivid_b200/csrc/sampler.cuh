@@ -1,10 +1,11 @@
-// Fused denoising-step kernels: classifier-free-guidance mix + DDPM / DDIM / DPM-Solver++(2M) update (+ multiview
+// Fused denoising-step kernels: classifier-free-guidance mix + DDPM / DDIM / DPM-Solver++(2M) / UniPC update (+ multiview
 // replace/constrain guidance) in ONE HBM pass over [N,4,H,W], coefficients read from a device-resident table and step
 // state (no per-step H2D).
 //   reference: ClassifierFreeGuidance.model_inference classifier_free_guidance.py:39-42
 //              DdpmSampler.p_mean_variance / sample_once   samplers/ddpm.py:85-100,127-131
 //              DdimSampler.sample_once                      samplers/ddim.py:81-103
 //              DPM-Solver++(2M), data-prediction multistep  Lu et al. 2022, arXiv:2211.01095 (no reference counterpart)
+//              UniPC, bh2 predictor-corrector               Zhao et al. 2023, arXiv:2302.04867 (no reference counterpart)
 //              InpaintCFG.make_cond_inputs                  frameworks/inpaint_cfg.py:33-49
 //              SuperResCFG.make_cond_inputs                 frameworks/sr_cfg.py:31-36
 #pragma once
@@ -73,6 +74,20 @@ struct DpmStep {
   float w0, w1;                // 1 + 1/(2r), -1/(2r)
   int order;                   // 1 or 2
   float c_z;                   // ODE: 0;                             SDE: sigma_p * sqrt(1 - exp(-2h)), 0 on the final step
+};
+
+// UniPC per-step coefficients (include/ivid_b200.h), computed in double by the step-state kernel and rounded to fp32 once
+// (sampler.cu: unipc_step_state), folded into two linear combinations over the step's planes, D0 = D_i and the history
+// H_j = D_{i-j}:
+//   corrector (corr_order >= 1):  x^c = a * base + v[0] * D0 + v[1] * H_1 + ... + v[corr_order] * H_corr_order
+//                 (corr_order 0):  x^c = x_t
+//   predictor:                    x_p = c * x^c + w[0] * D0 + w[1] * H_1 + ... + w[order - 1] * H_{order-1}
+// Only the terms of the two orders are evaluated: the history beyond them may hold anything.
+struct UniPcStep {
+  float a, v[4];
+  float c, w[3];
+  int corr_order;              // 0 (first step: no corrector) .. 3
+  int order;                   // predictor order 1..3 (1 on the final step, where c = 0, w[0] = 1: x_p = D0)
 };
 
 struct StepParams {
@@ -187,6 +202,29 @@ __device__ __forceinline__ float eps_x0(const StepParams& p, const StepCoef& k, 
 }
 // dynamic thresholding of one element of x_0 with its sample's s (see threshold_select_kernel)
 __device__ __forceinline__ float threshold_x0(float x0, float s) { return __fdiv_rn(fminf(fmaxf(x0, -s), s), s); }
+// the replace / constrain guidance of DDIM, DPM-Solver++ and UniPC on x_0 of one element (sample n, channel c, pixel pix);
+// nz = (t_prev != 0)
+__device__ __forceinline__ float guide_x0(const StepParams& p, float nz, int n, int c, size_t pix, float x0) {
+  auto mul = [](float a, float b) { return __fmul_rn(a, b); };
+  auto add = [](float a, float b) { return __fadd_rn(a, b); };
+  auto sub = [](float a, float b) { return __fsub_rn(a, b); };
+  if (c < 3) {
+    if (p.g.rgb != nullptr) {
+      const float y = p.g.rgb[(static_cast<size_t>(n) * 3 + c) * p.HW + pix];
+      const float m = p.g.rgb_mask[static_cast<size_t>(n) * p.HW + pix];
+      x0 = add(mul(sub(1.0f, nz), x0), mul(nz, add(mul(add(mul(p.g.w_rgb, y), mul(p.g.w_rgb_c, x0)), m), mul(x0, sub(1.0f, m)))));
+    }
+  } else if (p.g.depth != nullptr) {
+    const float y = p.g.depth[static_cast<size_t>(n) * p.HW + pix];
+    const float m = p.g.depth_mask[static_cast<size_t>(n) * p.HW + pix];
+    x0 = add(mul(add(mul(p.g.w_depth, y), mul(p.g.w_depth_c, x0)), m), mul(x0, sub(1.0f, m)));
+    if (p.g.convex != nullptr) {
+      const float cv = p.g.convex[static_cast<size_t>(n) * p.HW + pix];
+      x0 = add(mul(x0, m), mul(add(mul(p.g.w_convex, fmaxf(x0, cv)), mul(p.g.w_convex_c, x0)), sub(1.0f, m)));
+    }
+  }
+  return x0;
+}
 // x_{t-1} and x_0 of one element (sample n, channel c, pixel pix) from x_t, its x_0 after clipping or thresholding and the N(0,1)
 // draw z: the replace / constrain guidance, then the DDPM / DDIM / DPM-Solver++ update.  DPM-Solver++: z is read only by the SDE
 // variant (c_z != 0), dprev is D_{-1} of the element (read only at order 2) and x0o the guided D0.
@@ -203,21 +241,7 @@ __device__ __forceinline__ void step_update(const StepParams& p, const StepScala
     x0o = x0;
     return;
   }
-  if (c < 3) {
-    if (p.g.rgb != nullptr) {
-      const float y = p.g.rgb[(static_cast<size_t>(n) * 3 + c) * p.HW + pix];
-      const float m = p.g.rgb_mask[static_cast<size_t>(n) * p.HW + pix];
-      x0 = add(mul(sub(1.0f, s.nz), x0), mul(s.nz, add(mul(add(mul(p.g.w_rgb, y), mul(p.g.w_rgb_c, x0)), m), mul(x0, sub(1.0f, m)))));
-    }
-  } else if (p.g.depth != nullptr) {
-    const float y = p.g.depth[static_cast<size_t>(n) * p.HW + pix];
-    const float m = p.g.depth_mask[static_cast<size_t>(n) * p.HW + pix];
-    x0 = add(mul(add(mul(p.g.w_depth, y), mul(p.g.w_depth_c, x0)), m), mul(x0, sub(1.0f, m)));
-    if (p.g.convex != nullptr) {
-      const float cv = p.g.convex[static_cast<size_t>(n) * p.HW + pix];
-      x0 = add(mul(x0, m), mul(add(mul(p.g.w_convex, fmaxf(x0, cv)), mul(p.g.w_convex_c, x0)), sub(1.0f, m)));
-    }
-  }
+  x0 = guide_x0(p, s.nz, n, c, pix, x0);
   if (kKind == kStepDpm) {
     // D_{-1} is not read at order 1: the history may hold anything (first step of a run)
     const float d = s.d.order == 2 ? add(mul(s.d.w0, x0), mul(s.d.w1, dprev)) : x0;
@@ -390,6 +414,69 @@ struct Update {
   }
 };
 
+// The UniPC update of a quad (kind 2 with unipc = 1): corrector, predictor and the shift of the history, in place.  The
+// arena holds kUniPcPlanes planes of [N,C,H,W]: the history H_1 .. H_3 (D_{i-1} .. D_{i-3}) and the corrector's base.  Each
+// thread reads every plane of its elements before it writes them, so no other thread sees a plane half shifted.  depth =
+// the history planes a run keeps (its order); the pointers stay fixed across a run, so consecutive steps replay one graph.
+constexpr int kUniPcPlanes = 4;
+struct UniPcUpdate {
+  float* arena;                // planes 0..2: H_1..H_3, plane 3: base
+  size_t plane;                // elements per plane (N*C*H*W)
+  float* corrected;            // optional: x^c
+  const UniPcStep* u;          // device step state
+  int depth;                   // 1..3
+  struct Scalars { StepCoef k; float nz; UniPcStep u; };
+  __device__ __forceinline__ Scalars scalars(const StepParams& p) const {
+    return {p.table[*p.t_index], (*p.t_prev != 0) ? 1.0f : 0.0f, *u};
+  }
+  template <typename Load>
+  __device__ __forceinline__ void operator()(const StepParams& p, const Scalars& s, const Quad& q, Load&& load) const {
+    auto mul = [](float a, float b) { return __fmul_rn(a, b); };
+    auto add = [](float a, float b) { return __fadd_rn(a, b); };
+    const UniPcStep& u = s.u;
+    float h[3][4] = {}, base[4];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      if (j < depth) {
+        const float4 t = *reinterpret_cast<const float4*>(arena + j * plane + q.i);
+        h[j][0] = t.x; h[j][1] = t.y; h[j][2] = t.z; h[j][3] = t.w;
+      }
+    }
+    {
+      const float4 t = *reinterpret_cast<const float4*>(arena + 3 * plane + q.i);
+      base[0] = t.x; base[1] = t.y; base[2] = t.z; base[3] = t.w;
+    }
+    float xt[4], x0[4], xc[4], xo[4];
+    load(xt, x0);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float d = guide_x0(p, s.nz, q.n, q.c, q.pix + e, x0[e]);
+      x0[e] = d;
+      float v = xt[e];
+      if (u.corr_order >= 1) {
+        v = add(mul(u.a, base[e]), mul(u.v[0], d));
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+          if (j < u.corr_order) v = add(v, mul(u.v[j + 1], h[j][e]));
+      }
+      xc[e] = v;
+      float o = add(mul(u.c, v), mul(u.w[0], d));
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (j + 1 < u.order) o = add(o, mul(u.w[j + 1], h[j][e]));
+      xo[e] = o;
+    }
+    stg_f4(p.x_prev + q.i, make_float4(xo[0], xo[1], xo[2], xo[3]));
+    if (p.pred_x0) stg_f4(p.pred_x0 + q.i, make_float4(x0[0], x0[1], x0[2], x0[3]));
+    if (corrected) stg_f4(corrected + q.i, make_float4(xc[0], xc[1], xc[2], xc[3]));
+    stg_f4(arena + 3 * plane + q.i, make_float4(xc[0], xc[1], xc[2], xc[3]));
+#pragma unroll
+    for (int j = 2; j >= 1; --j)
+      if (j < depth) stg_f4(arena + j * plane + q.i, make_float4(h[j - 1][0], h[j - 1][1], h[j - 1][2], h[j - 1][3]));
+    stg_f4(arena + q.i, make_float4(x0[0], x0[1], x0[2], x0[3]));
+  }
+};
+
 // x_0 of a quad into a [N,C,H,W] buffer.  x0 may be the eps buffer of an EpsRows source (rows [0,N)): each element is read
 // before it is overwritten, by the same thread, so neither pointer is __restrict__.
 struct StoreX0 {
@@ -406,7 +493,7 @@ struct StoreX0 {
 
 template <typename Src, typename Sink>
 __global__ void __launch_bounds__(256) step_kernel(const StepParams p, const Src src, const Sink sink) {
-  const typename Sink::Scalars s = Sink::scalars(p);
+  const typename Sink::Scalars s = sink.scalars(p);
   const int cfg = step_cfg(p);
   const size_t units = src.units(p);
   for (size_t u = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; u < units; u += static_cast<size_t>(gridDim.x) * blockDim.x)

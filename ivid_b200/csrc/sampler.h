@@ -1,4 +1,4 @@
-// DDPM / DDIM / DPM-Solver++ samplers (host class).  See sampler.cu / sampler.cuh.
+// DDPM / DDIM / DPM-Solver++ / UniPC samplers (host class).  See sampler.cu / sampler.cuh.
 #pragma once
 #include <vector>
 
@@ -38,7 +38,8 @@ class Sampler {
   void* d_table_ = nullptr;
   void* d_state_ = nullptr;
   double* d_acp_ = nullptr;                // float64 alphas_cumprod (DPM-Solver++ step scalars)
-  float* d_hist_ = nullptr;                // DPM-Solver++ history D_{-1} [N,C,H,W], updated in place by the step kernels
+  float* d_hist_ = nullptr;                // DPM-Solver++ history D_{-1} [N,C,H,W], or UniPC's history and base (4 planes),
+                                           // updated in place by the step kernels
   size_t cap_hist_ = 0;
   int64_t* d_t_ = nullptr;
   int64_t* d_classes2_ = nullptr;

@@ -64,8 +64,8 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
-    (DPM-Solver++(2M)) wherever the reference runs DdimSampler, and solver="dpmpp_sde" its stochastic variant
-    (SDE-DPM-Solver++(2M)); DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
+    (DPM-Solver++(2M)) wherever the reference runs DdimSampler, solver="dpmpp_sde" its stochastic variant
+    (SDE-DPM-Solver++(2M)) and solver="unipc" UniPcSampler at order 2; DDPM at steps_uncond >= 1000 is kept.  precision="fp8"
     runs the ResBlock convs of both networks with e4m3 operands (AdmUnet2d.set_precision).  guidance_interval=(t_lo, t_hi)
     guides only the steps of both networks whose model time lies in [t_lo, t_hi] (the samplers' `guidance_interval`);
     the other steps run at strength 0 with one batch-N forward.  cache_interval=N, cache_branch=b reuse the deep features of
@@ -76,11 +76,12 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
         if fw is not None:
             _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
     _check_threshold(dynamic_threshold, False)
-    assert solver in ("ddim", "dpmpp", "dpmpp_sde"), f"solver must be 'ddim', 'dpmpp' or 'dpmpp_sde', got {solver!r}"
+    assert solver in ("ddim", "dpmpp", "dpmpp_sde", "unipc"), \
+        f"solver must be 'ddim', 'dpmpp', 'dpmpp_sde' or 'unipc', got {solver!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
             fw.backbone.set_precision(precision)
-    ode = samplers.DdimSampler if solver == "ddim" else samplers.DpmSolverSampler
+    ode = {"ddim": samplers.DdimSampler, "unipc": samplers.UniPcSampler}.get(solver, samplers.DpmSolverSampler)
     sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
     sde_kw = dict(sde=True) if solver == "dpmpp_sde" else {}
@@ -357,10 +358,10 @@ def build_arg_parser():
     ap.add_argument("--rng", choices=["philox", "torch"], default="philox",
                     help="per-step noise: 'philox' draws in-kernel (fast, default); 'torch' draws with the torch generator exactly "
                          "where the reference does (seed-for-seed reproduction of the reference's images needs this)")
-    ap.add_argument("--solver", choices=["ddim", "dpmpp", "dpmpp_sde"], default="ddim",
+    ap.add_argument("--solver", choices=["ddim", "dpmpp", "dpmpp_sde", "unipc"], default="ddim",
                     help="sampler of the DDIM-step views: 'ddim' as the reference, 'dpmpp' DPM-Solver++(2M), which needs fewer "
-                         "steps for the same convergence, 'dpmpp_sde' its stochastic variant SDE-DPM-Solver++(2M) "
-                         "(DDPM at --steps_uncond >= 1000 is unchanged)")
+                         "steps for the same convergence, 'dpmpp_sde' its stochastic variant SDE-DPM-Solver++(2M), 'unipc' the "
+                         "UniPC predictor-corrector at order 2 (DDPM at --steps_uncond >= 1000 is unchanged)")
     ap.add_argument("--precision", choices=["fp16", "fp8"], default="fp16",
                     help="operands of the ResBlock convs: 'fp16' (default) or 'fp8' (e4m3, faster, changes the numbers; DESIGN.md §2)")
     ap.add_argument("--guidance_interval", type=parse_interval, default=None, metavar="LO,HI",

@@ -1,1 +1,1 @@
-from .samplers import DdpmSampler, DdimSampler, DpmSolverSampler
+from .samplers import DdpmSampler, DdimSampler, DpmSolverSampler, UniPcSampler

@@ -1,6 +1,6 @@
 """DdpmSampler / DdimSampler — host-side mirrors of the reference samplers
 (diffusion/samplers/ddpm.py:12-187, diffusion/samplers/ddim.py:12-165) — and DpmSolverSampler, a DPM-Solver++(2M)
-sampler with the same surface that the reference does not have.
+sampler, and UniPcSampler, the UniPC predictor-corrector, with the same surface that the reference does not have.
 
 Same constructor (`Sampler(framework)`), same float64 numpy table attributes, same `.sample(...)` / `.sample_once(...)`
 signatures and return dict (`samples`, `pred_x_t`, `pred_x_0`).  The step itself — UNet forward with both
@@ -25,7 +25,7 @@ from .. import _lib
 from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG
 from ..utils import edict
 
-__all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler"]
+__all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler", "UniPcSampler"]
 
 
 def _unwrap(backbone):
@@ -77,6 +77,7 @@ def _check_threshold(dynamic_threshold, clip_denoised):
 
 class _NativeSampler:
     KIND = 0
+    UNIPC = False     # kind 2 only: the UniPC update instead of DPM-Solver++
 
     def __init__(self, framework):
         self.framework = framework
@@ -113,7 +114,7 @@ class _NativeSampler:
         return uses_cfg, float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
 
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None):
+                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None, prev_x=None, corrected=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -162,9 +163,19 @@ class _NativeSampler:
         if hw is not None:
             a.height, a.width = int(hw[0]), int(hw[1])
         a.order = int(order)
-        if prev is not None:
+        step_t = lambda t: int(t[0]) if torch.is_tensor(t) and t.dim() > 0 else int(t)
+        if self.UNIPC:
+            # up to three (t_last, pred_x_0) pairs, newest first, and the corrector's base
+            a.unipc = 1
+            slots = (("prev_x0_dev", "t_last"), ("prev2_x0_dev", "t_last2"), ("prev3_x0_dev", "t_last3"))
+            for (x_field, t_field), (t_last, x0_last) in zip(slots, prev or ()):
+                setattr(a, t_field, step_t(t_last))
+                setattr(a, x_field, P(x0_last))
+            a.prev_xt_dev = P(prev_x)
+            a.corrected_xt_dev = _lib.ptr(corrected).value
+        elif prev is not None:
             t_last, x0_last = prev
-            a.t_last = int(t_last[0]) if torch.is_tensor(t_last) and t_last.dim() > 0 else int(t_last)
+            a.t_last = step_t(t_last)
             a.prev_x0_dev = P(x0_last)
         a.sde = 1 if sde else 0
         interval = _check_interval(interval, len(fw.betas))
@@ -188,15 +199,16 @@ class _NativeSampler:
         return _unwrap(self.framework.backbone).num_res_blocks
 
     def _native_step(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                     sde=False, interval=None, cache=None, threshold=None):
+                     sde=False, interval=None, cache=None, threshold=None, prev_x=None):
         """One step.  `t` / `t_prev` are host ints (ivid_sampler_step) or the [N] tensors sample_once receives
         (ivid_sampler_step_dev: the step is read on the device, no host sync; t_prev None for DDPM)."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
+        corrected = torch.empty_like(x_t) if self.UNIPC else None
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
                                   hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache,
-                                  threshold=threshold)
+                                  threshold=threshold, prev_x=prev_x, corrected=corrected)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         L = _lib.lib()
@@ -210,10 +222,13 @@ class _NativeSampler:
                 rc = L.ivid_sampler_step(*head, int(t), int(t_prev), ctypes.byref(a), _lib.cur_stream(dev))
             _lib.check(rc)
         del keep
-        return edict({"pred_x_prev": x_prev, "pred_x_0": x0})
+        out = edict({"pred_x_prev": x_prev, "pred_x_0": x0})
+        if self.UNIPC:
+            out.corrected_x_t = corrected
+        return out
 
     def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, interval, reuse_features, cache_branch,
-                     order=0, prev=None, sde=False, dynamic_threshold=None):
+                     order=0, prev=None, sde=False, dynamic_threshold=None, prev_x=None):
         """The body of every sample_once: the host checks before any device work or torch draw, the step noise (drawn as
         the reference draws it, or the injected `noise` and kwargs' `cond_noise`), then the step with t / t_prev read on
         the device (all samples of a batch share the step, ddpm.py:177-179, ddim.py:154-158: no host sync)."""
@@ -230,7 +245,7 @@ class _NativeSampler:
         # the DPM-Solver++ ODE update reads no step noise
         return self._native_step(x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise if self.KIND != 2 or sde else None,
                                  cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold)
+                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold, prev_x=prev_x)
 
     def _draw_step_noise(self, x_t, kwargs):
         """torch draws in the reference's order: InpaintCFG rgb, depth (inside model_inference), then randn_like(x_t)."""
@@ -282,7 +297,7 @@ class _NativeSampler:
             else:
                 jump = T // nsteps
                 sched = [(jump * (i + 1), jump * i) for i in reversed(range(nsteps))]
-            prev = None
+            prev, prev_x = None, None
             reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
                                          cache_interval)
             for i, (t, t_prev) in enumerate(sched):
@@ -290,8 +305,10 @@ class _NativeSampler:
                 # the DPM-Solver++ ODE update draws z only to consume the torch RNG as DdimSampler does
                 out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if self.KIND != 2 or sde else None,
                                         cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                        cache=(0, cache_branch, reuse[i]), threshold=threshold)
-                if self.KIND == 2 and order != 1:
+                                        cache=(0, cache_branch, reuse[i]), threshold=threshold, prev_x=prev_x)
+                if self.UNIPC:
+                    prev, prev_x = ([(t, out.pred_x_0)] + (prev or []))[:order], out.corrected_x_t
+                elif self.KIND == 2 and order != 1:
                     prev = (t, out.pred_x_0)
                 img = out.pred_x_prev
                 if return_trajectory:
@@ -443,3 +460,50 @@ class DpmSolverSampler(_NativeSampler):
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
                          cache_branch=cache_branch, dynamic_threshold=dynamic_threshold)
+
+
+class UniPcSampler(_NativeSampler):
+    """UniPC (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework for Fast Sampling of Diffusion Models",
+    arXiv:2302.04867), data prediction with B(h) = e^h - 1 ("bh2"), multistep of order 1 to 3, on DdimSampler's time grid with
+    DpmSolverSampler's guidance (classifier-free mix, multiview replace / constrain applied to x_0).  Each step first corrects
+    the previous prediction x_t with the model output D0 this step computes anyway (the corrector UniC, which raises the order
+    by one at no extra network evaluation), then predicts x_{t_prev} from the corrected x_t (UniP, at orders 1 and 2 the
+    DPM-Solver++ update).  The network always sees the uncorrected prediction.  The corrector, predictor and history update
+    run fused into the output head (include/ivid_b200.h, kind 2 with unipc = 1)."""
+    KIND = 2
+    UNIPC = True
+
+    @torch.no_grad()
+    def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, prev_x=None, order=2, replace_rgb=None,
+                    replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
+                    cache_branch=0, dynamic_threshold=None, **kwargs):
+        """One UniPC step from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
+        `prev` is a list of up to three `(t_last, pred_x_0)` pairs of the previous steps, newest first, and `prev_x` the
+        previous step's `corrected_x_t` (the corrector's base; required with `prev`).  With n pairs (at most `order` are used)
+        the step corrects at order min(order, n) and predicts at order min(order, n + 1); the step to t_prev = 0 returns x_0.
+        Returns `pred_x_prev` (the prediction the next step's network sees), `pred_x_0` and `corrected_x_t` (x_t itself
+        without `prev`).  Chain steps with prev = ([(t, pred_x_0)] + prev)[:3] and prev_x = corrected_x_t.  `noise` is not used; the
+        torch RNG is consumed as DpmSolverSampler.sample_once consumes it.  `guidance_interval`, `reuse_features`,
+        `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once."""
+        assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
+        prev = list(prev) if prev is not None else []
+        assert len(prev) <= 3, f"prev holds at most three (t_last, pred_x_0) pairs, got {len(prev)}"
+        assert not prev or prev_x is not None, "prev needs prev_x, the previous step's corrected_x_t"
+        kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
+        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
+                                 cache_branch, order=order, prev=prev, dynamic_threshold=dynamic_threshold, prev_x=prev_x)
+
+    @torch.no_grad()
+    def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
+               rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
+               dynamic_threshold=None, **kwargs):
+        """Run `steps` UniPC steps of order `order` (1, 2 or 3; 2 is the paper's choice for guided sampling).  Step i predicts
+        at order min(order, i + 1) and corrects at the previous step's order; the first step has no corrector and the final
+        step (to t_prev = 0) returns x_0 as DDIM does.  pred_x_t holds the predictions the network saw.  Draws no step noise;
+        the torch RNG is consumed as DpmSolverSampler.sample(sde=False) consumes it.  `guidance_interval`, `cache_interval` /
+        `cache_branch` and `dynamic_threshold` as in DpmSolverSampler.sample: the history holds the D0 of whichever forward
+        ran, thresholded.  Same return dict as DdimSampler.sample."""
+        assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
+        return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
+                         order=order, interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
+                         dynamic_threshold=dynamic_threshold)
