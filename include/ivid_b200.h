@@ -251,6 +251,15 @@ typedef struct {
   int t_last3;
   const float* prev_xt_dev;
   float* corrected_xt_dev;
+  /* Partial run (SDEdit, Meng et al. 2022, arXiv:2108.01073), ivid_sampler_run only; zero runs the whole grid.
+   * ivid_sampler_run executes steps i = start_step .. steps-1 of the grid it builds (T steps for DDPM), from the x_inout_dev
+   * of step start_step (ivid_sampler_diffuse below makes one from an image).  Each executed step keeps its t, t_prev,
+   * Philox stream i, conditional-input noise and guidance-interval decision of a full run.  Multistep state counts from
+   * the first executed step: the DPM-Solver++ history, the UniPC order ramp and corrector, and the full forward of feature
+   * reuse all start at i = start_step as they start at i = 0 in a full run.  noise_all_dev, cond_noise_all_dev and the
+   * trajectories hold only the executed steps (index i - start_step).  0 <= start_step < steps, else
+   * IVID_ERR_INVALID_ARGUMENT.  The single-step entry points ignore it. */
+  int start_step;
   /* Dynamic thresholding of x0 (Saharia et al. 2022, "Imagen", arXiv:2205.11487, sec. 2.3), every kind; zero means off.
    * For every sample n, after the classifier-free guidance mix and x0 = sqrt(1/acp) * x_t - sqrt(1/acp - 1) * eps, where
    * clip_denoised would clamp it:
@@ -301,6 +310,15 @@ int ivid_cfg_mix(const float* eps2n_dev, float strength, float* out_dev, uint64_
 int ivid_sampler_run(ivid_sampler_t* s, ivid_unet_t* unet, float* x_inout_dev, int N, int steps,
                      const ivid_step_args_t* args, const float* noise_all_dev, const float* cond_noise_all_dev,
                      float* traj_x0_dev, float* traj_xt_dev, void* stream);
+
+/* GaussianDiffusion.diffuse (gaussian_diffusion.py:45-64), q(x_t | x_0): out = sqrt(acp[t]) * x0 + sqrt(1 - acp[t]) * z over
+ * N * count_per_sample fp32 elements (count_per_sample a multiple of 4; out overlaps neither x0 nor noise).  t is the step minus 1, as the
+ * reference passes it, 0 <= t < T.  The two coefficients are the float64 table values rounded once to fp32 (the reference's
+ * extract), and the expression is evaluated as fp32 mul, mul, add, so injected noise gives the reference's bits.
+ * noise_dev = z, or NULL: z = Philox(seed, stream 0xFFFFFFFF), a stream no sampler step uses, so a run that diffuses and
+ * samples with one seed is reproducible end to end.  Kernel name: ivid::diffuse_kernel. */
+int ivid_sampler_diffuse(ivid_sampler_t* s, const float* x0_dev, const float* noise_dev, int N, uint64_t count_per_sample,
+                         int t, uint64_t seed, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * RGBD novel-view warp — replaces rgbd_3d.utils.{linearize_depth, depth_to_mesh, aggregate_conditions, project_depth,

@@ -71,6 +71,7 @@ class StepArgsT(Structure):
         ("t_last3", c_int),
         ("prev_xt_dev", c_void_p),    # UniPC, single step: the corrector's base, the corrected x at t_last
         ("corrected_xt_dev", c_void_p),  # UniPC, optional output: this step's corrected x_t
+        ("start_step", c_int),        # ivid_sampler_run: execute grid steps start_step .. steps-1 only (0 = all)
         ("dynamic_threshold", c_int), # 1: threshold x_0 at the threshold_ratio-quantile of |x_0| of each sample
         ("threshold_ratio", c_double),
         ("threshold_max", c_double),  # upper bound of the threshold; <= 0 = none
@@ -140,6 +141,7 @@ SIGNATURES = {
     "ivid_cfg_mix": (c_int, [c_void_p, c_float, c_void_p, c_uint64, c_void_p]),
     "ivid_op_dynamic_threshold": (c_int, [c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_void_p, c_void_p]),
     "ivid_sampler_run": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(StepArgsT), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "ivid_sampler_diffuse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_uint64, c_int, c_uint64, c_void_p, c_void_p]),
     "ivid_op_conv2d": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int,
                                c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "ivid_op_group_norm": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,

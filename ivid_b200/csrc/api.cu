@@ -242,6 +242,14 @@ int ivid_sampler_run(ivid_sampler_t* s, ivid_unet_t* unet, float* x_inout_dev, i
                  static_cast<cudaStream_t>(stream));
   });
 }
+int ivid_sampler_diffuse(ivid_sampler_t* s, const float* x0_dev, const float* noise_dev, int N, uint64_t count_per_sample,
+                         int t, uint64_t seed, float* out_dev, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(s); IVID_NOT_NULL(x0_dev); IVID_NOT_NULL(out_dev);
+    s->impl->diffuse(x0_dev, noise_dev, N, static_cast<size_t>(count_per_sample), t, seed, out_dev,
+                     static_cast<cudaStream_t>(stream));
+  });
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // operator-level entry points (weights are packed per call: test / profiling paths, not the hot loop)

@@ -240,6 +240,19 @@ static void launch_step_tail(const StepParams& p, const Src& src, const StepTail
   update(ThresholdedX0{t.x0, t.s});
 }
 
+void Sampler::diffuse(const float* x0, const float* noise, int N, size_t per_sample, int t, uint64_t seed, float* out,
+                      cudaStream_t stream) const {
+  IVID_REQUIRE(N >= 1 && per_sample >= 1, "diffuse: N and count_per_sample must be positive");
+  IVID_REQUIRE(per_sample % 4 == 0, "diffuse: count_per_sample must be a multiple of 4");
+  IVID_REQUIRE(t >= 0 && t < T_, "diffuse: t out of range");
+  const size_t n4 = static_cast<size_t>(N) * per_sample / 4;
+  IVID_REQUIRE(n4 <= 0xFFFFFFFFull, "diffuse: more than 2^32 quads");   // the Philox index is 32-bit
+  // extract() of the reference: the float64 sqrt tables (gaussian_diffusion.py:41-42) rounded once to fp32
+  const float a = static_cast<float>(std::sqrt(acp_[t])), b = static_cast<float>(std::sqrt(1.0 - acp_[t]));
+  diffuse_kernel<<<elementwise_grid(n4), 256, 0, stream>>>(x0, noise, out, n4, a, b, seed);
+  IVID_CHECK_CUDA(cudaGetLastError());
+}
+
 void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double threshold_max, float* s_out, float* x_out,
                               cudaStream_t st) {
   IVID_REQUIRE(N >= 1 && M >= 1, "dynamic threshold: N and M must be positive");
@@ -614,6 +627,10 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   const bool dpm = a.kind == kStepDpm;
   if (!ddim) steps = T_;
   IVID_REQUIRE(steps >= 1 && steps <= T_, "steps out of range");
+  // a partial run executes steps s0 .. steps-1 of the same grid; k = i - s0 counts the executed steps, and multistep state
+  // (history, order ramp, the first full forward) starts at k = 0 as a full run's starts at i = 0
+  const int s0 = a.start_step;
+  IVID_REQUIRE(s0 >= 0 && s0 < steps, "start_step must satisfy 0 <= start_step < steps");
   const int jump = T_ / steps;                     // ddim.py:153
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));
   ensure_device(2 * N, 2 * img);
@@ -626,47 +643,48 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   // per denoising step the host then issues three calls: the step-state kernel, ONE CUDA-graph launch (the whole batch-2N
   // forward, batch-N for a step outside the guidance interval: each batch has its own plan and graphs) and the fused
   // guidance-mix + x_{t-1} update.  The first batch-2N step fills [classes, -1 ...] once for the whole reverse process.
-  // feature reuse: a full forward at step 0, at a switch between the batch-2N and batch-N plans, and every cache_interval
-  // steps after the last full one; reuse forwards in between
+  // feature reuse: a full forward at the first executed step, at a switch between the batch-2N and batch-N plans, and every
+  // cache_interval steps after the last full one; reuse forwards in between
   int last_full = 0;
   bool last_two = false, classes2_filled = false;
-  for (int i = 0; i < steps; ++i) {
+  for (int i = s0; i < steps; ++i) {
+    const int k = i - s0;
     int t, t_prev;
     if (ddim) { t = jump * (steps - i); t_prev = jump * (steps - 1 - i); }   // ddim.py:154
     else { t = T_ - 1 - i; t_prev = 0; }                                      // ddpm.py:177
     ivid_step_args_t ai = a;
-    ai.step_noise_dev = noise_all ? noise_all + static_cast<size_t>(i) * img : nullptr;
+    ai.step_noise_dev = noise_all ? noise_all + static_cast<size_t>(k) * img : nullptr;
     if (dpm) {
-      // multistep history: from the second step on, D_{-1} is the previous step's D0, already in the sampler's buffer
-      ai.prev_x0_dev = i > 0 ? d_hist_ : nullptr;
-      ai.t_last = i > 0 ? jump * (steps + 1 - i) : 0;
+      // multistep history: from the second executed step on, D_{-1} is the previous step's D0, already in the sampler's buffer
+      ai.prev_x0_dev = k > 0 ? d_hist_ : nullptr;
+      ai.t_last = k > 0 ? jump * (steps + 1 - i) : 0;
     }
     if (a.unipc) {
-      // UniPC: the arena's planes, D_{i-1-j} at t + jump * (1 + j) for the j < min(i, order) steps that have run, and the base
-      ai.prev2_x0_dev = i > 1 && a.order > 1 ? d_hist_ + img : nullptr;
-      ai.t_last2 = i > 1 ? jump * (steps + 2 - i) : 0;
-      ai.prev3_x0_dev = i > 2 && a.order > 2 ? d_hist_ + 2 * img : nullptr;
-      ai.t_last3 = i > 2 ? jump * (steps + 3 - i) : 0;
-      ai.prev_xt_dev = i > 0 ? d_hist_ + 3 * img : nullptr;
+      // UniPC: the arena's planes, D_{i-1-j} at t + jump * (1 + j) for the j < min(k, order) steps that have run, and the base
+      ai.prev2_x0_dev = k > 1 && a.order > 1 ? d_hist_ + img : nullptr;
+      ai.t_last2 = k > 1 ? jump * (steps + 2 - i) : 0;
+      ai.prev3_x0_dev = k > 2 && a.order > 2 ? d_hist_ + 2 * img : nullptr;
+      ai.t_last3 = k > 2 ? jump * (steps + 3 - i) : 0;
+      ai.prev_xt_dev = k > 0 ? d_hist_ + 3 * img : nullptr;
       ai.corrected_xt_dev = nullptr;
     }
     if (cond_noise_all && ai.cond.kind == 1)
-      ai.cond.noise_dev = cond_noise_all + static_cast<size_t>(i) * N * 4 * hw;
+      ai.cond.noise_dev = cond_noise_all + static_cast<size_t>(k) * N * 4 * hw;
     const bool two = plan_step(ai, N, t, t_prev, false).Nf == 2 * N;
-    const bool full = a.cache_interval <= 1 || i == 0 || two != last_two || i - last_full >= a.cache_interval;
-    if (full) last_full = i;
+    const bool full = a.cache_interval <= 1 || k == 0 || two != last_two || k - last_full >= a.cache_interval;
+    if (full) last_full = k;
     last_two = two;
     ai.cache_reuse = full ? 0 : 1;
-    float* dst = traj_xt ? traj_xt + static_cast<size_t>(i) * img : bufs[cur ^ 1];
-    float* x0 = traj_x0 ? traj_x0 + static_cast<size_t>(i) * img : nullptr;
-    const float* src = (traj_xt && i > 0) ? traj_xt + static_cast<size_t>(i - 1) * img : bufs[cur];
-    if (traj_xt && i == 0) src = x;
+    float* dst = traj_xt ? traj_xt + static_cast<size_t>(k) * img : bufs[cur ^ 1];
+    float* x0 = traj_x0 ? traj_x0 + static_cast<size_t>(k) * img : nullptr;
+    const float* src = (traj_xt && k > 0) ? traj_xt + static_cast<size_t>(k - 1) * img : bufs[cur];
+    if (traj_xt && k == 0) src = x;
     step_impl(unet, src, dst, x0, N, plan_step(ai, N, t, t_prev, false), ai, i, stream, nullptr, nullptr, allow_fuse,
               classes2_filled);
     classes2_filled = classes2_filled || two;
     if (!traj_xt) cur ^= 1;
   }
-  const float* last = traj_xt ? traj_xt + static_cast<size_t>(steps - 1) * img : bufs[cur];
+  const float* last = traj_xt ? traj_xt + static_cast<size_t>(steps - 1 - s0) * img : bufs[cur];
   if (last != x) IVID_CHECK_CUDA(cudaMemcpyAsync(x, last, img * 4, cudaMemcpyDeviceToDevice, stream));
 }
 

@@ -151,6 +151,22 @@ __global__ void __launch_bounds__(256) cfg_mix_kernel(const float* __restrict__ 
   }
 }
 
+// Philox stream of the forward diffusion's noise: no step uses it (steps use their index, below T)
+constexpr uint32_t kDiffuseStream = 0xFFFFFFFFu;
+
+// q(x_t | x_0): out = a * x0 + b * z with a = fp32(sqrt(acp[t])), b = fp32(sqrt(1 - acp[t])), rounded as the reference's two
+// fp32 tensor products and their sum (no FMA).  z is the injected noise, or Philox(seed, kDiffuseStream) indexed by quad as
+// the step kernels index their noise.
+__global__ void __launch_bounds__(256) diffuse_kernel(const float* __restrict__ x0, const float* __restrict__ noise,
+                                                      float* __restrict__ out, size_t n4, float a, float b, uint64_t seed) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n4; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const float4 z = noise != nullptr ? ldg_f4(noise + 4 * i) : philox_normal4(seed, kDiffuseStream, static_cast<uint32_t>(i));
+    const float4 x = ldg_f4(x0 + 4 * i);
+    stg_f4(out + 4 * i, make_float4(__fadd_rn(__fmul_rn(a, x.x), __fmul_rn(b, z.x)), __fadd_rn(__fmul_rn(a, x.y), __fmul_rn(b, z.y)),
+                                    __fadd_rn(__fmul_rn(a, x.z), __fmul_rn(b, z.z)), __fadd_rn(__fmul_rn(a, x.w), __fmul_rn(b, z.w))));
+  }
+}
+
 // Per-step scalars derived once per thread from the device-resident step state.
 struct StepScalars {
   StepCoef k;

@@ -20,7 +20,10 @@ class Sampler {
   void step(Unet& unet, const float* x_t, float* x_prev, float* pred_x0, int N, int t, int t_prev,
             const ivid_step_args_t& a, int stream_id, cudaStream_t stream, const int64_t* t_dev = nullptr,
             const int64_t* t_prev_dev = nullptr);
-  // the whole reverse process
+  // q(x_t | x_0) of the reference's step minus 1 t over N * per_sample elements; noise == nullptr draws Philox(seed)
+  void diffuse(const float* x0, const float* noise, int N, size_t per_sample, int t, uint64_t seed, float* out,
+               cudaStream_t stream) const;
+  // the whole reverse process (a.start_step: from that step of the grid on)
   void run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t& a, const float* noise_all,
            const float* cond_noise_all, float* traj_x0, float* traj_xt, cudaStream_t stream);
 

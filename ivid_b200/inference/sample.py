@@ -1,7 +1,7 @@
 """Multiview sampling driver — mirror of the reference's inference/sample.py (sample_all :30-147, per-rank sharding
 :199-202, view sets :304-338) with the per-view loop kept on the device:
 
-    view 0:  unconditional sampler  (DDPM 1000 / DDIM)                               -> RGBD on the GPU
+    view 0:  unconditional sampler  (DDPM 1000 / DDIM), or a given view (SDEdit of it)  -> RGBD on the GPU
     view j:  DeviceWarp.aggregate (CUDA mesh + rasterise + aggregate + post-filters)  -> condition maps on the GPU
              conditional DDIM sampler with replace / constrain guidance               -> RGBD on the GPU
 
@@ -30,6 +30,69 @@ from .utils import colorize_depth, parse_int_list, reorder, save_scene
 def shard(items, rank, world_size):
     """seeds / classes / per-sample modelviews of this rank (sample.py:199-202: [rank::world_size])."""
     return items[rank::world_size] if items is not None else None
+
+
+def preprocess_init_view(image, disparity, image_size, normalize=False, normalize_depth=False, prepocess_depth="none", near=0.5,
+                         far=100, **_):
+    """[4, S, S] RGBD of a photo and its disparity map, as the reference's datasets make a training x_0 (datasets/base.py:92-126,
+    BaseDataset.get_file / process_file, with their `dataset.args`): the disparity / 6250 rescaled so its maximum is at most
+    1 / near, floored at 1e-3 and mapped by `prepocess_depth`; the image resized to S on its short side (LANCZOS) and the
+    depth (NEAREST), both centre-cropped to S x S; each mapped to [-1, 1] when its normalize flag is set.
+    image: a PIL image; disparity: a 2-D array as the datasets store it (the `arr_0` of their .npz files)."""
+    from PIL import Image
+    assert prepocess_depth in ("none", "to_depth", "disparity_minmax", "depth_minmax", "z_buffer"), \
+        f"unknown depth preprocessing {prepocess_depth!r}"
+    depth = np.asarray(disparity).astype(np.float32)
+    assert depth.ndim == 2, f"the disparity map must be 2-D, got shape {depth.shape}"
+    depth /= 6250
+    if depth.max() > 1 / near:
+        depth /= depth.max() * near
+    depth = np.maximum(depth, 1e-3)
+    if prepocess_depth == "to_depth":
+        depth = 1 / depth
+    elif prepocess_depth == "disparity_minmax":
+        depth = (depth - depth.min()) / (depth.max() - depth.min())
+    elif prepocess_depth == "depth_minmax":
+        depth = 1 / depth
+        depth = (depth - depth.min()) / (depth.max() - depth.min())
+    elif prepocess_depth == "z_buffer":
+        depth = (depth - 1 / near) / (1 / far - 1 / near)
+        depth = np.clip(depth, 0, 1)
+
+    def resize_crop(img, resample):
+        # torchvision Resize(S) (short side to S, the long side truncated) then CenterCrop(S)
+        w, h = img.size
+        short, long = (w, h) if w <= h else (h, w)
+        new_long = int(image_size * long / short)
+        size = (image_size, new_long) if w <= h else (new_long, image_size)
+        if size != (w, h):
+            img = img.resize(size, resample)
+        w, h = img.size
+        top, left = int(round((h - image_size) / 2.0)), int(round((w - image_size) / 2.0))
+        return img.crop((left, top, left + image_size, top + image_size))
+
+    rgb = np.array(resize_crop(image, Image.LANCZOS))
+    rgb = torch.from_numpy(rgb if rgb.ndim == 3 else rgb[:, :, None]).permute(2, 0, 1).contiguous()
+    rgb = rgb.to(torch.float32).div(255) if rgb.dtype == torch.uint8 else rgb.to(torch.float32)
+    if rgb.shape[0] == 1:
+        rgb = rgb.repeat(3, 1, 1)
+    if rgb.shape[0] == 4:
+        rgb = rgb[:3]
+    if normalize:
+        rgb = rgb * 2 - 1
+    d = torch.from_numpy(np.array(resize_crop(Image.fromarray(depth), Image.NEAREST)).astype(np.float32))[None]
+    if normalize_depth:
+        d = d * 2 - 1
+    return torch.cat([rgb, d])
+
+
+def load_init_view(image_path, depth_path, dataset_args, image_size):
+    """preprocess_init_view of an image file and a disparity file (.npz with arr_0, or .npy)."""
+    from PIL import Image
+    disparity = np.load(depth_path)
+    if isinstance(disparity, np.lib.npyio.NpzFile):
+        disparity = disparity["arr_0"]
+    return preprocess_init_view(Image.open(image_path), disparity, image_size, **dataset_args)
 
 
 def build_modelviews(viewset, num_samples, rng=None):
@@ -61,7 +124,8 @@ def build_modelviews(viewset, num_samples, rng=None):
 @torch.no_grad()
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
-               precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None):
+               precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init_views=None,
+               init_strength=None):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, solver="dpmpp_sde" its stochastic variant
@@ -71,7 +135,17 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     the other steps run at strength 0 with one batch-N forward.  cache_interval=N, cache_branch=b reuse the deep features of
     both networks between full forwards every N steps (the samplers' `cache_interval` / `cache_branch`; None: no reuse).
     dynamic_threshold=p or (p, s_max) thresholds x_0 dynamically at every step of both networks (the samplers'
-    `dynamic_threshold`)."""
+    `dynamic_threshold`).
+    init_views [num_samples, 4, S, S] (RGBD in [-1, 1], one per sample of this rank, sharded like the seeds) starts every
+    scene from a given first view: without init_strength view 0 IS that view and the unconditional model does not run
+    (framework_uncond may be None); with init_strength view 0 is its SDEdit by the unconditional sampler (the samplers'
+    `init` / `init_strength`) with the sample's class, guidance, solver and options.  Views 1... grow from view 0 as always."""
+    if init_views is None:
+        assert init_strength is None, "init_strength needs init_views"
+    else:
+        assert init_views.dim() == 4 and init_views.shape[1] == 4, f"init_views must be [num_samples,4,S,S], got {tuple(init_views.shape)}"
+    assert framework_uncond is not None or (init_views is not None and init_strength is None), \
+        "framework_uncond is needed unless every view 0 is given (init_views without init_strength)"
     for fw in (framework_uncond, framework_cond):          # before any device work
         if fw is not None:
             _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
@@ -82,7 +156,9 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
         if fw is not None and fw.backbone.precision != precision:
             fw.backbone.set_precision(precision)
     ode = {"ddim": samplers.DdimSampler, "unipc": samplers.UniPcSampler}.get(solver, samplers.DpmSolverSampler)
-    sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
+    sampler_uncond = None
+    if framework_uncond is not None:
+        sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
     sde_kw = dict(sde=True) if solver == "dpmpp_sde" else {}
     gi_kw = dict(guidance_interval=tuple(guidance_interval)) if guidance_interval is not None else {}
@@ -91,9 +167,12 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     th_kw = dict(dynamic_threshold=dynamic_threshold) if dynamic_threshold is not None else {}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
-    net = framework_uncond.backbone
+    net = (framework_uncond if framework_uncond is not None else framework_cond).backbone
     S = net.image_size
     dev = net.device
+    if init_views is not None:
+        assert tuple(init_views.shape) == (num_samples, 4, S, S), \
+            f"init_views must be [{num_samples},4,{S},{S}] (one view per sample, at the backbone's size), got {tuple(init_views.shape)}"
     per_sample_views = isinstance(modelviews[0], list)
     wparams = dict(fov=fov, near=near, far=far, atol=atol, rtol=rtol, erode_rgb=erode_rgb)
     warps = {}
@@ -118,14 +197,20 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
             warp = warps[bs]
             warp.reset()
         samples, cond_color, cond_depth = [], [], []
-        cfg_u = isinstance(framework_uncond, frameworks.ClassifierFreeGuidance)
+        # guided frameworks take the guidance strength (without an unconditional model, the conditional one decides)
+        cfg_u = (isinstance(framework_uncond, frameworks.ClassifierFreeGuidance) if framework_uncond is not None
+                 else isinstance(framework_cond, frameworks.InpaintCFG))
         for j in range(n_views):
             mv_j = [views_of(k)[j] for k in range(bs)] if per_sample_views else views_of(0)[j]
-            if j == 0:
+            if j == 0 and init_views is not None and init_strength is None:
+                res = edict(samples=init_views[i: i + bs].to(device=dev, dtype=torch.float32).contiguous())
+            elif j == 0:
                 kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
                 if steps_uncond < 1000:
                     kw.update(sde_kw)
                 kw.update(th_kw)
+                if init_views is not None:     # SDEdit of the given view; the seeds' noise is the forward diffusion's z
+                    kw.update(init=init_views[i: i + bs].to(device=dev, dtype=torch.float32), init_strength=init_strength)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
             else:
                 cond = warp.aggregate(mv_j, **wparams)                   # [bs,7,S,S] in [0,1]
@@ -237,8 +322,11 @@ def main(rank, world_size, opt):
     torch.cuda.set_device(rank)
     dev = torch.device("cuda", rank)
     cfg_u = json.load(open(opt.config_uncond))
-    fw_u = _load_model(cfg_u, opt.ckpt_uncond, dev)
-    fw_c = _load_model(json.load(open(opt.config_cond)), opt.ckpt_cond, dev) if opt.viewset != "uncond" else None
+    init_image, init_strength = getattr(opt, "init_image", None), getattr(opt, "init_strength", None)
+    # a given first view without a strength needs no unconditional model
+    fw_u = _load_model(cfg_u, opt.ckpt_uncond, dev) if init_image is None or init_strength is not None else None
+    cfg_c = json.load(open(opt.config_cond)) if opt.viewset != "uncond" or init_image is not None else None
+    fw_c = _load_model(cfg_c, opt.ckpt_cond, dev) if opt.viewset != "uncond" else None
     seeds = parse_int_list(opt.seeds) if opt.num_samples is None else None
     num = len(seeds) if seeds is not None else opt.num_samples
     ncls = cfg_u["backbone"]["args"].get("num_classes")
@@ -261,6 +349,12 @@ def main(rank, world_size, opt):
     interval = getattr(opt, "guidance_interval", None)
     cache_interval, cache_branch = getattr(opt, "cache_interval", None), getattr(opt, "cache_branch", 0)
     dynamic_threshold = getattr(opt, "dynamic_threshold", None)
+    init_views = None
+    if init_image is not None:
+        # one view for every sample: the seeds vary the continuation (and, with a strength, the noising)
+        size = cfg_u["backbone"]["args"]["image_size"]
+        view = load_init_view(init_image, opt.init_depth, cfg_c["dataset"]["args"], size)
+        init_views = view[None].expand(len(idx), -1, -1, -1)
     out_dir = output_dir_name(opt)
     for sub in ("results", "grids", "conds", "scenes"):                 # sample.py:283-286
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
@@ -269,7 +363,7 @@ def main(rank, world_size, opt):
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
                      rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
                      precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                     dynamic_threshold=dynamic_threshold)
+                     dynamic_threshold=dynamic_threshold, init_views=init_views, init_strength=init_strength)
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -285,11 +379,14 @@ def output_dir_name(opt):
     interval = getattr(opt, "guidance_interval", None)
     cache_interval = getattr(opt, "cache_interval", None)
     dt = getattr(opt, "dynamic_threshold", None)
+    init_image, init_strength = getattr(opt, "init_image", None), getattr(opt, "init_strength", None)
     return os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
                         + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}")
                         + ("" if interval is None else f"_interval{interval[0]}-{interval[1]}")
                         + ("" if cache_interval is None else f"_cache{cache_interval}b{getattr(opt, 'cache_branch', 0)}")
-                        + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}"))
+                        + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}")
+                        + ("" if init_image is None else f"_init-{os.path.splitext(os.path.basename(init_image))[0]}")
+                        + ("" if init_strength is None else f"_strength{init_strength}"))
 
 
 def _int_at_least(lo):
@@ -334,6 +431,29 @@ def parse_threshold(s):
     return vals[0] if len(vals) == 1 else (vals[0], vals[1])
 
 
+def parse_strength(s):
+    """'S' -> S of --init_strength, 0 < S <= 1."""
+    try:
+        v = float(s)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected a number, got {s!r}") from None
+    if not 0.0 < v <= 1.0:
+        raise argparse.ArgumentTypeError(f"expected 0 < S <= 1, got {s!r}")
+    return v
+
+
+def parse_args(argv=None):
+    """build_arg_parser().parse_args with the checks between options: --init_image and --init_depth go together, and
+    --init_strength needs them."""
+    ap = build_arg_parser()
+    o = ap.parse_args(argv)
+    if (o.init_image is None) != (o.init_depth is None):
+        ap.error("--init_image and --init_depth go together")
+    if o.init_strength is not None and o.init_image is None:
+        ap.error("--init_strength needs --init_image and --init_depth")
+    return o
+
+
 def build_arg_parser():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config_uncond", default="configs/rgbd_imagenet_adm_128_large_cfg.json")
@@ -376,11 +496,19 @@ def build_arg_parser():
     ap.add_argument("--dynamic_threshold", type=parse_threshold, default=None, metavar="P[,MAX]",
                     help="dynamic thresholding of the predicted x_0 (Imagen): clamp each sample's x_0 to [-s, s] and divide by s, "
                          "s = min(max(P-quantile of |x_0|, 1), MAX); e.g. 0.995 (default: off; MAX defaults to no bound)")
+    ap.add_argument("--init_image", default=None, metavar="PATH",
+                    help="grow every scene from this RGB image as its first view (needs --init_depth); preprocessed as the "
+                         "dataset of --config_cond prepares its images")
+    ap.add_argument("--init_depth", default=None, metavar="PATH",
+                    help="the disparity map of --init_image as the reference's datasets store it: .npz with arr_0, or .npy")
+    ap.add_argument("--init_strength", type=parse_strength, default=None, metavar="S",
+                    help="with --init_image: re-sample the first view from it by SDEdit, running the last S of the unconditional "
+                         "schedule, 0 < S <= 1 (default: the given view is the first view as it is)")
     return ap
 
 
 if __name__ == "__main__":
-    o = build_arg_parser().parse_args()
+    o = parse_args()
     n = torch.cuda.device_count()
     if n <= 1:
         main(0, 1, o)

@@ -1,1 +1,1 @@
-from .samplers import DdpmSampler, DdimSampler, DpmSolverSampler, UniPcSampler
+from .samplers import DdpmSampler, DdimSampler, DpmSolverSampler, UniPcSampler, init_steps

@@ -25,7 +25,7 @@ from .. import _lib
 from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG
 from ..utils import edict
 
-__all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler", "UniPcSampler"]
+__all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler", "UniPcSampler", "init_steps"]
 
 
 def _unwrap(backbone):
@@ -73,6 +73,28 @@ def _check_threshold(dynamic_threshold, clip_denoised):
     assert real(s_max) and float(s_max) >= 1.0, f"dynamic_threshold s_max must be >= 1, got {s_max!r}"
     assert not clip_denoised, "clip_denoised and dynamic_threshold exclude each other"
     return float(p), float(s_max)
+
+
+def init_steps(init_strength, steps):
+    """Executed steps n of a run started from an image (SDEdit): round(init_strength * steps), at least 1 and at most steps.
+    The run then starts at grid step start_step = steps - n."""
+    return min(steps, max(1, int(init_strength * steps + 0.5)))
+
+
+def _check_init(init, init_strength, noise, image_size, channels):
+    """The arguments of a run started from an image, checked before any device work: init [N, channels, H, W] with
+    init_strength in (0, 1], noise (the z of the forward diffusion) of init's shape, and no image_size (init sets the size)."""
+    if init is None:
+        assert init_strength is None, "init_strength needs init"
+        return
+    assert init_strength is not None, "init needs init_strength, the share of the schedule to run in (0, 1]"
+    assert isinstance(init_strength, numbers.Real) and not isinstance(init_strength, bool) and 0.0 < init_strength <= 1.0, \
+        f"init_strength must be in (0, 1], got {init_strength!r}"
+    assert torch.is_tensor(init) and init.dim() == 4 and init.shape[1] == channels, \
+        f"init must be an [N,{channels},H,W] tensor, got {tuple(init.shape) if torch.is_tensor(init) else type(init).__name__}"
+    assert image_size is None, "init sets the sample size: do not pass image_size with it"
+    assert noise is None or tuple(noise.shape) == tuple(init.shape), \
+        f"noise (the forward diffusion's z) must have init's shape {tuple(init.shape)}, got {tuple(noise.shape)}"
 
 
 class _NativeSampler:
@@ -273,30 +295,48 @@ class _NativeSampler:
         return reuse
 
     def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
-             sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None):
+             sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init=None, init_strength=None):
         interval = _check_interval(interval, len(self.framework.betas))   # before any device work
         cache_interval = _check_cache(cache_interval, cache_branch, self._num_res_blocks())
         threshold = _check_threshold(dynamic_threshold, clip_denoised)
+        _check_init(init, init_strength, noise, image_size, _unwrap(self.framework.backbone).out_channels)
         net = self._net()
         net.eval()
         if image_size is None:
             image_size = net.image_size
         device = net.device
-        # as in the reference (ddpm.py:168-176), given noise is used as-is and defines the sample size
-        img = noise if noise is not None else torch.randn((num, net.out_channels, image_size, image_size), device=device)
-        assert img.dim() == 4 and img.shape[1] == net.out_channels, f"noise must be [N,{net.out_channels},H,W], got {tuple(img.shape)}"
-        img = _f32(img, device).clone()
+        if init is not None:
+            x_init = _f32(init, device)
+            img = torch.empty_like(x_init)
+        else:
+            # as in the reference (ddpm.py:168-176), given noise is used as-is and defines the sample size
+            img = noise if noise is not None else torch.randn((num, net.out_channels, image_size, image_size), device=device)
+            assert img.dim() == 4 and img.shape[1] == net.out_channels, f"noise must be [N,{net.out_channels},H,W], got {tuple(img.shape)}"
+            img = _f32(img, device).clone()
         num = img.shape[0]
         shape = tuple(img.shape)
         T = self.framework.timesteps
         nsteps = T if self.KIND == 0 else (steps if steps is not None else T)
         ret = edict({"samples": None, "pred_x_t": [], "pred_x_0": []})
+        start = 0
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if rng == "philox" else 0
+        if init is not None:
+            # SDEdit: x at grid step start = steps - n is q(x_t | init) at that step's model time, jump * n - 1 (n - 1 for DDPM)
+            n = init_steps(init_strength, nsteps)
+            start = nsteps - n
+            jump = 1 if self.KIND == 0 else T // nsteps
+            # z: the given noise, Philox(seed) on a stream no step uses, or (rng="torch") randn_like(x_0) as diffuse draws it
+            z = _f32(noise, device) if noise is not None else (torch.randn_like(x_init) if rng == "torch" else None)
+            with torch.cuda.device(device):
+                _lib.check(_lib.lib().ivid_sampler_diffuse(self._handle, _lib.ptr(x_init), _lib.ptr(z), num, x_init[0].numel(),
+                                                           jump * n - 1, seed, _lib.ptr(img), _lib.cur_stream(device)))
         if rng == "torch":
             if self.KIND == 0:
                 sched = [(i, 0) for i in range(T)][::-1]
             else:
                 jump = T // nsteps
                 sched = [(jump * (i + 1), jump * i) for i in reversed(range(nsteps))]
+            sched = sched[start:]
             prev, prev_x = None, None
             reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
                                          cache_interval)
@@ -315,13 +355,13 @@ class _NativeSampler:
                     ret.pred_x_t.append(out.pred_x_prev)
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
             a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
                                       interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold)
+            a.start_step = start
             traj0 = trajt = None
             if return_trajectory:
-                traj0 = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
-                trajt = torch.empty((nsteps,) + shape, dtype=torch.float32, device=device)
+                traj0 = torch.empty((nsteps - start,) + shape, dtype=torch.float32, device=device)
+                trajt = torch.empty((nsteps - start,) + shape, dtype=torch.float32, device=device)
             with torch.cuda.device(device):
                 _lib.check(_lib.lib().ivid_sampler_run(self._handle, net._handle, _lib.ptr(img), num, int(nsteps), ctypes.byref(a),
                                                        None, None, _lib.ptr(traj0), _lib.ptr(trajt), _lib.cur_stream(device)))
@@ -364,7 +404,7 @@ class DdpmSampler(_NativeSampler):
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
         """Run the full reverse process (ddpm.py:134-187).  `steps` is accepted and ignored exactly as in the reference.
         pred_x_t / pred_x_0 are only materialised with return_trajectory=True (the reference keeps 2x1000 tensors alive;
         its callers read `.samples` only: inference/sample.py:82).
@@ -385,10 +425,18 @@ class DdpmSampler(_NativeSampler):
         clip_denoised would clamp x_0, each sample's x_0 is clamped to [-s, s] and divided by s, s = min(max(q, 1), s_max) and q
         the p-quantile of |x_0| over the sample (linear interpolation, as numpy.quantile); s_max defaults to no bound, p in
         (0, 1], s_max >= 1.  The guidance and the update then read the thresholded x_0 (include/ivid_b200.h).  Excludes
-        clip_denoised; s_max = 1 is clip_denoised=True.  The noise and the torch RNG consumption are unchanged."""
+        clip_denoised; s_max = 1 is clip_denoised=True.  The noise and the torch RNG consumption are unchanged.
+
+        init=x_0, init_strength=s (extension; SDEdit, Meng et al. 2022, arXiv:2108.01073): start from the image x_0 ([N, C, H, W]
+        in the model's [-1, 1] range; it sets N and the size, so image_size must stay None) instead of x_T.  Of the schedule's
+        `steps` steps (T for DDPM) the last n = min(steps, max(1, round(s * steps))) run, 0 < s <= 1: x_0 is diffused to the
+        first of them by q(x_t | x_0) (GaussianDiffusion.diffuse at model time jump * n - 1), with `noise` as its z if given,
+        and the run goes on from there.  Low s stays close to x_0; s = 1 runs the whole schedule from a noised x_0.  Each
+        executed step is the step of a full run; the multistep history and feature reuse start afresh at the first one.
+        pred_x_t / pred_x_0 hold the n executed steps.  rng="torch" draws z with randn_like(x_0) before the steps."""
         return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold)
+                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
 
 
 class DdimSampler(_NativeSampler):
@@ -409,13 +457,13 @@ class DdimSampler(_NativeSampler):
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
                verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
         """Run `steps` DDIM steps (ddim.py:106-165).  `guidance_interval=(t_lo, t_hi)` as in DdpmSampler.sample, on the model
         time t - 1 of each step; `cache_interval` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample (the replace /
-        constrain guidance acts on the thresholded x_0)."""
+        constrain guidance acts on the thresholded x_0).  `init` / `init_strength` as in DdpmSampler.sample."""
         return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
                          interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold)
+                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -449,17 +497,18 @@ class DpmSolverSampler(_NativeSampler):
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, sde=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
         """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
         final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
         is drawn where DdimSampler draws it (`rng`).  `guidance_interval` as in DdimSampler.sample; the history D_{-1} of a
         step after an unguided one is that step's unguided D0.  `cache_interval` / `cache_branch` as in DdpmSampler.sample;
         the history D_{-1} of a step is that step's D0, from whichever forward ran.  `dynamic_threshold` as in
-        DdpmSampler.sample: D0 is the thresholded, guided x_0, and so is the history.  Same return dict as DdimSampler.sample."""
+        DdpmSampler.sample: D0 is the thresholded, guided x_0, and so is the history.  `init` / `init_strength` as in
+        DdpmSampler.sample; the first executed step is first order.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
-                         cache_branch=cache_branch, dynamic_threshold=dynamic_threshold)
+                         cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
 
 
 class UniPcSampler(_NativeSampler):
@@ -496,14 +545,15 @@ class UniPcSampler(_NativeSampler):
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
         """Run `steps` UniPC steps of order `order` (1, 2 or 3; 2 is the paper's choice for guided sampling).  Step i predicts
         at order min(order, i + 1) and corrects at the previous step's order; the first step has no corrector and the final
         step (to t_prev = 0) returns x_0 as DDIM does.  pred_x_t holds the predictions the network saw.  Draws no step noise;
         the torch RNG is consumed as DpmSolverSampler.sample(sde=False) consumes it.  `guidance_interval`, `cache_interval` /
         `cache_branch` and `dynamic_threshold` as in DpmSolverSampler.sample: the history holds the D0 of whichever forward
-        ran, thresholded.  Same return dict as DdimSampler.sample."""
+        ran, thresholded.  `init` / `init_strength` as in DdpmSampler.sample; the order ramp starts at the first executed step.
+        Same return dict as DdimSampler.sample."""
         assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold)
+                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
