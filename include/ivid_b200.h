@@ -136,6 +136,17 @@ int ivid_unet_forward_reuse(ivid_unet_t* h, const float* x_dev, int Nx, int H, i
                             const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, int cache_branch,
                             void* stream);
 
+/* Perturbed-attention forward (PAG, ivid_step_args_t.pag): ivid_unet_forward_hw in which rows [row0, N) replace the
+ * attention map of every attention layer in layers_host (num_layers indices into the attention layers in state-dict order,
+ * the layers whose "*.qkv.weight" keys they own) by the identity: the layer computes x + proj_out(V), V the fp16 value
+ * channels of its qkv projection.  Rows [0, row0) are the ordinary forward.  cache_branch = -1 runs the full forward,
+ * 0 <= b <= num_res_blocks the reuse forward at branch b (ivid_unet_forward_reuse), which perturbs the selected layers it
+ * recomputes.  Each (N, H, W, row0, layers) has a plan of its own, with its own graphs and feature cache.  row0 outside
+ * [0, N], num_layers < 1, or an index out of range or listed twice: IVID_ERR_INVALID_ARGUMENT. */
+int ivid_unet_forward_perturbed(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
+                                const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, int row0,
+                                const int* layers_host, int num_layers, int cache_branch, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Samplers — replace diffusion.samplers.DdpmSampler / DdimSampler (samplers/ddpm.py:12-187, samplers/ddim.py:12-165)
  * together with the framework's model_inference (classifier_free_guidance.py:23-42, inpaint_cfg.py:61-83,
@@ -251,6 +262,25 @@ typedef struct {
   int t_last3;
   const float* prev_xt_dev;
   float* corrected_xt_dev;
+  /* Perturbed-attention guidance (PAG; Ahn et al. 2024, "Self-Rectifying Diffusion Sampling with Perturbed-Attention
+   * Guidance", arXiv:2403.17377), every kind; zero means off.  The fields sit before start_step and the
+   * dynamic-threshold fields, which stay last.  With pag = 1 and pag_scale = w > 0 the forward gains N
+   * perturbed rows: the same x (read modulo N), t, class, conditional-input assembly and conditional-input noise as the
+   * conditional rows, with the attention map of every layer in pag_layers replaced by the identity (the layer outputs its V
+   * channels; ivid_unet_forward_perturbed).  The rows are [cond | null (only on a step with the classifier-free mix) |
+   * perturbed] and the classes [c, -1, c].  With G the eps of the step without PAG ((1+s) eps_c - s eps_u on a guided CFG
+   * step, (1+s) eps_c for strength < 0 with classes, eps_c otherwise), the step's eps is
+   *   eps = G + w * (eps_c - eps_perturbed)      (fp32, G first, then sub, mul, add each rounded to nearest),
+   * and everything after the mix (clipping or dynamic thresholding, replace / constrain, the updates, the history) reads it.
+   * The guidance interval gates both guidances: an unguided step runs one batch-N forward with eps = eps_c
+   * (ivid_sampler_step_dev keeps the full batch and ignores the extra rows).  pag = 0, or pag_scale = 0, runs no perturbed rows.
+   *   pag_layers: host array of pag_num_layers attention-layer indices, the positions of the attention layers ("*.qkv.weight")
+   *   in state-dict order; each in range and listed once.
+   * pag other than 0 / 1, or with pag_scale negative, infinite or NaN, or without layers: IVID_ERR_INVALID_ARGUMENT. */
+  int pag;
+  float pag_scale;
+  const int* pag_layers;
+  int pag_num_layers;
   /* Partial run (SDEdit, Meng et al. 2022, arXiv:2108.01073), ivid_sampler_run only; zero runs the whole grid.
    * ivid_sampler_run executes steps i = start_step .. steps-1 of the grid it builds (T steps for DDPM), from the x_inout_dev
    * of step start_step (ivid_sampler_diffuse below makes one from an image).  Each executed step keeps its t, t_prev,
@@ -300,6 +330,14 @@ int ivid_op_dynamic_threshold(const float* x_dev, int N, int M, double ratio, do
 /* ClassifierFreeGuidance.model_inference's mix alone (classifier_free_guidance.py:42): out = (1+s)*eps[0:count) -
  * s*eps[count:2*count) for the batch-2N forward's output (count = N*C*H*W, multiple of 4). */
 int ivid_cfg_mix(const float* eps2n_dev, float strength, float* out_dev, uint64_t count, void* stream);
+
+/* The whole guidance mix of a step alone, on the step kernels' element arithmetic (framework-level model_inference with
+ * perturbed-attention guidance).  eps_dev holds row blocks of count elements (count = N*C*H*W, multiple of 4): the conditional
+ * block, the null-class block when cfg = 1, the perturbed block when pag = 1.  out = G + pag_scale * (eps_c - eps_perturbed)
+ * (the term only with pag = 1), G = (1+s) eps_c - s eps_u (cfg 1), (1+s) eps_c (cfg 2) or eps_c (cfg 0), s = strength.
+ * cfg outside 0..2, pag outside 0 / 1, or pag_scale negative or not finite: IVID_ERR_INVALID_ARGUMENT. */
+int ivid_guidance_mix(const float* eps_dev, uint64_t count, int cfg, float strength, int pag, float pag_scale, float* out_dev,
+                      void* stream);
 
 /* sample: the whole reverse process on device (ddpm.py:134-187, ddim.py:106-165); x_inout_dev holds x_T on entry
  * and the samples on return.  `steps` = DDIM / DPM-Solver++ step count (ignored for DDPM, which runs all T).  Optional
@@ -472,6 +510,10 @@ int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, v
 /* The same with head width head_channels = C / heads (a multiple of 64, dividing C): qkv fp16 [N,T,3C] in the order
    [head][q|k|v][head_channels] -> fp16 [N,T,C].  head_channels = 64 computes exactly what ivid_op_attention computes. */
 int ivid_op_attention_heads(const void* qkv_dev, int N, int T, int C, int head_channels, void* out_dev, void* stream);
+/* The attention launch of a perturbed layer: rows [0, row0) as ivid_op_attention_heads over those rows alone, rows [row0, N)
+   the identity map, out[n, t, head_channels*h + c] = qkv[n, t, 3*head_channels*h + 2*head_channels + c] (0 <= row0 <= N). */
+int ivid_op_attention_perturbed(const void* qkv_dev, int N, int T, int C, int head_channels, int row0, void* out_dev,
+                                void* stream);
 
 #ifdef __cplusplus
 }

@@ -71,6 +71,10 @@ class StepArgsT(Structure):
         ("t_last3", c_int),
         ("prev_xt_dev", c_void_p),    # UniPC, single step: the corrector's base, the corrected x at t_last
         ("corrected_xt_dev", c_void_p),  # UniPC, optional output: this step's corrected x_t
+        ("pag", c_int),               # 1: perturbed-attention guidance, eps += pag_scale * (eps_c - eps_perturbed)
+        ("pag_scale", c_float),
+        ("pag_layers", POINTER(c_int)),   # host array: attention-layer indices in state-dict order
+        ("pag_num_layers", c_int),
         ("start_step", c_int),        # ivid_sampler_run: execute grid steps start_step .. steps-1 only (0 = all)
         ("dynamic_threshold", c_int), # 1: threshold x_0 at the threshold_ratio-quantile of |x_0| of each sample
         ("threshold_ratio", c_double),
@@ -129,6 +133,8 @@ SIGNATURES = {
                                      c_void_p]),
     "ivid_unet_forward_reuse": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p,
                                         c_int, c_int, c_void_p]),
+    "ivid_unet_forward_perturbed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(CondT), c_void_p, c_void_p, c_void_p,
+                                            c_int, c_int, POINTER(c_int), c_int, c_int, c_void_p]),
     "ivid_conv_tile": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "ivid_unet_debug_tap": (c_int, [c_void_p, c_int, c_char_p, c_void_p, c_uint64, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "ivid_unet_profile_begin": (c_int, [c_void_p]),
@@ -139,6 +145,7 @@ SIGNATURES = {
     "ivid_sampler_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(StepArgsT), c_void_p]),
     "ivid_sampler_step_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, POINTER(StepArgsT), c_void_p]),
     "ivid_cfg_mix": (c_int, [c_void_p, c_float, c_void_p, c_uint64, c_void_p]),
+    "ivid_guidance_mix": (c_int, [c_void_p, c_uint64, c_int, c_float, c_int, c_float, c_void_p, c_void_p]),
     "ivid_op_dynamic_threshold": (c_int, [c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_void_p, c_void_p]),
     "ivid_sampler_run": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(StepArgsT), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ivid_sampler_diffuse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_uint64, c_int, c_uint64, c_void_p, c_void_p]),
@@ -154,6 +161,7 @@ SIGNATURES = {
     "ivid_op_group_norm_apply": (c_int, [POINTER(OpGnT), c_void_p]),
     "ivid_op_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention_heads": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "ivid_op_attention_perturbed": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_warp_create": (c_int, [c_int, c_int, c_int, c_int, c_double, c_double, c_int, POINTER(c_void_p)]),
     "ivid_warp_destroy": (c_int, [c_void_p]),
     "ivid_warp_reset": (c_int, [c_void_p]),

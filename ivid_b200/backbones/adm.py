@@ -17,7 +17,10 @@ import torch.nn as nn
 
 from .. import _lib
 
-__all__ = ["AdmUnet2d"]
+__all__ = ["AdmUnet2d", "PAG_DEFAULT_LAYERS"]
+
+# perturbed-attention guidance: every ADM network has an attention layer in its middle block (not a claim that it is best)
+PAG_DEFAULT_LAYERS = ("middle_block.1",)
 
 
 class _Params(nn.Module):
@@ -184,6 +187,51 @@ class AdmUnet2d(nn.Module):
         return p.value, n.value
 
     # ------------------------------------------------------------------------------------------------------------
+    @property
+    def attention_layers(self):
+        """Names of the attention layers ("input_blocks.7.1", "middle_block.1", ...) in state-dict order; the position of a
+        name is the layer index of the C ABI's perturbed-attention entry points."""
+        return [k[: -len(".qkv.weight")] for k, _, _ in self._schema if k.endswith(".qkv.weight")]
+
+    def pag_layer_indices(self, layers):
+        """Indices of the named attention layers (AssertionError for an empty selection, an unknown or a repeated name)."""
+        assert not isinstance(layers, str), f"pag_layers must be a sequence of layer names, got the string {layers!r}"
+        layers = list(layers)
+        assert layers, "pag_layers must name at least one attention layer"
+        names = self.attention_layers
+        for name in layers:
+            assert name in names, f"{name!r} is not an attention layer of this network (attention layers: {names})"
+        assert len(set(layers)) == len(layers), f"pag_layers lists a layer twice: {layers}"
+        return [names.index(name) for name in layers]
+
+    def _check_input(self, x, classes):
+        """The input assertions of forward() and forward_perturbed() (adm.py:540-549)."""
+        assert classes is None or self.num_classes is not None, "this model is not class-conditioned"
+        if classes is not None:
+            assert bool(torch.all(classes >= 0)) or self.has_null_class, "this model does not have a null class"
+            assert classes.shape == (x.shape[0],), "classes must be a 1-D batch of labels"
+        assert x.dim() == 4 and x.shape[1] == self.in_channels, \
+            f"expected input [N,{self.in_channels},H,W], got {tuple(x.shape)}"
+
+    @torch.no_grad()
+    def forward_perturbed(self, x, times, classes=None, layers=PAG_DEFAULT_LAYERS):
+        """forward() with the attention map of every layer in `layers` replaced by the identity (perturbed-attention
+        guidance, Ahn et al. 2024, arXiv:2403.17377): each such layer computes x + proj_out(V), V the value channels of its
+        qkv projection.  Every row of the batch is perturbed.  Same arguments and return as forward()."""
+        idx = self.pag_layer_indices(layers)
+        self._check_input(x, classes)
+        self._ensure_packed()
+        N, _, H, W = x.shape
+        xx = x.to(torch.float32).contiguous()
+        tt = times.to(device=x.device, dtype=torch.int64).contiguous()
+        cc = classes.to(device=x.device, dtype=torch.int64).contiguous() if classes is not None else None
+        out = torch.empty((N, self.out_channels, H, W), dtype=torch.float32, device=x.device)
+        arr = (ctypes.c_int * len(idx))(*idx)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().ivid_unet_forward_perturbed(self._handle, _lib.ptr(xx), N, H, W, None, _lib.ptr(tt), _lib.ptr(cc),
+                                                              _lib.ptr(out), N, 0, arr, len(idx), -1, _lib.cur_stream(x.device)))
+        return out.type(x.dtype)
+
     @torch.no_grad()
     def forward(self, x, times, classes=None):
         """Apply the model to an input batch (reference adm.py:526-566).
@@ -192,12 +240,7 @@ class AdmUnet2d(nn.Module):
         H and W need not equal image_size (which only places the attention blocks): like the reference, any size divisible
         by 2^(len(channel_mult) - 1) runs, and other sizes raise RuntimeError.
         """
-        assert classes is None or self.num_classes is not None, "this model is not class-conditioned"
-        if classes is not None:
-            assert bool(torch.all(classes >= 0)) or self.has_null_class, "this model does not have a null class"
-            assert classes.shape == (x.shape[0],), "classes must be a 1-D batch of labels"
-        assert x.dim() == 4 and x.shape[1] == self.in_channels, \
-            f"expected input [N,{self.in_channels},H,W], got {tuple(x.shape)}"
+        self._check_input(x, classes)
         self._ensure_packed()
         N, _, H, W = x.shape
         xx = x.to(torch.float32).contiguous()

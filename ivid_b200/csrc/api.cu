@@ -141,6 +141,20 @@ int ivid_unet_forward_reuse(ivid_unet_t* h, const float* x_dev, int Nx, int H, i
                      cache_branch);
   });
 }
+int ivid_unet_forward_perturbed(ivid_unet_t* h, const float* x_dev, int Nx, int H, int W, const ivid_cond_t* cond,
+                                const int64_t* t_dev, const int64_t* classes_dev, float* eps_dev, int N, int row0,
+                                const int* layers_host, int num_layers, int cache_branch, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(h); IVID_NOT_NULL(x_dev); IVID_NOT_NULL(t_dev); IVID_NOT_NULL(eps_dev);
+    IVID_REQUIRE(num_layers >= 1 && layers_host != nullptr, "perturbed forward: at least one attention layer");
+    IVID_REQUIRE(row0 >= 0 && row0 <= N, "perturbed forward: row0 must lie in [0, N]");
+    AttnPerturb pert;
+    pert.row0 = row0;
+    pert.layers.assign(layers_host, layers_host + num_layers);
+    h->impl->forward(x_dev, Nx, H, W, cond, t_dev, classes_dev, eps_dev, N, static_cast<cudaStream_t>(stream), nullptr,
+                     cache_branch, &pert);
+  });
+}
 // the square forwards at the backbone's image_size
 int ivid_unet_forward(ivid_unet_t* h, const float* x_dev, int Nx, const int64_t* t_dev, const int64_t* classes_dev,
                       float* eps_dev, int N, void* stream) {
@@ -222,6 +236,13 @@ int ivid_cfg_mix(const float* eps2n_dev, float strength, float* out_dev, uint64_
   return guarded([&] {
     IVID_NOT_NULL(eps2n_dev); IVID_NOT_NULL(out_dev);
     launch_cfg_mix(eps2n_dev, out_dev, static_cast<size_t>(count), strength, static_cast<cudaStream_t>(stream));
+  });
+}
+int ivid_guidance_mix(const float* eps_dev, uint64_t count, int cfg, float strength, int pag, float pag_scale, float* out_dev,
+                      void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(eps_dev); IVID_NOT_NULL(out_dev);
+    launch_guidance_mix(eps_dev, out_dev, static_cast<size_t>(count), cfg, strength, pag, pag_scale, static_cast<cudaStream_t>(stream));
   });
 }
 int ivid_op_dynamic_threshold(const float* x_dev, int N, int M, double ratio, double threshold_max, float* s_out_dev,
@@ -402,6 +423,19 @@ int ivid_op_attention_heads(const void* qkv_dev, int N, int T, int C, int head_c
     IVID_NOT_NULL(qkv_dev); IVID_NOT_NULL(out_dev);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     std::unique_ptr<AttnLaunch, void (*)(AttnLaunch*)> l(attn_launch_create(qkv_dev, N, T, C, head_channels, out_dev), attn_launch_destroy);
+    attn_launch_run(l.get(), st);
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+  });
+}
+
+int ivid_op_attention_perturbed(const void* qkv_dev, int N, int T, int C, int head_channels, int row0, void* out_dev,
+                                void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(qkv_dev); IVID_NOT_NULL(out_dev);
+    IVID_REQUIRE(row0 >= 0 && row0 <= N, "attention: row0 must lie in [0, N]");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    std::unique_ptr<AttnLaunch, void (*)(AttnLaunch*)> l(attn_launch_create(qkv_dev, N, T, C, head_channels, out_dev, row0),
+                                                         attn_launch_destroy);
     attn_launch_run(l.get(), st);
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
   });

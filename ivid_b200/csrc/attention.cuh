@@ -190,4 +190,21 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant
   }
 }
 
+// Perturbed-attention rows (PAG, Ahn et al. 2024, arXiv:2403.17377): the attention map is replaced by the identity, so the
+// output of each head is its V channels, copied bit for bit.  Rows [row0, N) of qkv [N][T][3C] (head h of width d owns q|k|v
+// at channels [3dh, 3dh + 3d)) -> out [N][T][C] channel dh + c = qkv channel 3dh + 2d + c.  One 16-byte group of 8 channels
+// per work item (C and d are multiples of 64, so a group never straddles a head).
+__global__ void __launch_bounds__(256) attention_identity_kernel(const __half* __restrict__ qkv, __half* __restrict__ out,
+                                                                 size_t row0, size_t rows, int C, int d) {
+  const int groups = C / 8;
+  const size_t items = rows * groups;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < items; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t row = row0 + i / groups;                  // n * T + t
+    const int c8 = static_cast<int>(i % groups) * 8;
+    const int h = c8 / d, c = c8 - h * d;
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(qkv + row * 3 * C + 3 * d * h + 2 * d + c));
+    *reinterpret_cast<uint4*>(out + row * C + c8) = v;
+  }
+}
+
 }  // namespace ivid

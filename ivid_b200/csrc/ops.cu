@@ -247,6 +247,12 @@ void conv_launch_run(const ConvLaunch* l, cudaStream_t s) {
   }
 }
 
+static int ew_grid(size_t work_items, int block) {
+  const size_t blocks = (work_items + block - 1) / block;
+  const size_t cap = static_cast<size_t>(sm_count()) * 16;
+  return static_cast<int>(std::max<size_t>(1, std::min(blocks, cap)));
+}
+
 // --------------------------------------------------------------------------------------------------
 // attention
 // --------------------------------------------------------------------------------------------------
@@ -259,14 +265,23 @@ struct AttnLaunch {
   bool qres = false;
   int smem = 0;
   int grid;
+  // rows [row0, N) take the identity output (attention_identity_kernel); the softmax kernels run over rows [0, row0)
+  int N = 0, T = 0, C = 0, row0 = 0;
+  const __half* qkv = nullptr;
+  __half* out = nullptr;
 };
 
-AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out) {
+AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out, int row0) {
   if (head_ch <= 0 || head_ch % 64 != 0)
     throw Error(kErrNotImplemented, "attention: head width " + std::to_string(head_ch) + " is not a multiple of 64");
   IVID_REQUIRE(C % head_ch == 0, "attention: channels must be a multiple of the head width " + std::to_string(head_ch));
   IVID_REQUIRE(T >= 1, "attention: sequence length must be positive");
+  if (row0 < 0) row0 = N;
+  IVID_REQUIRE(row0 <= N, "attention: the perturbed-row start must lie in [0, N]");
   auto* l = new AttnLaunch();
+  l->N = N; l->T = T; l->C = C; l->row0 = row0;
+  l->qkv = static_cast<const __half*>(qkv);
+  l->out = static_cast<__half*>(out);
   l->head_ch = head_ch;
   l->p.N = N; l->p.T = T; l->p.C = C; l->p.heads = C / 64;
   l->p.q_tiles = (T + 127) / 128;
@@ -279,7 +294,7 @@ AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch
                             CU_TENSOR_MAP_SWIZZLE_128B);
   l->mapKV = make_tensor_map(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(qkv), dims, str, boxkv,
                              CU_TENSOR_MAP_SWIZZLE_128B);
-  l->grid = N * l->p.heads * l->p.q_tiles;
+  l->grid = row0 * l->p.heads * l->p.q_tiles;
   if (head_ch == 64) return l;
   // wider heads: k = d/64 chunks; ceil(k/4) output-column slices of nv <= 4 boxes (see attention_hd.cuh)
   using Cfg = AttnHdCfg;
@@ -299,7 +314,7 @@ AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch
   hp.stages = std::min(Cfg::MAX_STAGES, (budget - fixed) / Cfg::stage_bytes(l->qres));
   IVID_REQUIRE(hp.stages >= 4, "attention: shared-memory ring too shallow");
   l->smem = fixed + hp.stages * Cfg::stage_bytes(l->qres);
-  l->grid = N * hp.heads * hp.q_tiles * hp.slices;
+  l->grid = row0 * hp.heads * hp.q_tiles * hp.slices;
   return l;
 }
 void attn_launch_destroy(AttnLaunch* l) { delete l; }
@@ -315,6 +330,18 @@ static void run_attn_hd(const AttnLaunch* l, cudaStream_t s) {
 }
 
 void attn_launch_run(const AttnLaunch* l, cudaStream_t s) {
+  attn_launch_run_identity(l, s);
+  attn_launch_run_softmax(l, s);
+}
+void attn_launch_run_identity(const AttnLaunch* l, cudaStream_t s) {
+  if (l->row0 == l->N) return;
+  const size_t rows = static_cast<size_t>(l->N - l->row0) * l->T;
+  attention_identity_kernel<<<ew_grid(rows * (l->C / 8), 256), 256, 0, s>>>(l->qkv, l->out, static_cast<size_t>(l->row0) * l->T, rows,
+                                                                         l->C, l->head_ch);
+  IVID_CHECK_CUDA(cudaGetLastError());
+}
+void attn_launch_run_softmax(const AttnLaunch* l, cudaStream_t s) {
+  if (l->row0 == 0) return;
   if (l->head_ch != 64) {
     switch (l->nv * 2 + (l->qres ? 1 : 0)) {
       case 5: run_attn_hd<2, true>(l, s); break;
@@ -338,11 +365,6 @@ void attn_launch_run(const AttnLaunch* l, cudaStream_t s) {
 // --------------------------------------------------------------------------------------------------
 // element-wise / embedding
 // --------------------------------------------------------------------------------------------------
-static int ew_grid(size_t work_items, int block) {
-  const size_t blocks = (work_items + block - 1) / block;
-  const size_t cap = static_cast<size_t>(sm_count()) * 16;
-  return static_cast<int>(std::max<size_t>(1, std::min(blocks, cap)));
-}
 
 void launch_gn_stats(const float* x, double* stats, int N, int HW, int C, cudaStream_t s) {
   IVID_REQUIRE(C % 4 == 0, "gn_stats: C % 4");

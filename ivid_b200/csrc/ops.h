@@ -79,10 +79,14 @@ struct ConvPack {
 ConvPack conv_pack(const float* w, const float* b, int cout, int cin, int ksz, int pitch, const float* w2, const float* b2,
                    int cin2, int cin2a, bool e4m3);
 
-// head_ch = 64: attention_kernel; any other multiple of 64: attention_hd_kernel (kErrNotImplemented otherwise)
-AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out);
+// head_ch = 64: attention_kernel; any other multiple of 64: attention_hd_kernel (kErrNotImplemented otherwise).
+// row0 in [0, N] (-1: N): rows [0, row0) run that kernel, exactly as a launch over those rows alone; rows [row0, N) take the
+// perturbed-attention identity output, each head's V channels (attention_identity_kernel)
+AttnLaunch* attn_launch_create(const void* qkv, int N, int T, int C, int head_ch, void* out, int row0 = -1);
 void attn_launch_destroy(AttnLaunch* l);
-void attn_launch_run(const AttnLaunch* l, cudaStream_t s);
+void attn_launch_run(const AttnLaunch* l, cudaStream_t s);                    // both parts below
+void attn_launch_run_softmax(const AttnLaunch* l, cudaStream_t s);            // rows [0, row0) only (nothing at row0 = 0)
+void attn_launch_run_identity(const AttnLaunch* l, cudaStream_t s);           // rows [row0, N) only (nothing at row0 = N)
 
 void launch_gn_stats(const float* x, double* stats, int N, int HW, int C, cudaStream_t s);
 struct GnApplyDesc {
@@ -115,6 +119,9 @@ struct CondPackDesc {
 };
 void launch_cond_pack(const CondPackDesc& d, cudaStream_t s);   // sampler.cu
 void launch_cfg_mix(const float* eps2, float* out, size_t count, float strength, cudaStream_t s);   // sampler.cu
+// the step's guidance mix over row blocks of `count` elements (include/ivid_b200.h, ivid_guidance_mix)   // sampler.cu
+void launch_guidance_mix(const float* eps, float* out, size_t count, int cfg, float strength, int pag, float pag_scale,
+                         cudaStream_t s);
 // dynamic thresholding of x [N][M] (sampler.cuh): s_out [N] and x_out = clamp(x, -s, s) / s; threshold_max <= 0: no upper bound
 void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double threshold_max, float* s_out, float* x_out,
                               cudaStream_t s);   // sampler.cu

@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 
 #include "sampler.cuh"
 
@@ -188,6 +189,12 @@ __global__ void fill_classes_kernel(const int64_t* classes, int64_t* out, int N)
   for (int i = threadIdx.x + blockIdx.x * blockDim.x; i < 2 * N; i += blockDim.x * gridDim.x)
     out[i] = i < N ? classes[i] : -1;
 }
+// the classes of a forward with perturbed-attention rows: [c, -1, c] with the null-class block (cfg 1), [c, c] without
+__global__ void fill_classes_pag_kernel(const int64_t* classes, int64_t* out, int N, int null_block) {
+  const int blocks = null_block ? 3 : 2;
+  for (int i = threadIdx.x + blockIdx.x * blockDim.x; i < blocks * N; i += blockDim.x * gridDim.x)
+    out[i] = (null_block && i >= N && i < 2 * N) ? -1 : classes[i % N];
+}
 
 // blocks of 256 threads for a grid-stride loop over `units` work units: at most 8 per SM
 static int elementwise_grid(size_t units) {
@@ -198,6 +205,20 @@ void launch_cfg_mix(const float* eps2, float* out, size_t count, float strength,
   IVID_REQUIRE(count % 4 == 0, "cfg mix: element count must be a multiple of 4");
   const size_t n4 = count / 4;
   cfg_mix_kernel<<<elementwise_grid(n4), 256, 0, s>>>(eps2, out, n4, strength);
+  IVID_CHECK_CUDA(cudaGetLastError());
+}
+
+void launch_guidance_mix(const float* eps, float* out, size_t count, int cfg, float strength, int pag, float pag_scale,
+                         cudaStream_t s) {
+  IVID_REQUIRE(count % 4 == 0, "guidance mix: element count must be a multiple of 4");
+  IVID_REQUIRE(cfg >= 0 && cfg <= 2, "guidance mix: cfg must be 0, 1 or 2");
+  IVID_REQUIRE(pag == 0 || pag == 1, "guidance mix: pag must be 0 or 1");
+  IVID_REQUIRE(!pag || (std::isfinite(pag_scale) && pag_scale >= 0.0f), "guidance mix: pag_scale must be finite and >= 0");
+  StepParams p;
+  std::memset(&p, 0, sizeof(p));
+  p.cfg = cfg; p.strength = strength; p.pag = pag; p.pag_scale = pag_scale;
+  const size_t n4 = count / 4;
+  guidance_mix_kernel<<<elementwise_grid(n4), 256, 0, s>>>(eps, out, n4, p);
   IVID_CHECK_CUDA(cudaGetLastError());
 }
 
@@ -219,25 +240,33 @@ struct StepTail {
 
 // The tail of a step from x_0 source src (sampler.cuh: EpsRows after the forward, HeadTaps as the forward's last node): the
 // update, or with a dynamic threshold x_0 into t.x0, s of every sample and the update on the thresholded x_0.
-template <typename Src>
+template <bool kPag, typename Src>
 static void launch_step_tail(const StepParams& p, const Src& src, const StepTail& t, cudaStream_t st) {
   auto update = [&](const auto& from) {
+    using From = std::decay_t<decltype(from)>;
+    constexpr bool kP = kPag && !std::is_same_v<From, ThresholdedX0>;   // thresholded x_0 has the PAG term in it already
     const int grid = elementwise_grid(from.units(p));
-    if (t.unipc) step_kernel<<<grid, 256, 0, st>>>(p, from, t.uni);
-    else if (t.kind == kStepDdim) step_kernel<<<grid, 256, 0, st>>>(p, from, Update<kStepDdim>());
-    else if (t.kind == kStepDpm) step_kernel<<<grid, 256, 0, st>>>(p, from, Update<kStepDpm>());
-    else step_kernel<<<grid, 256, 0, st>>>(p, from, Update<kStepDdpm>());
+    if (t.unipc) step_kernel<From, UniPcUpdate, kP><<<grid, 256, 0, st>>>(p, from, t.uni);
+    else if (t.kind == kStepDdim) step_kernel<From, Update<kStepDdim>, kP><<<grid, 256, 0, st>>>(p, from, Update<kStepDdim>());
+    else if (t.kind == kStepDpm) step_kernel<From, Update<kStepDpm>, kP><<<grid, 256, 0, st>>>(p, from, Update<kStepDpm>());
+    else step_kernel<From, Update<kStepDdpm>, kP><<<grid, 256, 0, st>>>(p, from, Update<kStepDdpm>());
     IVID_CHECK_CUDA(cudaGetLastError());
   };
   if (!t.threshold) {
     update(src);
     return;
   }
-  step_kernel<<<elementwise_grid(src.units(p)), 256, 0, st>>>(p, src, StoreX0{t.x0});
+  step_kernel<Src, StoreX0, kPag><<<elementwise_grid(src.units(p)), 256, 0, st>>>(p, src, StoreX0{t.x0});
   IVID_CHECK_CUDA(cudaGetLastError());
   threshold_select_kernel<<<p.N, kSelectThreads, 0, st>>>(t.x0, p.C * p.HW, t.ratio, t.s_max, t.s);
   IVID_CHECK_CUDA(cudaGetLastError());
   update(ThresholdedX0{t.x0, t.s});
+}
+// the PAG instantiations only for a step with the perturbed rows (StepParams::pag)
+template <typename Src>
+static void launch_step_tail(const StepParams& p, const Src& src, const StepTail& t, cudaStream_t st) {
+  if (p.pag) launch_step_tail<true>(p, src, t, st);
+  else launch_step_tail<false>(p, src, t, st);
 }
 
 void Sampler::diffuse(const float* x0, const float* noise, int N, size_t per_sample, int t, uint64_t seed, float* out,
@@ -420,16 +449,32 @@ void Sampler::check_step_args(const ivid_step_args_t& a, const Unet& unet, int N
                "constrain_depth is applied inside replace_depth (ddim.py:90-95)");
   IVID_REQUIRE(a.kind != kStepDdpm || (a.replace_rgb_dev == nullptr && a.replace_depth_dev == nullptr),
                "replace/constrain guidance is DDIM / DPM-Solver++ only");
+  // perturbed-attention guidance: a flag, a finite scale >= 0 and at least one attention layer, each listed once
+  IVID_REQUIRE(a.pag == 0 || a.pag == 1, "pag must be 0 or 1");
+  if (a.pag) {
+    IVID_REQUIRE(std::isfinite(a.pag_scale) && a.pag_scale >= 0.0f, "pag_scale must be finite and >= 0");
+    IVID_REQUIRE(a.pag_layers != nullptr && a.pag_num_layers >= 1, "pag needs at least one attention layer (pag_layers)");
+    const int L = unet.num_attention_layers();
+    for (int i = 0; i < a.pag_num_layers; ++i) {
+      IVID_REQUIRE(a.pag_layers[i] >= 0 && a.pag_layers[i] < L,
+                   "pag_layers: attention layer index " + std::to_string(a.pag_layers[i]) + " out of range [0, " + std::to_string(L) + ")");
+      for (int j = 0; j < i; ++j) IVID_REQUIRE(a.pag_layers[j] != a.pag_layers[i], "pag_layers: a layer is listed twice");
+    }
+  }
 }
+
+// whether a step runs the perturbed-attention rows at all: pag with a positive scale (pag_scale 0 is the step without them)
+static bool pag_on(const ivid_step_args_t& a) { return a.pag != 0 && a.pag_scale > 0.0f; }
 
 // What one step runs, decided in one place from the arguments and the step.
 struct StepPlan {
   int t_index;        // table row of the model time: t for DDPM, t - 1 for DDIM / DPM-Solver++ (ddim.py:81)
   int t_prev;         // DDIM / DPM-Solver++: the previous actual step
-  bool gated;         // a guidance interval applies: use_cfg, classes and an interval
+  bool gated;         // a guidance interval applies: an interval and a guidance (use_cfg with classes, or pag)
   bool guided;        // host route: the model time lies inside the interval (or none applies); the device route sets true
   int cfg;            // StepParams::cfg
-  int Nf;             // the forward's batch: 2N exactly when cfg == 1
+  bool pag;           // the forward carries the perturbed-attention rows (last block of N)
+  int Nf;             // the forward's batch: N, + N null-class rows when cfg == 1, + N perturbed rows with pag
   int order;          // DPM-Solver++ order of the update: 2 with a previous data prediction unless order = 1, else 1;
                       // UniPC: the predictor order min(order, nhist + 1), 1 on the final step (device route: at most that)
   int corr_order;     // UniPC: the corrector order min(order, nhist), 0 without history (device route: at most that)
@@ -446,7 +491,8 @@ static StepPlan plan_step(const ivid_step_args_t& a, int N, int t, int t_prev, b
   // guidance interval: a step whose model time lies outside it is the step at strength 0, eps = eps_c of one forward.  The
   // host route knows t and runs that step as a batch-N forward; the device route keeps the batch-2N forward and the step
   // kernel reads the guided flag set_step_kernel writes.  Without classes (or use_cfg) only one forward runs anyway.
-  sp.gated = a.guidance_interval != 0 && a.use_cfg && has_classes;
+  // The interval gates perturbed-attention guidance too: an unguided step has neither term.
+  sp.gated = a.guidance_interval != 0 && ((a.use_cfg && has_classes) || pag_on(a));
   sp.guided = !sp.gated || t_on_device || (sp.t_index >= a.guidance_t_lo && sp.t_index <= a.guidance_t_hi);
   // classifier-free guidance: one batch-2N forward when strength > 0 and the model is class conditional (cfg 1).
   // inpaint_cfg.py:77-78 / sr_cfg.py:53-54: classes None -> single null-class forward, no (1+s) scaling.
@@ -455,7 +501,8 @@ static StepPlan plan_step(const ivid_step_args_t& a, int N, int t, int t_prev, b
   const bool two = a.use_cfg && has_classes && a.strength > 0.0f && sp.guided;
   const bool scale_only = a.use_cfg && a.strength < 0.0f && (has_classes || a.cond.kind == 0) && sp.guided;
   sp.cfg = two ? 1 : (scale_only ? 2 : 0);
-  sp.Nf = two ? 2 * N : N;
+  sp.pag = pag_on(a) && sp.guided;
+  sp.Nf = (two ? 2 * N : N) + (sp.pag ? N : 0);
   sp.order = (a.kind == kStepDpm && a.prev_x0_dev != nullptr && a.order != 1) ? 2 : 1;
   sp.corr_order = 0;
   sp.nhist = 0;
@@ -533,7 +580,16 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
                                          sp.gated ? 1 : 0, a.guidance_t_lo, a.guidance_t_hi, up);
   IVID_CHECK_CUDA(cudaGetLastError());
   const int64_t* cls = a.classes_dev;
-  if (sp.cfg == 1) {
+  if (sp.pag) {
+    // [c, -1, c] or [c, c] of the forward with perturbed rows; no classes stay no classes
+    if (cls != nullptr) {
+      if (!classes2_filled) {
+        fill_classes_pag_kernel<<<1, 256, 0, stream>>>(a.classes_dev, d_classes2_, N, sp.cfg == 1 ? 1 : 0);
+        IVID_CHECK_CUDA(cudaGetLastError());
+      }
+      cls = d_classes2_;
+    }
+  } else if (sp.cfg == 1) {
     // [classes, -1 ...] of the batch-2N forward
     if (!classes2_filled) {
       fill_classes_kernel<<<1, 256, 0, stream>>>(a.classes_dev, d_classes2_, N);
@@ -555,6 +611,7 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
   p.N = N; p.C = C; p.HW = HW;
   p.cfg = sp.cfg;
   p.strength = a.strength;
+  if (sp.pag) { p.pag = 1; p.pag_scale = a.pag_scale; }
   p.clip = a.clip_denoised; p.eta = a.eta; p.seed = a.seed; p.stream = 0;
   p.stream_dev = &state->stream;
   if (dpm && !a.unipc) {
@@ -612,8 +669,13 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
       launch_step_tail(p, HeadTaps{Y, bias, Hy, Wy, ldy}, tail, st);
     };
   }
+  AttnPerturb pert;
+  if (sp.pag) {
+    pert.row0 = sp.Nf - N;
+    pert.layers.assign(a.pag_layers, a.pag_layers + a.pag_num_layers);
+  }
   unet.forward(x_t, N, H, W, cond.kind ? &cond : nullptr, d_t_, cls, fuse ? nullptr : d_eps_, sp.Nf, stream, fuse ? &hook : nullptr,
-               sp.cache_branch);
+               sp.cache_branch, sp.pag ? &pert : nullptr);
   unet.set_cond_stream_dev(nullptr);
   if (!fuse) launch_step_tail(p, EpsRows{d_eps_}, tail, stream);
 }
@@ -633,7 +695,8 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   IVID_REQUIRE(s0 >= 0 && s0 < steps, "start_step must satisfy 0 <= start_step < steps");
   const int jump = T_ / steps;                     // ddim.py:153
   IVID_CHECK_CUDA(cudaSetDevice(unet.device()));
-  ensure_device(2 * N, 2 * img);
+  const int rows = pag_on(a) ? 3 : 2;             // the largest forward of the run, in blocks of N
+  ensure_device(rows * N, rows * img);
   if (dpm) ensure_hist(a.unipc ? kUniPcPlanes * img : img);   // before the loop: the history must not move between steps
   if (dpm && !a.sde) noise_all = nullptr;          // the ODE solver draws no step noise
   // the fused head step needs per-step pointers that stay the same from step to step
@@ -643,10 +706,10 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   // per denoising step the host then issues three calls: the step-state kernel, ONE CUDA-graph launch (the whole batch-2N
   // forward, batch-N for a step outside the guidance interval: each batch has its own plan and graphs) and the fused
   // guidance-mix + x_{t-1} update.  The first batch-2N step fills [classes, -1 ...] once for the whole reverse process.
-  // feature reuse: a full forward at the first executed step, at a switch between the batch-2N and batch-N plans, and every
-  // cache_interval steps after the last full one; reuse forwards in between
-  int last_full = 0;
-  bool last_two = false, classes2_filled = false;
+  // feature reuse: a full forward at the first executed step, at a switch between plans (batch 2N or 3N and batch N), and
+  // every cache_interval steps after the last full one; reuse forwards in between
+  int last_full = 0, last_nf = 0;
+  bool classes2_filled = false;
   for (int i = s0; i < steps; ++i) {
     const int k = i - s0;
     int t, t_prev;
@@ -670,10 +733,10 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
     }
     if (cond_noise_all && ai.cond.kind == 1)
       ai.cond.noise_dev = cond_noise_all + static_cast<size_t>(k) * N * 4 * hw;
-    const bool two = plan_step(ai, N, t, t_prev, false).Nf == 2 * N;
-    const bool full = a.cache_interval <= 1 || k == 0 || two != last_two || k - last_full >= a.cache_interval;
+    const int nf = plan_step(ai, N, t, t_prev, false).Nf;
+    const bool full = a.cache_interval <= 1 || k == 0 || nf != last_nf || k - last_full >= a.cache_interval;
     if (full) last_full = k;
-    last_two = two;
+    last_nf = nf;
     ai.cache_reuse = full ? 0 : 1;
     float* dst = traj_xt ? traj_xt + static_cast<size_t>(k) * img : bufs[cur ^ 1];
     float* x0 = traj_x0 ? traj_x0 + static_cast<size_t>(k) * img : nullptr;
@@ -681,7 +744,7 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
     if (traj_xt && k == 0) src = x;
     step_impl(unet, src, dst, x0, N, plan_step(ai, N, t, t_prev, false), ai, i, stream, nullptr, nullptr, allow_fuse,
               classes2_filled);
-    classes2_filled = classes2_filled || two;
+    classes2_filled = classes2_filled || nf > N;     // every guided step of a run has the same row layout
     if (!traj_xt) cur ^= 1;
   }
   const float* last = traj_xt ? traj_xt + static_cast<size_t>(steps - 1 - s0) * img : bufs[cur];

@@ -113,6 +113,10 @@ struct StepParams {
   // guidance interval on the device-timestep route (appended): device flag, 0 = this step is unguided, so eps = eps_c
   // whatever cfg says (the null-class rows are ignored); nullptr = always guided
   const int* guided;
+  // perturbed-attention guidance (appended): 1 = the eps rows hold a third block, the forward with identity attention maps,
+  // after the conditional (and, at cfg 1, the null-class) rows, and eps gains pag_scale * (eps_c - eps_perturbed)
+  int pag;
+  float pag_scale;
 };
 
 // (1 + strength) * eps_c - strength * eps_u (only evaluated with strength > 0).  Every product / sum of the step arithmetic is
@@ -121,21 +125,53 @@ struct StepParams {
 __device__ __forceinline__ float cfg_mix(float ec, float eu, float strength) {
   return __fsub_rn(__fmul_rn(__fadd_rn(1.0f, strength), ec), __fmul_rn(strength, eu));
 }
-// cfg of this step: p.cfg, or 0 when the device flag says the step lies outside the guidance interval
-__device__ __forceinline__ int step_cfg(const StepParams& p) { return (p.guided != nullptr && *p.guided == 0) ? 0 : p.cfg; }
-// the guidance-mixed eps of four elements, cfg = step_cfg(p): eps(false, e) loads the conditional eps, eps(true, e) the
-// unconditional one (called only when cfg == 1)
+// the guidance of this step: p.cfg in bits 0-1 and kPagBit when the perturbed-attention term applies; 0 when the device
+// flag says the step lies outside the guidance interval (which gates both guidances)
+constexpr int kPagBit = 4;
+__device__ __forceinline__ int step_cfg(const StepParams& p) {
+  return (p.guided != nullptr && *p.guided == 0) ? 0 : (p.cfg | (p.pag ? kPagBit : 0));
+}
+// row block of the perturbed eps: after the conditional rows, and after the null-class rows when cfg & 3 == 1
+__device__ __forceinline__ int pag_block(int cfg) { return (cfg & 3) == 1 ? 2 : 1; }
+// the guidance-mixed eps of four elements, cfg = step_cfg(p): eps(b, e) loads row block b of eps: 0 the conditional rows,
+// 1 the null-class rows (called only when cfg & 3 == 1), pag_block(cfg) the perturbed rows (only with kPagBit).  The
+// classifier-free part G is formed first, then G + pag_scale * (eps_c - eps_perturbed), each operation rounded on its own.
+// eps_c is loaded again for the PAG term rather than kept live across G (the same bits: every source is deterministic).  The
+// step kernels take the term as a compile-time switch (step_kernel's kPag): without it cfg & kPagBit is known to be 0, the
+// branch is not compiled, and the steps without PAG keep the code they had before it existed.
 template <typename Eps>
 __device__ __forceinline__ void mix_eps4(const StepParams& p, int cfg, Eps&& eps, float (&e)[4]) {
-  eps(false, e);
-  if (cfg == 1) {
+  eps(0, e);
+  if ((cfg & 3) == 1) {
     float eu[4];
-    eps(true, eu);
+    eps(1, eu);
 #pragma unroll
     for (int j = 0; j < 4; ++j) e[j] = cfg_mix(e[j], eu[j], p.strength);
-  } else if (cfg == 2) {
+  } else if ((cfg & 3) == 2) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) e[j] = __fmul_rn(__fadd_rn(1.0f, p.strength), e[j]);
+  }
+  if (cfg & kPagBit) {
+    float ec[4], ep[4];
+    eps(0, ec);
+    eps(pag_block(cfg), ep);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) e[j] = __fadd_rn(e[j], __fmul_rn(p.pag_scale, __fsub_rn(ec[j], ep[j])));
+  }
+}
+
+// the whole guidance mix of the step alone (framework.model_inference with perturbed-attention guidance): out = mix_eps4 over
+// the row blocks of eps, n4 quads each; p carries cfg, strength, pag and pag_scale
+__global__ void __launch_bounds__(256) guidance_mix_kernel(const float* __restrict__ eps, float* __restrict__ out, size_t n4,
+                                                           const StepParams p) {
+  const int cfg = step_cfg(p);
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n4; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    float e[4];
+    mix_eps4(p, cfg, [&](int b, float (&v)[4]) {
+      const float4 t = ldg_f4(eps + (b * n4 + i) * 4);
+      v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+    }, e);
+    stg_f4(out + 4 * i, make_float4(e[0], e[1], e[2], e[3]));
   }
 }
 
@@ -317,7 +353,8 @@ __device__ __forceinline__ Quad flat_quad(const StepParams& p, size_t u) {
   return q;
 }
 
-// x_0 from the eps buffer [2N or N,C,H,W]: rows [0,N) conditional, [N,2N) unconditional when cfg == 1.  One quad per unit.
+// x_0 from the eps buffer [N, 2N or 3N][C,H,W]: rows [0,N) conditional, then [N,2N) unconditional when cfg & 3 == 1, then the
+// perturbed rows with kPagBit.  One quad per unit.
 struct EpsRows {
   const float* eps;
   __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * p.C * p.HW / 4; }
@@ -327,9 +364,9 @@ struct EpsRows {
     const Quad q = flat_quad(p, u);
     f(q, [&](float (&xt)[4], float (&x0)[4]) {
       float e[4];
-      mix_eps4(p, cfg, [&](bool uncond, float (&v)[4]) {
+      mix_eps4(p, cfg, [&](int b, float (&v)[4]) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) v[j] = eps[(uncond ? total : 0) + q.i + j];
+        for (int j = 0; j < 4; ++j) v[j] = eps[b * total + q.i + j];
       }, e);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -343,11 +380,11 @@ struct EpsRows {
 // x_0 from the tap columns Y of the output head's 1x1 GEMM: eps is the shift-and-add of eps_gather_kernel (same summation
 // order), never written to HBM.  One unit = 4 consecutive pixels (one row segment) of one sample, all Co = 4 channels: 4 quads.
 struct HeadTaps {
-  const float* Y;              // [2N or N][H][W][ldy] tap columns (tap*Co + c)
+  const float* Y;              // [N, 2N or 3N][H][W][ldy] tap columns (tap*Co + c), row blocks as EpsRows
   const float* bias;           // [Co]
   int H, W, ldy;
   __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * H * (W / 4); }
-  // eps of pixel (x, y) of sample n (n >= N: the unconditional half), all 4 channels
+  // eps of pixel (x, y) of row n (row block n / N, as EpsRows), all 4 channels
   __device__ __forceinline__ void eps4(int n, int y, int x, float (&e)[4]) const {
     e[0] = e[1] = e[2] = e[3] = 0.f;
 #pragma unroll
@@ -369,7 +406,7 @@ struct HeadTaps {
     float e[4][4];                  // [pixel][channel]
 #pragma unroll
     for (int j = 0; j < 4; ++j)
-      mix_eps4(p, cfg, [&](bool uncond, float (&v)[4]) { eps4(uncond ? n + p.N : n, y, xg * 4 + j, v); }, e[j]);
+      mix_eps4(p, cfg, [&](int b, float (&v)[4]) { eps4(n + b * p.N, y, xg * 4 + j, v); }, e[j]);
     const size_t pix = static_cast<size_t>(y) * W + xg * 4;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -507,10 +544,11 @@ struct StoreX0 {
   }
 };
 
-template <typename Src, typename Sink>
+// kPag: the instantiation for steps with perturbed-attention guidance (p.pag = 1); the others mask kPagBit off at compile time
+template <typename Src, typename Sink, bool kPag>
 __global__ void __launch_bounds__(256) step_kernel(const StepParams p, const Src src, const Sink sink) {
   const typename Sink::Scalars s = sink.scalars(p);
-  const int cfg = step_cfg(p);
+  const int cfg = kPag ? step_cfg(p) : (step_cfg(p) & 3);
   const size_t units = src.units(p);
   for (size_t u = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; u < units; u += static_cast<size_t>(gridDim.x) * blockDim.x)
     src.quads(p, s.k, cfg, u, [&](const Quad& q, auto&& load) { sink(p, s, q, load); });

@@ -431,6 +431,7 @@ Unet::~Unet() {
 struct Plan {
   int N = 0;
   int H = 0, W = 0;        // input geometry
+  AttnPerturb pert;        // normalised: row0 = N and no layers when unperturbed, layers sorted
   uint64_t last_use = 0;   // Unet::plan_uses_ at the latest forward
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
@@ -544,25 +545,29 @@ void Unet::check_geometry(int H, int W) const {
                                " (2^(levels-1)): the skip connections' sizes would not match after " + std::to_string(levels - 1) + " downsamplings");
 }
 
-Plan* Unet::get_plan(int N, int H, int W) {
+Plan* Unet::get_plan(int N, int H, int W, const AttnPerturb& pert) {
   Plan* found = nullptr;
-  for (auto& p : plans_) if (p->N == N && p->H == H && p->W == W) found = p.get();
+  for (auto& p : plans_)
+    if (p->N == N && p->H == H && p->W == W && p->pert.row0 == pert.row0 && p->pert.layers == pert.layers) found = p.get();
   if (found == nullptr) {
     check_geometry(H, W);
     if (plans_.size() >= 4) {
       IVID_CHECK_CUDA(cudaDeviceSynchronize());     // the evicted plan's workspace may still be in use by queued kernels
       plans_.erase(plans_.begin());
     }
-    plans_.emplace_back(build_plan(N, H, W));
+    plans_.emplace_back(build_plan(N, H, W, pert));
     found = plans_.back().get();
   }
   found->last_use = ++plan_uses_;
   return found;
 }
 
-Plan* Unet::build_plan(int N, int SH, int SW) {
+Plan* Unet::build_plan(int N, int SH, int SW, const AttnPerturb& pert) {
   std::unique_ptr<Plan> plan(new Plan());
   plan->N = N;
+  plan->pert = pert;
+  std::vector<bool> perturbed(attn_.size(), false);
+  for (int i : pert.layers) perturbed[i] = true;
   plan->H = SH; plan->W = SW;
   plan->n_blocks = static_cast<int>(blocks_.size());
   plan->block_stats.assign(blocks_.size(), 0);      // block 0, the stem, takes the first statistics
@@ -818,7 +823,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
       if (create) pl->taps.push_back({r.pfx, out.data, out.d16, out.C, out.H, out.W});
       return out;
     };
-    auto run_attn = [&](const AttnBlockDef& a, const Act& x) -> Act {
+    auto run_attn = [&](const AttnBlockDef& a, int idx, const Act& x) -> Act {
       IVID_REQUIRE(x.C == a.C, "internal: attention width mismatch at " + a.pfx);
       const int T = x.H * x.W;
       void* a1 = s16(kA1, x.H, x.W, a.C);
@@ -836,11 +841,17 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
         add_conv(d);
       }
       if (create) {
-        AttnLaunch* l = attn_launch_create(qkv, N, T, a.C, a.head_ch, a2);
+        // PAG: rows [row0, N) of a perturbed layer take the identity map (their own op); the softmax op covers the rest
+        const int row0 = perturbed[idx] ? pert.row0 : N;
+        AttnLaunch* l = attn_launch_create(qkv, N, T, a.C, a.head_ch, a2, row0);
         pl->attns.push_back(l);
-        pl->add_op("attention", 4.0 * N * static_cast<double>(T) * T * a.C, static_cast<double>(N) * T * a.C * 8,
-                   "T=" + std::to_string(T) + " heads=" + std::to_string(a.C / a.head_ch) + " d=" + std::to_string(a.head_ch),
-                   [l](cudaStream_t s) { attn_launch_run(l, s); });
+        const std::string shape = "T=" + std::to_string(T) + " heads=" + std::to_string(a.C / a.head_ch) + " d=" + std::to_string(a.head_ch);
+        if (row0 > 0)
+          pl->add_op("attention", 4.0 * row0 * static_cast<double>(T) * T * a.C, static_cast<double>(row0) * T * a.C * 8, shape,
+                     [l](cudaStream_t s) { attn_launch_run_softmax(l, s); });
+        if (row0 < N)
+          pl->add_op("attention_identity", 0, static_cast<double>(N - row0) * T * a.C * 4, shape + " rows=" + std::to_string(N - row0),
+                     [l](cudaStream_t s) { attn_launch_run_identity(l, s); });
       }
       Act out = new_act(a.C, x.H, x.W, false);
       {
@@ -911,7 +922,7 @@ Plan* Unet::build_plan(int N, int SH, int SW) {
               cur = run_res(res_[l.idx], cur, nullptr);
             }
             break;
-          case LayerKind::kAttention: cur = run_attn(attn_[l.idx], cur); break;
+          case LayerKind::kAttention: cur = run_attn(attn_[l.idx], l.idx, cur); break;
           case LayerKind::kResample: cur = run_resample(resample_[l.idx], cur); break;
         }
         first = false;
@@ -993,7 +1004,7 @@ bool Unet::can_fuse_head(int W) const {
 }
 
 void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes,
-                   float* eps, int N, cudaStream_t stream, const HeadHook* hook, int cache_branch) {
+                   float* eps, int N, cudaStream_t stream, const HeadHook* hook, int cache_branch, const AttnPerturb* pert) {
   if (!finalized()) throw Error(kErrState, "AdmUnet2d: forward before .cuda()/finalize");
   IVID_REQUIRE(cache_branch >= -1 && cache_branch <= cfg_.num_res_blocks,
                "cache_branch must be in [0, num_res_blocks] = [0, " + std::to_string(cfg_.num_res_blocks) + "]");
@@ -1009,8 +1020,23 @@ void Unet::forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond
   IVID_REQUIRE(cnd.kind != 2 || (cnd.sr_scale >= 0 && H % std::max(cnd.sr_scale, 1) == 0 && W % std::max(cnd.sr_scale, 1) == 0),
                "forward: the super-resolution scale must divide the input size");
   IVID_REQUIRE(hook != nullptr || eps != nullptr, "forward: eps output missing");
+  AttnPerturb pt;
+  pt.row0 = N;
+  if (pert != nullptr && !pert->layers.empty()) {
+    IVID_REQUIRE(pert->row0 >= 0 && pert->row0 <= N, "forward: the perturbed-row start must lie in [0, N]");
+    pt.layers = pert->layers;
+    std::sort(pt.layers.begin(), pt.layers.end());
+    for (size_t i = 0; i < pt.layers.size(); ++i) {
+      IVID_REQUIRE(pt.layers[i] >= 0 && pt.layers[i] < num_attention_layers(),
+                   "forward: attention layer index " + std::to_string(pt.layers[i]) + " out of range [0, " +
+                       std::to_string(num_attention_layers()) + ")");
+      IVID_REQUIRE(i == 0 || pt.layers[i] != pt.layers[i - 1], "forward: an attention layer is listed twice");
+    }
+    pt.row0 = pert->row0;
+    if (pt.row0 == N) pt.layers.clear();
+  }
 
-  Plan* pl = get_plan(N, H, W);
+  Plan* pl = get_plan(N, H, W, pt);
   if (cache_branch >= 0 && !pl->cache_valid)
     throw Error(kErrState, "reuse forward: no full forward of this batch size and input size has run since the plan was built");
   pl->x = x; pl->Nx = Nx; pl->t = t; pl->classes = classes; pl->eps = eps;

@@ -85,6 +85,14 @@ struct HeadHook {
   uint64_t key = 0;
 };
 
+// Perturbed-attention guidance (PAG, Ahn et al. 2024, arXiv:2403.17377): rows [row0, N) of a forward replace the attention
+// map of every listed attention layer (indices into the attention layers in state-dict order) by the identity, so those
+// layers output their V channels.  Rows [0, row0) run the ordinary forward.  No layers (or row0 = N): no perturbation.
+struct AttnPerturb {
+  int row0 = 0;
+  std::vector<int> layers;
+};
+
 class Unet {
  public:
   explicit Unet(const std::string& cfg_json);
@@ -107,8 +115,14 @@ class Unet {
   // include/ivid_b200.h), which runs the embeddings, input packing, input blocks 0..b, output blocks L-1-b..L-1 and the head,
   // and reads the output of output block L-2-b that the plan's last full forward left in place; kErrState before any full
   // forward of the plan.
+  // pert: perturbed rows and layers (nullptr: none).  A perturbed forward runs on a plan of its own, keyed by the
+  // perturbation as well as (N, H, W), so its graphs and its feature cache are never shared with an unperturbed forward.
   void forward(const float* x, int Nx, int H, int W, const ivid_cond_t* cond, const int64_t* t, const int64_t* classes,
-               float* eps, int N, cudaStream_t stream, const HeadHook* hook = nullptr, int cache_branch = -1);
+               float* eps, int N, cudaStream_t stream, const HeadHook* hook = nullptr, int cache_branch = -1,
+               const AttnPerturb* pert = nullptr);
+  // attention layers in state-dict order: their count and names ("middle_block.1", "input_blocks.7.1", ...)
+  int num_attention_layers() const { return static_cast<int>(attn_.size()); }
+  const std::string& attention_layer_name(int i) const { return attn_.at(i).pfx; }
   // whether the output head of an H x W forward runs as the tap-column GEMM whose last kernel a HeadHook can replace
   bool can_fuse_head(int W) const;
   // inputs the network accepts: H and W positive multiples of 2^(levels - 1), as in the reference (its skip concatenations
@@ -126,8 +140,8 @@ class Unet {
   void build_topology();
   int add_param(const std::string& name, std::vector<int64_t> shape, bool is_buffer = false);
   const ParamSpec& P(const std::string& name) const;
-  Plan* get_plan(int N, int H, int W);
-  Plan* build_plan(int N, int H, int W);
+  Plan* get_plan(int N, int H, int W, const AttnPerturb& pert);
+  Plan* build_plan(int N, int H, int W, const AttnPerturb& pert);
 
   UnetConfig cfg_;
   int embed_dim_ = 0;
@@ -159,7 +173,7 @@ class Unet {
   bool profile_ = false;
   std::map<std::string, ProfAgg> profile_acc_;
   std::string profile_ops_;
-  std::vector<std::unique_ptr<Plan>> plans_;       // keyed by (N, H, W)
+  std::vector<std::unique_ptr<Plan>> plans_;       // keyed by (N, H, W, perturbation)
   uint64_t plan_uses_ = 0;                         // debug_tap reads the most recently run plan of a batch size
   friend struct Plan;
 };

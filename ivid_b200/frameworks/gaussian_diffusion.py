@@ -12,6 +12,8 @@ from __future__ import annotations
 
 import ctypes
 import inspect
+import math
+import numbers
 
 import numpy as np
 import torch
@@ -34,6 +36,21 @@ def _extract(arr, timesteps, broadcast_shape):
 
 def _unwrap(backbone):
     return backbone.module if hasattr(backbone, "module") else backbone
+
+
+def check_pag(pag_scale, pag_layers, net):
+    """Perturbed-attention guidance arguments, checked before any device work: pag_scale None or a finite real >= 0, and
+    pag_layers None (the default layers) or a non-empty sequence of distinct attention-layer names of `net`.  Returns
+    (pag_scale, layer indices) when the perturbed rows run (pag_scale > 0), else None.  pag_layers without pag_scale is an
+    error: it would silently do nothing."""
+    from ..backbones.adm import PAG_DEFAULT_LAYERS
+    if pag_scale is None:
+        assert pag_layers is None, "pag_layers needs pag_scale"
+        return None
+    assert isinstance(pag_scale, numbers.Real) and not isinstance(pag_scale, bool), f"pag_scale must be a real number, got {pag_scale!r}"
+    assert math.isfinite(pag_scale) and pag_scale >= 0, f"pag_scale must be finite and >= 0, got {pag_scale!r}"
+    idx = _unwrap(net).pag_layer_indices(PAG_DEFAULT_LAYERS if pag_layers is None else pag_layers)
+    return (float(pag_scale), idx) if pag_scale > 0 else None
 
 
 class GaussianDiffusion:
@@ -67,13 +84,15 @@ class GaussianDiffusion:
                 / _extract(self.sqrt_alphas_cumprod, t, x_t.shape))
 
     # --- native helpers -------------------------------------------------------------------------------------------
-    def _native_forward(self, x, t, classes, strength, cond=None, keep=()):
+    def _native_forward(self, x, t, classes, strength, cond=None, keep=(), pag=None):
         """eps of one call of `model_inference`, entirely behind the C ABI.
 
         strength > 0 with a class-conditional model: both classifier-free-guidance halves run as ONE batch-2N forward
         sharing x (the second half gets the null class), then `ivid_cfg_mix` forms (1+s)*eps_c - s*eps_u.  Otherwise a
         single forward, scaled by (1+strength) as the reference does (classifier_free_guidance.py:40-41).
-        `cond` is an `_lib.CondT` describing the conditional-input assembly (InpaintCFG / SuperResCFG) or None."""
+        `cond` is an `_lib.CondT` describing the conditional-input assembly (InpaintCFG / SuperResCFG) or None.
+        `pag` = (pag_scale, layer indices) from check_pag adds N perturbed rows to the same forward (classes [c, -1, c]) and
+        mixes all blocks with `ivid_guidance_mix`, the step kernels' arithmetic."""
         net = _unwrap(self.backbone)
         net._ensure_packed()
         L = _lib.lib()
@@ -88,6 +107,8 @@ class GaussianDiffusion:
             assert net.num_classes is not None, "this model is not class-conditioned"
             assert net.has_null_class, "this model does not have a null class"
         nf = 2 * N if two else N
+        if pag is not None:
+            return self._pag_forward(net, xx, t, classes, strength, two, cond, pag)
         tt = t.to(device=dev, dtype=torch.int64)
         if two:
             tt = tt.repeat(2)
@@ -109,12 +130,43 @@ class GaussianDiffusion:
         del keep
         return out
 
-    def _cfg_forward(self, x, t, classes, strength):
-        return self._native_forward(x, t, classes, strength)
+    def _pag_forward(self, net, xx, t, classes, strength, two, cond, pag):
+        """[cond | null (two) | perturbed] rows in one forward, then G + w (eps_c - eps_perturbed) (include/ivid_b200.h)."""
+        L = _lib.lib()
+        dev = xx.device
+        N, _, H, W = xx.shape
+        blocks = 3 if two else 2
+        tt = t.to(device=dev, dtype=torch.int64).repeat(blocks).contiguous()
+        cc = None
+        if classes is not None:
+            c = classes.to(dev, torch.int64)
+            parts = [c, torch.full((N,), -1, dtype=torch.int64, device=dev), c] if two else [c, c]
+            cc = torch.cat(parts).contiguous()
+        # G as _native_forward forms it: the mix (two), (1+s) eps_c for strength < 0, eps_c otherwise
+        cfg = 1 if two else (2 if strength < 0 else 0)
+        w, idx = pag
+        arr = (ctypes.c_int * len(idx))(*idx)
+        eps = torch.empty((blocks * N, net.out_channels, H, W), dtype=torch.float32, device=dev)
+        out = torch.empty((N, net.out_channels, H, W), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            st = _lib.cur_stream(dev)
+            _lib.check(L.ivid_unet_forward_perturbed(net._handle, _lib.ptr(xx), N, H, W, ctypes.byref(cond) if cond is not None else None,
+                                                     _lib.ptr(tt), _lib.ptr(cc), _lib.ptr(eps), blocks * N, (blocks - 1) * N, arr,
+                                                     len(idx), -1, st))
+            _lib.check(L.ivid_guidance_mix(_lib.ptr(eps), out.numel(), cfg, float(strength), 1, w, _lib.ptr(out), st))
+        return out
+
+    def _cfg_forward(self, x, t, classes, strength, pag=None):
+        return self._native_forward(x, t, classes, strength, pag=pag)
 
     @torch.no_grad()
-    def model_inference(self, x, t, classes=None, **kwargs):
-        """Predicted noise (gaussian_diffusion.py:76-91)."""
+    def model_inference(self, x, t, classes=None, pag_scale=None, pag_layers=None, **kwargs):
+        """Predicted noise (gaussian_diffusion.py:76-91).  pag_scale=w > 0 (extension; perturbed-attention guidance, Ahn et
+        al. 2024, arXiv:2403.17377) returns eps_c + w (eps_c - eps_perturbed), eps_perturbed the forward with the attention
+        maps of `pag_layers` (names, default ("middle_block.1",)) replaced by the identity, both rows of one forward."""
+        pag = check_pag(pag_scale, pag_layers, self.backbone)
+        if pag is not None:
+            return self._native_forward(x, t, classes, 0.0, pag=pag)
         kwargs = {k: v for k, v in kwargs.items() if k in self.backbone_args}
         return self.backbone(x, t, classes, **kwargs)
 
@@ -130,9 +182,10 @@ class ClassifierFreeGuidance(GaussianDiffusion):
         self.p_uncond = p_uncond
 
     @torch.no_grad()
-    def model_inference(self, x, t, classes=None, strength=3.0, **kwargs):
-        # classifier_free_guidance.py:38-42
-        return self._cfg_forward(x, t, classes, strength)
+    def model_inference(self, x, t, classes=None, strength=3.0, pag_scale=None, pag_layers=None, **kwargs):
+        # classifier_free_guidance.py:38-42; pag_scale / pag_layers as in GaussianDiffusion.model_inference, added to the mix
+        pag = check_pag(pag_scale, pag_layers, self.backbone)
+        return self._cfg_forward(x, t, classes, strength, pag=pag)
 
 
 class InpaintCFG(GaussianDiffusion):
@@ -165,9 +218,11 @@ class InpaintCFG(GaussianDiffusion):
         return torch.cat([x, torch.randn_like(x), x.new_zeros(x[:, :1].shape)], dim=1)
 
     @torch.no_grad()
-    def model_inference(self, x, t, y, mask, classes=None, strength=3.0, noise=None, **kwargs):
+    def model_inference(self, x, t, y, mask, classes=None, strength=3.0, noise=None, pag_scale=None, pag_layers=None, **kwargs):
         """inpaint_cfg.py:61-83.  The conditional input is assembled inside the native forward (cond_pack_kernel);
-        `noise` [N,4,H,W] injects the hole-filling draws, default = torch draws in the reference's order."""
+        `noise` [N,4,H,W] injects the hole-filling draws, default = torch draws in the reference's order.  pag_scale /
+        pag_layers as in GaussianDiffusion.model_inference; the perturbed rows share the conditional rows' hole noise."""
+        pag = check_pag(pag_scale, pag_layers, self.backbone)
         dev = x.device
         f32 = lambda v: None if v is None else v.to(device=dev, dtype=torch.float32).contiguous()
         yy, mm, mr = f32(y), f32(mask), f32(kwargs.get("mask_rgb"))
@@ -176,7 +231,7 @@ class InpaintCFG(GaussianDiffusion):
         cond.kind = 1
         cond.y_dev, cond.mask_dev, cond.mask_rgb_dev, cond.noise_dev = yy.data_ptr(), mm.data_ptr(), (mr.data_ptr() if mr is not None else None), zz.data_ptr()
         # classes None -> single null-class forward without (1+s) scaling (inpaint_cfg.py:77-78)
-        return self._native_forward(x, t, classes, strength if classes is not None else 0.0, cond, keep=(yy, mm, mr, zz))
+        return self._native_forward(x, t, classes, strength if classes is not None else 0.0, cond, keep=(yy, mm, mr, zz), pag=pag)
 
 
 class SuperResCFG(GaussianDiffusion):
@@ -202,11 +257,12 @@ class SuperResCFG(GaussianDiffusion):
         return s
 
     @torch.no_grad()
-    def model_inference(self, x, t, y, classes=None, strength=3.0, **kwargs):
-        # sr_cfg.py:39-60
+    def model_inference(self, x, t, y, classes=None, strength=3.0, pag_scale=None, pag_layers=None, **kwargs):
+        # sr_cfg.py:39-60; pag_scale / pag_layers as in GaussianDiffusion.model_inference
+        pag = check_pag(pag_scale, pag_layers, self.backbone)
         yy = y.to(device=x.device, dtype=torch.float32).contiguous()
         cond = _lib.CondT()
         cond.kind = 2
         cond.sr_scale = self._scale(x, yy)
         cond.y_dev = yy.data_ptr()
-        return self._native_forward(x, t, classes, strength if classes is not None else 0.0, cond, keep=(yy,))
+        return self._native_forward(x, t, classes, strength if classes is not None else 0.0, cond, keep=(yy,), pag=pag)

@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import argparse
 import json
+import math
 import os
 import threading
 
@@ -20,6 +21,8 @@ import numpy as np
 import torch
 
 from .. import backbones, frameworks, samplers
+from ..backbones.adm import PAG_DEFAULT_LAYERS
+from ..frameworks.gaussian_diffusion import check_pag
 from ..samplers.samplers import _check_cache, _check_threshold
 from ..rgbd_3d import DeviceWarp, glm_compat as glm
 from ..rgbd_3d import utils as rgbd_utils
@@ -125,7 +128,7 @@ def build_modelviews(viewset, num_samples, rng=None):
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
                precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init_views=None,
-               init_strength=None):
+               init_strength=None, pag_scale=None, pag_layers=None):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, solver="dpmpp_sde" its stochastic variant
@@ -139,7 +142,9 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     init_views [num_samples, 4, S, S] (RGBD in [-1, 1], one per sample of this rank, sharded like the seeds) starts every
     scene from a given first view: without init_strength view 0 IS that view and the unconditional model does not run
     (framework_uncond may be None); with init_strength view 0 is its SDEdit by the unconditional sampler (the samplers'
-    `init` / `init_strength`) with the sample's class, guidance, solver and options.  Views 1... grow from view 0 as always."""
+    `init` / `init_strength`) with the sample's class, guidance, solver and options.  Views 1... grow from view 0 as always.
+    pag_scale=w, pag_layers=names add perturbed-attention guidance to every step of both networks (the samplers'
+    `pag_scale` / `pag_layers`), the class-free unconditional network included; the guidance interval gates it there too."""
     if init_views is None:
         assert init_strength is None, "init_strength needs init_views"
     else:
@@ -149,6 +154,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     for fw in (framework_uncond, framework_cond):          # before any device work
         if fw is not None:
             _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
+            check_pag(pag_scale, pag_layers, fw.backbone)
     _check_threshold(dynamic_threshold, False)
     assert solver in ("ddim", "dpmpp", "dpmpp_sde", "unipc"), \
         f"solver must be 'ddim', 'dpmpp', 'dpmpp_sde' or 'unipc', got {solver!r}"
@@ -165,6 +171,9 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     if cache_interval is not None:
         gi_kw.update(cache_interval=cache_interval, cache_branch=cache_branch)
     th_kw = dict(dynamic_threshold=dynamic_threshold) if dynamic_threshold is not None else {}
+    pag_kw = dict(pag_scale=pag_scale, pag_layers=pag_layers) if pag_scale is not None else {}
+    # a framework without classifier-free guidance takes the interval only to gate perturbed-attention guidance
+    plain_kw = {k: v for k, v in gi_kw.items() if k.startswith("cache") or (pag_kw and k == "guidance_interval")}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
     net = (framework_uncond if framework_uncond is not None else framework_cond).backbone
@@ -205,10 +214,10 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
             if j == 0 and init_views is not None and init_strength is None:
                 res = edict(samples=init_views[i: i + bs].to(device=dev, dtype=torch.float32).contiguous())
             elif j == 0:
-                kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
+                kw = dict(strength=guidance, **gi_kw) if cfg_u else dict(plain_kw)
                 if steps_uncond < 1000:
                     kw.update(sde_kw)
-                kw.update(th_kw)
+                kw.update(th_kw, **pag_kw)
                 if init_views is not None:     # SDEdit of the given view; the seeds' noise is the forward diffusion's z
                     kw.update(init=init_views[i: i + bs].to(device=dev, dtype=torch.float32), init_strength=init_strength)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
@@ -220,8 +229,8 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 cond_depth.append(cond[:, 3:4] * 2 - 1)
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
-                kw = dict(strength=guidance, **gi_kw) if cfg_u else {k: v for k, v in gi_kw.items() if k.startswith("cache")}
-                kw.update(sde_kw, **th_kw)
+                kw = dict(strength=guidance, **gi_kw) if cfg_u else dict(plain_kw)
+                kw.update(sde_kw, **th_kw, **pag_kw)
                 res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
             samples.append(res.samples)
             if warp is not None:
@@ -363,7 +372,8 @@ def main(rank, world_size, opt):
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
                      rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
                      precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                     dynamic_threshold=dynamic_threshold, init_views=init_views, init_strength=init_strength)
+                     dynamic_threshold=dynamic_threshold, init_views=init_views, init_strength=init_strength,
+                     pag_scale=getattr(opt, "pag_scale", None), pag_layers=getattr(opt, "pag_layers", None))
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -386,7 +396,16 @@ def output_dir_name(opt):
                         + ("" if cache_interval is None else f"_cache{cache_interval}b{getattr(opt, 'cache_branch', 0)}")
                         + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}")
                         + ("" if init_image is None else f"_init-{os.path.splitext(os.path.basename(init_image))[0]}")
-                        + ("" if init_strength is None else f"_strength{init_strength}"))
+                        + ("" if init_strength is None else f"_strength{init_strength}")
+                        + _pag_suffix(opt))
+
+
+def _pag_suffix(opt):
+    """_pag{W}, plus the layers ('+'-joined) when they are not the default."""
+    w, layers = getattr(opt, "pag_scale", None), getattr(opt, "pag_layers", None)
+    if w is None:
+        return ""
+    return f"_pag{w}" + ("" if layers is None or tuple(layers) == PAG_DEFAULT_LAYERS else "-" + "+".join(layers))
 
 
 def _int_at_least(lo):
@@ -431,6 +450,25 @@ def parse_threshold(s):
     return vals[0] if len(vals) == 1 else (vals[0], vals[1])
 
 
+def parse_pag_scale(s):
+    """'W' -> W of --pag_scale, a finite number >= 0."""
+    try:
+        v = float(s)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected a number, got {s!r}") from None
+    if not (math.isfinite(v) and v >= 0.0):
+        raise argparse.ArgumentTypeError(f"expected a finite W >= 0, got {s!r}")
+    return v
+
+
+def parse_pag_layers(s):
+    """'NAME[,NAME...]' -> the tuple of attention-layer names of --pag_layers (checked against the network when it is built)."""
+    names = tuple(n.strip() for n in s.split(","))
+    if not names or any(not n for n in names):
+        raise argparse.ArgumentTypeError(f"expected NAME[,NAME...], got {s!r}")
+    return names
+
+
 def parse_strength(s):
     """'S' -> S of --init_strength, 0 < S <= 1."""
     try:
@@ -451,6 +489,8 @@ def parse_args(argv=None):
         ap.error("--init_image and --init_depth go together")
     if o.init_strength is not None and o.init_image is None:
         ap.error("--init_strength needs --init_image and --init_depth")
+    if o.pag_layers is not None and o.pag_scale is None:
+        ap.error("--pag_layers needs --pag_scale")
     return o
 
 
@@ -504,6 +544,11 @@ def build_arg_parser():
     ap.add_argument("--init_strength", type=parse_strength, default=None, metavar="S",
                     help="with --init_image: re-sample the first view from it by SDEdit, running the last S of the unconditional "
                          "schedule, 0 < S <= 1 (default: the given view is the first view as it is)")
+    ap.add_argument("--pag_scale", type=parse_pag_scale, default=None, metavar="W",
+                    help="perturbed-attention guidance of both networks at scale W >= 0: adds W * (eps - eps with identity "
+                         "attention maps) at every guided step; works without classes (default: off)")
+    ap.add_argument("--pag_layers", type=parse_pag_layers, default=None, metavar="NAME[,NAME...]",
+                    help="with --pag_scale: the attention layers to perturb, by state-dict name (default: middle_block.1)")
     return ap
 
 

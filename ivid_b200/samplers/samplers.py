@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from .. import _lib
-from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG
+from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG, check_pag
 from ..utils import edict
 
 __all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler", "UniPcSampler", "init_steps"]
@@ -136,7 +136,7 @@ class _NativeSampler:
         return uses_cfg, float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
 
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None, prev_x=None, corrected=None):
+                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None, prev_x=None, corrected=None, pag=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -210,6 +210,10 @@ class _NativeSampler:
             a.dynamic_threshold = 1
             a.threshold_ratio = threshold[0]
             a.threshold_max = 0.0 if math.isinf(threshold[1]) else threshold[1]
+        if pag is not None:
+            layers = (ctypes.c_int * len(pag[1]))(*pag[1])
+            keep.append(layers)
+            a.pag, a.pag_scale, a.pag_layers, a.pag_num_layers = 1, pag[0], layers, len(pag[1])
         return a, keep
 
     def _net(self):
@@ -221,7 +225,7 @@ class _NativeSampler:
         return _unwrap(self.framework.backbone).num_res_blocks
 
     def _native_step(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                     sde=False, interval=None, cache=None, threshold=None, prev_x=None):
+                     sde=False, interval=None, cache=None, threshold=None, prev_x=None, pag=None):
         """One step.  `t` / `t_prev` are host ints (ivid_sampler_step) or the [N] tensors sample_once receives
         (ivid_sampler_step_dev: the step is read on the device, no host sync; t_prev None for DDPM)."""
         net = self._net()
@@ -230,7 +234,7 @@ class _NativeSampler:
         corrected = torch.empty_like(x_t) if self.UNIPC else None
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
                                   hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache,
-                                  threshold=threshold, prev_x=prev_x, corrected=corrected)
+                                  threshold=threshold, prev_x=prev_x, corrected=corrected, pag=pag)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         L = _lib.lib()
@@ -250,7 +254,7 @@ class _NativeSampler:
         return out
 
     def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, interval, reuse_features, cache_branch,
-                     order=0, prev=None, sde=False, dynamic_threshold=None, prev_x=None):
+                     order=0, prev=None, sde=False, dynamic_threshold=None, prev_x=None, pag_scale=None, pag_layers=None):
         """The body of every sample_once: the host checks before any device work or torch draw, the step noise (drawn as
         the reference draws it, or the injected `noise` and kwargs' `cond_noise`), then the step with t / t_prev read on
         the device (all samples of a batch share the step, ddpm.py:177-179, ddim.py:154-158: no host sync)."""
@@ -260,6 +264,7 @@ class _NativeSampler:
         _check_interval(interval, len(self.framework.betas))
         _check_cache(None, cache_branch, self._num_res_blocks())
         threshold = _check_threshold(dynamic_threshold, clip_denoised)
+        pag = check_pag(pag_scale, pag_layers, self.framework.backbone)
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kwargs)
         else:
@@ -267,7 +272,7 @@ class _NativeSampler:
         # the DPM-Solver++ ODE update reads no step noise
         return self._native_step(x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise if self.KIND != 2 or sde else None,
                                  cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold, prev_x=prev_x)
+                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold, prev_x=prev_x, pag=pag)
 
     def _draw_step_noise(self, x_t, kwargs):
         """torch draws in the reference's order: InpaintCFG rgb, depth (inside model_inference), then randn_like(x_t)."""
@@ -279,24 +284,27 @@ class _NativeSampler:
             cond_noise = torch.cat([n_rgb, n_d], dim=1)
         return torch.randn_like(x_t), cond_noise
 
-    def _reuse_schedule(self, model_times, classes, kwargs, interval, cache_interval):
+    def _reuse_schedule(self, model_times, classes, kwargs, interval, cache_interval, pag=None):
         """Whether each step of a run reuses the cached features, by ivid_sampler_run's rule: a full forward at the first
-        step, where the forward switches between the guided batch-2N and the unguided batch-N plan, and cache_interval steps
-        after the last full one."""
+        step, where the forward switches plans (the guided batch of 2N or 3N rows and the unguided batch-N plan), and
+        cache_interval steps after the last full one."""
         _, strength = self._guidance(kwargs)
-        reuse, last_full, last_two = [], 0, False
+        reuse, last_full, last_rows = [], 0, 0
         for i, tm in enumerate(model_times):
-            two = classes is not None and strength > 0 and (interval is None or interval[0] <= tm <= interval[1])
-            full = cache_interval <= 1 or i == 0 or two != last_two or i - last_full >= cache_interval
+            inside = interval is None or interval[0] <= tm <= interval[1]
+            rows = 1 + (classes is not None and strength > 0 and inside) + (pag is not None and inside)
+            full = cache_interval <= 1 or i == 0 or rows != last_rows or i - last_full >= cache_interval
             if full:
                 last_full = i
-            last_two = two
+            last_rows = rows
             reuse.append(not full)
         return reuse
 
     def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
-             sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init=None, init_strength=None):
+             sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init=None, init_strength=None,
+             pag_scale=None, pag_layers=None):
         interval = _check_interval(interval, len(self.framework.betas))   # before any device work
+        pag = check_pag(pag_scale, pag_layers, self.framework.backbone)
         cache_interval = _check_cache(cache_interval, cache_branch, self._num_res_blocks())
         threshold = _check_threshold(dynamic_threshold, clip_denoised)
         _check_init(init, init_strength, noise, image_size, _unwrap(self.framework.backbone).out_channels)
@@ -339,13 +347,13 @@ class _NativeSampler:
             sched = sched[start:]
             prev, prev_x = None, None
             reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
-                                         cache_interval)
+                                         cache_interval, pag)
             for i, (t, t_prev) in enumerate(sched):
                 z, cond_noise = self._draw_step_noise(img, kwargs)
                 # the DPM-Solver++ ODE update draws z only to consume the torch RNG as DdimSampler does
                 out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if self.KIND != 2 or sde else None,
                                         cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                        cache=(0, cache_branch, reuse[i]), threshold=threshold, prev_x=prev_x)
+                                        cache=(0, cache_branch, reuse[i]), threshold=threshold, prev_x=prev_x, pag=pag)
                 if self.UNIPC:
                     prev, prev_x = ([(t, out.pred_x_0)] + (prev or []))[:order], out.corrected_x_t
                 elif self.KIND == 2 and order != 1:
@@ -356,7 +364,7 @@ class _NativeSampler:
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
-                                      interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold)
+                                      interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold, pag=pag)
             a.start_step = start
             traj0 = trajt = None
             if return_trajectory:
@@ -391,20 +399,21 @@ class DdpmSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, dynamic_threshold=None, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
         """x_{t-1} from x_t (ddpm.py:111-131).  `t` is the [N] tensor of steps minus 1 (all equal).
         `noise` (extension) injects the randn_like draw; default draws it with torch like the reference.
         `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`).
         `reuse_features=True` (extension): the step's forward reuses the deep features of the last full forward of the same
         batch and size at branch `cache_branch` (see `sample`); RuntimeError if no full forward has run on it.
-        `dynamic_threshold=p` or `(p, s_max)` (extension): dynamic thresholding of x_0 (see `sample`)."""
+        `dynamic_threshold=p` or `(p, s_max)` (extension): dynamic thresholding of x_0 (see `sample`).
+        `pag_scale` / `pag_layers` (extension): perturbed-attention guidance (see `sample`)."""
         return self._sample_once(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, guidance_interval, reuse_features,
-                                 cache_branch, dynamic_threshold=dynamic_threshold)
+                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers)
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
         """Run the full reverse process (ddpm.py:134-187).  `steps` is accepted and ignored exactly as in the reference.
         pred_x_t / pred_x_0 are only materialised with return_trajectory=True (the reference keeps 2x1000 tensors alive;
         its callers read `.samples` only: inference/sample.py:82).
@@ -433,10 +442,18 @@ class DdpmSampler(_NativeSampler):
         first of them by q(x_t | x_0) (GaussianDiffusion.diffuse at model time jump * n - 1), with `noise` as its z if given,
         and the run goes on from there.  Low s stays close to x_0; s = 1 runs the whole schedule from a noised x_0.  Each
         executed step is the step of a full run; the multistep history and feature reuse start afresh at the first one.
-        pred_x_t / pred_x_0 hold the n executed steps.  rng="torch" draws z with randn_like(x_0) before the steps."""
+        pred_x_t / pred_x_0 hold the n executed steps.  rng="torch" draws z with randn_like(x_0) before the steps.
+
+        pag_scale=w, pag_layers=names (extension; perturbed-attention guidance, Ahn et al. 2024, arXiv:2403.17377): every
+        guided step adds N rows to its forward, the conditional forward with the attention maps of the named attention layers
+        (default ("middle_block.1",)) replaced by the identity, and uses eps = G + w (eps_c - eps_perturbed), G the eps of the
+        step without it (the classifier-free mix, if any).  It works without classes, so it guides class-free models too.  The
+        guidance interval gates it like classifier-free guidance.  w >= 0; None or 0 is the run without it, bit for bit.  The
+        noise and the torch RNG consumption are unchanged (the InpaintCFG hole noise is shared by the perturbed rows)."""
         return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
+                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
+                         pag_layers=pag_layers)
 
 
 class DdimSampler(_NativeSampler):
@@ -446,24 +463,26 @@ class DdimSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, eta=0.0, replace_rgb=None,
                     replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, dynamic_threshold=None, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
         """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step).
         `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi].
-        `reuse_features` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample_once."""
+        `reuse_features` / `cache_branch` / `dynamic_threshold` / `pag_scale` / `pag_layers` as in DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, dynamic_threshold=dynamic_threshold)
+                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
                verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
         """Run `steps` DDIM steps (ddim.py:106-165).  `guidance_interval=(t_lo, t_hi)` as in DdpmSampler.sample, on the model
         time t - 1 of each step; `cache_interval` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample (the replace /
-        constrain guidance acts on the thresholded x_0).  `init` / `init_strength` as in DdpmSampler.sample."""
+        constrain guidance acts on the thresholded x_0).  `init` / `init_strength` and `pag_scale` / `pag_layers` as in
+        DdpmSampler.sample."""
         return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
                          interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
+                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
+                         pag_layers=pag_layers)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -482,33 +501,36 @@ class DpmSolverSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
                     constrain_depth=None, noise=None, sde=False, guidance_interval=None, reuse_features=False, cache_branch=0,
-                    dynamic_threshold=None, **kwargs):
+                    dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
         """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
         With sde=True `noise` is the injected z of the update; with sde=False the update does not use it.  When it is None
         the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
         randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval`, `reuse_features`,
-        `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once (D0, and so pred_x_0, is thresholded)."""
+        `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once (D0, and so pred_x_0, is thresholded);
+        `pag_scale` / `pag_layers` as for DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
                                  cache_branch, order=2 if prev is not None else 1, prev=prev, sde=sde,
-                                 dynamic_threshold=dynamic_threshold)
+                                 dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, sde=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
         """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
         final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
         is drawn where DdimSampler draws it (`rng`).  `guidance_interval` as in DdimSampler.sample; the history D_{-1} of a
         step after an unguided one is that step's unguided D0.  `cache_interval` / `cache_branch` as in DdpmSampler.sample;
         the history D_{-1} of a step is that step's D0, from whichever forward ran.  `dynamic_threshold` as in
         DdpmSampler.sample: D0 is the thresholded, guided x_0, and so is the history.  `init` / `init_strength` as in
-        DdpmSampler.sample; the first executed step is first order.  Same return dict as DdimSampler.sample."""
+        DdpmSampler.sample; the first executed step is first order.  `pag_scale` / `pag_layers` as in DdpmSampler.sample; the
+        history holds the PAG-guided D0.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
-                         cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
+                         cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength,
+                         pag_scale=pag_scale, pag_layers=pag_layers)
 
 
 class UniPcSampler(_NativeSampler):
@@ -525,7 +547,7 @@ class UniPcSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, prev_x=None, order=2, replace_rgb=None,
                     replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, dynamic_threshold=None, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
         """One UniPC step from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev` is a list of up to three `(t_last, pred_x_0)` pairs of the previous steps, newest first, and `prev_x` the
         previous step's `corrected_x_t` (the corrector's base; required with `prev`).  With n pairs (at most `order` are used)
@@ -533,27 +555,29 @@ class UniPcSampler(_NativeSampler):
         Returns `pred_x_prev` (the prediction the next step's network sees), `pred_x_0` and `corrected_x_t` (x_t itself
         without `prev`).  Chain steps with prev = ([(t, pred_x_0)] + prev)[:3] and prev_x = corrected_x_t.  `noise` is not used; the
         torch RNG is consumed as DpmSolverSampler.sample_once consumes it.  `guidance_interval`, `reuse_features`,
-        `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once."""
+        `cache_branch`, `dynamic_threshold` and `pag_scale` / `pag_layers` as for DdimSampler.sample_once."""
         assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
         prev = list(prev) if prev is not None else []
         assert len(prev) <= 3, f"prev holds at most three (t_last, pred_x_0) pairs, got {len(prev)}"
         assert not prev or prev_x is not None, "prev needs prev_x, the previous step's corrected_x_t"
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, order=order, prev=prev, dynamic_threshold=dynamic_threshold, prev_x=prev_x)
+                                 cache_branch, order=order, prev=prev, dynamic_threshold=dynamic_threshold, prev_x=prev_x,
+                                 pag_scale=pag_scale, pag_layers=pag_layers)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
         """Run `steps` UniPC steps of order `order` (1, 2 or 3; 2 is the paper's choice for guided sampling).  Step i predicts
         at order min(order, i + 1) and corrects at the previous step's order; the first step has no corrector and the final
         step (to t_prev = 0) returns x_0 as DDIM does.  pred_x_t holds the predictions the network saw.  Draws no step noise;
         the torch RNG is consumed as DpmSolverSampler.sample(sde=False) consumes it.  `guidance_interval`, `cache_interval` /
         `cache_branch` and `dynamic_threshold` as in DpmSolverSampler.sample: the history holds the D0 of whichever forward
-        ran, thresholded.  `init` / `init_strength` as in DdpmSampler.sample; the order ramp starts at the first executed step.
-        Same return dict as DdimSampler.sample."""
+        ran, thresholded.  `init` / `init_strength` and `pag_scale` / `pag_layers` as in DdpmSampler.sample; the order ramp
+        starts at the first executed step.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength)
+                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
+                         pag_layers=pag_layers)
