@@ -281,6 +281,35 @@ typedef struct {
   float pag_scale;
   const int* pag_layers;
   int pag_num_layers;
+  /* Adaptive projected guidance (APG; Sadat, Hilliges, Weber, "Eliminating Oversaturation and Artifacts of High Guidance
+   * Scales in Diffusion Models", ICLR 2025, arXiv:2410.02416), every kind; zero means off.  The fields sit before
+   * start_step and the dynamic-threshold fields, which stay last.  It replaces the classifier-free
+   * mix of a guided step (use_cfg = 1, classes_dev, strength = s > 0) by an update in x0 space.  For every sample n, over
+   * its M = C*H*W elements (all channels):
+   *   D_c = sqrt(1/acp) * x_t - sqrt(1/acp - 1) * eps_c, D_u the same from eps_u (the null-class rows);
+   *   m = (D_c - D_u) + beta * m_prev       (beta = apg_momentum; m_prev = 0 at the first guided step);
+   *   c = min(1, r / |m|)                   (r = apg_norm; r = 0 or m = 0: c = 1);
+   *   k = (1 - eta) * <m, D_c> / max(|D_c|^2, tiny)    (eta = apg_eta, tiny = DBL_MIN);
+   *   D = D_c + s * c * (m - k * D_c)       (+ pag_scale * (D_c - D_p) with PAG, D_p the x0 of the perturbed rows).
+   * m becomes the next m_prev.  Everything after the mix (clip_denoised or dynamic thresholding, replace / constrain, the
+   * updates, the multistep history, pred_x0) reads D as its x0.  eta = 1, r = 0, beta = 0 is the classifier-free step
+   * (1+s) D_c - s D_u in real arithmetic, not bit for bit.  Rounding: D_c as the step's x0; D_c - D_u = sqrt(1/acp - 1) *
+   * (eps_u - eps_c) and the PAG term sqrt(1/acp - 1) * (pag_scale * (eps_p - eps_c)) in fp32; beta rounded to fp32 once,
+   * m = D_c - D_u + beta * m_prev in fp32; |m|^2, <m, D_c> and |D_c|^2 accumulated in double in an order fixed by the
+   * sample's own elements; c rounded to fp32, a = fp32(s * c), b = fp32(s * c * k) rounded once; D = D_c + (a * m - b * D_c)
+   * in fp32, each operation rounded to nearest, then + the PAG term.  A sample's result depends on its own elements only.
+   * Steps that are not guided (outside the guidance interval, or the device flag of ivid_sampler_step_dev) are the unguided
+   * step and leave m_prev as it is.
+   *   apg_state_dev: ivid_sampler_step / ivid_sampler_step_dev: [N,C,H,W] fp32 m_prev on entry, m after a guided step;
+   *     NULL is zero history (and m is not returned).  ivid_sampler_run keeps its own state, zeroed at start_step, and
+   *     ignores this field.
+   * apg other than 0 / 1, or apg = 1 without use_cfg, classes_dev or strength > 0 (finite), apg_eta or apg_norm negative or
+   * not finite, apg_momentum outside (-1, 1): IVID_ERR_INVALID_ARGUMENT. */
+  int apg;
+  double apg_eta;
+  double apg_norm;
+  double apg_momentum;
+  float* apg_state_dev;
   /* Partial run (SDEdit, Meng et al. 2022, arXiv:2108.01073), ivid_sampler_run only; zero runs the whole grid.
    * ivid_sampler_run executes steps i = start_step .. steps-1 of the grid it builds (T steps for DDPM), from the x_inout_dev
    * of step start_step (ivid_sampler_diffuse below makes one from an image).  Each executed step keeps its t, t_prev,
@@ -326,6 +355,14 @@ int ivid_sampler_step_dev(ivid_sampler_t* s, ivid_unet_t* unet, const float* x_t
  * threshold_max as threshold_ratio and threshold_max there (IVID_ERR_INVALID_ARGUMENT outside them).  Synchronises the stream. */
 int ivid_op_dynamic_threshold(const float* x_dev, int N, int M, double ratio, double threshold_max, float* s_out_dev,
                               float* x_out_dev, void* stream);
+
+/* The adaptive projected guidance of ivid_step_args_t alone, on the reduction and element functions the step runs (tests
+ * drive it with crafted data): d_c_dev and d_u_dev fp32 [N][M] are D_c and D_u; state_inout_dev [N][M] holds m_prev on entry
+ * (zeros for the first step) and m on return; out_dev [N][M] receives D.  Here D_c - D_u is one fp32 subtraction.  s > 0
+ * (finite), eta, r and beta as apg_eta, apg_norm and apg_momentum there (IVID_ERR_INVALID_ARGUMENT outside them).
+ * Synchronises the stream. */
+int ivid_op_apg(const float* d_c_dev, const float* d_u_dev, float* state_inout_dev, int N, int M, float s, double eta,
+                double r, double beta, float* out_dev, void* stream);
 
 /* ClassifierFreeGuidance.model_inference's mix alone (classifier_free_guidance.py:42): out = (1+s)*eps[0:count) -
  * s*eps[count:2*count) for the batch-2N forward's output (count = N*C*H*W, multiple of 4). */

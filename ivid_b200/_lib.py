@@ -75,6 +75,11 @@ class StepArgsT(Structure):
         ("pag_scale", c_float),
         ("pag_layers", POINTER(c_int)),   # host array: attention-layer indices in state-dict order
         ("pag_num_layers", c_int),
+        ("apg", c_int),               # 1: adaptive projected guidance replaces the classifier-free mix
+        ("apg_eta", c_double),        # weight of the update's part parallel to D_c
+        ("apg_norm", c_double),       # bound r on the update's norm; 0 = none
+        ("apg_momentum", c_double),   # beta in (-1, 1)
+        ("apg_state_dev", c_void_p),  # single step: [N,C,H,W] m_prev in, m out; NULL = zero history
         ("start_step", c_int),        # ivid_sampler_run: execute grid steps start_step .. steps-1 only (0 = all)
         ("dynamic_threshold", c_int), # 1: threshold x_0 at the threshold_ratio-quantile of |x_0| of each sample
         ("threshold_ratio", c_double),
@@ -147,6 +152,7 @@ SIGNATURES = {
     "ivid_cfg_mix": (c_int, [c_void_p, c_float, c_void_p, c_uint64, c_void_p]),
     "ivid_guidance_mix": (c_int, [c_void_p, c_uint64, c_int, c_float, c_int, c_float, c_void_p, c_void_p]),
     "ivid_op_dynamic_threshold": (c_int, [c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_void_p, c_void_p]),
+    "ivid_op_apg": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_double, c_double, c_double, c_void_p, c_void_p]),
     "ivid_sampler_run": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(StepArgsT), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ivid_sampler_diffuse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_uint64, c_int, c_uint64, c_void_p, c_void_p]),
     "ivid_op_conv2d": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int,

@@ -254,6 +254,15 @@ int ivid_op_dynamic_threshold(const float* x_dev, int N, int M, double ratio, do
     IVID_CHECK_CUDA(cudaStreamSynchronize(st));
   });
 }
+int ivid_op_apg(const float* d_c_dev, const float* d_u_dev, float* state_inout_dev, int N, int M, float s, double eta,
+                double r, double beta, float* out_dev, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(d_c_dev); IVID_NOT_NULL(d_u_dev); IVID_NOT_NULL(state_inout_dev); IVID_NOT_NULL(out_dev);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_apg(d_c_dev, d_u_dev, state_inout_dev, N, M, s, eta, r, beta, out_dev, st);
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+  });
+}
 int ivid_sampler_run(ivid_sampler_t* s, ivid_unet_t* unet, float* x_inout_dev, int N, int steps,
                      const ivid_step_args_t* args, const float* noise_all_dev, const float* cond_noise_all_dev,
                      float* traj_x0_dev, float* traj_xt_dev, void* stream) {

@@ -125,6 +125,9 @@ void launch_guidance_mix(const float* eps, float* out, size_t count, int cfg, fl
 // dynamic thresholding of x [N][M] (sampler.cuh): s_out [N] and x_out = clamp(x, -s, s) / s; threshold_max <= 0: no upper bound
 void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double threshold_max, float* s_out, float* x_out,
                               cudaStream_t s);   // sampler.cu
+// adaptive projected guidance of x_0 rows [N][M] (include/ivid_b200.h, ivid_op_apg): state holds m_prev on entry and m on return
+void launch_apg(const float* dc, const float* du, float* state, int N, int M, float s, double eta, double norm, double beta,
+                float* out, cudaStream_t st);   // sampler.cu
 
 void launch_posenc(const int64_t* t, int Nt, const float* freqs, int half, float* out, int N, cudaStream_t s);
 // FiLM table (all ResBlock emb_layers as one product): out = silu(emb) * Wp^T + bias, Wp in the swizzled K-chunk-major

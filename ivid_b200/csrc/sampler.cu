@@ -236,10 +236,13 @@ struct StepTail {
   float* s;
   bool unipc;
   UniPcUpdate uni;
+  bool apg;          // adaptive projected guidance (StepPlan::apg) with its planes and parameters
+  ApgParams ap;
 };
 
 // The tail of a step from x_0 source src (sampler.cuh: EpsRows after the forward, HeadTaps as the forward's last node): the
-// update, or with a dynamic threshold x_0 into t.x0, s of every sample and the update on the thresholded x_0.
+// update, or with a dynamic threshold x_0 into t.x0, s of every sample and the update on the thresholded x_0.  With APG the
+// source first feeds ApgStore, and ApgX0 is the x_0 source of the rest.
 template <bool kPag, typename Src>
 static void launch_step_tail(const StepParams& p, const Src& src, const StepTail& t, cudaStream_t st) {
   auto update = [&](const auto& from) {
@@ -252,15 +255,27 @@ static void launch_step_tail(const StepParams& p, const Src& src, const StepTail
     else step_kernel<From, Update<kStepDdpm>, kP><<<grid, 256, 0, st>>>(p, from, Update<kStepDdpm>());
     IVID_CHECK_CUDA(cudaGetLastError());
   };
-  if (!t.threshold) {
-    update(src);
+  auto finish = [&](const auto& from) {
+    using From = std::decay_t<decltype(from)>;
+    if (!t.threshold) {
+      update(from);
+      return;
+    }
+    step_kernel<From, StoreX0, kPag><<<elementwise_grid(from.units(p)), 256, 0, st>>>(p, from, StoreX0{t.x0});
+    IVID_CHECK_CUDA(cudaGetLastError());
+    threshold_select_kernel<<<p.N, kSelectThreads, 0, st>>>(t.x0, p.C * p.HW, t.ratio, t.s_max, t.s);
+    IVID_CHECK_CUDA(cudaGetLastError());
+    update(ThresholdedX0{t.x0, t.s});
+  };
+  if (!t.apg) {
+    finish(src);
     return;
   }
-  step_kernel<Src, StoreX0, kPag><<<elementwise_grid(src.units(p)), 256, 0, st>>>(p, src, StoreX0{t.x0});
+  step_kernel<Src, ApgStore, kPag><<<elementwise_grid(src.units(p)), 256, 0, st>>>(p, src, ApgStore{t.ap});
   IVID_CHECK_CUDA(cudaGetLastError());
-  threshold_select_kernel<<<p.N, kSelectThreads, 0, st>>>(t.x0, p.C * p.HW, t.ratio, t.s_max, t.s);
+  apg_reduce_kernel<<<p.N, kApgThreads, 0, st>>>(t.ap.dc, t.ap.m, p.C * p.HW, p.strength, t.ap.eta, t.ap.norm, p.guided, t.ap.scal);
   IVID_CHECK_CUDA(cudaGetLastError());
-  update(ThresholdedX0{t.x0, t.s});
+  finish(ApgX0{t.ap});
 }
 // the PAG instantiations only for a step with the perturbed rows (StepParams::pag)
 template <typename Src>
@@ -293,6 +308,30 @@ void launch_dynamic_threshold(const float* x, int N, int M, double ratio, double
   const size_t total = static_cast<size_t>(N) * M;
   threshold_apply_kernel<<<elementwise_grid(total), 256, 0, st>>>(x, s_out, x_out, static_cast<size_t>(M), total);
   IVID_CHECK_CUDA(cudaGetLastError());
+}
+
+// the APG parameters, as ivid_step_args_t documents them
+static void check_apg_params(double eta, double norm, double beta) {
+  IVID_REQUIRE(std::isfinite(eta) && eta >= 0.0, "apg_eta must be finite and >= 0");
+  IVID_REQUIRE(std::isfinite(norm) && norm >= 0.0, "apg_norm must be finite and >= 0");
+  IVID_REQUIRE(std::isfinite(beta) && beta > -1.0 && beta < 1.0, "apg_momentum must lie in (-1, 1)");
+}
+
+void launch_apg(const float* dc, const float* du, float* state, int N, int M, float s, double eta, double norm, double beta,
+                float* out, cudaStream_t st) {
+  IVID_REQUIRE(N >= 1 && M >= 1, "apg: N and M must be positive");
+  IVID_REQUIRE(std::isfinite(s) && s > 0.0f, "apg: strength must be finite and > 0");
+  check_apg_params(eta, norm, beta);
+  const size_t total = static_cast<size_t>(N) * M;
+  float* scal = nullptr;
+  IVID_CHECK_CUDA(cudaMallocAsync(&scal, sizeof(float) * 2 * N, st));
+  apg_momentum_kernel<<<elementwise_grid(total), 256, 0, st>>>(dc, du, state, static_cast<float>(beta), total);
+  IVID_CHECK_CUDA(cudaGetLastError());
+  apg_reduce_kernel<<<N, kApgThreads, 0, st>>>(dc, state, M, s, eta, norm, nullptr, scal);
+  IVID_CHECK_CUDA(cudaGetLastError());
+  apg_apply_kernel<<<elementwise_grid(total), 256, 0, st>>>(dc, state, scal, out, static_cast<size_t>(M), total);
+  IVID_CHECK_CUDA(cudaGetLastError());
+  IVID_CHECK_CUDA(cudaFreeAsync(scal, st));
 }
 
 void launch_cond_pack(const CondPackDesc& d, cudaStream_t s) {
@@ -348,6 +387,7 @@ Sampler::~Sampler() {
   if (d_acp_) cudaFree(d_acp_);
   if (d_hist_) cudaFree(d_hist_);
   if (d_thr_s_) cudaFree(d_thr_s_);
+  if (d_apg_) cudaFree(d_apg_);
 }
 
 const std::vector<double>& Sampler::table(int which) const {
@@ -408,6 +448,29 @@ void Sampler::ensure_hist(size_t elems) {
   cap_hist_ = elems;
 }
 
+// APG planes of [N,C,H,W]: D_c, m (the momentum state) and the PAG term, then the scalars [N][2]
+constexpr int kApgPlanes = 3;
+void Sampler::ensure_apg(size_t img, int N) {
+  const size_t elems = kApgPlanes * img + 2 * static_cast<size_t>(N);
+  if (elems <= cap_apg_ && img == apg_img_) return;
+  if (d_apg_) cudaFree(d_apg_);
+  IVID_CHECK_CUDA(cudaMalloc(&d_apg_, elems * 4));
+  cap_apg_ = elems;
+  apg_img_ = img;
+}
+
+ApgParams Sampler::apg_params(const ivid_step_args_t& a) const {
+  ApgParams ap;
+  ap.dc = d_apg_;
+  ap.m = d_apg_ + apg_img_;
+  ap.pag = d_apg_ + 2 * apg_img_;
+  ap.scal = d_apg_ + kApgPlanes * apg_img_;
+  ap.beta = static_cast<float>(a.apg_momentum);
+  ap.eta = a.apg_eta;
+  ap.norm = a.apg_norm;
+  return ap;
+}
+
 // sample size H x W: 0 means the backbone's image_size
 static int sample_dim(int v, const Unet& unet) { return v > 0 ? v : unet.cfg().image_size; }
 
@@ -461,6 +524,14 @@ void Sampler::check_step_args(const ivid_step_args_t& a, const Unet& unet, int N
       for (int j = 0; j < i; ++j) IVID_REQUIRE(a.pag_layers[j] != a.pag_layers[i], "pag_layers: a layer is listed twice");
     }
   }
+  // adaptive projected guidance: a flag, acting on the classifier-free mix only (use_cfg, classes, strength > 0)
+  IVID_REQUIRE(a.apg == 0 || a.apg == 1, "apg must be 0 or 1");
+  if (a.apg) {
+    IVID_REQUIRE(a.use_cfg && a.classes_dev != nullptr && a.strength > 0.0f,
+                 "apg needs classifier-free guidance: use_cfg = 1, classes_dev and strength > 0");
+    IVID_REQUIRE(std::isfinite(a.strength), "apg: strength must be finite");
+    check_apg_params(a.apg_eta, a.apg_norm, a.apg_momentum);
+  }
 }
 
 // whether a step runs the perturbed-attention rows at all: pag with a positive scale (pag_scale 0 is the step without them)
@@ -474,6 +545,7 @@ struct StepPlan {
   bool guided;        // host route: the model time lies inside the interval (or none applies); the device route sets true
   int cfg;            // StepParams::cfg
   bool pag;           // the forward carries the perturbed-attention rows (last block of N)
+  bool apg;           // the classifier-free mix of this step runs as adaptive projected guidance (cfg == 1)
   int Nf;             // the forward's batch: N, + N null-class rows when cfg == 1, + N perturbed rows with pag
   int order;          // DPM-Solver++ order of the update: 2 with a previous data prediction unless order = 1, else 1;
                       // UniPC: the predictor order min(order, nhist + 1), 1 on the final step (device route: at most that)
@@ -502,6 +574,7 @@ static StepPlan plan_step(const ivid_step_args_t& a, int N, int t, int t_prev, b
   const bool scale_only = a.use_cfg && a.strength < 0.0f && (has_classes || a.cond.kind == 0) && sp.guided;
   sp.cfg = two ? 1 : (scale_only ? 2 : 0);
   sp.pag = pag_on(a) && sp.guided;
+  sp.apg = a.apg != 0 && sp.cfg == 1;
   sp.Nf = (two ? 2 * N : N) + (sp.pag ? N : 0);
   sp.order = (a.kind == kStepDpm && a.prev_x0_dev != nullptr && a.order != 1) ? 2 : 1;
   sp.corr_order = 0;
@@ -574,6 +647,19 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
     if (sp.order == 2 && a.prev_x0_dev != d_hist_)
       IVID_CHECK_CUDA(cudaMemcpyAsync(d_hist_, a.prev_x0_dev, img * 4, cudaMemcpyDeviceToDevice, stream));
   }
+  // APG: m_prev lives in the sampler's plane (a fixed pointer).  run() passes that plane itself; a caller's state is copied
+  // in and receives m after the step, NULL is zero history
+  float* apg_state_out = nullptr;
+  if (sp.apg) {
+    ensure_apg(img, N);
+    float* m = d_apg_ + apg_img_;
+    if (a.apg_state_dev == nullptr) {
+      IVID_CHECK_CUDA(cudaMemsetAsync(m, 0, img * 4, stream));
+    } else if (a.apg_state_dev != m) {
+      IVID_CHECK_CUDA(cudaMemcpyAsync(m, a.apg_state_dev, img * 4, cudaMemcpyDeviceToDevice, stream));
+      apg_state_out = a.apg_state_dev;
+    }
+  }
   StepState* state = reinterpret_cast<StepState*>(d_state_);
   set_step_kernel<<<1, 128, 0, stream>>>(state, d_t_, sp.Nf, sp.t_index, sp.t_prev, stream_id, t_dev, t_prev_dev,
                                          kind != kStepDdpm ? 1 : 0, T_, dpm ? d_acp_ : nullptr, a.t_last, sp.order, a.sde,
@@ -634,6 +720,10 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
     tail.unipc = true;
     tail.uni = UniPcUpdate{d_hist_, img, a.corrected_xt_dev, &state->uni, a.order};
   }
+  if (sp.apg) {
+    tail.apg = true;
+    tail.ap = apg_params(a);
+  }
 
   unet.set_cond_stream_dev(cond.kind != 0 && cond.noise_dev == nullptr ? &state->stream : nullptr);
   // Fused route: the output head's last kernel IS the step (step_kernel<HeadTaps, ...>): eps never reaches HBM and the update is
@@ -663,6 +753,12 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
       mix(&u.arena, sizeof(u.arena)); mix(&u.plane, sizeof(u.plane)); mix(&u.corrected, sizeof(u.corrected));
       mix(&u.u, sizeof(u.u)); mix(&u.depth, sizeof(u.depth));
     }
+    if (tail.apg) {           // APG: its planes and parameters, field by field
+      const ApgParams& g = tail.ap;
+      h ^= 0xA9600000ull;
+      mix(&g.dc, sizeof(g.dc)); mix(&g.m, sizeof(g.m)); mix(&g.pag, sizeof(g.pag)); mix(&g.scal, sizeof(g.scal));
+      mix(&g.beta, sizeof(g.beta)); mix(&g.eta, sizeof(g.eta)); mix(&g.norm, sizeof(g.norm));
+    }
     hook.key = h | 1ull;
     hook.launch = [p, tail](const float* Y, const float* bias, int, int Hy, int Wy, int Co, int ldy, cudaStream_t st) {
       IVID_REQUIRE(Co == 4 && Wy % 4 == 0, "fused head step: 4 output channels, width % 4 == 0");
@@ -678,6 +774,8 @@ void Sampler::step_impl(Unet& unet, const float* x_t, float* x_prev, float* pred
                sp.cache_branch, sp.pag ? &pert : nullptr);
   unet.set_cond_stream_dev(nullptr);
   if (!fuse) launch_step_tail(p, EpsRows{d_eps_}, tail, stream);
+  if (apg_state_out != nullptr)
+    IVID_CHECK_CUDA(cudaMemcpyAsync(apg_state_out, d_apg_ + apg_img_, img * 4, cudaMemcpyDeviceToDevice, stream));
 }
 
 void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t& a, const float* noise_all,
@@ -698,6 +796,13 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
   const int rows = pag_on(a) ? 3 : 2;             // the largest forward of the run, in blocks of N
   ensure_device(rows * N, rows * img);
   if (dpm) ensure_hist(a.unipc ? kUniPcPlanes * img : img);   // before the loop: the history must not move between steps
+  float* apg_state = nullptr;
+  if (a.apg) {
+    // the APG planes likewise; the momentum state starts at zero at the first executed step
+    ensure_apg(img, N);
+    apg_state = d_apg_ + apg_img_;
+    IVID_CHECK_CUDA(cudaMemsetAsync(apg_state, 0, img * 4, stream));
+  }
   if (dpm && !a.sde) noise_all = nullptr;          // the ODE solver draws no step noise
   // the fused head step needs per-step pointers that stay the same from step to step
   const bool allow_fuse = noise_all == nullptr && cond_noise_all == nullptr && traj_x0 == nullptr && traj_xt == nullptr;
@@ -717,6 +822,7 @@ void Sampler::run(Unet& unet, float* x, int N, int steps, const ivid_step_args_t
     else { t = T_ - 1 - i; t_prev = 0; }                                      // ddpm.py:177
     ivid_step_args_t ai = a;
     ai.step_noise_dev = noise_all ? noise_all + static_cast<size_t>(k) * img : nullptr;
+    ai.apg_state_dev = apg_state;
     if (dpm) {
       // multistep history: from the second executed step on, D_{-1} is the previous step's D0, already in the sampler's buffer
       ai.prev_x0_dev = k > 0 ? d_hist_ : nullptr;

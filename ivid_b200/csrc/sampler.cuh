@@ -6,9 +6,12 @@
 //              DdimSampler.sample_once                      samplers/ddim.py:81-103
 //              DPM-Solver++(2M), data-prediction multistep  Lu et al. 2022, arXiv:2211.01095 (no reference counterpart)
 //              UniPC, bh2 predictor-corrector               Zhao et al. 2023, arXiv:2302.04867 (no reference counterpart)
+//              adaptive projected guidance                  Sadat et al. 2025, arXiv:2410.02416 (no reference counterpart)
 //              InpaintCFG.make_cond_inputs                  frameworks/inpaint_cfg.py:33-49
 //              SuperResCFG.make_cond_inputs                 frameworks/sr_cfg.py:31-36
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ivid {
@@ -353,25 +356,92 @@ __device__ __forceinline__ Quad flat_quad(const StepParams& p, size_t u) {
   return q;
 }
 
+// What a source makes of the eps row blocks of a quad.  GuidedX0 (every step): the guided, clipped x_0 of each element, from
+// mix_eps4.  ApgInputs (the first pass of an APG step, below): the three inputs of adaptive projected guidance.  mix() runs
+// before x_t is read, x0() per element after.
+struct GuidedX0 {
+  using Eps = float[1][4];
+  using Out = float[4];
+  template <typename Ld>
+  __device__ __forceinline__ static void mix(const StepParams& p, int cfg, Ld&& eps, Eps& e) { mix_eps4(p, cfg, eps, e[0]); }
+  __device__ __forceinline__ static void x0(const StepParams& p, const StepCoef& k, int j, float xt, const Eps& e, Out& o) {
+    o[j] = eps_x0(p, k, xt, e[0][j]);
+  }
+};
+
+// ----------------------------------------------------------------------------------------------
+// Adaptive projected guidance (APG; Sadat, Hilliges, Weber, ICLR 2025, arXiv:2410.02416), per sample n over its M = C*H*W
+// elements, on a step with the classifier-free mix (include/ivid_b200.h):
+//   D_c = x_0 of eps_c, D_u = x_0 of eps_u, m = (D_c - D_u) + beta * m_prev, c = min(1, r / |m|),
+//   k = (1 - eta) <m, D_c> / max(|D_c|^2, tiny), D = D_c + s c (m - k D_c) (+ the PAG term w (D_c - D_p)).
+// A step in this mode runs step_kernel<Src, ApgStore> (D_c, m and the PAG term into sampler-owned planes, from HeadTaps on
+// the fused route and EpsRows on the separate one), apg_reduce_kernel (the two scalars of every sample) and
+// step_kernel<ApgX0, sink> (D, then the update, or StoreX0 and the dynamic threshold).  Both routes share the last two.
+// ----------------------------------------------------------------------------------------------
+struct ApgParams {
+  float* dc;                   // [N,C,H,W] D_c
+  float* m;                    // [N,C,H,W] m_prev on entry, m after the first pass (in place)
+  float* pag;                  // [N,C,H,W] the PAG term w (D_c - D_p) (steps with PAG only)
+  float* scal;                 // [N][2]: fp32(s * c) and fp32(s * c * k)
+  float beta;                  // momentum, rounded to fp32 once
+  double eta, norm;            // parallel weight and norm bound r (0: no bound), used in double
+};
+// the momentum update of one element: m = delta + beta * m_prev (beta = 0: m = delta, m_prev is not read)
+__device__ __forceinline__ float apg_momentum(float delta, float beta, float m_prev) {
+  return beta != 0.0f ? __fadd_rn(delta, __fmul_rn(beta, m_prev)) : delta;
+}
+// the guided x_0 of one element: D_c + (s c * m - s c k * D_c)
+__device__ __forceinline__ float apg_guide(float dc, float m, float sc, float sck) {
+  return __fadd_rn(dc, __fsub_rn(__fmul_rn(sc, m), __fmul_rn(sck, dc)));
+}
+// The first pass's inputs of an element: o[0] = D_c = x_0 of eps_c (never clipped), o[1] = D_c - D_u, o[2] = the PAG term
+// w (D_c - D_p).  The differences are taken in eps, where the x_t terms cancel: D_c - D_u = sqrt(1/acp - 1) (eps_u - eps_c)
+// and D_c - D_p = sqrt(1/acp - 1) (eps_p - eps_c).  On a step the device flag leaves unguided (cfg 0) only o[0] is formed.
+struct ApgInputs {
+  using Eps = float[3][4];     // eps_c, eps_u - eps_c, w (eps_p - eps_c)
+  using Out = float[3][4];
+  template <typename Ld>
+  __device__ __forceinline__ static void mix(const StepParams& p, int cfg, Ld&& eps, Eps& e) {
+    eps(0, e[0]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) e[1][j] = e[2][j] = 0.f;
+    if ((cfg & 3) == 1) {
+      eps(1, e[1]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) e[1][j] = __fsub_rn(e[1][j], e[0][j]);
+    }
+    if (cfg & kPagBit) {
+      eps(pag_block(cfg), e[2]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) e[2][j] = __fmul_rn(p.pag_scale, __fsub_rn(e[2][j], e[0][j]));
+    }
+  }
+  __device__ __forceinline__ static void x0(const StepParams&, const StepCoef& k, int j, float xt, const Eps& e, Out& o) {
+    o[0][j] = step_x0(k, xt, e[0][j]);
+    o[1][j] = __fmul_rn(k.sqrt_recipm1_acp, e[1][j]);
+    o[2][j] = __fmul_rn(k.sqrt_recipm1_acp, e[2][j]);
+  }
+};
+
 // x_0 from the eps buffer [N, 2N or 3N][C,H,W]: rows [0,N) conditional, then [N,2N) unconditional when cfg & 3 == 1, then the
 // perturbed rows with kPagBit.  One quad per unit.
 struct EpsRows {
   const float* eps;
   __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * p.C * p.HW / 4; }
-  template <typename F>
+  template <typename R = GuidedX0, typename F>
   __device__ __forceinline__ void quads(const StepParams& p, const StepCoef& k, int cfg, size_t u, F&& f) const {
     const size_t total = static_cast<size_t>(p.N) * p.C * p.HW;
     const Quad q = flat_quad(p, u);
-    f(q, [&](float (&xt)[4], float (&x0)[4]) {
-      float e[4];
-      mix_eps4(p, cfg, [&](int b, float (&v)[4]) {
+    f(q, [&](float (&xt)[4], typename R::Out& x0) {
+      typename R::Eps e;
+      R::mix(p, cfg, [&](int b, float (&v)[4]) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) v[j] = eps[b * total + q.i + j];
       }, e);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         xt[j] = p.x_t[q.i + j];
-        x0[j] = eps_x0(p, k, xt[j], e[j]);
+        R::x0(p, k, j, xt[j], e, x0);
       }
     });
   }
@@ -397,16 +467,16 @@ struct HeadTaps {
 #pragma unroll
     for (int c = 0; c < 4; ++c) e[c] += __ldg(bias + c);
   }
-  template <typename F>
+  template <typename R = GuidedX0, typename F>
   __device__ __forceinline__ void quads(const StepParams& p, const StepCoef& k, int cfg, size_t g, F&& f) const {
     const int w4 = W / 4;
     const int xg = static_cast<int>(g % w4);
     const int y = static_cast<int>((g / w4) % H);
     const int n = static_cast<int>(g / (static_cast<size_t>(w4) * H));
-    float e[4][4];                  // [pixel][channel]
+    typename R::Eps e[4];           // [pixel][block][channel]
 #pragma unroll
     for (int j = 0; j < 4; ++j)
-      mix_eps4(p, cfg, [&](int b, float (&v)[4]) { eps4(n + b * p.N, y, xg * 4 + j, v); }, e[j]);
+      R::mix(p, cfg, [&](int b, float (&v)[4]) { eps4(n + b * p.N, y, xg * 4 + j, v); }, e[j]);
     const size_t pix = static_cast<size_t>(y) * W + xg * 4;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -415,11 +485,16 @@ struct HeadTaps {
       q.pix = pix;
       q.n = n;
       q.c = c;
-      f(q, [&](float (&xt)[4], float (&x0)[4]) {
+      f(q, [&](float (&xt)[4], typename R::Out& x0) {
         const float4 v = ldg_f4(p.x_t + q.i);
         xt[0] = v.x; xt[1] = v.y; xt[2] = v.z; xt[3] = v.w;
+        typename R::Eps ec;          // channel c of the four pixels
 #pragma unroll
-        for (int j = 0; j < 4; ++j) x0[j] = eps_x0(p, k, xt[j], e[j][c]);
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int b = 0; b < static_cast<int>(sizeof(ec) / sizeof(ec[0])); ++b) ec[b][j] = e[j][b][c];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) R::x0(p, k, j, xt[j], ec, x0);
       });
     }
   }
@@ -544,14 +619,136 @@ struct StoreX0 {
   }
 };
 
-// kPag: the instantiation for steps with perturbed-attention guidance (p.pag = 1); the others mask kPagBit off at compile time
+// The first pass of an APG step (a source reading ApgInputs): D_c, m = (D_c - D_u) + beta * m_prev and the PAG term of a
+// quad into the planes of a.  On a step the device flag leaves unguided only D_c is written and m_prev stays as it was.
+struct ApgStore {
+  ApgParams a;
+  using Reader = ApgInputs;
+  struct Scalars { StepCoef k; int guided; };
+  __device__ __forceinline__ static Scalars scalars(const StepParams& p) { return {p.table[*p.t_index], step_cfg(p) & 3}; }
+  template <typename Load>
+  __device__ __forceinline__ void operator()(const StepParams& p, const Scalars& s, const Quad& q, Load&& load) const {
+    float xt[4], in[3][4];
+    load(xt, in);
+    stg_f4(a.dc + q.i, make_float4(in[0][0], in[0][1], in[0][2], in[0][3]));
+    if (!s.guided) return;
+    float mp[4] = {0.f, 0.f, 0.f, 0.f}, m[4];
+    if (a.beta != 0.0f) {
+      const float4 t = *reinterpret_cast<const float4*>(a.m + q.i);
+      mp[0] = t.x; mp[1] = t.y; mp[2] = t.z; mp[3] = t.w;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) m[j] = apg_momentum(in[1][j], a.beta, mp[j]);
+    stg_f4(a.m + q.i, make_float4(m[0], m[1], m[2], m[3]));
+    if (p.pag) stg_f4(a.pag + q.i, make_float4(in[2][0], in[2][1], in[2][2], in[2][3]));
+  }
+};
+
+// x_0 of an APG step from the planes of the first pass and the scalars of apg_reduce_kernel: D = D_c + s c (m - k D_c), plus
+// the PAG term (cfg & kPagBit), clipped when p.clip is set; D_c alone (then clipped) on a step the device flag leaves
+// unguided (cfg 0), which is the unguided step's x_0 bit for bit.  One quad per unit.
+struct ApgX0 {
+  ApgParams a;
+  __host__ __device__ size_t units(const StepParams& p) const { return static_cast<size_t>(p.N) * p.C * p.HW / 4; }
+  template <typename F>
+  __device__ __forceinline__ void quads(const StepParams& p, const StepCoef&, int cfg, size_t u, F&& f) const {
+    const Quad q = flat_quad(p, u);
+    f(q, [&](float (&xt)[4], float (&x0)[4]) {
+      const float4 d = ldg_f4(a.dc + q.i);
+      const float dc[4] = {d.x, d.y, d.z, d.w};
+      float dv[4] = {dc[0], dc[1], dc[2], dc[3]};
+      if (cfg & 3) {
+        const float sc = a.scal[2 * q.n], sck = a.scal[2 * q.n + 1];
+        const float4 m = ldg_f4(a.m + q.i);
+        const float mv[4] = {m.x, m.y, m.z, m.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) dv[j] = apg_guide(dc[j], mv[j], sc, sck);
+        if (cfg & kPagBit) {
+          const float4 g = ldg_f4(a.pag + q.i);
+          dv[0] = __fadd_rn(dv[0], g.x); dv[1] = __fadd_rn(dv[1], g.y);
+          dv[2] = __fadd_rn(dv[2], g.z); dv[3] = __fadd_rn(dv[3], g.w);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        xt[j] = p.x_t[q.i + j];
+        x0[j] = p.clip ? fminf(fmaxf(dv[j], -1.0f), 1.0f) : dv[j];
+      }
+    });
+  }
+};
+
+// kPag: the instantiation for steps with perturbed-attention guidance (p.pag = 1); the others mask kPagBit off at compile time.
+// The APG first pass (Sink = ApgStore) has its source read ApgInputs instead of the guided x_0.
 template <typename Src, typename Sink, bool kPag>
 __global__ void __launch_bounds__(256) step_kernel(const StepParams p, const Src src, const Sink sink) {
   const typename Sink::Scalars s = sink.scalars(p);
   const int cfg = kPag ? step_cfg(p) : (step_cfg(p) & 3);
   const size_t units = src.units(p);
-  for (size_t u = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; u < units; u += static_cast<size_t>(gridDim.x) * blockDim.x)
-    src.quads(p, s.k, cfg, u, [&](const Quad& q, auto&& load) { sink(p, s, q, load); });
+  for (size_t u = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; u < units; u += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    if constexpr (std::is_same_v<Sink, ApgStore>)
+      src.template quads<ApgInputs>(p, s.k, cfg, u, [&](const Quad& q, auto&& load) { sink(p, s, q, load); });
+    else
+      src.quads(p, s.k, cfg, u, [&](const Quad& q, auto&& load) { sink(p, s, q, load); });
+  }
+}
+
+// The two scalars of APG for every sample n (one block per sample) from the first pass's planes D_c and m over its M elements:
+// |m|^2, <m, D_c> and |D_c|^2 in double, each thread over elements threadIdx.x + j * kApgThreads in order, then a fixed
+// tree over the block, so the sums depend on the sample's own elements only.  c = min(1, r / |m|) (1 for r = 0 or m = 0),
+// k = (1 - eta) <m, D_c> / max(|D_c|^2, tiny); scal[n] = {fp32(s) * fp32(c), fp32(s * fp32(c) * k)}.  guided != nullptr
+// and 0: the step is unguided and nothing is written.
+constexpr int kApgThreads = 512;
+__global__ void __launch_bounds__(kApgThreads) apg_reduce_kernel(const float* __restrict__ dc, const float* __restrict__ m, int M,
+                                                                 float s, double eta, double r, const int* guided,
+                                                                 float* __restrict__ scal) {
+  if (guided != nullptr && *guided == 0) return;
+  __shared__ double part[3][kApgThreads / 32];
+  const size_t base = static_cast<size_t>(blockIdx.x) * M;
+  double mm = 0.0, md = 0.0, dd = 0.0;
+  for (int i = threadIdx.x; i < M; i += kApgThreads) {
+    const double mv = m[base + i], dv = dc[base + i];
+    mm = __fma_rn(mv, mv, mm);
+    md = __fma_rn(mv, dv, md);
+    dd = __fma_rn(dv, dv, dd);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mm = __dadd_rn(mm, __shfl_xor_sync(0xFFFFFFFFu, mm, o));
+    md = __dadd_rn(md, __shfl_xor_sync(0xFFFFFFFFu, md, o));
+    dd = __dadd_rn(dd, __shfl_xor_sync(0xFFFFFFFFu, dd, o));
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { part[0][warp] = mm; part[1][warp] = md; part[2][warp] = dd; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mm = md = dd = 0.0;
+    for (int w = 0; w < kApgThreads / 32; ++w) {
+      mm = __dadd_rn(mm, part[0][w]);
+      md = __dadd_rn(md, part[1][w]);
+      dd = __dadd_rn(dd, part[2][w]);
+    }
+    const double nm = sqrt(mm);
+    const float c = (r > 0.0 && nm > 0.0) ? static_cast<float>(fmin(1.0, r / nm)) : 1.0f;
+    const double k = (1.0 - eta) * md / fmax(dd, 2.2250738585072014e-308);
+    scal[2 * blockIdx.x] = __fmul_rn(s, c);
+    scal[2 * blockIdx.x + 1] = static_cast<float>(static_cast<double>(s) * c * k);
+  }
+}
+
+// The element passes of ivid_op_apg over [N][M]: m = (d_c - d_u) + beta * m_prev in place, then out = apg_guide
+__global__ void __launch_bounds__(256) apg_momentum_kernel(const float* __restrict__ dc, const float* __restrict__ du, float* m,
+                                                           float beta, size_t total) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    m[i] = apg_momentum(__fsub_rn(dc[i], du[i]), beta, m[i]);
+}
+__global__ void __launch_bounds__(256) apg_apply_kernel(const float* __restrict__ dc, const float* __restrict__ m,
+                                                        const float* __restrict__ scal, float* __restrict__ out, size_t M,
+                                                        size_t total) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t n = i / M;
+    out[i] = apg_guide(dc[i], m[i], scal[2 * n], scal[2 * n + 1]);
+  }
 }
 
 // ----------------------------------------------------------------------------------------------

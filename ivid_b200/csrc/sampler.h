@@ -7,6 +7,7 @@
 namespace ivid {
 
 struct StepPlan;   // what one step runs (sampler.cu)
+struct ApgParams;  // the planes and parameters of an APG step (sampler.cuh)
 
 class Sampler {
  public:
@@ -36,6 +37,10 @@ class Sampler {
                  const int64_t* t_prev_dev, bool allow_fuse, bool classes2_filled);
   void ensure_device(int N2, size_t eps_elems);
   void ensure_hist(size_t elems);
+  // APG planes and scalars for samples of img = N*C*H*W elements (sampler.cu: kApgPlanes); the buffer moves only when img
+  // changes or N outgrows it
+  void ensure_apg(size_t img, int N);
+  ApgParams apg_params(const ivid_step_args_t& a) const;
   int T_;
   std::vector<double> betas_, acp_, acp_prev_, srac_, srm1_, pvar_, plogvar_, pc1_, pc2_;
   void* d_table_ = nullptr;
@@ -47,6 +52,8 @@ class Sampler {
   int64_t* d_t_ = nullptr;
   int64_t* d_classes2_ = nullptr;
   float* d_thr_s_ = nullptr;               // dynamic thresholding: s of every sample [cap_n_]
+  float* d_apg_ = nullptr;                 // adaptive projected guidance: D_c, m, the PAG term and the scalars
+  size_t cap_apg_ = 0, apg_img_ = 0;
   float* d_eps_ = nullptr;
   float* d_xtmp_ = nullptr;
   int cap_n_ = 0;

@@ -23,7 +23,7 @@ import torch
 from .. import backbones, frameworks, samplers
 from ..backbones.adm import PAG_DEFAULT_LAYERS
 from ..frameworks.gaussian_diffusion import check_pag
-from ..samplers.samplers import _check_cache, _check_threshold
+from ..samplers.samplers import _check_apg, _check_cache, _check_threshold
 from ..rgbd_3d import DeviceWarp, glm_compat as glm
 from ..rgbd_3d import utils as rgbd_utils
 from ..utils import edict
@@ -128,7 +128,7 @@ def build_modelviews(viewset, num_samples, rng=None):
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
                precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init_views=None,
-               init_strength=None, pag_scale=None, pag_layers=None):
+               init_strength=None, pag_scale=None, pag_layers=None, apg=None):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, solver="dpmpp_sde" its stochastic variant
@@ -144,7 +144,9 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     (framework_uncond may be None); with init_strength view 0 is its SDEdit by the unconditional sampler (the samplers'
     `init` / `init_strength`) with the sample's class, guidance, solver and options.  Views 1... grow from view 0 as always.
     pag_scale=w, pag_layers=names add perturbed-attention guidance to every step of both networks (the samplers'
-    `pag_scale` / `pag_layers`), the class-free unconditional network included; the guidance interval gates it there too."""
+    `pag_scale` / `pag_layers`), the class-free unconditional network included; the guidance interval gates it there too.
+    apg=eta, (eta, r) or (eta, r, beta) runs the classifier-free mix of both networks as adaptive projected guidance (the
+    samplers' `apg`); both frameworks must have classifier-free guidance, and classes are needed."""
     if init_views is None:
         assert init_strength is None, "init_strength needs init_views"
     else:
@@ -156,6 +158,10 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
             _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
             check_pag(pag_scale, pag_layers, fw.backbone)
     _check_threshold(dynamic_threshold, False)
+    if apg is not None:
+        for fw in (framework_uncond, framework_cond):
+            if fw is not None:
+                _check_apg(apg, fw, classes, guidance)
     assert solver in ("ddim", "dpmpp", "dpmpp_sde", "unipc"), \
         f"solver must be 'ddim', 'dpmpp', 'dpmpp_sde' or 'unipc', got {solver!r}"
     for fw in (framework_uncond, framework_cond):
@@ -172,6 +178,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
         gi_kw.update(cache_interval=cache_interval, cache_branch=cache_branch)
     th_kw = dict(dynamic_threshold=dynamic_threshold) if dynamic_threshold is not None else {}
     pag_kw = dict(pag_scale=pag_scale, pag_layers=pag_layers) if pag_scale is not None else {}
+    apg_kw = dict(apg=apg) if apg is not None else {}
     # a framework without classifier-free guidance takes the interval only to gate perturbed-attention guidance
     plain_kw = {k: v for k, v in gi_kw.items() if k.startswith("cache") or (pag_kw and k == "guidance_interval")}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
@@ -217,7 +224,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 kw = dict(strength=guidance, **gi_kw) if cfg_u else dict(plain_kw)
                 if steps_uncond < 1000:
                     kw.update(sde_kw)
-                kw.update(th_kw, **pag_kw)
+                kw.update(th_kw, **pag_kw, **apg_kw)
                 if init_views is not None:     # SDEdit of the given view; the seeds' noise is the forward diffusion's z
                     kw.update(init=init_views[i: i + bs].to(device=dev, dtype=torch.float32), init_strength=init_strength)
                 res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
@@ -230,7 +237,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
                 kw = dict(strength=guidance, **gi_kw) if cfg_u else dict(plain_kw)
-                kw.update(sde_kw, **th_kw, **pag_kw)
+                kw.update(sde_kw, **th_kw, **pag_kw, **apg_kw)
                 res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
             samples.append(res.samples)
             if warp is not None:
@@ -373,7 +380,8 @@ def main(rank, world_size, opt):
                      rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
                      precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch,
                      dynamic_threshold=dynamic_threshold, init_views=init_views, init_strength=init_strength,
-                     pag_scale=getattr(opt, "pag_scale", None), pag_layers=getattr(opt, "pag_layers", None))
+                     pag_scale=getattr(opt, "pag_scale", None), pag_layers=getattr(opt, "pag_layers", None),
+                     apg=getattr(opt, "apg", None))
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -397,7 +405,7 @@ def output_dir_name(opt):
                         + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}")
                         + ("" if init_image is None else f"_init-{os.path.splitext(os.path.basename(init_image))[0]}")
                         + ("" if init_strength is None else f"_strength{init_strength}")
-                        + _pag_suffix(opt))
+                        + _pag_suffix(opt) + _apg_suffix(opt))
 
 
 def _pag_suffix(opt):
@@ -406,6 +414,14 @@ def _pag_suffix(opt):
     if w is None:
         return ""
     return f"_pag{w}" + ("" if layers is None or tuple(layers) == PAG_DEFAULT_LAYERS else "-" + "+".join(layers))
+
+
+def _apg_suffix(opt):
+    """_apg{ETA}, then ,{R} and ,{BETA} as given."""
+    apg = getattr(opt, "apg", None)
+    if apg is None:
+        return ""
+    return "_apg" + ",".join(str(v) for v in (apg if isinstance(apg, tuple) else (apg,)))
 
 
 def _int_at_least(lo):
@@ -448,6 +464,25 @@ def parse_threshold(s):
     if len(vals) == 2 and not vals[1] >= 1.0:
         raise argparse.ArgumentTypeError(f"expected MAX >= 1, got {s!r}")
     return vals[0] if len(vals) == 1 else (vals[0], vals[1])
+
+
+def parse_apg(s):
+    """'ETA', 'ETA,R' or 'ETA,R,BETA' -> ETA or the tuple of --apg: ETA >= 0, the norm bound R >= 0 (0: none) and the
+    momentum -1 < BETA < 1, all finite."""
+    parts = s.split(",")
+    if len(parts) not in (1, 2, 3):
+        raise argparse.ArgumentTypeError(f"expected ETA[,R[,BETA]], got {s!r}")
+    try:
+        vals = [float(v) for v in parts]
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected numbers ETA[,R[,BETA]], got {s!r}") from None
+    if not all(math.isfinite(v) for v in vals):
+        raise argparse.ArgumentTypeError(f"expected finite numbers, got {s!r}")
+    if vals[0] < 0.0 or (len(vals) > 1 and vals[1] < 0.0):
+        raise argparse.ArgumentTypeError(f"expected ETA >= 0 and R >= 0, got {s!r}")
+    if len(vals) == 3 and not -1.0 < vals[2] < 1.0:
+        raise argparse.ArgumentTypeError(f"expected -1 < BETA < 1, got {s!r}")
+    return vals[0] if len(vals) == 1 else tuple(vals)
 
 
 def parse_pag_scale(s):
@@ -549,6 +584,10 @@ def build_arg_parser():
                          "attention maps) at every guided step; works without classes (default: off)")
     ap.add_argument("--pag_layers", type=parse_pag_layers, default=None, metavar="NAME[,NAME...]",
                     help="with --pag_scale: the attention layers to perturb, by state-dict name (default: middle_block.1)")
+    ap.add_argument("--apg", type=parse_apg, default=None, metavar="ETA[,R[,BETA]]",
+                    help="adaptive projected guidance of both networks: the guidance update split into its parts parallel and "
+                         "orthogonal to the conditional x_0, the parallel part weighted by ETA, the update's norm bounded by R "
+                         "(0: no bound) and a momentum BETA across steps; e.g. 0,0,-0.5 (default: plain classifier-free guidance)")
     return ap
 
 

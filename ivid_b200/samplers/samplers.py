@@ -75,6 +75,26 @@ def _check_threshold(dynamic_threshold, clip_denoised):
     return float(p), float(s_max)
 
 
+def _check_apg(apg, framework, classes, strength):
+    """Adaptive projected guidance argument: None, eta, (eta, r) or (eta, r, beta), eta >= 0, the norm bound r >= 0 (0: none)
+    and the momentum beta in (-1, 1), all finite; r and beta default to 0.  It acts on the classifier-free mix, so it needs
+    a framework with one, classes and strength > 0.  Returns (eta, r, beta) as floats, or None."""
+    if apg is None:
+        return None
+    vals = tuple(apg) if isinstance(apg, (tuple, list)) else (apg,)
+    assert 1 <= len(vals) <= 3, f"apg must be eta, (eta, r) or (eta, r, beta), got {apg!r}"
+    eta, r, beta = vals + (0.0,) * (3 - len(vals))
+    real = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool) and math.isfinite(v)
+    assert real(eta) and eta >= 0.0, f"apg eta must be finite and >= 0, got {eta!r}"
+    assert real(r) and r >= 0.0, f"apg norm bound r must be finite and >= 0, got {r!r}"
+    assert real(beta) and -1.0 < beta < 1.0, f"apg momentum beta must lie in (-1, 1), got {beta!r}"
+    assert isinstance(framework, (ClassifierFreeGuidance, InpaintCFG, SuperResCFG)), \
+        f"apg acts on classifier-free guidance, which {type(framework).__name__} does not have"
+    assert classes is not None, "apg acts on classifier-free guidance, which needs classes"
+    assert math.isfinite(strength) and strength > 0.0, f"apg needs a guidance strength > 0, got {strength!r}"
+    return float(eta), float(r), float(beta)
+
+
 def init_steps(init_strength, steps):
     """Executed steps n of a run started from an image (SDEdit): round(init_strength * steps), at least 1 and at most steps.
     The run then starts at grid step start_step = steps - n."""
@@ -136,7 +156,8 @@ class _NativeSampler:
         return uses_cfg, float(kwargs.get("strength", 3.0)) if uses_cfg else 0.0
 
     def _step_args(self, device, classes, clip_denoised, eta, kwargs, step_noise=None, cond_noise=None, seed=0, hw=None,
-                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None, prev_x=None, corrected=None, pag=None):
+                   order=0, prev=None, sde=False, interval=None, cache=None, threshold=None, prev_x=None, corrected=None, pag=None,
+                   apg=None, apg_state=None):
         fw = self.framework
         a = _lib.StepArgsT()
         keep = []
@@ -214,6 +235,10 @@ class _NativeSampler:
             layers = (ctypes.c_int * len(pag[1]))(*pag[1])
             keep.append(layers)
             a.pag, a.pag_scale, a.pag_layers, a.pag_num_layers = 1, pag[0], layers, len(pag[1])
+        if apg is not None:
+            a.apg = 1
+            a.apg_eta, a.apg_norm, a.apg_momentum = apg
+            a.apg_state_dev = _lib.ptr(apg_state).value
         return a, keep
 
     def _net(self):
@@ -225,16 +250,20 @@ class _NativeSampler:
         return _unwrap(self.framework.backbone).num_res_blocks
 
     def _native_step(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
-                     sde=False, interval=None, cache=None, threshold=None, prev_x=None, pag=None):
+                     sde=False, interval=None, cache=None, threshold=None, prev_x=None, pag=None, apg=None, apg_state=None):
         """One step.  `t` / `t_prev` are host ints (ivid_sampler_step) or the [N] tensors sample_once receives
-        (ivid_sampler_step_dev: the step is read on the device, no host sync; t_prev None for DDPM)."""
+        (ivid_sampler_step_dev: the step is read on the device, no host sync; t_prev None for DDPM).  With `apg`, the
+        momentum state m_prev (None: zero history) is copied, and the copy receives m: it is the returned `apg_state`."""
         net = self._net()
         dev = x_t.device
         x_t = _f32(x_t, dev)
         corrected = torch.empty_like(x_t) if self.UNIPC else None
+        if apg is not None:
+            apg_state = torch.zeros_like(x_t) if apg_state is None else _f32(apg_state, dev).clone()
         a, keep = self._step_args(dev, classes, clip_denoised, eta, kwargs, step_noise=noise, cond_noise=cond_noise,
                                   hw=x_t.shape[-2:], order=order, prev=prev, sde=sde, interval=interval, cache=cache,
-                                  threshold=threshold, prev_x=prev_x, corrected=corrected, pag=pag)
+                                  threshold=threshold, prev_x=prev_x, corrected=corrected, pag=pag, apg=apg,
+                                  apg_state=apg_state)
         x_prev = torch.empty_like(x_t)
         x0 = torch.empty_like(x_t)
         L = _lib.lib()
@@ -251,10 +280,13 @@ class _NativeSampler:
         out = edict({"pred_x_prev": x_prev, "pred_x_0": x0})
         if self.UNIPC:
             out.corrected_x_t = corrected
+        if apg is not None:
+            out.apg_state = apg_state
         return out
 
     def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, interval, reuse_features, cache_branch,
-                     order=0, prev=None, sde=False, dynamic_threshold=None, prev_x=None, pag_scale=None, pag_layers=None):
+                     order=0, prev=None, sde=False, dynamic_threshold=None, prev_x=None, pag_scale=None, pag_layers=None,
+                     apg=None, apg_state=None):
         """The body of every sample_once: the host checks before any device work or torch draw, the step noise (drawn as
         the reference draws it, or the injected `noise` and kwargs' `cond_noise`), then the step with t / t_prev read on
         the device (all samples of a batch share the step, ddpm.py:177-179, ddim.py:154-158: no host sync)."""
@@ -265,6 +297,10 @@ class _NativeSampler:
         _check_cache(None, cache_branch, self._num_res_blocks())
         threshold = _check_threshold(dynamic_threshold, clip_denoised)
         pag = check_pag(pag_scale, pag_layers, self.framework.backbone)
+        apg = _check_apg(apg, self.framework, classes, self._guidance(kwargs)[1])
+        assert apg_state is None or apg is not None, "apg_state needs apg"
+        assert apg_state is None or tuple(apg_state.shape) == tuple(x_t.shape), \
+            f"apg_state must have x_t's shape {tuple(x_t.shape)}, got {tuple(apg_state.shape)}"
         if noise is None:
             noise, cond_noise = self._draw_step_noise(x_t, kwargs)
         else:
@@ -272,7 +308,8 @@ class _NativeSampler:
         # the DPM-Solver++ ODE update reads no step noise
         return self._native_step(x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise if self.KIND != 2 or sde else None,
                                  cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold, prev_x=prev_x, pag=pag)
+                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold, prev_x=prev_x, pag=pag,
+                                 apg=apg, apg_state=apg_state)
 
     def _draw_step_noise(self, x_t, kwargs):
         """torch draws in the reference's order: InpaintCFG rgb, depth (inside model_inference), then randn_like(x_t)."""
@@ -302,9 +339,10 @@ class _NativeSampler:
 
     def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
              sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init=None, init_strength=None,
-             pag_scale=None, pag_layers=None):
+             pag_scale=None, pag_layers=None, apg=None):
         interval = _check_interval(interval, len(self.framework.betas))   # before any device work
         pag = check_pag(pag_scale, pag_layers, self.framework.backbone)
+        apg = _check_apg(apg, self.framework, classes, self._guidance(kwargs)[1])
         cache_interval = _check_cache(cache_interval, cache_branch, self._num_res_blocks())
         threshold = _check_threshold(dynamic_threshold, clip_denoised)
         _check_init(init, init_strength, noise, image_size, _unwrap(self.framework.backbone).out_channels)
@@ -345,7 +383,7 @@ class _NativeSampler:
                 jump = T // nsteps
                 sched = [(jump * (i + 1), jump * i) for i in reversed(range(nsteps))]
             sched = sched[start:]
-            prev, prev_x = None, None
+            prev, prev_x, apg_state = None, None, None
             reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
                                          cache_interval, pag)
             for i, (t, t_prev) in enumerate(sched):
@@ -353,7 +391,10 @@ class _NativeSampler:
                 # the DPM-Solver++ ODE update draws z only to consume the torch RNG as DdimSampler does
                 out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if self.KIND != 2 or sde else None,
                                         cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                        cache=(0, cache_branch, reuse[i]), threshold=threshold, prev_x=prev_x, pag=pag)
+                                        cache=(0, cache_branch, reuse[i]), threshold=threshold, prev_x=prev_x, pag=pag,
+                                        apg=apg, apg_state=apg_state)
+                if apg is not None:
+                    apg_state = out.apg_state
                 if self.UNIPC:
                     prev, prev_x = ([(t, out.pred_x_0)] + (prev or []))[:order], out.corrected_x_t
                 elif self.KIND == 2 and order != 1:
@@ -364,7 +405,8 @@ class _NativeSampler:
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
-                                      interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold, pag=pag)
+                                      interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold, pag=pag,
+                                      apg=apg)
             a.start_step = start
             traj0 = trajt = None
             if return_trajectory:
@@ -399,21 +441,25 @@ class DdpmSampler(_NativeSampler):
 
     @torch.no_grad()
     def sample_once(self, x_t, t, classes=None, clip_denoised=False, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, apg=None, apg_state=None, **kwargs):
         """x_{t-1} from x_t (ddpm.py:111-131).  `t` is the [N] tensor of steps minus 1 (all equal).
         `noise` (extension) injects the randn_like draw; default draws it with torch like the reference.
         `guidance_interval=(t_lo, t_hi)` (extension): the step is guided only if t lies in [t_lo, t_hi] (see `sample`).
         `reuse_features=True` (extension): the step's forward reuses the deep features of the last full forward of the same
         batch and size at branch `cache_branch` (see `sample`); RuntimeError if no full forward has run on it.
         `dynamic_threshold=p` or `(p, s_max)` (extension): dynamic thresholding of x_0 (see `sample`).
-        `pag_scale` / `pag_layers` (extension): perturbed-attention guidance (see `sample`)."""
+        `pag_scale` / `pag_layers` (extension): perturbed-attention guidance (see `sample`).
+        `apg` (extension): adaptive projected guidance (see `sample`).  `apg_state` is the momentum state the previous step
+        returned as `out.apg_state` (None at the first step: zero history); the step returns its own, so steps chained with
+        apg_state = out.apg_state reproduce a run, as `prev` / `prev_x` chain the multistep samplers."""
         return self._sample_once(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, guidance_interval, reuse_features,
-                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers)
+                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers,
+                                 apg=apg, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, apg=None, **kwargs):
         """Run the full reverse process (ddpm.py:134-187).  `steps` is accepted and ignored exactly as in the reference.
         pred_x_t / pred_x_0 are only materialised with return_trajectory=True (the reference keeps 2x1000 tensors alive;
         its callers read `.samples` only: inference/sample.py:82).
@@ -449,11 +495,21 @@ class DdpmSampler(_NativeSampler):
         (default ("middle_block.1",)) replaced by the identity, and uses eps = G + w (eps_c - eps_perturbed), G the eps of the
         step without it (the classifier-free mix, if any).  It works without classes, so it guides class-free models too.  The
         guidance interval gates it like classifier-free guidance.  w >= 0; None or 0 is the run without it, bit for bit.  The
-        noise and the torch RNG consumption are unchanged (the InpaintCFG hole noise is shared by the perturbed rows)."""
+        noise and the torch RNG consumption are unchanged (the InpaintCFG hole noise is shared by the perturbed rows).
+
+        apg=eta, (eta, r) or (eta, r, beta) (extension; adaptive projected guidance, Sadat, Hilliges, Weber, ICLR 2025,
+        arXiv:2410.02416): every guided step replaces the classifier-free mix by an update in x_0 space.  Per sample, with
+        D_c / D_u the x_0 of the conditional / null-class eps and m = (D_c - D_u) + beta m_prev (momentum across guided steps),
+        the update is scaled to norm at most r and its part parallel to D_c weighted by eta: D = D_c + s c (m - k D_c),
+        c = min(1, r / |m|), k = (1 - eta) <m, D_c> / |D_c|^2, s the strength (include/ivid_b200.h).  eta >= 0, r >= 0 (0: no
+        bound, the default), -1 < beta < 1 (default 0).  eta = 1, r = 0, beta = 0 is classifier-free guidance up to rounding.
+        Needs a classifier-free-guidance framework, classes and strength > 0.  Clipping or dynamic thresholding, the
+        multiview guidance and the update read D.  The noise and the torch RNG consumption are unchanged; None (default) is
+        the run without it, bit for bit."""
         return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
                          dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
-                         pag_layers=pag_layers)
+                         pag_layers=pag_layers, apg=apg)
 
 
 class DdimSampler(_NativeSampler):
@@ -463,26 +519,28 @@ class DdimSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, eta=0.0, replace_rgb=None,
                     replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, apg=None, apg_state=None, **kwargs):
         """x_{t_prev} from x_t (ddim.py:48-103).  t / t_prev are [N] tensors of actual steps (1 means one step).
         `guidance_interval=(t_lo, t_hi)`: the step is guided only if its model time t - 1 lies in [t_lo, t_hi].
-        `reuse_features` / `cache_branch` / `dynamic_threshold` / `pag_scale` / `pag_layers` as in DdpmSampler.sample_once."""
+        `reuse_features` / `cache_branch` / `dynamic_threshold` / `pag_scale` / `pag_layers` / `apg` / `apg_state` as in
+        DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers)
+                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers,
+                                 apg=apg, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
                verbose=True, rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, apg=None, **kwargs):
         """Run `steps` DDIM steps (ddim.py:106-165).  `guidance_interval=(t_lo, t_hi)` as in DdpmSampler.sample, on the model
         time t - 1 of each step; `cache_interval` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample (the replace /
-        constrain guidance acts on the thresholded x_0).  `init` / `init_strength` and `pag_scale` / `pag_layers` as in
-        DdpmSampler.sample."""
+        constrain guidance acts on the thresholded x_0).  `init` / `init_strength`, `pag_scale` / `pag_layers` and `apg` as
+        in DdpmSampler.sample (the replace / constrain guidance acts on the APG-guided x_0)."""
         return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
                          interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
                          dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
-                         pag_layers=pag_layers)
+                         pag_layers=pag_layers, apg=apg)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -501,23 +559,24 @@ class DpmSolverSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, replace_rgb=None, replace_depth=None,
                     constrain_depth=None, noise=None, sde=False, guidance_interval=None, reuse_features=False, cache_branch=0,
-                    dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
+                    dynamic_threshold=None, pag_scale=None, pag_layers=None, apg=None, apg_state=None, **kwargs):
         """x_{t_prev} from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev = (t_last, pred_x_0)` of the previous step selects the second-order update, None the first-order one.
         With sde=True `noise` is the injected z of the update; with sde=False the update does not use it.  When it is None
         the torch RNG is consumed exactly as DdimSampler.sample_once consumes it (InpaintCFG hole noise, then one
         randn_like(x_t), which is z for sde=True); `cond_noise` injects the hole noise.  `guidance_interval`, `reuse_features`,
         `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once (D0, and so pred_x_0, is thresholded);
-        `pag_scale` / `pag_layers` as for DdpmSampler.sample_once."""
+        `pag_scale` / `pag_layers` and `apg` / `apg_state` as for DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
                                  cache_branch, order=2 if prev is not None else 1, prev=prev, sde=sde,
-                                 dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers)
+                                 dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers, apg=apg,
+                                 apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, sde=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, apg=None, **kwargs):
         """Run `steps` DPM-Solver++ steps of order `order` (1 or 2), the SDE variant with sde=True.  The first step and the
         final step (to t_prev = 0, which returns x_0 as DDIM does and draws no noise) are first order.  The SDE's step noise
         is drawn where DdimSampler draws it (`rng`).  `guidance_interval` as in DdimSampler.sample; the history D_{-1} of a
@@ -525,12 +584,13 @@ class DpmSolverSampler(_NativeSampler):
         the history D_{-1} of a step is that step's D0, from whichever forward ran.  `dynamic_threshold` as in
         DdpmSampler.sample: D0 is the thresholded, guided x_0, and so is the history.  `init` / `init_strength` as in
         DdpmSampler.sample; the first executed step is first order.  `pag_scale` / `pag_layers` as in DdpmSampler.sample; the
-        history holds the PAG-guided D0.  Same return dict as DdimSampler.sample."""
+        history holds the PAG-guided D0.  `apg` as in DdpmSampler.sample; the history holds the APG-guided D0.  Same return
+        dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
                          cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength,
-                         pag_scale=pag_scale, pag_layers=pag_layers)
+                         pag_scale=pag_scale, pag_layers=pag_layers, apg=apg)
 
 
 class UniPcSampler(_NativeSampler):
@@ -547,7 +607,7 @@ class UniPcSampler(_NativeSampler):
     @torch.no_grad()
     def sample_once(self, x_t, t, t_prev, classes=None, clip_denoised=False, prev=None, prev_x=None, order=2, replace_rgb=None,
                     replace_depth=None, constrain_depth=None, noise=None, guidance_interval=None, reuse_features=False,
-                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, **kwargs):
+                    cache_branch=0, dynamic_threshold=None, pag_scale=None, pag_layers=None, apg=None, apg_state=None, **kwargs):
         """One UniPC step from x_t.  t / t_prev are [N] tensors of actual steps, as for DdimSampler.sample_once.
         `prev` is a list of up to three `(t_last, pred_x_0)` pairs of the previous steps, newest first, and `prev_x` the
         previous step's `corrected_x_t` (the corrector's base; required with `prev`).  With n pairs (at most `order` are used)
@@ -555,7 +615,7 @@ class UniPcSampler(_NativeSampler):
         Returns `pred_x_prev` (the prediction the next step's network sees), `pred_x_0` and `corrected_x_t` (x_t itself
         without `prev`).  Chain steps with prev = ([(t, pred_x_0)] + prev)[:3] and prev_x = corrected_x_t.  `noise` is not used; the
         torch RNG is consumed as DpmSolverSampler.sample_once consumes it.  `guidance_interval`, `reuse_features`,
-        `cache_branch`, `dynamic_threshold` and `pag_scale` / `pag_layers` as for DdimSampler.sample_once."""
+        `cache_branch`, `dynamic_threshold`, `pag_scale` / `pag_layers` and `apg` / `apg_state` as for DdimSampler.sample_once."""
         assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
         prev = list(prev) if prev is not None else []
         assert len(prev) <= 3, f"prev holds at most three (t_last, pred_x_0) pairs, got {len(prev)}"
@@ -563,21 +623,21 @@ class UniPcSampler(_NativeSampler):
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
         return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
                                  cache_branch, order=order, prev=prev, dynamic_threshold=dynamic_threshold, prev_x=prev_x,
-                                 pag_scale=pag_scale, pag_layers=pag_layers)
+                                 pag_scale=pag_scale, pag_layers=pag_layers, apg=apg, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
                rng="philox", return_trajectory=False, guidance_interval=None, cache_interval=None, cache_branch=0,
-               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, **kwargs):
+               dynamic_threshold=None, init=None, init_strength=None, pag_scale=None, pag_layers=None, apg=None, **kwargs):
         """Run `steps` UniPC steps of order `order` (1, 2 or 3; 2 is the paper's choice for guided sampling).  Step i predicts
         at order min(order, i + 1) and corrects at the previous step's order; the first step has no corrector and the final
         step (to t_prev = 0) returns x_0 as DDIM does.  pred_x_t holds the predictions the network saw.  Draws no step noise;
         the torch RNG is consumed as DpmSolverSampler.sample(sde=False) consumes it.  `guidance_interval`, `cache_interval` /
         `cache_branch` and `dynamic_threshold` as in DpmSolverSampler.sample: the history holds the D0 of whichever forward
-        ran, thresholded.  `init` / `init_strength` and `pag_scale` / `pag_layers` as in DdpmSampler.sample; the order ramp
-        starts at the first executed step.  Same return dict as DdimSampler.sample."""
+        ran, thresholded.  `init` / `init_strength`, `pag_scale` / `pag_layers` and `apg` as in DdpmSampler.sample; the order
+        ramp starts at the first executed step.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
         return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
                          order=order, interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
                          dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
-                         pag_layers=pag_layers)
+                         pag_layers=pag_layers, apg=apg)
