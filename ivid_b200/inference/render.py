@@ -1,9 +1,9 @@
 """Free-view fusion rendering of sampled scenes (reference inference/render.py:41-89): every stored view of a scene is
 re-meshed (load_scene, numeric padding) and all of them are aggregated by the CUDA AggregationRenderer at 5x
 super-sampling from a camera trajectory; frames are LANCZOS-resolved to 128x128 (colour) and point-sampled + inferno
-colour-mapped (depth).
+colour-mapped (depth) at the size of the stored views (128x128 for the pipeline's scenes, 256x256 after super-resolution).
 
-    python -m ivid_b200.inference.render --scene_dir samples/... [--traj swing|random] [--frames 60]
+    python -m ivid_b200.inference.render --scene_dir samples/... [--traj swing|random] [--frames 60] [--image_size N]
 
 Differences from the reference script: frames are written as PNG sequences + one .npz per scene when `imageio` (mp4
 writer) is not installed; the random trajectory takes a seed.
@@ -18,7 +18,7 @@ import numpy as np
 from PIL import Image
 
 from ..rgbd_3d import glm_compat as glm
-from .utils import colorize_depth, load_scene
+from .utils import colorize_depth, load_scene, load_scene_views
 
 SSAA = 5                      # render.py:64
 
@@ -76,12 +76,19 @@ def render_scene(renderer, scene_path, modelviews, atol=0.03, rtol=0.03, erode_r
     depth colour map run on the device (AggregationRenderer.render_resolved); resolve_on_device=False keeps the reference's
     numpy / PIL / cv2 steps on the host (`resolve_frame`), bit-identical by construction."""
     meshes, colors = load_scene(scene_path, atol=atol, rtol=rtol, erode_rgb=erode_rgb)
+    assert all(c.shape[0] == renderer.image_size for c in colors), \
+        f"{scene_path}: the views are {colors[0].shape[0]}x{colors[0].shape[0]}, the renderer's image_size is {renderer.image_size}"
     if resolve_on_device:
         return renderer.render_resolved(meshes, colors, list(modelviews), lut=depth_colour_table())
     res = renderer.render(meshes, colors, list(modelviews))
     frames = res if isinstance(res, list) else [res]
     cols, deps = zip(*(resolve_frame(f, renderer.image_size) for f in frames))
     return np.stack(cols, axis=0), np.stack(deps, axis=0)
+
+
+def scene_image_size(path):
+    """The size n of the n x n views stored in a scene file."""
+    return int(load_scene_views(path)[0].color.shape[0])
 
 
 def main(argv=None):
@@ -94,6 +101,7 @@ def main(argv=None):
     ap.add_argument("--atol", type=float, default=0.03)
     ap.add_argument("--rtol", type=float, default=0.03)
     ap.add_argument("--erode_rgb", type=int, default=3)
+    ap.add_argument("--image_size", type=int, default=None, help="frame size (default: the size of the first scene's views)")
     opt = ap.parse_args(argv)
     out_dir = opt.output_dir or opt.scene_dir
     os.makedirs(os.path.join(out_dir, "results"), exist_ok=True)
@@ -108,7 +116,8 @@ def main(argv=None):
         raise NotImplementedError(opt.traj)
 
     from .. import rgbd_3d
-    renderer = rgbd_3d.AggregationRenderer(128 * SSAA, 128, near=0.1, far=200, device=0)
+    n = opt.image_size if opt.image_size is not None else (scene_image_size(scenes[0]) if scenes else 128)
+    renderer = rgbd_3d.AggregationRenderer(n * SSAA, n, near=0.1, far=200, device=0)
     try:
         import imageio
     except ImportError:

@@ -4,6 +4,7 @@
     view 0:  unconditional sampler  (DDPM 1000 / DDIM), or a given view (SDEdit of it)  -> RGBD on the GPU
     view j:  DeviceWarp.aggregate (CUDA mesh + rasterise + aggregate + post-filters)  -> condition maps on the GPU
              conditional DDIM sampler with replace / constrain guidance               -> RGBD on the GPU
+    then, with a super-resolution network, every view again at its size (superres.superresolve_views)
 
 Nothing crosses PCIe inside the loop; samples are copied to the host once per batch for saving.
 
@@ -27,7 +28,11 @@ from ..samplers.samplers import _check_apg, _check_cache, _check_threshold
 from ..rgbd_3d import DeviceWarp, glm_compat as glm
 from ..rgbd_3d import utils as rgbd_utils
 from ..utils import edict
+from .superres import check_options as _check_sr_options, check_superres, superresolve_views
 from .utils import colorize_depth, parse_int_list, reorder, save_scene
+
+
+_SR_STREAM = 0x2A5AC0DE5EED0001      # mixed into the reseed of an unseeded super-resolution stage
 
 
 def shard(items, rank, world_size):
@@ -128,7 +133,8 @@ def build_modelviews(viewset, num_samples, rng=None):
 def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_uncond, steps_cond, modelviews, fov=45, near=0.6,
                far=5, atol=0.03, rtol=0.03, erode_rgb=2, classes=None, guidance=3.0, batchsize=10, rng="philox", solver="ddim",
                precision="fp16", guidance_interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init_views=None,
-               init_strength=None, pag_scale=None, pag_layers=None, apg=None):
+               init_strength=None, pag_scale=None, pag_layers=None, apg=None, framework_sr=None, steps_sr=50, sr_size=None,
+               sr_guidance=None, sr_replace=(0.1, 0.2)):
     """Generator over finished samples: (meshes, colors, samples [V,4,H,W], conds) — signature of sample.py:30-46.
     `meshes[v]` carries what save_scene needs (linear depth, fov, modelview).  solver="dpmpp" runs DpmSolverSampler
     (DPM-Solver++(2M)) wherever the reference runs DdimSampler, solver="dpmpp_sde" its stochastic variant
@@ -146,7 +152,14 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     pag_scale=w, pag_layers=names add perturbed-attention guidance to every step of both networks (the samplers'
     `pag_scale` / `pag_layers`), the class-free unconditional network included; the guidance interval gates it there too.
     apg=eta, (eta, r) or (eta, r, beta) runs the classifier-free mix of both networks as adaptive projected guidance (the
-    samplers' `apg`); both frameworks must have classifier-free guidance, and classes are needed."""
+    samplers' `apg`); both frameworks must have classifier-free guidance, and classes are needed.
+    framework_sr (a SuperResCFG) super-resolves every batch once all its views exist (superres.superresolve_views, with
+    steps_sr steps, output size sr_size or its backbone's image_size, guidance sr_guidance or `guidance`, replace weights
+    sr_replace, the batch's seeds and every option above).  The stage draws from a fork of the torch RNG, so the views at S
+    are bit for bit those of the call without it, seeded or not (unseeded, the fork is reseeded from one draw of the RNG,
+    so the stage's draws do not repeat the next batch's); the generator yields the S' views as
+    `samples`, their meshes and colours at S', and the S views as conds["lowres"] [V,4,S,S] (conds is created for it when
+    the view set has no conditional views)."""
     if init_views is None:
         assert init_strength is None, "init_strength needs init_views"
     else:
@@ -164,6 +177,14 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 _check_apg(apg, fw, classes, guidance)
     assert solver in ("ddim", "dpmpp", "dpmpp_sde", "unipc"), \
         f"solver must be 'ddim', 'dpmpp', 'dpmpp_sde' or 'unipc', got {solver!r}"
+    net = (framework_uncond if framework_uncond is not None else framework_cond).backbone
+    S = net.image_size
+    dev = net.device
+    if framework_sr is not None:
+        check_superres(framework_sr, S, sr_size, sr_replace)
+        _check_sr_options(framework_sr, classes, guidance if sr_guidance is None else sr_guidance, solver, guidance_interval,
+                          cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        assert isinstance(steps_sr, int) and steps_sr >= 1, f"steps_sr must be an integer >= 1, got {steps_sr!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
             fw.backbone.set_precision(precision)
@@ -183,15 +204,13 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
     plain_kw = {k: v for k, v in gi_kw.items() if k.startswith("cache") or (pag_kw and k == "guidance_interval")}
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
-    net = (framework_uncond if framework_uncond is not None else framework_cond).backbone
-    S = net.image_size
-    dev = net.device
     if init_views is not None:
         assert tuple(init_views.shape) == (num_samples, 4, S, S), \
             f"init_views must be [{num_samples},4,{S},{S}] (one view per sample, at the backbone's size), got {tuple(init_views.shape)}"
     per_sample_views = isinstance(modelviews[0], list)
     wparams = dict(fov=fov, near=near, far=far, atol=atol, rtol=rtol, erode_rgb=erode_rgb)
     warps = {}
+    sr_cache = {}
 
     for i in range(0, num_samples, batchsize):
         bs = min(batchsize, num_samples - i)
@@ -244,6 +263,24 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 warp.add_view(res.samples, mv_j, **wparams)
         samples = torch.stack(samples, dim=1)                           # [bs, V, 4, S, S]
         conds = {"color": torch.stack(cond_color, dim=1), "depth": torch.stack(cond_depth, dim=1)} if cond_color else None
+        if framework_sr is not None:
+            conds = dict(conds or {}, lowres=samples)
+            # the stage draws from a fork of the torch RNG (CPU and this device), so the batches after it draw what they draw
+            # without it; unseeded, the fork is reseeded first, else it would repeat the next batch's draws
+            cuda_idx = ([dev.index if dev.index is not None else torch.cuda.current_device()] if dev.type == "cuda" else [])
+            with torch.random.fork_rng(devices=cuda_idx):
+                if seeds is None:
+                    sr_seed = int(torch.randint(0, 2 ** 62, (1,)).item()) ^ _SR_STREAM
+                    torch.random.default_generator.manual_seed(sr_seed)
+                    for k in cuda_idx:
+                        torch.cuda.default_generators[k].manual_seed(sr_seed)
+                samples = superresolve_views(
+                    framework_sr, samples, [views_of(k) for k in range(bs)] if per_sample_views else views_of(0),
+                    steps=steps_sr, size=sr_size, classes=b_classes, guidance=guidance if sr_guidance is None else sr_guidance,
+                    seeds=seeds[i: i + bs] if seeds is not None else None, replace=sr_replace, rng=rng, solver=solver,
+                    precision=precision, guidance_interval=guidance_interval, cache_interval=cache_interval,
+                    cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale,
+                    pag_layers=pag_layers, apg=apg, cache=sr_cache, **wparams)           # [bs, V, 4, S', S']
         rgbd = samples.permute(0, 1, 3, 4, 2).cpu().numpy() * 0.5 + 0.5   # one D2H per batch
         for k in range(bs):
             meshes = [edict(depth=rgbd_utils.linearize_depth(rgbd[k, v, :, :, 3:], near, far), fov=fov,
@@ -283,24 +320,31 @@ def async_save(meshes, colors, samples, conds, suffix, cfg):
          viewset uncond: results/rgb_*.png + scenes/scene_*.npz
          viewset random: grids/rgb_*.png (both views), conds/rgb_*.png (view 0), results/rgb_*.png (view 1)
          viewset 3x9   : grids/{rgb,depth}_*.png, conds/{rgb_cond,depth_cond}_*.png (3x9 mosaics, `reorder`), scenes/scene_*.npz
+    After the super-resolution stage (conds["lowres"] holds the views before it) the results, grids and scene are at the
+    super-resolved size, conds/ keeps the conditions the conditional model saw, and random / 3x9 add grids/rgb_lowres_*.png.
     The 8-bit images are packed on the device on the caller's stream and copied to pinned host memory asynchronously; a
     worker thread waits for that copy, encodes the PNGs and writes the scene, while the main thread goes on sampling."""
     from PIL import Image
     out = cfg.output_dir
     jobs = []       # (relative path, device uint8 HWC tensor)
     vs = cfg.viewset
+    lowres = conds.get("lowres") if conds is not None else None
     if vs == "uncond":
         jobs.append((os.path.join("results", f"rgb_{suffix}.png"), to_u8(samples[0, :3])))
     elif vs == "random":
         jobs.append((os.path.join("grids", f"rgb_{suffix}.png"), image_grid_u8(samples[:, :3], 2)))
-        jobs.append((os.path.join("conds", f"rgb_{suffix}.png"), to_u8(samples[0, :3])))
+        jobs.append((os.path.join("conds", f"rgb_{suffix}.png"), to_u8((samples if lowres is None else lowres)[0, :3])))
         jobs.append((os.path.join("results", f"rgb_{suffix}.png"), to_u8(samples[1, :3])))
+        if lowres is not None:
+            jobs.append((os.path.join("grids", f"rgb_lowres_{suffix}.png"), image_grid_u8(lowres[:, :3], 2)))
     elif vs == "3x9":
         dev = samples.device
         jobs.append((os.path.join("grids", f"rgb_{suffix}.png"), image_grid_u8(reorder(samples[:, :3], vs), 9)))
         jobs.append((os.path.join("grids", f"depth_{suffix}.png"), image_grid_u8(reorder(colorize_depth(samples[:, 3:]).to(dev), vs), 9)))
         jobs.append((os.path.join("conds", f"rgb_cond_{suffix}.png"), image_grid_u8(reorder(conds["color"][:, :3], vs), 9)))
         jobs.append((os.path.join("conds", f"depth_cond_{suffix}.png"), image_grid_u8(reorder(colorize_depth(conds["depth"]).to(dev), vs), 9)))
+        if lowres is not None:
+            jobs.append((os.path.join("grids", f"rgb_lowres_{suffix}.png"), image_grid_u8(reorder(lowres[:, :3], vs), 9)))
     else:
         raise NotImplementedError
     host = []
@@ -343,6 +387,8 @@ def main(rank, world_size, opt):
     fw_u = _load_model(cfg_u, opt.ckpt_uncond, dev) if init_image is None or init_strength is not None else None
     cfg_c = json.load(open(opt.config_cond)) if opt.viewset != "uncond" or init_image is not None else None
     fw_c = _load_model(cfg_c, opt.ckpt_cond, dev) if opt.viewset != "uncond" else None
+    config_sr = getattr(opt, "config_sr", None)
+    fw_sr = _load_model(json.load(open(config_sr)), getattr(opt, "ckpt_sr", None), dev) if config_sr is not None else None
     seeds = parse_int_list(opt.seeds) if opt.num_samples is None else None
     num = len(seeds) if seeds is not None else opt.num_samples
     ncls = cfg_u["backbone"]["args"].get("num_classes")
@@ -381,7 +427,8 @@ def main(rank, world_size, opt):
                      precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch,
                      dynamic_threshold=dynamic_threshold, init_views=init_views, init_strength=init_strength,
                      pag_scale=getattr(opt, "pag_scale", None), pag_layers=getattr(opt, "pag_layers", None),
-                     apg=getattr(opt, "apg", None))
+                     apg=getattr(opt, "apg", None), framework_sr=fw_sr, steps_sr=getattr(opt, "steps_sr", 50),
+                     sr_replace=getattr(opt, "sr_replace", SR_REPLACE_DEFAULT))
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -405,7 +452,7 @@ def output_dir_name(opt):
                         + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}")
                         + ("" if init_image is None else f"_init-{os.path.splitext(os.path.basename(init_image))[0]}")
                         + ("" if init_strength is None else f"_strength{init_strength}")
-                        + _pag_suffix(opt) + _apg_suffix(opt))
+                        + _pag_suffix(opt) + _apg_suffix(opt) + _sr_suffix(opt))
 
 
 def _pag_suffix(opt):
@@ -422,6 +469,34 @@ def _apg_suffix(opt):
     if apg is None:
         return ""
     return "_apg" + ",".join(str(v) for v in (apg if isinstance(apg, tuple) else (apg,)))
+
+
+SR_REPLACE_DEFAULT = (0.1, 0.2)
+
+
+def _sr_suffix(opt):
+    """_sr{STEPS} with --config_sr, then -replace{RGB}-{DEPTH} or -noreplace when the replace weights are not the default."""
+    if getattr(opt, "config_sr", None) is None:
+        return ""
+    rep = getattr(opt, "sr_replace", SR_REPLACE_DEFAULT)
+    tail = "" if rep == SR_REPLACE_DEFAULT else ("-noreplace" if rep is None else f"-replace{rep[0]}-{rep[1]}")
+    return f"_sr{getattr(opt, 'steps_sr', 50)}" + tail
+
+
+def parse_sr_replace(s):
+    """'RGB,DEPTH' -> (RGB, DEPTH) of --sr_replace, both in [0, 1]; 'none' -> None (views super-resolved independently)."""
+    if s.strip().lower() == "none":
+        return None
+    parts = s.split(",")
+    if len(parts) != 2:
+        raise argparse.ArgumentTypeError(f"expected RGB,DEPTH or none, got {s!r}")
+    try:
+        vals = tuple(float(v) for v in parts)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected two numbers RGB,DEPTH, got {s!r}") from None
+    if not all(0.0 <= v <= 1.0 for v in vals):
+        raise argparse.ArgumentTypeError(f"expected weights in [0, 1], got {s!r}")
+    return vals
 
 
 def _int_at_least(lo):
@@ -526,7 +601,36 @@ def parse_args(argv=None):
         ap.error("--init_strength needs --init_image and --init_depth")
     if o.pag_layers is not None and o.pag_scale is None:
         ap.error("--pag_layers needs --pag_scale")
+    check_sr_flags(ap, o)
     return o
+
+
+def add_sr_flags(ap, required=False):
+    """The super-resolution flags.  --steps_sr and --sr_replace default to argparse.SUPPRESS so that check_sr_flags can
+    tell a given flag from its default."""
+    ap.add_argument("--config_sr", required=required, default=None, metavar="PATH",
+                    help="super-resolve every scene with this SuperResCFG config (e.g. rgbd_imagenet_adm_256_128_small_sr.json) "
+                         "once its views exist: results, grids and scenes at the network's image_size (default: off)")
+    ap.add_argument("--ckpt_sr", default=None, metavar="PATH", help="checkpoint of --config_sr (default: random weights)")
+    ap.add_argument("--steps_sr", type=_int_at_least(1), default=argparse.SUPPRESS, metavar="N",
+                    help="sampler steps of every super-resolved view (default 50)")
+    ap.add_argument("--sr_replace", type=parse_sr_replace, default=argparse.SUPPRESS, metavar="RGB,DEPTH|none",
+                    help="replace-guidance weights of the super-resolved views towards the earlier ones, warped at the new size "
+                         "(default 0.1,0.2, the conditional stage's, not tuned for super-resolution); 'none' super-resolves "
+                         "every view on its own")
+
+
+def check_sr_flags(ap, o):
+    """--ckpt_sr, --steps_sr and --sr_replace need --config_sr; fills the defaults of the last two."""
+    if o.config_sr is None:
+        for flag, given in (("ckpt_sr", o.ckpt_sr is not None), ("steps_sr", hasattr(o, "steps_sr")),
+                            ("sr_replace", hasattr(o, "sr_replace"))):
+            if given:
+                ap.error(f"--{flag} needs --config_sr")
+    if not hasattr(o, "steps_sr"):
+        o.steps_sr = 50
+    if not hasattr(o, "sr_replace"):
+        o.sr_replace = SR_REPLACE_DEFAULT
 
 
 def build_arg_parser():
@@ -588,6 +692,7 @@ def build_arg_parser():
                     help="adaptive projected guidance of both networks: the guidance update split into its parts parallel and "
                          "orthogonal to the conditional x_0, the parallel part weighted by ETA, the update's norm bounded by R "
                          "(0: no bound) and a momentum BETA across steps; e.g. 0,0,-0.5 (default: plain classifier-free guidance)")
+    add_sr_flags(ap)
     return ap
 
 
