@@ -16,6 +16,7 @@ CPU restatement of the reference's RGBD novel-view warp.
 from __future__ import annotations
 
 import ctypes
+import ctypes.util
 import os
 import subprocess
 
@@ -48,8 +49,19 @@ def look_at(eye, center, up) -> np.ndarray:
     return m
 
 
+def _tanf():
+    libm = ctypes.CDLL(ctypes.util.find_library("m"))
+    libm.tanf.restype, libm.tanf.argtypes = ctypes.c_float, [ctypes.c_float]
+    return libm.tanf
+
+
+_TANF = _tanf()
+
+
 def perspective(fovy_rad, aspect, near, far) -> np.ndarray:
-    t = np.float32(np.tan(np.float32(fovy_rad) / np.float32(2)))
+    # glm::perspective takes tan of the float32 half angle with the C library's tanf; numpy's float32 tan differs from it
+    # by one ulp at some angles (30 degrees is one), which moves every snapped vertex of a render at that fov
+    t = np.float32(_TANF(float(np.float32(fovy_rad) / np.float32(2))))
     m = np.zeros((4, 4), dtype=np.float32)
     m[0, 0] = np.float32(1) / (np.float32(aspect) * t)
     m[1, 1] = np.float32(1) / t
