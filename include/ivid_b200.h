@@ -473,6 +473,33 @@ int ivid_warp_forward_backward(ivid_warp_t* w, const float* lin_depth0_host, con
                                void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Mesh export: TSDF fusion of a scene's RGBD views and surface-nets extraction (no reference counterpart; the rule is
+ * oracle/fusion_ref.py, which these entry points follow bit for bit).  Volumes are dense [dims[2]][dims[1]][dims[0]]
+ * (x fastest); voxel (i,j,k) is centred at origin + (index + 0.5) * voxel in world space.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  float origin[3];
+  float voxel;     /* edge length, > 0 */
+  int dims[3];     /* voxels along x, y, z; each >= 2, product < 2^31 - 1 */
+} ivid_fusion_grid_t;
+/* Integrate V views (views in index order, one pass per voxel, no atomics):
+ *   depth_dev fp32 [V,n,n] linear depth, valid_dev uint8 [V,n,n] (0 = skip the pixel), color_dev fp32 [V,n,n,3];
+ *   modelviews_host fp32 [V,16] row-major world -> camera (the camera looks down -z); focal = 0.5 / tan(fov / 2);
+ *   trunc: truncation distance in voxels.
+ * Writes the caller-allocated device volumes tsdf_sum (sum of min(1, sdf / (trunc * voxel))), weight (its sample count),
+ * color_sum [.., 3] and color_weight (samples with |sdf| <= trunc * voxel).  Arguments are checked before any launch. */
+int ivid_fusion_integrate(const float* depth_dev, const uint8_t* valid_dev, const float* color_dev, const float* modelviews_host,
+                          int num_views, int image_size, float focal, const ivid_fusion_grid_t* grid, float trunc,
+                          float* tsdf_sum_dev, float* weight_dev, float* color_sum_dev, float* color_weight_dev, void* stream);
+/* Surface nets over the volumes of ivid_fusion_integrate: *num_vertices and *num_faces always receive the mesh size; with
+ * vertices_dev fp32 [max_vertices,3], colors_dev uint8 [max_vertices,3] and faces_dev int64 [max_faces,3] all non-NULL the
+ * mesh is also written (IVID_ERR_INVALID_ARGUMENT if it does not fit).  With all three NULL only the counts are computed:
+ * call once to size the buffers and once to fill them.  Vertices are numbered in cell order, faces in edge order. */
+int ivid_fusion_extract(const ivid_fusion_grid_t* grid, const float* tsdf_sum_dev, const float* weight_dev, const float* color_sum_dev,
+                        const float* color_weight_dev, int64_t max_vertices, int64_t max_faces, float* vertices_dev,
+                        uint8_t* colors_dev, int64_t* faces_dev, int64_t* num_vertices, int64_t* num_faces, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Operator-level entry points (unit parity tests, profiling): the kernels the UNet is assembled from.
  * ------------------------------------------------------------------------------------------------------------------ */
 

@@ -117,6 +117,10 @@ class WarpParamsT(Structure):
                 ("erode_rgb", c_int), ("padding", c_double)]
 
 
+class FusionGridT(Structure):
+    _fields_ = [("origin", c_float * 3), ("voxel", c_float), ("dims", c_int * 3)]
+
+
 # name -> (restype, argtypes); also the list tests/test_abi.py checks against the header
 SIGNATURES = {
     "ivid_last_error": (c_char_p, []),
@@ -182,6 +186,10 @@ SIGNATURES = {
     "ivid_warp_render_simple": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ivid_warp_forward_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, POINTER(WarpParamsT), c_void_p, c_void_p]),
     "ivid_warp_postfilter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(WarpParamsT), c_void_p, c_void_p]),
+    "ivid_fusion_integrate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, POINTER(FusionGridT), c_float,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "ivid_fusion_extract": (c_int, [POINTER(FusionGridT), c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
+                                    c_void_p, POINTER(c_int64), POINTER(c_int64), c_void_p]),
 }
 
 _lib = None

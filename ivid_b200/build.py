@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libivid_b200.so")
 OBJ_DIR = os.path.join(HERE, "_build")
-SOURCES = ["host_util.cu", "ops.cu", "unet.cu", "sampler.cu", "warp.cu", "api.cu"]
+SOURCES = ["host_util.cu", "ops.cu", "unet.cu", "sampler.cu", "warp.cu", "fusion.cu", "api.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
@@ -24,8 +24,9 @@ NVCC_FLAGS = [
 ]
 
 
-# warp.cu mirrors the CPU oracle's fp32 rounding (oracle/raster_ref.c is built with -ffp-contract=off)
-EXTRA_FLAGS = {"warp.cu": ["-fmad=false"]}
+# warp.cu mirrors the CPU oracle's fp32 rounding (oracle/raster_ref.c is built with -ffp-contract=off); fusion.cu that of
+# the numpy oracle/fusion_ref.py
+EXTRA_FLAGS = {"warp.cu": ["-fmad=false"], "fusion.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:
