@@ -569,6 +569,26 @@ typedef struct {
   void* out_dev; int out_e4m3; void* out_lo_dev; void* out_raw16_dev; float* out_raw32_dev;
 } ivid_op_gn_t;
 int ivid_op_group_norm_apply(const ivid_op_gn_t* args, void* stream);
+/* The separate GroupNorm statistics pass the UNet runs where no conv epilogue takes them: per-(sample, channel) sum and
+ * sum of squares of x_dev fp32 NHWC [N,H,W,C] (C % 4 == 0) added to stats_dev fp64 [N,C,2] (zero it first).  Synchronises
+ * the stream. */
+int ivid_op_gn_stats(const float* x_dev, int N, int H, int W, int C, double* stats_dev, void* stream);
+/* One plain resampling layer (resblock_updown = False) as the UNet runs it, input [N,H,W,C] (C % 8 == 0):
+ *   mode 2 conv 1: Downsample2d's 3x3 stride-2 pad-1 conv (H, W even), the nine taps gathered into 9C operand channels and
+ *                  multiplied as one 1x1 conv; mode 1 conv 1: Upsample2d, nearest 2x then a 3x3 pad-1 conv.  x_dev fp16
+ *                  NHWC; w_host fp32 [C,C,3,3], b_host [C] or NULL;
+ *   mode 2 conv 0: AvgPool2d(2) (H, W even); mode 1 conv 0: nearest 2x.  x_dev fp32 NHWC;
+ *   out_dev fp32 NHWC [N,Ho,Wo,C]; out16_dev optional fp16 copy of it; stats_dev optional fp64 [N,C,2] sums of out_dev as
+ *   the next GroupNorm reads them (zero it first), taken in the conv epilogue where ivid_conv_tile(Ho, Wo) reports
+ *   fused_stats and by the separate statistics pass otherwise; operand_dev optional (conv 1): receives the conv's fp16
+ *   operand, [N,Ho,Wo,9C] for mode 2 and [N,Ho,Wo,C] for mode 1.  Synchronises the stream. */
+typedef struct {
+  int mode, conv;
+  const void* x_dev; int N, H, W, C;
+  const float* w_host; const float* b_host;
+  float* out_dev; void* out16_dev; double* stats_dev; void* operand_dev;
+} ivid_op_resample_t;
+int ivid_op_resample(const ivid_op_resample_t* args, void* stream);
 /* QKVAttention (adm.py:233-253): qkv fp16 [N,T,3C] (legacy head-major q|k|v order) -> fp16 [N,T,C]. */
 int ivid_op_attention(const void* qkv_dev, int N, int T, int C, void* out_dev, void* stream);
 /* The same with head width head_channels = C / heads (a multiple of 64, dividing C): qkv fp16 [N,T,3C] in the order

@@ -112,6 +112,15 @@ class OpGnT(Structure):
     ]
 
 
+class OpResampleT(Structure):
+    _fields_ = [
+        ("mode", c_int), ("conv", c_int),
+        ("x_dev", c_void_p), ("N", c_int), ("H", c_int), ("W", c_int), ("C", c_int),
+        ("w_host", c_void_p), ("b_host", c_void_p),
+        ("out_dev", c_void_p), ("out16_dev", c_void_p), ("stats_dev", c_void_p), ("operand_dev", c_void_p),
+    ]
+
+
 class WarpParamsT(Structure):
     _fields_ = [("fov_deg", c_double), ("near", c_double), ("far", c_double), ("atol", c_double), ("rtol", c_double),
                 ("erode_rgb", c_int), ("padding", c_double)]
@@ -169,6 +178,8 @@ SIGNATURES = {
                                         c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_conv2d_ex": (c_int, [POINTER(OpConvT), c_void_p]),
     "ivid_op_group_norm_apply": (c_int, [POINTER(OpGnT), c_void_p]),
+    "ivid_op_gn_stats": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "ivid_op_resample": (c_int, [POINTER(OpResampleT), c_void_p]),
     "ivid_op_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention_heads": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "ivid_op_attention_perturbed": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

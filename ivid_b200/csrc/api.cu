@@ -393,6 +393,60 @@ int ivid_op_group_norm_apply(const ivid_op_gn_t* a, void* stream) {
   });
 }
 
+int ivid_op_gn_stats(const float* x_dev, int N, int H, int W, int C, double* stats_dev, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(x_dev); IVID_NOT_NULL(stats_dev);
+    IVID_REQUIRE(N > 0 && N <= 65535 && H > 0 && W > 0 && C > 0 && C % 4 == 0,
+                 "gn_stats: N in [1, 65535], positive H and W, C a positive multiple of 4");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_gn_stats(x_dev, stats_dev, N, H * W, C, st);
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+  });
+}
+
+// One Downsample2d / Upsample2d with the launches and descriptor fields of run_resample in unet.cu: the same weight pitch
+// (C for the stride-2 conv's gathered taps, conv_pad_k(C) for the upsample conv), and the statistics from the conv
+// epilogue where add_conv fuses them, from gn_stats otherwise and after every pooling / nearest layer.
+int ivid_op_resample(const ivid_op_resample_t* a, void* stream) {
+  return guarded([&] {
+    IVID_NOT_NULL(a);
+    IVID_NOT_NULL(a->x_dev); IVID_NOT_NULL(a->out_dev);
+    IVID_REQUIRE(a->mode == 1 || a->mode == 2, "resample: mode must be 1 (up) or 2 (down)");
+    IVID_REQUIRE(a->conv == 0 || a->conv == 1, "resample: conv must be 0 or 1");
+    const int N = a->N, H = a->H, W = a->W, C = a->C;
+    IVID_REQUIRE(N > 0 && N <= 65535 && H > 0 && W > 0 && C > 0 && C % 8 == 0,
+                 "resample: N in [1, 65535], positive H and W, C a positive multiple of 8");
+    IVID_REQUIRE(a->mode == 1 || (H % 2 == 0 && W % 2 == 0), "resample: downsampling needs an even H and W");
+    IVID_REQUIRE(a->conv == 1 || a->operand_dev == nullptr, "resample: operand_dev belongs to the conv forms");
+    if (a->conv) IVID_NOT_NULL(a->w_host);
+    const int Ho = a->mode == 1 ? 2 * H : H / 2, Wo = a->mode == 1 ? 2 * W : W / 2;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (a->conv) {
+      const ConvPack pk = conv_pack(a->w_host, a->b_host, C, C, 3, a->mode == 2 ? C : conv_pad_k(C), nullptr, nullptr, 0, 0, false);
+      const size_t op_elems = static_cast<size_t>(N) * Ho * Wo * (a->mode == 2 ? 9 * C : C);
+      DevBuf dw(pk.w16.size() * 2), db(pk.bias.size() * 4), dop(a->operand_dev ? 0 : op_elems * 2);
+      void* opnd = a->operand_dev ? a->operand_dev : dop.p;
+      IVID_CHECK_CUDA(cudaMemcpyAsync(dw.p, pk.w16.data(), pk.w16.size() * 2, cudaMemcpyHostToDevice, st));
+      IVID_CHECK_CUDA(cudaMemcpyAsync(db.p, pk.bias.data(), pk.bias.size() * 4, cudaMemcpyHostToDevice, st));
+      ConvDesc d;
+      d.act0 = opnd; d.C0 = a->mode == 2 ? 9 * C : C; d.taps0 = a->mode == 2 ? 1 : 9;
+      d.weight = dw.p; d.cout_pad = pk.cout_pad; d.cout = C; d.bias = static_cast<const float*>(db.p);
+      d.out = a->out_dev; d.out16 = a->out16_dev; d.out_mode = 0; d.ldc = C; d.N = N; d.H = Ho; d.W = Wo;
+      const bool fused = a->stats_dev != nullptr && conv_can_fuse_stats(Ho, Wo);
+      if (fused) d.stats = a->stats_dev;
+      std::unique_ptr<ConvLaunch, void (*)(ConvLaunch*)> l(conv_launch_create(d), conv_launch_destroy);   // may refuse: before any launch
+      if (a->mode == 2) launch_im2col_s2(a->x_dev, opnd, N, H, W, C, st);
+      else launch_upsample2x_h16(a->x_dev, opnd, N, H, W, C, st);
+      conv_launch_run(l.get(), st);
+      if (a->stats_dev != nullptr && !fused) launch_gn_stats(a->out_dev, a->stats_dev, N, Ho * Wo, C, st);
+    } else {
+      launch_resample_f32(static_cast<const float*>(a->x_dev), a->out_dev, a->out16_dev, N, H, W, C, a->mode, st);
+      if (a->stats_dev != nullptr) launch_gn_stats(a->out_dev, a->stats_dev, N, Ho * Wo, C, st);
+    }
+    IVID_CHECK_CUDA(cudaStreamSynchronize(st));
+  });
+}
+
 static int op_group_norm(const float* x0_dev, int C0, const float* x1_dev, int C1, int N, int H, int W, int groups,
                          float eps, const float* gamma_host, const float* beta_host, const float* film_dev, int silu,
                          int mode, void* out_dev, bool e4m3, void* stream) {

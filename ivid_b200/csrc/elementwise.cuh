@@ -4,8 +4,9 @@
 //                      GroupNorm32 statistics (reference adm.py:36-41) are later formed per group from these, which
 //                      is what makes GroupNorm over a *virtual* channel concat (groups straddling the seam,
 //                      adm.py:563 + :158) free of any concat copy.
-//                      Only used below 32 pixels per sample: everywhere else the producing conv's epilogue accumulates
-//                      the statistics.
+//                      Only used below 32 pixels per sample and after the pooling / nearest resampling layers: everywhere
+//                      else the producing conv's epilogue accumulates the statistics.  Each thread sums its pixels in
+//                      fp32, at most ceil(min(HW, 256) / rows) of them (rows = 256 / min(C/4, 256)); the rest is fp64.
 //   gn_prologue      : (device function, per block) per-(sample, channel) affine y = x*A + B that folds mean/rstd,
 //                      gamma/beta and the FiLM scale/shift  h = GN(h)*(1+scale)+shift  (adm.py:216-217).
 //   gn_apply_h16_kernel: y = [SiLU](x*A+B), fp16 NHWC sources (hidden tensor, fp16 copies of block outputs, virtual
@@ -37,9 +38,13 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
   const int p0 = blockIdx.x * kStatsPixPerBlock;
   const int p1 = min(p0 + kStatsPixPerBlock, HW);
   const float* base = x + (static_cast<size_t>(n) * HW) * C;
-  for (int cc = tx; cc < c4; cc += cols) {
+  // Every thread runs the same ceil(c4 / cols) rounds, so the whole block reaches each barrier.  When C/4 > 256 is not a
+  // multiple of 256 the last round leaves columns cc >= c4 idle: they load nothing and store nothing to the statistics.
+  for (int cc0 = 0; cc0 < c4; cc0 += cols) {
+    const int cc = cc0 + tx;
+    const bool live = cc < c4;
     float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
-    if (ty < rows) {
+    if (ty < rows && live) {
       for (int p = p0 + ty; p < p1; p += rows) {
         const float4 v = ldg_f4(base + static_cast<size_t>(p) * C + cc * 4);
         s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
@@ -56,7 +61,7 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
       }
     }
     __syncthreads();
-    if (ty == 0) {
+    if (ty == 0 && live) {
       double ds[4], dq[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) { ds[j] = 0.0; dq[j] = 0.0; }
