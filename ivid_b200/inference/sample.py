@@ -14,21 +14,20 @@ from __future__ import annotations
 
 import argparse
 import json
-import math
 import os
 import threading
+from dataclasses import asdict
 
 import numpy as np
 import torch
 
 from .. import backbones, frameworks, samplers
-from ..backbones.adm import PAG_DEFAULT_LAYERS
-from ..frameworks.gaussian_diffusion import check_pag
-from ..samplers.samplers import _check_apg, _check_cache, _check_threshold
 from ..rgbd_3d import DeviceWarp, glm_compat as glm
 from ..rgbd_3d import utils as rgbd_utils
+from ..samplers.options import (SamplerOptions, add_arguments, check_arguments, int_at_least,
+                                parse_apg, solver_sampler)  # noqa: F401  (parse_apg: the --apg parser, part of this CLI's surface)
 from ..utils import edict
-from .superres import check_options as _check_sr_options, check_superres, superresolve_views
+from .superres import check_superres, superresolve_views
 from .utils import colorize_depth, parse_int_list, reorder, save_scene
 
 
@@ -166,42 +165,29 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
         assert init_views.dim() == 4 and init_views.shape[1] == 4, f"init_views must be [num_samples,4,S,S], got {tuple(init_views.shape)}"
     assert framework_uncond is not None or (init_views is not None and init_strength is None), \
         "framework_uncond is needed unless every view 0 is given (init_views without init_strength)"
+    opts = SamplerOptions(guidance_interval, cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
     for fw in (framework_uncond, framework_cond):          # before any device work
         if fw is not None:
-            _check_cache(cache_interval, cache_branch, fw.backbone.num_res_blocks)
-            check_pag(pag_scale, pag_layers, fw.backbone)
-    _check_threshold(dynamic_threshold, False)
-    if apg is not None:
-        for fw in (framework_uncond, framework_cond):
-            if fw is not None:
-                _check_apg(apg, fw, classes, guidance)
-    assert solver in ("ddim", "dpmpp", "dpmpp_sde", "unipc"), \
-        f"solver must be 'ddim', 'dpmpp', 'dpmpp_sde' or 'unipc', got {solver!r}"
+            opts.resolve(fw, classes, guidance)
+    ode, sde = solver_sampler(solver)
     net = (framework_uncond if framework_uncond is not None else framework_cond).backbone
     S = net.image_size
     dev = net.device
     if framework_sr is not None:
         check_superres(framework_sr, S, sr_size, sr_replace)
-        _check_sr_options(framework_sr, classes, guidance if sr_guidance is None else sr_guidance, solver, guidance_interval,
-                          cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        opts.resolve(framework_sr, classes, guidance if sr_guidance is None else sr_guidance)
         assert isinstance(steps_sr, int) and steps_sr >= 1, f"steps_sr must be an integer >= 1, got {steps_sr!r}"
     for fw in (framework_uncond, framework_cond):
         if fw is not None and fw.backbone.precision != precision:
             fw.backbone.set_precision(precision)
-    ode = {"ddim": samplers.DdimSampler, "unipc": samplers.UniPcSampler}.get(solver, samplers.DpmSolverSampler)
     sampler_uncond = None
     if framework_uncond is not None:
         sampler_uncond = ode(framework_uncond) if steps_uncond < 1000 else samplers.DdpmSampler(framework_uncond)
     sampler_cond = ode(framework_cond) if framework_cond is not None else None
-    sde_kw = dict(sde=True) if solver == "dpmpp_sde" else {}
-    gi_kw = dict(guidance_interval=tuple(guidance_interval)) if guidance_interval is not None else {}
-    if cache_interval is not None:
-        gi_kw.update(cache_interval=cache_interval, cache_branch=cache_branch)
-    th_kw = dict(dynamic_threshold=dynamic_threshold) if dynamic_threshold is not None else {}
-    pag_kw = dict(pag_scale=pag_scale, pag_layers=pag_layers) if pag_scale is not None else {}
-    apg_kw = dict(apg=apg) if apg is not None else {}
-    # a framework without classifier-free guidance takes the interval only to gate perturbed-attention guidance
-    plain_kw = {k: v for k, v in gi_kw.items() if k.startswith("cache") or (pag_kw and k == "guidance_interval")}
+    sde_kw = dict(sde=True) if sde else {}
+    # as in the reference, the unconditional model decides whether both networks take the guidance strength (without
+    # one, the conditional model decides)
+    kw = opts.sampler_kwargs(framework_uncond if framework_uncond is not None else framework_cond, guidance)
     num_samples = seeds_or_num_samples if not isinstance(seeds_or_num_samples, list) else len(seeds_or_num_samples)
     seeds = seeds_or_num_samples if isinstance(seeds_or_num_samples, list) else None
     if init_views is not None:
@@ -232,21 +218,15 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
             warp = warps[bs]
             warp.reset()
         samples, cond_color, cond_depth = [], [], []
-        # guided frameworks take the guidance strength (without an unconditional model, the conditional one decides)
-        cfg_u = (isinstance(framework_uncond, frameworks.ClassifierFreeGuidance) if framework_uncond is not None
-                 else isinstance(framework_cond, frameworks.InpaintCFG))
         for j in range(n_views):
             mv_j = [views_of(k)[j] for k in range(bs)] if per_sample_views else views_of(0)[j]
             if j == 0 and init_views is not None and init_strength is None:
                 res = edict(samples=init_views[i: i + bs].to(device=dev, dtype=torch.float32).contiguous())
             elif j == 0:
-                kw = dict(strength=guidance, **gi_kw) if cfg_u else dict(plain_kw)
-                if steps_uncond < 1000:
-                    kw.update(sde_kw)
-                kw.update(th_kw, **pag_kw, **apg_kw)
+                kw_u = dict(kw, **sde_kw) if steps_uncond < 1000 else dict(kw)
                 if init_views is not None:     # SDEdit of the given view; the seeds' noise is the forward diffusion's z
-                    kw.update(init=init_views[i: i + bs].to(device=dev, dtype=torch.float32), init_strength=init_strength)
-                res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw)
+                    kw_u.update(init=init_views[i: i + bs].to(device=dev, dtype=torch.float32), init_strength=init_strength)
+                res = sampler_uncond.sample(bs, noise=noise, classes=b_classes, steps=steps_uncond, verbose=False, rng=rng, **kw_u)
             else:
                 cond = warp.aggregate(mv_j, **wparams)                   # [bs,7,S,S] in [0,1]
                 y = cond[:, 0:4] * 2 - 1                                 # sample.py:103
@@ -255,9 +235,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                 cond_depth.append(cond[:, 3:4] * 2 - 1)
                 args = dict(y=y, mask=mask, mask_rgb=mask_rgb, replace_rgb=(0.1, y[:, :3], mask_rgb),
                             replace_depth=(0.2, y[:, 3:], mask), constrain_depth=(0.5, cond[:, 6:7] * 2 - 1))   # sample.py:104-119
-                kw = dict(strength=guidance, **gi_kw) if cfg_u else dict(plain_kw)
-                kw.update(sde_kw, **th_kw, **pag_kw, **apg_kw)
-                res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw)
+                res = sampler_cond.sample(bs, classes=b_classes, steps=steps_cond, verbose=False, rng=rng, **args, **kw, **sde_kw)
             samples.append(res.samples)
             if warp is not None:
                 warp.add_view(res.samples, mv_j, **wparams)
@@ -278,9 +256,7 @@ def sample_all(framework_uncond, framework_cond, seeds_or_num_samples, steps_unc
                     framework_sr, samples, [views_of(k) for k in range(bs)] if per_sample_views else views_of(0),
                     steps=steps_sr, size=sr_size, classes=b_classes, guidance=guidance if sr_guidance is None else sr_guidance,
                     seeds=seeds[i: i + bs] if seeds is not None else None, replace=sr_replace, rng=rng, solver=solver,
-                    precision=precision, guidance_interval=guidance_interval, cache_interval=cache_interval,
-                    cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale,
-                    pag_layers=pag_layers, apg=apg, cache=sr_cache, **wparams)           # [bs, V, 4, S', S']
+                    precision=precision, cache=sr_cache, **asdict(opts), **wparams)           # [bs, V, 4, S', S']
         rgbd = samples.permute(0, 1, 3, 4, 2).cpu().numpy() * 0.5 + 0.5   # one D2H per batch
         for k in range(bs):
             meshes = [edict(depth=rgbd_utils.linearize_depth(rgbd[k, v, :, :, 3:], near, far), fov=fov,
@@ -406,11 +382,6 @@ def main(rank, world_size, opt):
     seeds_r, classes_r = shard(seeds, rank, world_size), shard(classes, rank, world_size)
     idx = list(range(num))[rank::world_size]
     mvs_r = shard(mvs, rank, world_size) if isinstance(mvs[0], list) else mvs
-    solver = getattr(opt, "solver", "ddim")
-    precision = getattr(opt, "precision", "fp16")
-    interval = getattr(opt, "guidance_interval", None)
-    cache_interval, cache_branch = getattr(opt, "cache_interval", None), getattr(opt, "cache_branch", 0)
-    dynamic_threshold = getattr(opt, "dynamic_threshold", None)
     init_views = None
     if init_image is not None:
         # one view for every sample: the seeds vary the continuation (and, with a strength, the noising)
@@ -423,12 +394,10 @@ def main(rank, world_size, opt):
     save_cfg = edict(output_dir=out_dir, viewset=opt.viewset)
     gen = sample_all(fw_u, fw_c, seeds_r if seeds_r is not None else len(idx), opt.steps_uncond, opt.steps_cond, mvs_r, classes=classes_r,
                      guidance=opt.guidance, batchsize=opt.batchsize, fov=opt.fov, near=opt.near, far=opt.far, atol=opt.atol,
-                     rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=solver,
-                     precision=precision, guidance_interval=interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                     dynamic_threshold=dynamic_threshold, init_views=init_views, init_strength=init_strength,
-                     pag_scale=getattr(opt, "pag_scale", None), pag_layers=getattr(opt, "pag_layers", None),
-                     apg=getattr(opt, "apg", None), framework_sr=fw_sr, steps_sr=getattr(opt, "steps_sr", 50),
-                     sr_replace=getattr(opt, "sr_replace", SR_REPLACE_DEFAULT))
+                     rtol=opt.rtol, erode_rgb=opt.erode_rgb, rng=opt.rng, solver=getattr(opt, "solver", "ddim"),
+                     precision=getattr(opt, "precision", "fp16"), init_views=init_views, init_strength=init_strength,
+                     framework_sr=fw_sr, steps_sr=getattr(opt, "steps_sr", 50),
+                     sr_replace=getattr(opt, "sr_replace", SR_REPLACE_DEFAULT), **asdict(SamplerOptions.from_args(opt)))
     threads = []
     for i, (meshes, colors, samples, conds) in enumerate(gen):
         tag = (f"class{classes_r[i]:03d}_" if classes_r is not None else "") + (f"seed{seeds_r[i]:05d}" if seeds_r is not None else f"{idx[i]:05d}")
@@ -441,34 +410,13 @@ def output_dir_name(opt):
     """Output directory of a run: the reference's name, with a suffix for every extension that changes the samples."""
     solver = getattr(opt, "solver", "ddim")
     precision = getattr(opt, "precision", "fp16")
-    interval = getattr(opt, "guidance_interval", None)
-    cache_interval = getattr(opt, "cache_interval", None)
-    dt = getattr(opt, "dynamic_threshold", None)
     init_image, init_strength = getattr(opt, "init_image", None), getattr(opt, "init_strength", None)
+    head, tail = SamplerOptions.from_args(opt).dir_suffixes()
     return os.path.join(opt.output_dir, f"viewset_{opt.viewset}_steps_u{opt.steps_uncond}_c{opt.steps_cond}_guidance{opt.guidance}"
-                        + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}")
-                        + ("" if interval is None else f"_interval{interval[0]}-{interval[1]}")
-                        + ("" if cache_interval is None else f"_cache{cache_interval}b{getattr(opt, 'cache_branch', 0)}")
-                        + ("" if dt is None else f"_dthresh{dt}" if not isinstance(dt, tuple) else f"_dthresh{dt[0]}-{dt[1]}")
+                        + ("" if solver == "ddim" else f"_{solver}") + ("" if precision == "fp16" else f"_{precision}") + head
                         + ("" if init_image is None else f"_init-{os.path.splitext(os.path.basename(init_image))[0]}")
                         + ("" if init_strength is None else f"_strength{init_strength}")
-                        + _pag_suffix(opt) + _apg_suffix(opt) + _sr_suffix(opt))
-
-
-def _pag_suffix(opt):
-    """_pag{W}, plus the layers ('+'-joined) when they are not the default."""
-    w, layers = getattr(opt, "pag_scale", None), getattr(opt, "pag_layers", None)
-    if w is None:
-        return ""
-    return f"_pag{w}" + ("" if layers is None or tuple(layers) == PAG_DEFAULT_LAYERS else "-" + "+".join(layers))
-
-
-def _apg_suffix(opt):
-    """_apg{ETA}, then ,{R} and ,{BETA} as given."""
-    apg = getattr(opt, "apg", None)
-    if apg is None:
-        return ""
-    return "_apg" + ",".join(str(v) for v in (apg if isinstance(apg, tuple) else (apg,)))
+                        + tail + _sr_suffix(opt))
 
 
 SR_REPLACE_DEFAULT = (0.1, 0.2)
@@ -499,86 +447,6 @@ def parse_sr_replace(s):
     return vals
 
 
-def _int_at_least(lo):
-    def parse(s):
-        try:
-            v = int(s)
-        except ValueError:
-            raise argparse.ArgumentTypeError(f"expected an integer, got {s!r}") from None
-        if v < lo:
-            raise argparse.ArgumentTypeError(f"expected an integer >= {lo}, got {s!r}")
-        return v
-    return parse
-
-
-def parse_interval(s):
-    """'LO,HI' -> (LO, HI), the inclusive model-time bounds of --guidance_interval."""
-    parts = s.split(",")
-    if len(parts) != 2:
-        raise argparse.ArgumentTypeError(f"expected LO,HI, got {s!r}")
-    try:
-        lo, hi = int(parts[0]), int(parts[1])
-    except ValueError:
-        raise argparse.ArgumentTypeError(f"expected two integers LO,HI, got {s!r}") from None
-    if not 0 <= lo <= hi:
-        raise argparse.ArgumentTypeError(f"expected 0 <= LO <= HI, got {s!r}")
-    return lo, hi
-
-
-def parse_threshold(s):
-    """'P' or 'P,MAX' -> P or (P, MAX) of --dynamic_threshold: the quantile ratio 0 < P <= 1 and the bound MAX >= 1."""
-    parts = s.split(",")
-    if len(parts) not in (1, 2):
-        raise argparse.ArgumentTypeError(f"expected P or P,MAX, got {s!r}")
-    try:
-        vals = [float(v) for v in parts]
-    except ValueError:
-        raise argparse.ArgumentTypeError(f"expected numbers P[,MAX], got {s!r}") from None
-    if not 0.0 < vals[0] <= 1.0:
-        raise argparse.ArgumentTypeError(f"expected 0 < P <= 1, got {s!r}")
-    if len(vals) == 2 and not vals[1] >= 1.0:
-        raise argparse.ArgumentTypeError(f"expected MAX >= 1, got {s!r}")
-    return vals[0] if len(vals) == 1 else (vals[0], vals[1])
-
-
-def parse_apg(s):
-    """'ETA', 'ETA,R' or 'ETA,R,BETA' -> ETA or the tuple of --apg: ETA >= 0, the norm bound R >= 0 (0: none) and the
-    momentum -1 < BETA < 1, all finite."""
-    parts = s.split(",")
-    if len(parts) not in (1, 2, 3):
-        raise argparse.ArgumentTypeError(f"expected ETA[,R[,BETA]], got {s!r}")
-    try:
-        vals = [float(v) for v in parts]
-    except ValueError:
-        raise argparse.ArgumentTypeError(f"expected numbers ETA[,R[,BETA]], got {s!r}") from None
-    if not all(math.isfinite(v) for v in vals):
-        raise argparse.ArgumentTypeError(f"expected finite numbers, got {s!r}")
-    if vals[0] < 0.0 or (len(vals) > 1 and vals[1] < 0.0):
-        raise argparse.ArgumentTypeError(f"expected ETA >= 0 and R >= 0, got {s!r}")
-    if len(vals) == 3 and not -1.0 < vals[2] < 1.0:
-        raise argparse.ArgumentTypeError(f"expected -1 < BETA < 1, got {s!r}")
-    return vals[0] if len(vals) == 1 else tuple(vals)
-
-
-def parse_pag_scale(s):
-    """'W' -> W of --pag_scale, a finite number >= 0."""
-    try:
-        v = float(s)
-    except ValueError:
-        raise argparse.ArgumentTypeError(f"expected a number, got {s!r}") from None
-    if not (math.isfinite(v) and v >= 0.0):
-        raise argparse.ArgumentTypeError(f"expected a finite W >= 0, got {s!r}")
-    return v
-
-
-def parse_pag_layers(s):
-    """'NAME[,NAME...]' -> the tuple of attention-layer names of --pag_layers (checked against the network when it is built)."""
-    names = tuple(n.strip() for n in s.split(","))
-    if not names or any(not n for n in names):
-        raise argparse.ArgumentTypeError(f"expected NAME[,NAME...], got {s!r}")
-    return names
-
-
 def parse_strength(s):
     """'S' -> S of --init_strength, 0 < S <= 1."""
     try:
@@ -599,8 +467,7 @@ def parse_args(argv=None):
         ap.error("--init_image and --init_depth go together")
     if o.init_strength is not None and o.init_image is None:
         ap.error("--init_strength needs --init_image and --init_depth")
-    if o.pag_layers is not None and o.pag_scale is None:
-        ap.error("--pag_layers needs --pag_scale")
+    check_arguments(ap, o)
     check_sr_flags(ap, o)
     return o
 
@@ -612,7 +479,7 @@ def add_sr_flags(ap, required=False):
                     help="super-resolve every scene with this SuperResCFG config (e.g. rgbd_imagenet_adm_256_128_small_sr.json) "
                          "once its views exist: results, grids and scenes at the network's image_size (default: off)")
     ap.add_argument("--ckpt_sr", default=None, metavar="PATH", help="checkpoint of --config_sr (default: random weights)")
-    ap.add_argument("--steps_sr", type=_int_at_least(1), default=argparse.SUPPRESS, metavar="N",
+    ap.add_argument("--steps_sr", type=int_at_least(1), default=argparse.SUPPRESS, metavar="N",
                     help="sampler steps of every super-resolved view (default 50)")
     ap.add_argument("--sr_replace", type=parse_sr_replace, default=argparse.SUPPRESS, metavar="RGB,DEPTH|none",
                     help="replace-guidance weights of the super-resolved views towards the earlier ones, warped at the new size "
@@ -657,24 +524,7 @@ def build_arg_parser():
     ap.add_argument("--rng", choices=["philox", "torch"], default="philox",
                     help="per-step noise: 'philox' draws in-kernel (fast, default); 'torch' draws with the torch generator exactly "
                          "where the reference does (seed-for-seed reproduction of the reference's images needs this)")
-    ap.add_argument("--solver", choices=["ddim", "dpmpp", "dpmpp_sde", "unipc"], default="ddim",
-                    help="sampler of the DDIM-step views: 'ddim' as the reference, 'dpmpp' DPM-Solver++(2M), which needs fewer "
-                         "steps for the same convergence, 'dpmpp_sde' its stochastic variant SDE-DPM-Solver++(2M), 'unipc' the "
-                         "UniPC predictor-corrector at order 2 (DDPM at --steps_uncond >= 1000 is unchanged)")
-    ap.add_argument("--precision", choices=["fp16", "fp8"], default="fp16",
-                    help="operands of the ResBlock convs: 'fp16' (default) or 'fp8' (e4m3, faster, changes the numbers; DESIGN.md §2)")
-    ap.add_argument("--guidance_interval", type=parse_interval, default=None, metavar="LO,HI",
-                    help="apply classifier-free guidance only at the steps whose model time t (0 <= t < T, the t the network "
-                         "receives) lies in [LO, HI]; the other steps run unguided with half the network work (default: every step)")
-    ap.add_argument("--cache_interval", type=_int_at_least(1), default=None, metavar="N",
-                    help="reuse the deep UNet features between denoising steps (DeepCache): a full forward every N steps, shallow "
-                         "forwards in between; approximates the samples (default: every forward in full)")
-    ap.add_argument("--cache_branch", type=_int_at_least(0), default=0, metavar="B",
-                    help="with --cache_interval: the shallow forwards recompute input blocks 0..B and the last B+1 output blocks, "
-                         "0 <= B <= num_res_blocks (default 0, the cheapest)")
-    ap.add_argument("--dynamic_threshold", type=parse_threshold, default=None, metavar="P[,MAX]",
-                    help="dynamic thresholding of the predicted x_0 (Imagen): clamp each sample's x_0 to [-s, s] and divide by s, "
-                         "s = min(max(P-quantile of |x_0|, 1), MAX); e.g. 0.995 (default: off; MAX defaults to no bound)")
+    add_arguments(ap)
     ap.add_argument("--init_image", default=None, metavar="PATH",
                     help="grow every scene from this RGB image as its first view (needs --init_depth); preprocessed as the "
                          "dataset of --config_cond prepares its images")
@@ -683,15 +533,6 @@ def build_arg_parser():
     ap.add_argument("--init_strength", type=parse_strength, default=None, metavar="S",
                     help="with --init_image: re-sample the first view from it by SDEdit, running the last S of the unconditional "
                          "schedule, 0 < S <= 1 (default: the given view is the first view as it is)")
-    ap.add_argument("--pag_scale", type=parse_pag_scale, default=None, metavar="W",
-                    help="perturbed-attention guidance of both networks at scale W >= 0: adds W * (eps - eps with identity "
-                         "attention maps) at every guided step; works without classes (default: off)")
-    ap.add_argument("--pag_layers", type=parse_pag_layers, default=None, metavar="NAME[,NAME...]",
-                    help="with --pag_scale: the attention layers to perturb, by state-dict name (default: middle_block.1)")
-    ap.add_argument("--apg", type=parse_apg, default=None, metavar="ETA[,R[,BETA]]",
-                    help="adaptive projected guidance of both networks: the guidance update split into its parts parallel and "
-                         "orthogonal to the conditional x_0, the parallel part weighted by ETA, the update's norm bounded by R "
-                         "(0: no bound) and a momentum BETA across steps; e.g. 0,0,-0.5 (default: plain classifier-free guidance)")
     add_sr_flags(ap)
     return ap
 

@@ -16,14 +16,11 @@ import numbers
 
 import torch
 
-from .. import frameworks, samplers
-from ..frameworks.gaussian_diffusion import check_pag
+from .. import frameworks
 from ..rgbd_3d import DeviceWarp
-from ..samplers.samplers import _check_apg, _check_cache, _check_interval, _check_threshold
+from ..samplers.options import SamplerOptions, solver_sampler
 
 __all__ = ["superresolve_views", "check_superres"]
-
-SOLVERS = ("ddim", "dpmpp", "dpmpp_sde", "unipc")
 
 
 def _unwrap(backbone):
@@ -49,19 +46,6 @@ def check_superres(framework_sr, S, size=None, replace=(0.1, 0.2)):
             if not (isinstance(w, numbers.Real) and not isinstance(w, bool) and 0.0 <= w <= 1.0):
                 raise ValueError(f"replace weights must lie in [0, 1], got {replace!r}")
     return out, out // S
-
-
-def check_options(framework_sr, classes, guidance, solver, guidance_interval, cache_interval, cache_branch,
-                  dynamic_threshold, pag_scale, pag_layers, apg):
-    """The sampler options of the stage through the samplers' own checks (AssertionError), before any device work."""
-    net = _unwrap(framework_sr.backbone)
-    assert solver in SOLVERS, f"solver must be one of {SOLVERS}, got {solver!r}"
-    _check_interval(guidance_interval, len(framework_sr.betas))
-    _check_cache(cache_interval, cache_branch, net.num_res_blocks)
-    check_pag(pag_scale, pag_layers, net)
-    _check_threshold(dynamic_threshold, False)
-    if apg is not None:
-        _check_apg(apg, framework_sr, classes, guidance)
 
 
 def _per_sample(modelviews):
@@ -103,31 +87,21 @@ def superresolve_views(framework_sr, views, modelviews, steps=50, size=None, cla
     assert isinstance(steps, numbers.Integral) and steps >= 1, f"steps must be an integer >= 1, got {steps!r}"
     assert seeds is None or len(seeds) == B, f"seeds must hold one seed per sample ({B}), got {len(seeds)}"
     assert classes is None or len(classes) == B, f"classes must hold one class per sample ({B}), got {len(classes)}"
-    check_options(framework_sr, classes, guidance, solver, guidance_interval, cache_interval, cache_branch, dynamic_threshold,
-                  pag_scale, pag_layers, apg)
+    ode, sde = solver_sampler(solver)
+    opts = SamplerOptions(guidance_interval, cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+    opts.resolve(framework_sr, classes, guidance)
     net = _unwrap(framework_sr.backbone)
     if net.precision != precision:
         net.set_precision(precision)
     dev = net.device
     cache = {} if cache is None else cache
-    ode = {"ddim": samplers.DdimSampler, "unipc": samplers.UniPcSampler}.get(solver, samplers.DpmSolverSampler)
     key = ("sampler", id(framework_sr), ode)
     if key not in cache:
         cache[key] = ode(framework_sr)
     sampler = cache[key]
-    kw = dict(strength=guidance, steps=steps, verbose=False, rng=rng)
-    if solver == "dpmpp_sde":
+    kw = dict(steps=steps, verbose=False, rng=rng, **opts.sampler_kwargs(framework_sr, guidance))
+    if sde:
         kw["sde"] = True
-    if guidance_interval is not None:
-        kw["guidance_interval"] = tuple(guidance_interval)
-    if cache_interval is not None:
-        kw.update(cache_interval=cache_interval, cache_branch=cache_branch)
-    if dynamic_threshold is not None:
-        kw["dynamic_threshold"] = dynamic_threshold
-    if pag_scale is not None:
-        kw.update(pag_scale=pag_scale, pag_layers=pag_layers)
-    if apg is not None:
-        kw["apg"] = apg
     b_classes = None
     if classes is not None:
         b_classes = (classes if torch.is_tensor(classes) else torch.tensor(list(classes))).to(device=dev, dtype=torch.int64)

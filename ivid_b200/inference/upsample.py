@@ -17,12 +17,14 @@ import glob
 import json
 import os
 import re
+from dataclasses import asdict
 
 import numpy as np
 import torch
 from PIL import Image
 
 from ..rgbd_3d import utils as rgbd_utils
+from ..samplers.options import SamplerOptions, add_arguments, check_arguments
 from ..utils import edict
 from . import sample as sample_cli
 from .superres import superresolve_views
@@ -71,19 +73,10 @@ def main(argv=None):
     ap.add_argument("--erode_rgb", type=int, default=3)
     ap.add_argument("--guidance", type=float, default=3.0)
     ap.add_argument("--rng", choices=["philox", "torch"], default="philox")
-    ap.add_argument("--solver", choices=["ddim", "dpmpp", "dpmpp_sde", "unipc"], default="ddim")
-    ap.add_argument("--precision", choices=["fp16", "fp8"], default="fp16")
-    ap.add_argument("--guidance_interval", type=sample_cli.parse_interval, default=None, metavar="LO,HI")
-    ap.add_argument("--cache_interval", type=sample_cli._int_at_least(1), default=None, metavar="N")
-    ap.add_argument("--cache_branch", type=sample_cli._int_at_least(0), default=0, metavar="B")
-    ap.add_argument("--dynamic_threshold", type=sample_cli.parse_threshold, default=None, metavar="P[,MAX]")
-    ap.add_argument("--pag_scale", type=sample_cli.parse_pag_scale, default=None, metavar="W")
-    ap.add_argument("--pag_layers", type=sample_cli.parse_pag_layers, default=None, metavar="NAME[,NAME...]")
-    ap.add_argument("--apg", type=sample_cli.parse_apg, default=None, metavar="ETA[,R[,BETA]]")
+    add_arguments(ap)
     opt = ap.parse_args(argv)
     sample_cli.check_sr_flags(ap, opt)
-    if opt.pag_layers is not None and opt.pag_scale is None:
-        ap.error("--pag_layers needs --pag_scale")
+    check_arguments(ap, opt)
     scenes = sorted(glob.glob(os.path.join(opt.scene_dir, "scenes", "*.npz")))
     print(f"Found {len(scenes)} scenes.")
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -92,9 +85,7 @@ def main(argv=None):
     for sub in ("scenes", "results"):
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
     stage_kw = dict(replace=opt.sr_replace, atol=opt.atol, rtol=opt.rtol, erode_rgb=opt.erode_rgb, guidance=opt.guidance,
-                    rng=opt.rng, solver=opt.solver, precision=opt.precision, guidance_interval=opt.guidance_interval,
-                    cache_interval=opt.cache_interval, cache_branch=opt.cache_branch, dynamic_threshold=opt.dynamic_threshold,
-                    pag_scale=opt.pag_scale, pag_layers=opt.pag_layers, apg=opt.apg, cache={})
+                    rng=opt.rng, solver=opt.solver, precision=opt.precision, cache={}, **asdict(SamplerOptions.from_args(opt)))
     for path in scenes:
         name = os.path.basename(path)
         out, views = upsample_scene(fw, path, steps=opt.steps_sr, near=opt.near, far=opt.far, **stage_kw)

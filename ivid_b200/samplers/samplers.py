@@ -22,8 +22,9 @@ import numpy as np
 import torch
 
 from .. import _lib
-from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG, check_pag
+from ..frameworks.gaussian_diffusion import ClassifierFreeGuidance, GaussianDiffusion, InpaintCFG, SuperResCFG
 from ..utils import edict
+from .options import SamplerOptions
 
 __all__ = ["DdpmSampler", "DdimSampler", "DpmSolverSampler", "UniPcSampler", "init_steps"]
 
@@ -221,7 +222,6 @@ class _NativeSampler:
             a.t_last = step_t(t_last)
             a.prev_x0_dev = P(x0_last)
         a.sde = 1 if sde else 0
-        interval = _check_interval(interval, len(fw.betas))
         if interval is not None:
             a.guidance_interval = 1
             a.guidance_t_lo, a.guidance_t_hi = interval
@@ -245,9 +245,6 @@ class _NativeSampler:
         net = _unwrap(self.framework.backbone)
         net._ensure_packed()
         return net
-
-    def _num_res_blocks(self):
-        return _unwrap(self.framework.backbone).num_res_blocks
 
     def _native_step(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, cond_noise, order=0, prev=None,
                      sde=False, interval=None, cache=None, threshold=None, prev_x=None, pag=None, apg=None, apg_state=None):
@@ -284,21 +281,16 @@ class _NativeSampler:
             out.apg_state = apg_state
         return out
 
-    def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, interval, reuse_features, cache_branch,
-                     order=0, prev=None, sde=False, dynamic_threshold=None, prev_x=None, pag_scale=None, pag_layers=None,
-                     apg=None, apg_state=None):
+    def _sample_once(self, x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise, opts, reuse_features, order=0,
+                     prev=None, sde=False, prev_x=None, apg_state=None):
         """The body of every sample_once: the host checks before any device work or torch draw, the step noise (drawn as
         the reference draws it, or the injected `noise` and kwargs' `cond_noise`), then the step with t / t_prev read on
         the device (all samples of a batch share the step, ddpm.py:177-179, ddim.py:154-158: no host sync)."""
         B = x_t.shape[0]
         assert t.shape == (B,), "t must be a 1D tensor of shape (B,)"
         assert self.KIND == 0 or t_prev.shape == (B,), "t_prev must be a 1D tensor of shape (B,)"
-        _check_interval(interval, len(self.framework.betas))
-        _check_cache(None, cache_branch, self._num_res_blocks())
-        threshold = _check_threshold(dynamic_threshold, clip_denoised)
-        pag = check_pag(pag_scale, pag_layers, self.framework.backbone)
-        apg = _check_apg(apg, self.framework, classes, self._guidance(kwargs)[1])
-        assert apg_state is None or apg is not None, "apg_state needs apg"
+        opts = opts.resolve(self.framework, classes, self._guidance(kwargs)[1], clip_denoised)
+        assert apg_state is None or opts.apg is not None, "apg_state needs apg"
         assert apg_state is None or tuple(apg_state.shape) == tuple(x_t.shape), \
             f"apg_state must have x_t's shape {tuple(x_t.shape)}, got {tuple(apg_state.shape)}"
         if noise is None:
@@ -307,9 +299,8 @@ class _NativeSampler:
             cond_noise = kwargs.pop("cond_noise", None)
         # the DPM-Solver++ ODE update reads no step noise
         return self._native_step(x_t, t, t_prev, classes, clip_denoised, eta, kwargs, noise if self.KIND != 2 or sde else None,
-                                 cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                 cache=(0, cache_branch, bool(reuse_features)), threshold=threshold, prev_x=prev_x, pag=pag,
-                                 apg=apg, apg_state=apg_state)
+                                 cond_noise, order=order, prev=prev, sde=sde, prev_x=prev_x, apg_state=apg_state,
+                                 **opts.step_kwargs(reuse_features))
 
     def _draw_step_noise(self, x_t, kwargs):
         """torch draws in the reference's order: InpaintCFG rgb, depth (inside model_inference), then randn_like(x_t)."""
@@ -337,14 +328,9 @@ class _NativeSampler:
             reuse.append(not full)
         return reuse
 
-    def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, order=0,
-             sde=False, interval=None, cache_interval=None, cache_branch=0, dynamic_threshold=None, init=None, init_strength=None,
-             pag_scale=None, pag_layers=None, apg=None):
-        interval = _check_interval(interval, len(self.framework.betas))   # before any device work
-        pag = check_pag(pag_scale, pag_layers, self.framework.backbone)
-        apg = _check_apg(apg, self.framework, classes, self._guidance(kwargs)[1])
-        cache_interval = _check_cache(cache_interval, cache_branch, self._num_res_blocks())
-        threshold = _check_threshold(dynamic_threshold, clip_denoised)
+    def _run(self, num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, opts,
+             order=0, sde=False, init=None, init_strength=None):
+        opts = opts.resolve(self.framework, classes, self._guidance(kwargs)[1], clip_denoised)   # before any device work
         _check_init(init, init_strength, noise, image_size, _unwrap(self.framework.backbone).out_channels)
         net = self._net()
         net.eval()
@@ -384,16 +370,15 @@ class _NativeSampler:
                 sched = [(jump * (i + 1), jump * i) for i in reversed(range(nsteps))]
             sched = sched[start:]
             prev, prev_x, apg_state = None, None, None
-            reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, interval,
-                                         cache_interval, pag)
+            reuse = self._reuse_schedule([t if self.KIND == 0 else t - 1 for (t, _) in sched], classes, kwargs, opts.interval,
+                                         opts.cache_interval, opts.pag)
             for i, (t, t_prev) in enumerate(sched):
                 z, cond_noise = self._draw_step_noise(img, kwargs)
                 # the DPM-Solver++ ODE update draws z only to consume the torch RNG as DdimSampler does
                 out = self._native_step(img, t, t_prev, classes, clip_denoised, eta, kwargs, z if self.KIND != 2 or sde else None,
-                                        cond_noise, order=order, prev=prev, sde=sde, interval=interval,
-                                        cache=(0, cache_branch, reuse[i]), threshold=threshold, prev_x=prev_x, pag=pag,
-                                        apg=apg, apg_state=apg_state)
-                if apg is not None:
+                                        cond_noise, order=order, prev=prev, sde=sde, prev_x=prev_x, apg_state=apg_state,
+                                        **opts.step_kwargs(reuse[i]))
+                if opts.apg is not None:
                     apg_state = out.apg_state
                 if self.UNIPC:
                     prev, prev_x = ([(t, out.pred_x_0)] + (prev or []))[:order], out.corrected_x_t
@@ -405,8 +390,7 @@ class _NativeSampler:
                     ret.pred_x_0.append(out.pred_x_0)
         elif rng == "philox":
             a, keep = self._step_args(device, classes, clip_denoised, eta, kwargs, seed=seed, hw=shape[-2:], order=order, sde=sde,
-                                      interval=interval, cache=(cache_interval, cache_branch, 0), threshold=threshold, pag=pag,
-                                      apg=apg)
+                                      **opts.step_kwargs())
             a.start_step = start
             traj0 = trajt = None
             if return_trajectory:
@@ -452,9 +436,8 @@ class DdpmSampler(_NativeSampler):
         `apg` (extension): adaptive projected guidance (see `sample`).  `apg_state` is the momentum state the previous step
         returned as `out.apg_state` (None at the first step: zero history); the step returns its own, so steps chained with
         apg_state = out.apg_state reproduce a run, as `prev` / `prev_x` chain the multistep samplers."""
-        return self._sample_once(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, guidance_interval, reuse_features,
-                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers,
-                                 apg=apg, apg_state=apg_state)
+        opts = SamplerOptions(guidance_interval, None, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._sample_once(x_t, t, None, classes, clip_denoised, 0.0, kwargs, noise, opts, reuse_features, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, steps=None, image_size=None, noise=None, classes=None, clip_denoised=False, verbose=True,
@@ -506,10 +489,9 @@ class DdpmSampler(_NativeSampler):
         Needs a classifier-free-guidance framework, classes and strength > 0.  Clipping or dynamic thresholding, the
         multiview guidance and the update read D.  The noise and the torch RNG consumption are unchanged; None (default) is
         the run without it, bit for bit."""
-        return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
-                         pag_layers=pag_layers, apg=apg)
+        opts = SamplerOptions(guidance_interval, cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._run(num, image_size, noise, classes, None, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs, opts,
+                         init=init, init_strength=init_strength)
 
 
 class DdimSampler(_NativeSampler):
@@ -525,9 +507,8 @@ class DdimSampler(_NativeSampler):
         `reuse_features` / `cache_branch` / `dynamic_threshold` / `pag_scale` / `pag_layers` / `apg` / `apg_state` as in
         DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
-        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers,
-                                 apg=apg, apg_state=apg_state)
+        opts = SamplerOptions(guidance_interval, None, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, eta, kw, noise, opts, reuse_features, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, clip_denoised=False, eta=0.0,
@@ -537,10 +518,9 @@ class DdimSampler(_NativeSampler):
         time t - 1 of each step; `cache_interval` / `cache_branch` / `dynamic_threshold` as in DdpmSampler.sample (the replace /
         constrain guidance acts on the thresholded x_0).  `init` / `init_strength`, `pag_scale` / `pag_layers` and `apg` as
         in DdpmSampler.sample (the replace / constrain guidance acts on the APG-guided x_0)."""
-        return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs,
-                         interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
-                         pag_layers=pag_layers, apg=apg)
+        opts = SamplerOptions(guidance_interval, cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._run(num, image_size, noise, classes, steps, clip_denoised, eta, verbose, rng, return_trajectory, kwargs, opts,
+                         init=init, init_strength=init_strength)
 
 
 class DpmSolverSampler(_NativeSampler):
@@ -568,10 +548,9 @@ class DpmSolverSampler(_NativeSampler):
         `cache_branch` and `dynamic_threshold` as for DdimSampler.sample_once (D0, and so pred_x_0, is thresholded);
         `pag_scale` / `pag_layers` and `apg` / `apg_state` as for DdpmSampler.sample_once."""
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
-        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, order=2 if prev is not None else 1, prev=prev, sde=sde,
-                                 dynamic_threshold=dynamic_threshold, pag_scale=pag_scale, pag_layers=pag_layers, apg=apg,
-                                 apg_state=apg_state)
+        opts = SamplerOptions(guidance_interval, None, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, opts, reuse_features,
+                                 order=2 if prev is not None else 1, prev=prev, sde=sde, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
@@ -587,10 +566,9 @@ class DpmSolverSampler(_NativeSampler):
         history holds the PAG-guided D0.  `apg` as in DdpmSampler.sample; the history holds the APG-guided D0.  Same return
         dict as DdimSampler.sample."""
         assert order in (1, 2), f"order must be 1 or 2, got {order}"
-        return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         order=order, sde=bool(sde), interval=guidance_interval, cache_interval=cache_interval,
-                         cache_branch=cache_branch, dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength,
-                         pag_scale=pag_scale, pag_layers=pag_layers, apg=apg)
+        opts = SamplerOptions(guidance_interval, cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs, opts,
+                         order=order, sde=bool(sde), init=init, init_strength=init_strength)
 
 
 class UniPcSampler(_NativeSampler):
@@ -621,9 +599,9 @@ class UniPcSampler(_NativeSampler):
         assert len(prev) <= 3, f"prev holds at most three (t_last, pred_x_0) pairs, got {len(prev)}"
         assert not prev or prev_x is not None, "prev needs prev_x, the previous step's corrected_x_t"
         kw = dict(kwargs, replace_rgb=replace_rgb, replace_depth=replace_depth, constrain_depth=constrain_depth)
-        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, guidance_interval, reuse_features,
-                                 cache_branch, order=order, prev=prev, dynamic_threshold=dynamic_threshold, prev_x=prev_x,
-                                 pag_scale=pag_scale, pag_layers=pag_layers, apg=apg, apg_state=apg_state)
+        opts = SamplerOptions(guidance_interval, None, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._sample_once(x_t, t, t_prev, classes, clip_denoised, 0.0, kw, noise, opts, reuse_features,
+                                 order=order, prev=prev, prev_x=prev_x, apg_state=apg_state)
 
     @torch.no_grad()
     def sample(self, num, image_size=None, noise=None, classes=None, steps=None, order=2, clip_denoised=False, verbose=True,
@@ -637,7 +615,6 @@ class UniPcSampler(_NativeSampler):
         ran, thresholded.  `init` / `init_strength`, `pag_scale` / `pag_layers` and `apg` as in DdpmSampler.sample; the order
         ramp starts at the first executed step.  Same return dict as DdimSampler.sample."""
         assert order in (1, 2, 3), f"order must be 1, 2 or 3, got {order}"
-        return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs,
-                         order=order, interval=guidance_interval, cache_interval=cache_interval, cache_branch=cache_branch,
-                         dynamic_threshold=dynamic_threshold, init=init, init_strength=init_strength, pag_scale=pag_scale,
-                         pag_layers=pag_layers, apg=apg)
+        opts = SamplerOptions(guidance_interval, cache_interval, cache_branch, dynamic_threshold, pag_scale, pag_layers, apg)
+        return self._run(num, image_size, noise, classes, steps, clip_denoised, 0.0, verbose, rng, return_trajectory, kwargs, opts,
+                         order=order, init=init, init_strength=init_strength)

@@ -27,7 +27,7 @@ import bench                                      # noqa: E402  (MODELS, GUIDANC
 import ivid_b200.backbones as backbones           # noqa: E402
 import ivid_b200.frameworks as frameworks         # noqa: E402
 import ivid_b200.samplers as samplers             # noqa: E402
-from ivid_b200.inference.sample import parse_interval   # noqa: E402
+from ivid_b200.samplers.options import parse_interval   # noqa: E402
 from oracle import unet_ref                       # noqa: E402
 
 
